@@ -1,0 +1,358 @@
+// Host-side orchestration of the CLIP-FlanT5 VQAScore forward: CLIP ViT -> projector -> T5 encoder over the spliced sequence -> T5 decoder
+// -> lm_head with the log-softmax gather of the labels. A fixed sequence of kernel launches on the caller's stream.
+#pragma once
+#include "host.cuh"
+#include "attention.cuh"
+#include "attention_sm90.cuh"
+#include "qwen_kernels.cuh"   // cast_f32_bf16_kernel
+
+static int clipt5_finalize(vqa_handle* h) {
+    const vqa_clipt5_config& c = h->cfg;
+    bool ok = true;
+    const int P = (c.image_size / c.patch_size) * (c.image_size / c.patch_size);
+    const int Dv = c.vit_hidden, Dm = c.d_model, inner = c.n_heads * 64;
+    h->patch_w = need(h, "vit.patch_embed.weight", Dv, h->kpad, ok);
+    h->cls = need(h, "vit.class_embedding", Dv, 1, ok);
+    h->pos = need(h, "vit.position_embedding", P + 1, Dv, ok);
+    h->pre_ln_w = need(h, "vit.pre_ln.weight", Dv, 1, ok);
+    h->pre_ln_b = need(h, "vit.pre_ln.bias", Dv, 1, ok);
+    h->vit.resize(c.vit_layers_run);
+    for (int i = 0; i < c.vit_layers_run; ++i) {
+        const std::string p = "vit.layers." + std::to_string(i) + ".";
+        VitLayerW& L = h->vit[i];
+        L.ln1_w = need(h, p + "ln1.weight", Dv, 1, ok); L.ln1_b = need(h, p + "ln1.bias", Dv, 1, ok);
+        L.qkv_w = need(h, p + "qkv.weight", 3 * Dv, Dv, ok); L.qkv_b = need(h, p + "qkv.bias", 3 * Dv, 1, ok);
+        L.out_w = need(h, p + "out.weight", Dv, Dv, ok); L.out_b = need(h, p + "out.bias", Dv, 1, ok);
+        L.ln2_w = need(h, p + "ln2.weight", Dv, 1, ok); L.ln2_b = need(h, p + "ln2.bias", Dv, 1, ok);
+        L.fc1_w = need(h, p + "fc1.weight", c.vit_mlp, Dv, ok); L.fc1_b = need(h, p + "fc1.bias", c.vit_mlp, 1, ok);
+        L.fc2_w = need(h, p + "fc2.weight", Dv, c.vit_mlp, ok); L.fc2_b = need(h, p + "fc2.bias", Dv, 1, ok);
+    }
+    h->proj0_w = need(h, "proj.0.weight", Dm, Dv, ok); h->proj0_b = need(h, "proj.0.bias", Dm, 1, ok);
+    h->proj2_w = need(h, "proj.2.weight", Dm, Dm, ok); h->proj2_b = need(h, "proj.2.bias", Dm, 1, ok);
+    h->shared = need(h, "t5.shared", c.vocab, Dm, ok);
+    h->enc_rel = need(h, "t5.enc.rel_bias", c.rel_buckets, c.n_heads, ok);
+    h->dec_rel = need(h, "t5.dec.rel_bias", c.rel_buckets, c.n_heads, ok);
+    h->enc_final_ln = need(h, "t5.enc.final_ln", Dm, 1, ok);
+    h->dec_final_ln = need(h, "t5.dec.final_ln", Dm, 1, ok);
+    h->lm_head = need(h, "t5.lm_head", c.vocab, Dm, ok);
+    h->enc.resize(c.enc_layers);
+    for (int i = 0; i < c.enc_layers; ++i) {
+        const std::string p = "t5.enc." + std::to_string(i) + ".";
+        T5EncLayerW& L = h->enc[i];
+        L.ln0 = need(h, p + "ln0", Dm, 1, ok); L.qkv = need(h, p + "qkv", 3 * inner, Dm, ok);
+        L.o = need(h, p + "o", Dm, inner, ok); L.ln1 = need(h, p + "ln1", Dm, 1, ok);
+        L.wi = need(h, p + "wi", 2 * c.d_ff, Dm, ok); L.wo = need(h, p + "wo", Dm, c.d_ff, ok);
+        if (c.emulate_bf16_rounding & VQA_FLAG_FUSE_NORMS) {
+            L.qkv_g = need(h, p + "qkv_g", 3 * inner, Dm, ok);
+            L.wi_g = need(h, p + "wi_g", 2 * c.d_ff, Dm, ok);
+        }
+    }
+    h->dec.resize(c.dec_layers);
+    for (int i = 0; i < c.dec_layers; ++i) {
+        const std::string p = "t5.dec." + std::to_string(i) + ".";
+        T5DecLayerW& L = h->dec[i];
+        L.ln0 = need(h, p + "ln0", Dm, 1, ok); L.qkv = need(h, p + "qkv", 3 * inner, Dm, ok);
+        L.o = need(h, p + "o", Dm, inner, ok); L.ln1 = need(h, p + "ln1", Dm, 1, ok);
+        L.cq = need(h, p + "cq", inner, Dm, ok); L.ckv = need(h, p + "ckv", 2 * inner, Dm, ok);
+        L.co = need(h, p + "co", Dm, inner, ok); L.ln2 = need(h, p + "ln2", Dm, 1, ok);
+        L.wi = need(h, p + "wi", 2 * c.d_ff, Dm, ok); L.wo = need(h, p + "wo", Dm, c.d_ff, ok);
+        L.ckT = nullptr;
+        if (c.cross_attention_mode == 0) L.ckT = need(h, p + "ckT", Dm, inner, ok);
+    }
+    return ok ? VQA_OK : VQA_ERR_MISSING_WEIGHT;
+}
+
+// ------------------------------------------------------------------------------------------------ workspace plan
+struct ClipT5Workspace {
+    // vision
+    size_t patches, patch_out, hv, vn, vqkv, vattn, vmlp, proj1, proj2;
+    // t5
+    size_t x, xn, qkv, attn, ff, bias_table, seq_lens, ckv, ssq_a, ssq_b;
+    size_t y, yn, dqkv, dattn, dq, dff, splitk, splitk_bytes;
+    size_t xt, qt, csc, cctx;   // absorbed cross-attention: Xenc^T, q~ = Wk^T q, scores/probs, context sum p.h
+    size_t lse_max, lse_sum, label_logit;
+    size_t total;
+};
+static int ssq_stride(int d_model) { return (d_model / 32 + 3) / 4 * 4; }
+static ClipT5Workspace plan_workspace(const vqa_handle* h, int B, int NI, int L, int T) {
+    const vqa_clipt5_config& c = h->cfg;
+    const int P = (c.image_size / c.patch_size) * (c.image_size / c.patch_size);
+    const size_t Mv = (size_t)NI * (P + 1), Mp = (size_t)NI * P;
+    const int S = L - 1 + P;
+    const size_t M = (size_t)B * S, Md = (size_t)B * T;
+    const size_t inner = (size_t)c.n_heads * 64;
+    Plan pl;
+    ClipT5Workspace w;
+    w.patches = pl.take(Mp * h->kpad * 2);
+    w.patch_out = pl.take(Mp * c.vit_hidden * 2);
+    w.hv = pl.take(Mv * c.vit_hidden * 4);      // fp32: the vision tower's residual stream (see the vision loop)
+    w.vn = pl.take(Mv * c.vit_hidden * 2);
+    w.vqkv = pl.take(Mv * 3 * c.vit_hidden * 2);
+    w.vattn = pl.take(Mv * c.vit_hidden * 2);
+    w.vmlp = pl.take(Mv * c.vit_mlp * 2);
+    w.proj1 = pl.take(Mv * c.d_model * 2);
+    w.proj2 = pl.take(Mv * c.d_model * 2);
+    w.x = pl.take(M * c.d_model * 2);
+    w.xn = pl.take(M * c.d_model * 2);
+    w.qkv = pl.take(M * 3 * inner * 2);
+    w.attn = pl.take(M * inner * 2);
+    w.ff = pl.take(M * c.d_ff * 2);
+    // fused-norm mode: per-row partial sums of squares of the residual stream, two buffers (the stream is rewritten twice per layer);
+    // worst case one partial per 32 output columns
+    w.ssq_a = pl.take(M * (size_t)ssq_stride(c.d_model) * 4);
+    w.ssq_b = pl.take(M * (size_t)ssq_stride(c.d_model) * 4);
+    w.bias_table = pl.take((size_t)c.n_heads * (2 * S - 1) * 4);
+    w.seq_lens = pl.take((size_t)B * 4);
+    const size_t Sp = (size_t)(S + 7) / 8 * 8;
+    const size_t TH = (size_t)T * c.n_heads;
+    if (c.cross_attention_mode == 0) {
+        w.ckv = 0;
+        w.xt = pl.take((size_t)B * c.d_model * Sp * 2);
+        w.qt = pl.take((size_t)B * TH * c.d_model * 2);
+        w.csc = pl.take(((size_t)B * TH + 256) * Sp * 2);
+        w.cctx = pl.take((size_t)B * TH * c.d_model * 2);
+    } else {
+        w.ckv = pl.take(M * 2 * inner * 2);
+        w.xt = w.qt = w.csc = w.cctx = 0;
+    }
+    w.y = pl.take(Md * c.d_model * 2);
+    w.yn = pl.take(Md * c.d_model * 2);
+    w.dqkv = pl.take(Md * 3 * inner * 2);
+    w.dattn = pl.take(Md * inner * 2);
+    w.dq = pl.take(Md * inner * 2);
+    w.dff = pl.take(Md * c.d_ff * 2);
+    {   // fp32 partial tiles of the decoder's split-K GEMMs (largest of the eligible shapes; 0 when none is)
+        size_t sk = 0;
+        const int shapes[4][2] = {{(int)(3 * inner), c.d_model}, {c.d_model, (int)inner}, {(int)inner, c.d_model}, {c.d_model, c.d_ff}};
+        for (const auto& nk : shapes) {
+            const int s = splitk_slices((int)Md, nk[0], nk[1], h->num_sms);
+            if (s > 1) sk = std::max(sk, (size_t)s * Md * nk[0] * 4);
+        }
+        w.splitk = pl.take(sk);
+        w.splitk_bytes = sk;
+    }
+    const size_t ntiles = (size_t)LMHEAD_PARTS * ((c.vocab + LMHEAD_BN - 1) / LMHEAD_BN);
+    w.lse_max = pl.take(Md * ntiles * 4);
+    w.lse_sum = pl.take(Md * ntiles * 4);
+    w.label_logit = pl.take(Md * 4);
+    w.total = pl.off;
+    return w;
+}
+
+// Sum of squares of every row of x (bf16 [rows, D]) into slot 0 of its partial-sum row (the other slots are zero): seeds the fused
+// RMSNorm chain for the encoder's input embeddings. One warp per row.
+__global__ void __launch_bounds__(256) row_ssq_kernel(const bf16* __restrict__ x, float* __restrict__ ssq, int rows, int D, int stride) {
+    pdl_launch_dependents();
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= rows) return;
+    const int lane = threadIdx.x & 31;
+    const uint4* xr = reinterpret_cast<const uint4*>(x + (size_t)row * D);
+    float ss = 0.f;
+    for (int i = lane; i < D / 8; i += 32) {
+        const uint4 v = xr[i];
+        const uint32_t* u = reinterpret_cast<const uint32_t*>(&v);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = unpack_bf16x2(u[e]);
+            ss = fmaf(f.x, f.x, ss);
+            ss = fmaf(f.y, f.y, ss);
+        }
+    }
+    ss = warp_sum(ss);
+    if (lane == 0) ssq[(size_t)row * stride] = ss;
+}
+
+// ------------------------------------------------------------------------------------------------ forward
+// Arguments as vqa_clipt5_score, already validated.
+static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int n_images, const int* image_index, const int* input_ids,
+                        const int* text_lens, const int* labels, int B, int L, int T, float* out_scores, float* out_logprobs, void* workspace,
+                        size_t workspace_bytes, cudaStream_t st) {
+    const vqa_clipt5_config& c = h->cfg;
+    const ClipT5Workspace w = plan_workspace(h, B, n_images, L, T);
+    if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+    Forward f(h, workspace, st);
+    auto P_ = [&](size_t off) { return f.at(off); };
+    const int rnd = c.emulate_bf16_rounding & VQA_FLAG_ROUND_DECODER;
+    const bool round_attn = (c.emulate_bf16_rounding & VQA_FLAG_ROUND_ATTN_SCORES) != 0;
+    const bool fuse_norms = (c.emulate_bf16_rounding & VQA_FLAG_FUSE_NORMS) != 0;
+
+    const int grid_w = c.image_size / c.patch_size;
+    const int P = grid_w * grid_w;
+    const int Dv = c.vit_hidden, Dm = c.d_model, H = c.n_heads, inner = H * 64, Hv = c.vit_heads;
+    const int Mp = n_images * P, Mv = n_images * (P + 1);
+    const int S = L - 1 + P;
+    const int M = B * S, Md = B * T;
+
+    // Precision of the vision tower's residual stream: the reference runs CLIPVisionModel under torch.autocast(bf16). nn.LayerNorm is on
+    // autocast's fp32 list, so pre_layrnorm hands the encoder an fp32 tensor, every `residual + hidden_states` (modeling_clip.py:371,
+    // :376) promotes to fp32, and only the Linear inputs are cast to bf16. hidden_states[-2] is therefore an fp32 tensor, rounded to
+    // bf16 once where the projector's first Linear consumes it. The engine keeps the same: hv is fp32, the out_proj / fc2 epilogues add
+    // the bf16 Linear output into it unrounded, the LayerNorms read fp32 and write the bf16 GEMM operand.
+    float* hv = f.at<float>(w.hv);
+
+    // ---------------- vision tower (CLIP ViT, layers 0 .. vit_layers_run-1; hidden_states[-2]) ----------------
+    if (pixel_dtype == VQA_DTYPE_F32)
+        TRY(f.launch(CAT_OTHER, 0, "patchify", patchify_kernel<float>, Mp, 128, 0, reinterpret_cast<const float*>(pixels), P_(w.patches),
+                     n_images, c.image_size, c.image_size, c.patch_size, h->kpad));
+    else
+        TRY(f.launch(CAT_OTHER, 0, "patchify", patchify_kernel<bf16>, Mp, 128, 0, reinterpret_cast<const bf16*>(pixels), P_(w.patches),
+                     n_images, c.image_size, c.image_size, c.patch_size, h->kpad));
+    TRY(f.gemm(Gemm(P_(w.patches), h->patch_w, P_(w.patch_out), Mp, Dv, h->kpad)));
+    if (Dv == 1024)
+        TRY(f.launch(CAT_NORM, 0, "clip_embed_ln", clip_embed_ln_kernel<1024>, (Mv + 7) / 8, 256, 0, P_(w.patch_out), h->cls, h->pos,
+                     h->pre_ln_w, h->pre_ln_b, hv, n_images, P, c.vit_ln_eps));
+    else if (Dv == 256)
+        TRY(f.launch(CAT_NORM, 0, "clip_embed_ln", clip_embed_ln_kernel<256>, (Mv + 7) / 8, 256, 0, P_(w.patch_out), h->cls, h->pos,
+                     h->pre_ln_w, h->pre_ln_b, hv, n_images, P, c.vit_ln_eps));
+    else
+        return fail(h, VQA_ERR_UNSUPPORTED, "vit_hidden must be 1024 or 256");
+    for (int l = 0; l < c.vit_layers_run; ++l) {
+        const VitLayerW& Lw = h->vit[l];
+        TRY(f.layernorm_f32(hv, Lw.ln1_w, Lw.ln1_b, P_(w.vn), Mv, Dv, c.vit_ln_eps));
+        TRY(f.gemm(Gemm(P_(w.vn), Lw.qkv_w, P_(w.vqkv), Mv, 3 * Dv, Dv).with_bias(Lw.qkv_b)));
+        TRY(f.attention(4.0 * n_images * (double)Hv * (P + 1) * (P + 1) * 64, "vit attention", [&] {
+            return launch_attn_tc(P_(w.vqkv), 3 * Dv, 0, Dv, 2 * Dv, P_(w.vattn), Dv, n_images, P + 1, Hv, nullptr, nullptr, 0.125f, 0,
+                                  round_attn, st);
+        }));
+        TRY(f.gemm(Gemm(P_(w.vattn), Lw.out_w, hv, Mv, Dv, Dv).with_bias(Lw.out_b).accumulate_f32(), "gemm (fp32 residual)"));
+        TRY(f.layernorm_f32(hv, Lw.ln2_w, Lw.ln2_b, P_(w.vn), Mv, Dv, c.vit_ln_eps));
+        TRY(f.gemm(Gemm(P_(w.vn), Lw.fc1_w, P_(w.vmlp), Mv, c.vit_mlp, Dv).with_bias(Lw.fc1_b).with_epilogue(EPI_QUICK_GELU)));
+        TRY(f.gemm(Gemm(P_(w.vmlp), Lw.fc2_w, hv, Mv, Dv, c.vit_mlp).with_bias(Lw.fc2_b).accumulate_f32(), "gemm (fp32 residual)"));
+    }
+    // hidden_states[-2] -> bf16 (`.to(images.dtype)` / the projector Linear's autocast cast): the single rounding of the tower's output
+    const size_t n_hv = (size_t)Mv * Dv;
+    TRY(f.launch(CAT_OTHER, 0, "vision output cast", cast_f32_bf16_kernel, (unsigned)((n_hv / 4 + 255) / 256 + 1), 256, 0, hv, P_(w.vn), n_hv));
+    // mlp2x_gelu projector (Linear -> GELU(erf) -> Linear), applied to every row; the CLS rows are simply not spliced
+    TRY(f.gemm(Gemm(P_(w.vn), h->proj0_w, P_(w.proj1), Mv, Dm, Dv).with_bias(h->proj0_b).with_epilogue(EPI_GELU_ERF)));
+    TRY(f.gemm(Gemm(P_(w.proj1), h->proj2_w, P_(w.proj2), Mv, Dm, Dm).with_bias(h->proj2_b)));
+
+    // ---------------- multimodal splice -> T5 encoder input ----------------
+    int* seq_lens = f.at<int>(w.seq_lens);
+    float* bias_table = f.at<float>(w.bias_table);
+    {
+        auto g = f.group(CAT_OTHER);
+        // feature block of an image = P + 1 rows, first patch row = 1 (drop CLS: mm_vision_select_feature='patch')
+        TRY(f.launch(CAT_OTHER, 0, "splice", splice_embed_kernel, B * S, 128, 0, input_ids, text_lens, image_index, h->shared, P_(w.proj2),
+                     Dm, 1, P + 1, P_(w.x), seq_lens, B, L, S, P, Dm, c.image_token_id));
+        TRY(f.launch(CAT_OTHER, 0, "bias table", bias_table_from_lut_kernel, (H * (2 * S - 1) + 255) / 256, 256, 0, h->enc_rel, h->lut_bidir,
+                     c.rel_max_distance, bias_table, H, S));
+    }
+
+    // ---------------- T5 encoder ----------------
+    // fuse_norms: the two T5LayerNorms of a layer never run as kernels. The GEMMs that write the residual stream (o, wo) leave per-row
+    // partial sums of squares of what they stored; the GEMMs that read it (qkv, wi) take x itself with gamma folded into their weights and
+    // scale their accumulator rows by rsqrt(mean(x^2) + eps) in the epilogue (gemm_sm90.cuh, GemmParams::ssq_*).
+    NormFuse nf_cons, nf_prod;
+    float* ssq_cur = f.at<float>(w.ssq_a);
+    float* ssq_nxt = f.at<float>(w.ssq_b);
+    if (fuse_norms) {
+        const int parts = ssq_parts_for(pick_variant(M, Dm, EPI_STORE), Dm);
+        const int stride = (parts + 3) / 4 * 4;
+        if (stride > ssq_stride(Dm)) return fail(h, VQA_ERR_UNSUPPORTED, "fused norms: partial-sum stride exceeds the workspace plan");
+        nf_cons.stride = nf_prod.stride = stride;
+        nf_cons.inv_dim = 1.0f / (float)Dm;
+        nf_cons.eps = c.t5_ln_eps;
+        auto g = f.group(CAT_NORM);
+        TRY(f.memset0(ssq_cur, (size_t)M * stride * 4, "ssq clear"));
+        TRY(f.memset0(ssq_nxt, (size_t)M * stride * 4, "ssq clear"));
+        TRY(f.launch(CAT_NORM, 0, "row ssq", row_ssq_kernel, (M + 7) / 8, 256, 0, P_(w.x), ssq_cur, M, Dm, stride));
+    }
+    for (int l = 0; l < c.enc_layers; ++l) {
+        const T5EncLayerW& Lw = h->enc[l];
+        if (fuse_norms) {
+            nf_cons.ssq_in = ssq_cur;
+            TRY(f.gemm(Gemm(P_(w.x), Lw.qkv_g, P_(w.qkv), M, 3 * inner, Dm).with_norm(nf_cons)));
+        } else {
+            TRY(f.rmsnorm(P_(w.x), Lw.ln0, P_(w.xn), M, Dm, c.t5_ln_eps));
+            TRY(f.gemm(Gemm(P_(w.xn), Lw.qkv, P_(w.qkv), M, 3 * inner, Dm)));
+        }
+        TRY(f.attention(4.0 * B * (double)H * S * S * 64, "t5 encoder attention", [&] {
+            return launch_attn_tc(P_(w.qkv), 3 * inner, 0, inner, 2 * inner, P_(w.attn), inner, B, S, H, seq_lens, bias_table, 1.0f,
+                                  c.rel_max_distance, round_attn, st);
+        }));
+        if (fuse_norms) {
+            nf_prod.ssq_out = ssq_nxt;
+            TRY(f.gemm(Gemm(P_(w.attn), Lw.o, P_(w.x), M, Dm, inner).with_residual(P_(w.x)).with_norm(nf_prod)));
+            std::swap(ssq_cur, ssq_nxt);
+            nf_cons.ssq_in = ssq_cur;
+            TRY(f.gemm(Gemm(P_(w.x), Lw.wi_g, P_(w.ff), M, 2 * c.d_ff, Dm).with_epilogue(EPI_GATED_GELU, c.d_ff).with_norm(nf_cons)));
+            nf_prod.ssq_out = ssq_nxt;
+            TRY(f.gemm(Gemm(P_(w.ff), Lw.wo, P_(w.x), M, Dm, c.d_ff).with_residual(P_(w.x)).with_norm(nf_prod)));
+            std::swap(ssq_cur, ssq_nxt);
+        } else {
+            TRY(f.gemm(Gemm(P_(w.attn), Lw.o, P_(w.x), M, Dm, inner).with_residual(P_(w.x))));
+            TRY(f.rmsnorm(P_(w.x), Lw.ln1, P_(w.xn), M, Dm, c.t5_ln_eps));
+            TRY(f.gemm(Gemm(P_(w.xn), Lw.wi, P_(w.ff), M, 2 * c.d_ff, Dm).with_epilogue(EPI_GATED_GELU, c.d_ff)));
+            TRY(f.gemm(Gemm(P_(w.ff), Lw.wo, P_(w.x), M, Dm, c.d_ff).with_residual(P_(w.x))));
+        }
+    }
+    TRY(f.rmsnorm(P_(w.x), h->enc_final_ln, P_(w.xn), M, Dm, c.t5_ln_eps));  // encoder output lives in xn from here on
+    const int Sp = (S + 7) / 8 * 8;
+    if (c.cross_attention_mode == 0)
+        TRY(f.launch(CAT_OTHER, 0, "encoder transpose", transpose_bsd_kernel, dim3((Sp + 31) / 32, (Dm + 31) / 32, B), dim3(32, 8), 0,
+                     P_(w.xn), P_(w.xt), S, Dm, Sp));
+
+    // ---------------- T5 decoder (T target rows per pair) ----------------
+    TRY(f.launch(CAT_OTHER, 0, "decoder embed", decoder_embed_kernel, Md, 128, 0, labels, h->shared, P_(w.y), T, Dm, c.decoder_start_id,
+                 c.pad_token_id));
+    // decoder store-GEMMs: M = B*T rows against 4096-row weights -> split-K when that fills the SMs, else the plain path
+    auto dec = [&](Gemm g) {
+        const int sl = splitk_slices(g.M, g.N, g.K, f.nsm);
+        if (sl > 1 && (size_t)sl * g.M * g.N * 4 <= w.splitk_bytes) g.split_k(sl, f.at<float>(w.splitk));
+        return g;
+    };
+    for (int l = 0; l < c.dec_layers; ++l) {
+        const T5DecLayerW& Lw = h->dec[l];
+        // self-attention
+        TRY(f.rmsnorm(P_(w.y), Lw.ln0, P_(w.yn), Md, Dm, c.t5_ln_eps));
+        TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.qkv, P_(w.dqkv), Md, 3 * inner, Dm))));
+        TRY(f.launch(CAT_ATTENTION, 4.0 * B * (double)H * T * T * 64, "decoder self attention", t5_decoder_self_attn_kernel, (B * H * T + 3) / 4,
+                     128, 4 * T * sizeof(float), P_(w.dqkv), P_(w.dattn), h->dec_rel, h->lut_unidir, c.rel_max_distance, B, T, H, rnd));
+        TRY(f.gemm(dec(Gemm(P_(w.dattn), Lw.o, P_(w.y), Md, Dm, inner).with_residual(P_(w.y)))));
+        TRY(f.rmsnorm(P_(w.y), Lw.ln1, P_(w.yn), Md, Dm, c.t5_ln_eps));
+        TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.cq, P_(w.dq), Md, inner, Dm))));
+        if (c.cross_attention_mode != 0) {
+            // reference association: K/V projection of all S encoder rows in every layer (modeling_t5.py:297-299)
+            TRY(f.gemm(Gemm(P_(w.xn), Lw.ckv, P_(w.ckv), M, 2 * inner, Dm)));
+            TRY(f.launch(CAT_ATTENTION, 4.0 * B * (double)H * T * S * 64, "cross attention", t5_cross_attn_kernel<8>, B * H, 128, 0, P_(w.dq),
+                         P_(w.ckv), P_(w.dattn), seq_lens, 2 * inner, B, T, S, H, rnd));
+        } else {
+            // absorbed association (exact in real arithmetic; 30x fewer FLOPs because only T rows per pair attend):
+            //   q.(Wk x_s) = (Wk^T q).x_s          sum_s p_s (Wv x_s) = Wv (sum_s p_s x_s)
+            const int TH = T * H;
+            // (1) q~[b,t,h,:] = Wk[h]^T q[b,t,h,:]   -- per head: [B*T, 64] x ckT[:, h*64:(h+1)*64]^T -> rows (b*T+t)*H + h
+            Gemm g1(P_(w.dq), Lw.ckT, P_(w.qt), Md, Dm, 64);
+            g1.lda = inner; g1.ldw = inner; g1.ldc = H * Dm;
+            TRY(f.gemm(g1.batched(BatchSpec{H, 0, 64, 0, 64, (long long)Dm, Md, inner, Dm, inner}, Dm >= 256 ? 2561 : 1281), "batched gemm"));
+            // (2) scores[b,(t,h),s] = q~[b,(t,h),:] . x[b,s,:]   -- per pair: [T*H, d] x [S, d]^T
+            Gemm g2(P_(w.qt), P_(w.xn), P_(w.csc), TH, Sp, Dm);
+            TRY(f.gemm(g2.batched(BatchSpec{B, TH, 0, S, 0, (long long)TH * Sp, (long long)B * TH, Dm, (long long)B * S, Dm}, 1281), "batched gemm"));
+            TRY(f.launch(CAT_ATTENTION, 0, "cross softmax", cross_softmax_kernel, (B * TH + 7) / 8, 256, 0, P_(w.csc), seq_lens, TH, B * TH, S, Sp));
+            // (3) ctx[b,(t,h),:] = sum_s p[b,(t,h),s] x[b,s,:]   -- per pair: [T*H, Sp] x (x[b]^T)[d, Sp]^T
+            Gemm g3(P_(w.csc), P_(w.xt), P_(w.cctx), TH, Dm, Sp);
+            TRY(f.gemm(g3.batched(BatchSpec{B, TH, 0, Dm, 0, (long long)TH * Dm, (long long)B * TH, Sp, (long long)B * Dm, Sp}, Dm >= 256 ? 2561 : 1281),
+                       "batched gemm"));
+            // (4) o[b,t,h,:] = Wv[h] ctx[b,t,h,:]   -- per head: [B*T, d] (cols h*d..) x Wv[h*64:(h+1)*64, :]^T -> cols h*64..
+            Gemm g4(P_(w.cctx), Lw.ckv + (size_t)inner * Dm, P_(w.dattn), Md, 64, Dm);
+            g4.lda = H * Dm; g4.ldc = inner;
+            TRY(f.gemm(g4.batched(BatchSpec{H, 0, Dm, 64, 0, 64, Md, (long long)H * Dm, inner, Dm}, 641), "batched gemm"));
+        }
+        TRY(f.gemm(dec(Gemm(P_(w.dattn), Lw.co, P_(w.y), Md, Dm, inner).with_residual(P_(w.y)))));
+        // gated FFN
+        TRY(f.rmsnorm(P_(w.y), Lw.ln2, P_(w.yn), Md, Dm, c.t5_ln_eps));
+        TRY(f.gemm(Gemm(P_(w.yn), Lw.wi, P_(w.dff), Md, 2 * c.d_ff, Dm).with_epilogue(EPI_GATED_GELU, c.d_ff)));
+        TRY(f.gemm(dec(Gemm(P_(w.dff), Lw.wo, P_(w.y), Md, Dm, c.d_ff).with_residual(P_(w.y)))));
+    }
+    TRY(f.rmsnorm(P_(w.y), h->dec_final_ln, P_(w.yn), Md, Dm, c.t5_ln_eps));
+
+    // ---------------- lm_head x hidden, fused log-sum-exp + label gather; logits never reach HBM ----------------
+    float* lse_max = f.at<float>(w.lse_max);
+    float* lse_sum = f.at<float>(w.lse_sum);
+    float* label_logit = f.at<float>(w.label_logit);
+    const int ntiles = LMHEAD_PARTS * ((c.vocab + LMHEAD_BN - 1) / LMHEAD_BN);
+    TRY(f.gemm(Gemm(P_(w.yn), h->lm_head, nullptr, Md, c.vocab, Dm).lse(labels, lse_max, lse_sum, label_logit), "lm_head"));
+    TRY(f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, lse_max, lse_sum, label_logit, labels, out_scores,
+                 out_logprobs, B, T, ntiles));
+    return VQA_OK;
+}

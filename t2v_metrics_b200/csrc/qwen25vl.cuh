@@ -1,7 +1,9 @@
 // Host-side orchestration of the Qwen2.5-VL VQAScore forward: P(answer token | image, question) for a batch of prompts
 // in ONE prefill (the reference runs generate(max_new_tokens=1) per sample: qwen2vl_model.py:190-230).
-// Included by vqa_b200.cu (it uses that file's handle, GEMM/norm wrappers and ProfScope).
 #pragma once
+#include "host.cuh"
+#include "attention_sm90.cuh"
+#include "qwen_kernels.cuh"
 
 struct QwenVisLayerW {
     const bf16 *norm1, *norm2, *qkv_w, *qkv_b, *proj_w, *proj_b, *gu_w, *gu_b, *down_w, *down_b;
@@ -131,184 +133,123 @@ static int qwen_score(vqa_handle* h, QwenState& q, const void* pixel_patches, in
     const vqa_qwen25vl_config& c = q.cfg;
     const QwenWorkspace w = pk ? qwen_plan_rows(c, B, (size_t)pk->total_rows, n_patches) : qwen_plan(c, B, S, n_patches);
     if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
-    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    auto P_ = [&](size_t off) { return reinterpret_cast<bf16*>(ws + off); };
-    auto F_ = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
-    auto P8_ = [&](size_t off) { return ws + off; };
-    h->launches = 0;
-    h->prof.clear();
-    h->ev_used = 0;
-    int64_t* lc = &h->launches;
-    const int nsm = h->num_sms;
-#define TRY(x) do { int _rc = (x); if (_rc) return _rc; } while (0)
-    auto cuda_ok = [&](cudaError_t e, const char* what) -> int {
-        if (e == cudaSuccess) e = cudaGetLastError();
-        if (e != cudaSuccess) return fail(h, VQA_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-        return 0;
-    };
-    auto gemm = [&](const bf16* A, int lda, const bf16* W, int ldw, int w_rows, bf16* C, int ldc, int M_, int N_, int K_,
-                    const bf16* bias, const bf16* res, int ldr, int epi, int gate_off) -> int {
-        const double n_out = epi_is_gated(epi) ? N_ / 2 : N_;
-        const double bytes = 2.0 * ((double)M_ * K_ + (double)N_ * K_ + (double)M_ * n_out * (res ? 2 : 1));
-        ProfScope ps(h, CAT_GEMM, 2.0 * M_ * (double)N_ * K_, st, bytes);
-        return cuda_ok(run_gemm(A, lda, W, ldw, w_rows, C, ldc, M_, N_, K_, bias, res, ldr, epi, gate_off, 0, nsm, st, lc), "gemm");
-    };
-    auto rms = [&](const bf16* x, const bf16* wgt, bf16* y, int rows, int D_) -> int {
-        ProfScope ps(h, CAT_NORM, 0, st);
-        return cuda_ok(run_rmsnorm(x, wgt, y, rows, D_, c.rms_eps, st, lc), "rmsnorm");
-    };
+    Forward f(h, workspace, st);
+    auto P_ = [&](size_t off) { return f.at(off); };
+    auto F_ = [&](size_t off) { return f.at<float>(off); };
     const int L = n_patches, Dv = c.vit_hidden, Hv = c.vit_heads, hdv = c.vit_head_dim;
     const int unit = c.spatial_merge * c.spatial_merge, mlp_pad = qwen_mlp_pad(c.vit_mlp);
     const int D = c.hidden, M = pk ? pk->total_rows : B * S;
 
     // ---------------- vision tower ----------------
     {
-        ProfScope ps(h, CAT_OTHER, 0, st);
-        *lc += 3;
+        auto g = f.group(CAT_OTHER);
         const size_t n = (size_t)L * c.patch_dim;
-        bf16* patches = P_(w.patches);
         if (pixel_dtype == VQA_DTYPE_F32)
-            cast_f32_bf16_kernel<<<(unsigned)((n / 4 + 255) / 256 + 1), 256, 0, st>>>(reinterpret_cast<const float*>(pixel_patches), patches, n);
+            TRY(f.launch(CAT_OTHER, 0, "pixel cast", cast_f32_bf16_kernel, (unsigned)((n / 4 + 255) / 256 + 1), 256, 0,
+                         reinterpret_cast<const float*>(pixel_patches), P_(w.patches), n));
         else
-            CUDA_TRY(h, cudaMemcpyAsync(patches, pixel_patches, n * 2, cudaMemcpyDeviceToDevice, st));
+            TRY(f.copy(P_(w.patches), pixel_patches, n * 2, "pixel copy"));
         // rotary table of the (already window-ordered) patch positions: [h freqs | w freqs] duplicated (:404-409, :487)
-        rope_table_kernel<<<(L * (hdv / 2) + 255) / 256, 256, 0, st>>>(vis_pos_hw, L, q.vis_axis, q.vis_inv_freq, hdv / 2, F_(w.vcos), F_(w.vsin), 0);
-        TRY(cuda_ok(cudaSuccess, "vision prologue"));
+        TRY(f.launch(CAT_OTHER, 0, "vision rope table", rope_table_kernel, (L * (hdv / 2) + 255) / 256, 256, 0, vis_pos_hw, L, q.vis_axis,
+                     q.vis_inv_freq, hdv / 2, F_(w.vcos), F_(w.vsin), 0));
     }
     // patch embedding (Conv3d == GEMM), then re-order 2x2 groups into window order (:470-472)
-    TRY(gemm(P_(w.patches), c.patch_dim, q.patch_w, c.patch_dim, Dv, P_(w.vxn), Dv, L, Dv, c.patch_dim, nullptr, nullptr, 0, EPI_STORE, 0));
+    TRY(f.gemm(Gemm(P_(w.patches), q.patch_w, P_(w.vxn), L, Dv, c.patch_dim)));
     {
-        ProfScope ps(h, CAT_OTHER, 0, st);
-        ++*lc;
-        gather_rows_kernel<<<L, 128, 0, st>>>(P_(w.vxn), P_(w.vx), window_index, unit, Dv);
-        TRY(cuda_ok(cudaSuccess, "window reorder"));
-        if (hdv < 128) {   // the qkv GEMMs write head_dim of every 128-wide head slot; the attention kernel contracts q.k over all 128: zero the rest once
-            ++*lc;
-            CUDA_TRY(h, cudaMemsetAsync(P_(w.vqkv), 0, (size_t)L * 3 * Hv * 128 * 2, st));
-        }
+        auto g = f.group(CAT_OTHER);
+        TRY(f.launch(CAT_OTHER, 0, "window reorder", gather_rows_kernel, L, 128, 0, P_(w.vxn), P_(w.vx), window_index, unit, Dv));
+        // the qkv GEMMs write head_dim of every 128-wide head slot; the attention kernel contracts q.k over all 128: zero the rest once
+        if (hdv < 128) TRY(f.memset0(P_(w.vqkv), (size_t)L * 3 * Hv * 128 * 2, "vision qkv clear"));
     }
     const float vscale = 1.0f / sqrtf((float)hdv);
     for (int l = 0; l < c.vit_depth; ++l) {
         const QwenVisLayerW& Lw = q.vis[l];
         const bool full = (c.fullatt_mask >> l) & 1ull;
-        TRY(rms(P_(w.vx), Lw.norm1, P_(w.vxn), L, Dv));
-        {
-            const double nq = 3.0 * Hv * hdv;
-            ProfScope ps(h, CAT_GEMM, 2.0 * L * nq * Dv, st, 2.0 * ((double)L * Dv + nq * Dv + (double)L * nq));
-            TRY(cuda_ok(run_gemm(P_(w.vxn), Dv, Lw.qkv_w, Dv, 3 * Hv * hdv, P_(w.vqkv), 3 * Hv * 128, L, 3 * Hv * hdv, Dv, Lw.qkv_b, nullptr, 0, EPI_STORE,
-                                 0, 0, nsm, st, lc, false, nullptr, hdv < 128 ? hdv : 0, 128), "vision qkv gemm"));
-        }
-        {
-            ProfScope ps(h, CAT_OTHER, 0, st);
-            ++*lc;
-            const long long nthr = (long long)L * 2 * Hv * (hdv / 16);
-            rope_inplace_kernel<<<(unsigned)((nthr + 255) / 256), 256, 0, st>>>(P_(w.vqkv), 3 * Hv * 128, 0, 2 * Hv, 128, hdv, F_(w.vcos),
-                                                                            F_(w.vsin), L, 0);
-            TRY(cuda_ok(cudaSuccess, "vision rope"));
-        }
-        {
-            const int nseq = full ? n_frames : n_windows, mlen = full ? max_frame_len : max_window_len;
-            ProfScope ps(h, CAT_ATTENTION, 4.0 * (double)L * mlen * Hv * hdv, st);
-            ++*lc;
-            static const bool no_pairs = getenv("VQA_ATTN128_NO_PAIRS") != nullptr;     // A/B switch
-            TRY(cuda_ok(launch_attn_tc128(P_(w.vqkv), 3 * Hv * 128, L, 0, Hv * 128, 2 * Hv * 128, P_(w.vattn), Hv * hdv, nseq, mlen, 0, Hv, 1,
-                                          full ? cu_frames : cu_window, nullptr, vscale, false, st, nullptr,
-                                          /*two windows per tile*/ !full && max_window_len <= 64 && !no_pairs, /*compact heads*/ hdv, hdv),
-                        "vision attention"));
-        }
-        TRY(gemm(P_(w.vattn), Hv * hdv, Lw.proj_w, Hv * hdv, Dv, P_(w.vx), Dv, L, Dv, Hv * hdv, Lw.proj_b, P_(w.vx), Dv, EPI_STORE, 0));
-        TRY(rms(P_(w.vx), Lw.norm2, P_(w.vxn), L, Dv));
-        TRY(gemm(P_(w.vxn), Dv, Lw.gu_w, Dv, 2 * mlp_pad, P_(w.vff), mlp_pad, L, 2 * mlp_pad, Dv, Lw.gu_b, nullptr, 0, EPI_GATED_SILU, mlp_pad));
-        TRY(gemm(P_(w.vff), mlp_pad, Lw.down_w, mlp_pad, Dv, P_(w.vx), Dv, L, Dv, mlp_pad, Lw.down_b, P_(w.vx), Dv, EPI_STORE, 0));
+        TRY(f.rmsnorm(P_(w.vx), Lw.norm1, P_(w.vxn), L, Dv, c.rms_eps));
+        Gemm qkv(P_(w.vxn), Lw.qkv_w, P_(w.vqkv), L, 3 * Hv * hdv, Dv);
+        qkv.ldc = 3 * Hv * 128;
+        if (hdv < 128) { qkv.c_group_in = hdv; qkv.c_group_out = 128; }
+        TRY(f.gemm(qkv.with_bias(Lw.qkv_b), "vision qkv gemm"));
+        const long long nthr = (long long)L * 2 * Hv * (hdv / 16);
+        TRY(f.launch(CAT_OTHER, 0, "vision rope", rope_inplace_kernel, (unsigned)((nthr + 255) / 256), 256, 0, P_(w.vqkv), 3 * Hv * 128, 0, 2 * Hv,
+                     128, hdv, F_(w.vcos), F_(w.vsin), L, 0));
+        const int nseq = full ? n_frames : n_windows, mlen = full ? max_frame_len : max_window_len;
+        static const bool no_pairs = getenv("VQA_ATTN128_NO_PAIRS") != nullptr;     // A/B switch
+        TRY(f.attention(4.0 * (double)L * mlen * Hv * hdv, "vision attention", [&] {
+            return launch_attn_tc128(P_(w.vqkv), 3 * Hv * 128, L, 0, Hv * 128, 2 * Hv * 128, P_(w.vattn), Hv * hdv, nseq, mlen, 0, Hv, 1,
+                                     full ? cu_frames : cu_window, nullptr, vscale, false, st, nullptr,
+                                     /*two windows per tile*/ !full && max_window_len <= 64 && !no_pairs, /*compact heads*/ hdv, hdv);
+        }));
+        TRY(f.gemm(Gemm(P_(w.vattn), Lw.proj_w, P_(w.vx), L, Dv, Hv * hdv).with_bias(Lw.proj_b).with_residual(P_(w.vx))));
+        TRY(f.rmsnorm(P_(w.vx), Lw.norm2, P_(w.vxn), L, Dv, c.rms_eps));
+        TRY(f.gemm(Gemm(P_(w.vxn), Lw.gu_w, P_(w.vff), L, 2 * mlp_pad, Dv).with_bias(Lw.gu_b).with_epilogue(EPI_GATED_SILU, mlp_pad)));
+        TRY(f.gemm(Gemm(P_(w.vff), Lw.down_w, P_(w.vx), L, Dv, mlp_pad).with_bias(Lw.down_b).with_residual(P_(w.vx))));
     }
     // merger: RMSNorm -> [L/4, 4*Dv] -> Linear + GELU -> Linear; back to the original token order (:144-146, :512-513)
-    TRY(rms(P_(w.vx), q.merger_ln, P_(w.vmerge_in), L, Dv));
-    TRY(gemm(P_(w.vmerge_in), Dv * unit, q.fc1_w, Dv * unit, Dv * unit, P_(w.vfc1), Dv * unit, L / unit, Dv * unit, Dv * unit, q.fc1_b, nullptr, 0,
-             EPI_GELU_ERF, 0));
-    TRY(gemm(P_(w.vfc1), Dv * unit, q.fc2_w, Dv * unit, c.out_hidden, P_(w.vfeat), c.out_hidden, L / unit, c.out_hidden, Dv * unit, q.fc2_b, nullptr,
-             0, EPI_STORE, 0));
+    TRY(f.rmsnorm(P_(w.vx), q.merger_ln, P_(w.vmerge_in), L, Dv, c.rms_eps));
+    TRY(f.gemm(Gemm(P_(w.vmerge_in), q.fc1_w, P_(w.vfc1), L / unit, Dv * unit, Dv * unit).with_bias(q.fc1_b).with_epilogue(EPI_GELU_ERF)));
+    TRY(f.gemm(Gemm(P_(w.vfc1), q.fc2_w, P_(w.vfeat), L / unit, c.out_hidden, Dv * unit).with_bias(q.fc2_b)));
     {
-        ProfScope ps(h, CAT_OTHER, 0, st);
-        *lc += 3;
-        gather_rows_kernel<<<L / unit, 128, 0, st>>>(P_(w.vfeat), P_(w.vfeat_orig), reverse_index, 1, c.out_hidden);
+        auto g = f.group(CAT_OTHER);
+        TRY(f.launch(CAT_OTHER, 0, "merger reorder", gather_rows_kernel, L / unit, 128, 0, P_(w.vfeat), P_(w.vfeat_orig), reverse_index, 1,
+                     c.out_hidden));
         // ---------------- language model input ----------------
         // packed rows: one "sample" of M rows, all valid (its length is the last entry of cu_seqlens)
-        qwen_embed_kernel<<<M, 128, 0, st>>>(input_ids, feat_index, pk ? pk->cu_seqlens + pk->n_seq : seq_lens, q.embed, P_(w.vfeat_orig), P_(w.x),
-                                             pk ? M : S, D);
-        rope_table_kernel<<<(M * 64 + 255) / 256, 256, 0, st>>>(position_ids, M, q.text_axis, q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1);
-        TRY(cuda_ok(cudaSuccess, "llm prologue"));
+        TRY(f.launch(CAT_OTHER, 0, "llm embed", qwen_embed_kernel, M, 128, 0, input_ids, feat_index, pk ? pk->cu_seqlens + pk->n_seq : seq_lens,
+                     q.embed, P_(w.vfeat_orig), P_(w.x), pk ? M : S, D));
+        TRY(f.launch(CAT_OTHER, 0, "llm rope table", rope_table_kernel, (M * 64 + 255) / 256, 256, 0, position_ids, M, q.text_axis,
+                     q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1));
     }
     const int Hq = c.heads, Hkv = c.kv_heads, qkv_cols = (Hq + 2 * Hkv) * 128;
     const float tscale = 1.0f / sqrtf(128.0f);
     for (int l = 0; l < c.layers; ++l) {
         const QwenLlmLayerW& Lw = q.llm[l];
-        TRY(rms(P_(w.x), Lw.ln1, P_(w.xn), M, D));
-        TRY(gemm(P_(w.xn), D, Lw.qkv_w, D, qkv_cols, P_(w.qkv), qkv_cols, M, qkv_cols, D, Lw.qkv_b, nullptr, 0, EPI_STORE, 0));
-        {
-            ProfScope ps(h, CAT_OTHER, 0, st);
-            ++*lc;
-            // q heads and k heads are contiguous in the packed buffer -> one launch rotates Hq + Hkv heads
-            const long long nthr = (long long)M * (Hq + Hkv) * 8;
-            rope_inplace_kernel<<<(unsigned)((nthr + 255) / 256), 256, 0, st>>>(P_(w.qkv), qkv_cols, 0, Hq + Hkv, 128, 128, F_(w.cos), F_(w.sin), M,
-                                                                            c.emulate_bf16_rounding);
-            TRY(cuda_ok(cudaSuccess, "llm rope"));
-        }
-        {
-            ProfScope ps(h, CAT_ATTENTION, 2.0 * B * (double)Hq * S * S * 128, st);
-            ++*lc;
+        TRY(f.rmsnorm(P_(w.x), Lw.ln1, P_(w.xn), M, D, c.rms_eps));
+        TRY(f.gemm(Gemm(P_(w.xn), Lw.qkv_w, P_(w.qkv), M, qkv_cols, D).with_bias(Lw.qkv_b)));
+        // q heads and k heads are contiguous in the packed buffer -> one launch rotates Hq + Hkv heads
+        const long long nthr = (long long)M * (Hq + Hkv) * 8;
+        TRY(f.launch(CAT_OTHER, 0, "llm rope", rope_inplace_kernel, (unsigned)((nthr + 255) / 256), 256, 0, P_(w.qkv), qkv_cols, 0, Hq + Hkv,
+                     128, 128, F_(w.cos), F_(w.sin), M, c.emulate_bf16_rounding));
+        TRY(f.attention(2.0 * B * (double)Hq * S * S * 128, pk ? "llm attention (packed)" : "llm attention", [&] {
             if (pk)
-                TRY(cuda_ok(launch_attn_tc128(P_(w.qkv), qkv_cols, M, 0, Hq * 128, (Hq + Hkv) * 128, P_(w.attn), Hq * 128, pk->n_seq, pk->max_seq_len, 0,
-                                              Hq, Hq / Hkv, pk->cu_seqlens, nullptr, tscale, true, st, pk->kv_prefix), "llm attention (packed)"));
-            else
-                TRY(cuda_ok(launch_attn_tc128(P_(w.qkv), qkv_cols, M, 0, Hq * 128, (Hq + Hkv) * 128, P_(w.attn), Hq * 128, B, S, S, Hq, Hq / Hkv, nullptr,
-                                              seq_lens, tscale, true, st), "llm attention"));
-        }
-        TRY(gemm(P_(w.attn), Hq * 128, Lw.o_w, Hq * 128, D, P_(w.x), D, M, D, Hq * 128, nullptr, P_(w.x), D, EPI_STORE, 0));
-        TRY(rms(P_(w.x), Lw.ln2, P_(w.xn), M, D));
-        TRY(gemm(P_(w.xn), D, Lw.gu_w, D, 2 * c.mlp, P_(w.ff), c.mlp, M, 2 * c.mlp, D, nullptr, nullptr, 0, EPI_GATED_SILU, c.mlp));
-        TRY(gemm(P_(w.ff), c.mlp, Lw.down_w, c.mlp, D, P_(w.x), D, M, D, c.mlp, nullptr, P_(w.x), D, EPI_STORE, 0));
+                return launch_attn_tc128(P_(w.qkv), qkv_cols, M, 0, Hq * 128, (Hq + Hkv) * 128, P_(w.attn), Hq * 128, pk->n_seq, pk->max_seq_len,
+                                         0, Hq, Hq / Hkv, pk->cu_seqlens, nullptr, tscale, true, st, pk->kv_prefix);
+            return launch_attn_tc128(P_(w.qkv), qkv_cols, M, 0, Hq * 128, (Hq + Hkv) * 128, P_(w.attn), Hq * 128, B, S, S, Hq, Hq / Hkv, nullptr,
+                                     seq_lens, tscale, true, st);
+        }));
+        TRY(f.gemm(Gemm(P_(w.attn), Lw.o_w, P_(w.x), M, D, Hq * 128).with_residual(P_(w.x))));
+        TRY(f.rmsnorm(P_(w.x), Lw.ln2, P_(w.xn), M, D, c.rms_eps));
+        TRY(f.gemm(Gemm(P_(w.xn), Lw.gu_w, P_(w.ff), M, 2 * c.mlp, D).with_epilogue(EPI_GATED_SILU, c.mlp)));
+        TRY(f.gemm(Gemm(P_(w.ff), Lw.down_w, P_(w.x), M, D, c.mlp).with_residual(P_(w.x))));
     }
     // ---------------- last position -> final norm -> lm_head with fused log-softmax gather ----------------
-    {
-        ProfScope ps(h, CAT_OTHER, 0, st);
-        ++*lc;
-        if (pk) gather_rows_by_index_kernel<<<B, 128, 0, st>>>(P_(w.x), pk->pair_row, P_(w.last), D);
-        else    gather_last_rows_kernel<<<B, 128, 0, st>>>(P_(w.x), seq_lens, P_(w.last), S, D);
-        TRY(cuda_ok(cudaSuccess, "last-row gather"));
-    }
-    TRY(rms(P_(w.last), q.final_norm, P_(w.lastn), B, D));
+    if (pk) TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_rows_by_index_kernel, B, 128, 0, P_(w.x), pk->pair_row, P_(w.last), D));
+    else    TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_last_rows_kernel, B, 128, 0, P_(w.x), seq_lens, P_(w.last), S, D));
+    TRY(f.rmsnorm(P_(w.last), q.final_norm, P_(w.lastn), B, D, c.rms_eps));
     const int ntiles = LMHEAD_PARTS * ((c.vocab + LMHEAD_BN - 1) / LMHEAD_BN);
     const int pen_words = (c.vocab + 31) / 32;
     const bool penalise = repetition_penalty != 1.0f;
+    uint32_t* bitmap = f.at<uint32_t>(w.pen_bitmap);
     if (penalise) {
         // HF applies RepetitionPenaltyLogitsProcessor over the prompt ids before the scores are returned (generation/utils.py:2762-2770,
         // logits_process.py): one bit per (sample, vocabulary id) that occurs in the sample's prompt.
-        ProfScope ps(h, CAT_OTHER, 0, st);
-        *lc += 2;
-        TRY(cuda_ok(cudaMemsetAsync(P8_(w.pen_bitmap), 0, (size_t)B * pen_words * 4, st), "penalty bitmap clear"));
+        auto g = f.group(CAT_OTHER);
+        TRY(f.memset0(bitmap, (size_t)B * pen_words * 4, "penalty bitmap clear"));
         if (pk)
-            token_bitmap_packed_kernel<<<dim3((pk->max_prompt_len + 255) / 256, B), 256, 0, st>>>(input_ids, pk->cu_seqlens, pk->kv_prefix, pk->pair_seq,
-                                                                                                   c.vocab, reinterpret_cast<uint32_t*>(P8_(w.pen_bitmap)), pen_words);
+            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_packed_kernel, dim3((pk->max_prompt_len + 255) / 256, B), 256, 0, input_ids,
+                         pk->cu_seqlens, pk->kv_prefix, pk->pair_seq, c.vocab, bitmap, pen_words));
         else
-            token_bitmap_kernel<<<(B * S + 255) / 256, 256, 0, st>>>(input_ids, seq_lens, B, S, c.vocab,
-                                                                     reinterpret_cast<uint32_t*>(P8_(w.pen_bitmap)), pen_words);
-        TRY(cuda_ok(cudaSuccess, "penalty bitmap"));
+            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_kernel, (B * S + 255) / 256, 256, 0, input_ids, seq_lens, B, S, c.vocab,
+                         bitmap, pen_words));
     }
-    {
-        ProfScope ps(h, CAT_GEMM, 2.0 * B * (double)c.vocab * D, st, 2.0 * ((double)B * D + (double)c.vocab * D));
-        TRY(cuda_ok(run_lmhead(P_(w.lastn), D, q.lm_head, D, B, c.vocab, D, answer_ids, F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit), nsm, st,
-                               lc, 1.0f / temperature, penalise ? reinterpret_cast<const uint32_t*>(P8_(w.pen_bitmap)) : nullptr, pen_words,
-                               repetition_penalty), "lm_head"));
-    }
-    {
-        ProfScope ps(h, CAT_OTHER, 0, st);
-        ++*lc;
-        // T = 1 target per row: score = exp(logprob) = softmax(logits / T)[answer] (qwen2vl_model.py:160-167)
-        lse_finalize_kernel<<<(B + 3) / 4, 128, 0, st>>>(F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit), answer_ids, out_probs,
-                                                        out_logprobs ? out_logprobs : F_(w.logprob), B, 1, ntiles);
-        TRY(cuda_ok(cudaSuccess, "lse finalize"));
-    }
-#undef TRY
+    Gemm lm(P_(w.lastn), q.lm_head, nullptr, B, c.vocab, D);
+    lm.lse(answer_ids, F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit));
+    lm.lse_scale = 1.0f / temperature;
+    lm.penalty_bitmap = penalise ? bitmap : nullptr; lm.penalty_words = pen_words; lm.penalty = repetition_penalty;
+    TRY(f.gemm(lm, "lm_head"));
+    // T = 1 target per row: score = exp(logprob) = softmax(logits / T)[answer] (qwen2vl_model.py:160-167)
+    TRY(f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit),
+                 answer_ids, out_probs, out_logprobs ? out_logprobs : F_(w.logprob), B, 1, ntiles));
     return VQA_OK;
 }
 
@@ -326,10 +267,9 @@ static int qwen_topk(vqa_handle* h, QwenState& q, int B, size_t rows, int n_patc
     const int pen_words = (c.vocab + 31) / 32;
     const bool penalise = repetition_penalty != 1.0f;
     const uint32_t* bitmap = reinterpret_cast<const uint32_t*>(ws + w.pen_bitmap);      // built by the scoring call with the same penalty
-    CUDA_TRY(h, run_gemm(lastn, c.hidden, q.lm_head, c.hidden, c.vocab, logits, c.vocab, B, c.vocab, c.hidden, nullptr, nullptr, 0, EPI_STORE, 0, 0,
-                         h->num_sms, st, nullptr));
-    topk_softmax_kernel<<<B, 256, 0, st>>>(logits, (long long)c.vocab, c.vocab, 1.0f / temperature, penalise ? bitmap : nullptr, pen_words,
-                                           repetition_penalty, K, out_ids, out_probs);
-    CUDA_TRY(h, cudaGetLastError());
-    return VQA_OK;
+    cudaError_t e = run_gemm(Gemm(lastn, q.lm_head, logits, B, c.vocab, c.hidden), h->num_sms, st);
+    if (e == cudaSuccess)
+        topk_softmax_kernel<<<B, 256, 0, st>>>(logits, (long long)c.vocab, c.vocab, 1.0f / temperature, penalise ? bitmap : nullptr, pen_words,
+                                               repetition_penalty, K, out_ids, out_probs);
+    return cuda_status(h, e, "top-k");
 }

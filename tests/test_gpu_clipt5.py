@@ -184,6 +184,33 @@ def test_cuda_graph_replay_equals_direct_launches(golden_dir, dev):
     assert torch.equal(g3, direct)
 
 
+
+def captured_node_count(fn):
+    """Nodes of a CUDA graph capturing one call of fn, after one uncaptured warm-up call (as score_tensors_graphed does): every kernel,
+    memset and device copy the call enqueues."""
+    import ctypes
+    fn()
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph(keep_graph=True)
+    with torch.cuda.graph(graph):
+        fn()
+    n = ctypes.c_size_t(0)
+    assert ctypes.CDLL("libcuda.so.1").cuGraphGetNodes(ctypes.c_void_p(graph.raw_cuda_graph()), None, ctypes.byref(n)) == 0
+    return n.value
+
+
+@pytest.mark.parametrize("kw,d_ff", [({}, 512), (dict(fuse_norms=True), 512), (dict(cross_attention_mode="reference"), 512), ({}, 2048)])
+def test_launch_count_equals_captured_graph_nodes(kw, d_ff, dev):
+    """last_launch_count() (bench.py's gpu_launches) is what the forward really enqueues. d_ff = 2048 splits the decoder's wo GEMM
+    (K = d_ff) into K slices: one GEMM, two launches."""
+    cfg = orc.ClipT5Config.tiny(d_ff=d_ff)
+    sd = orc.make_synthetic_state_dict(cfg, seed=0, label_ids=(37, 1))
+    inp = orc.make_synthetic_inputs(cfg, 3, 12, seed=1, ragged=True, label_ids=(37, 1))
+    eng = make_engine(cfg, sd, dev, **kw)
+    i32 = lambda t: t.to(dev, torch.int32)
+    args = [inp["pixels"].to(dev), i32(inp["input_ids"]), i32(inp["text_lens"]), i32(inp["labels"])]
+    assert captured_node_count(lambda: eng.score_tensors(*args)) == eng.last_launch_count()
+
 def test_full_size_xxl_properties(dev):
     """BASELINE config-2 size (clip-flant5-xxl dims, B=64, S_enc=672): determinism, finite scores in [0,1], and batch
     invariance of the first pairs (B=64 vs B=4), which exercises every kernel at its production shape."""

@@ -165,6 +165,30 @@ def test_qwen_engine_matches_oracle(dev, hw, n_images):
     assert float((torch.log(pT) - torch.log(refT)).abs().max()) <= 2.0 * gap + 2e-2
 
 
+
+@pytest.mark.parametrize("packed,pen", [(False, 1.0), (True, 1.0), (False, 1.3), (True, 1.3)])
+def test_qwen_launch_count_equals_captured_graph_nodes(dev, packed, pen):
+    """last_launch_count() is what one forward enqueues (the nodes of a CUDA graph that captures it), padded and packed, with and
+    without the repetition-penalty bitmap."""
+    from t2v_metrics_b200 import qwen_host
+    from test_gpu_clipt5 import captured_node_count
+    cfg = qo.Qwen25VLConfig.tiny(**TINY)
+    inp = qo.make_synthetic_inputs(cfg, 4, (56, 84), 12, ragged=True, n_images=2)
+    eng = make_engine(cfg, qo.make_synthetic_state_dict(cfg, seed=0), dev)
+    ec = eng.cfg
+    grids = [tuple(map(int, g)) for g in inp["grid_thw"]]
+    build = qwen_host.build_packed_indices if packed else qwen_host.build_batch_indices
+    idx = build([x.tolist() for x in inp["input_ids"]], grids, list(inp["image_of_sample"]), ec.image_token_id, ec.spatial_merge_size,
+                ec.tokens_per_second, video_token_id=ec.video_token_id)
+    d = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in idx.items()}
+    ans = torch.as_tensor(list(map(int, inp["answer_ids"])), dtype=torch.int32).to(dev)
+    pix = inp["pixel_patches"].to(dev)
+    if packed:
+        fn = lambda: eng.score_packed(pix, grids, d, ans, repetition_penalty=pen)
+    else:
+        fn = lambda: eng.score_tensors(pix, grids, d["input_ids"], d["seq_lens"], d["feat_index"], d["position_ids"], ans, repetition_penalty=pen)
+    assert captured_node_count(fn) == eng.last_launch_count()
+
 @pytest.mark.parametrize("frames,hw", [(2, (56, 84)), (4, (84, 56))])
 def test_qwen_engine_video_grid(dev, frames, hw):
     """SURVEY 8(d) config 5: a video is a grid with t > 1 temporal patches -- same tower (windows and full attention are per
