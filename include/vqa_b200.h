@@ -204,6 +204,32 @@ int vqa_qwen25vl_score_packed(vqa_handle* h, const void* pixel_patches, int32_t 
                               float repetition_penalty, float* out_probs, float* out_logprobs, void* workspace, size_t workspace_bytes,
                               void* stream);
 
+/* ---- Qwen2.5-VL greedy generation (reference Qwen2VLModel.generate, qwen2vl_model.py:495-563: generate(do_sample=False)) ----
+ * One prefill, then one decode step per further token, all on the caller's stream. The prefill runs the vision tower and the padded-row
+ * prefill of vqa_qwen25vl_score (same index arrays, no answer ids), stores every layer's post-rope K/V rows in a cache inside the workspace
+ * (capacity seq_len + max_new_tokens per prompt), and selects the first token. A step feeds each prompt's last token through the
+ * language model and selects the next one. Selection: bf16 lm_head logits -> fp32 -> HF's RepetitionPenaltyLogitsProcessor over the
+ * prompt ids and the tokens generated so far (repetition_penalty 1.0 = off) -> arg-max, ties to the lowest id. A prompt finishes after
+ * emitting one of eos_ids (which is kept in its output) or max_new_tokens tokens; later steps leave it unchanged.
+ *   first_position [batch]  mRoPE position of the first generated token: the last prompt token's position + 1; token t sits at that + t
+ *                           on all three axes (what transformers' generate() feeds)
+ *   eos_ids [n_eos]         DEVICE; n_eos may be 0
+ *   out_tokens [batch, max_new_tokens]  generated ids, -1 after a prompt's last one; out_lengths [batch] tokens generated so far;
+ *   all_done [1]            1 once every prompt has finished
+ * Every step-dependent value lives in device memory: the step takes the same arguments every time, so one CUDA graph of it can be
+ * replayed for every token. The prefill and the steps must use the same workspace, sizes and pointers. batch <= 128. */
+size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, int32_t max_new_tokens);
+int vqa_qwen25vl_generate_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches, const int32_t* vis_pos_hw,
+                                  const int32_t* window_index, const int32_t* reverse_index, const int32_t* cu_window, int32_t n_windows,
+                                  int32_t max_window_len, const int32_t* cu_frames, int32_t n_frames, int32_t max_frame_len,
+                                  const int32_t* input_ids, const int32_t* seq_lens, const int32_t* feat_index, const int32_t* position_ids,
+                                  const int32_t* first_position, int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos,
+                                  int32_t max_new_tokens, float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+int vqa_qwen25vl_generate_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
+                               int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
+                               int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Number of kernels the last vqa_clipt5_score call launched (for bench.py's gpu_launches). */
 int64_t vqa_last_launch_count(vqa_handle* h);
 

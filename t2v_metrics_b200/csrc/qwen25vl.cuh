@@ -4,6 +4,7 @@
 #include "host.cuh"
 #include "attention_sm90.cuh"
 #include "qwen_kernels.cuh"
+#include "qwen_decode.cuh"
 
 struct QwenVisLayerW {
     const bf16 *norm1, *norm2, *qkv_w, *qkv_b, *proj_w, *proj_b, *gu_w, *gu_b, *down_w, *down_b;
@@ -123,17 +124,34 @@ static int qwen_finalize(vqa_handle* h, QwenState& q) {
     return VQA_OK;
 }
 
-static int qwen_score(vqa_handle* h, QwenState& q, const void* pixel_patches, int pixel_dtype, int n_patches,
-                      const int* vis_pos_hw, const int* window_index, const int* reverse_index, const int* cu_window,
-                      int n_windows, int max_window_len, const int* cu_frames, int n_frames, int max_frame_len,
-                      const int* input_ids, const int* seq_lens, const int* feat_index, const int* position_ids,
-                      const int* answer_ids, int B, int S, float temperature, float repetition_penalty, float* out_probs,
-                      float* out_logprobs,
-                      void* workspace, size_t workspace_bytes, cudaStream_t st, const QwenPacked* pk = nullptr) {
+// The vision and prompt inputs of one prefill (see vqa_qwen25vl_score)
+struct QwenPrompts {
+    const void* pixel_patches; int pixel_dtype, n_patches;
+    const int *vis_pos_hw, *window_index, *reverse_index, *cu_window; int n_windows, max_window_len;
+    const int* cu_frames; int n_frames, max_frame_len;
+    const int *input_ids, *seq_lens, *feat_index, *position_ids;
+    int B, S;
+};
+
+// K/V cache of a generate prefill: layer l's K and V at kc + l * layer_elems and vc + l * layer_elems, each [B, Hkv, cap, 128]
+struct QwenKVCache {
+    bf16 *kc, *vc;
+    size_t layer_elems;
+    int cap;
+};
+
+// Vision tower, embedding splice and every language-model layer of one prefill, into w.x. With `kv`, each layer's post-rope K/V rows are
+// also stored in the cache (one launch per layer after the rope).
+static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const QwenPrompts& in, const QwenPacked* pk,
+                        const QwenKVCache* kv = nullptr) {
     const vqa_qwen25vl_config& c = q.cfg;
-    const QwenWorkspace w = pk ? qwen_plan_rows(c, B, (size_t)pk->total_rows, n_patches) : qwen_plan(c, B, S, n_patches);
-    if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
-    Forward f(h, workspace, st);
+    cudaStream_t st = f.st;
+    const void* pixel_patches = in.pixel_patches;
+    const int pixel_dtype = in.pixel_dtype, n_patches = in.n_patches, B = in.B, S = in.S;
+    const int *vis_pos_hw = in.vis_pos_hw, *window_index = in.window_index, *reverse_index = in.reverse_index, *cu_window = in.cu_window;
+    const int n_windows = in.n_windows, max_window_len = in.max_window_len, n_frames = in.n_frames, max_frame_len = in.max_frame_len;
+    const int *cu_frames = in.cu_frames, *input_ids = in.input_ids, *seq_lens = in.seq_lens, *feat_index = in.feat_index;
+    const int* position_ids = in.position_ids;
     auto P_ = [&](size_t off) { return f.at(off); };
     auto F_ = [&](size_t off) { return f.at<float>(off); };
     const int L = n_patches, Dv = c.vit_hidden, Hv = c.vit_heads, hdv = c.vit_head_dim;
@@ -210,6 +228,10 @@ static int qwen_score(vqa_handle* h, QwenState& q, const void* pixel_patches, in
         const long long nthr = (long long)M * (Hq + Hkv) * 8;
         TRY(f.launch(CAT_OTHER, 0, "llm rope", rope_inplace_kernel, (unsigned)((nthr + 255) / 256), 256, 0, P_(w.qkv), qkv_cols, 0, Hq + Hkv,
                      128, 128, F_(w.cos), F_(w.sin), M, c.emulate_bf16_rounding));
+        if (kv)
+            TRY(f.launch(CAT_OTHER, 0, "kv cache write", kv_cache_write_kernel, (unsigned)(((long long)M * Hkv * 16 + 255) / 256), 256, 0, P_(w.qkv),
+                         qkv_cols, Hq * 128, (Hq + Hkv) * 128, Hkv, S, (long long)M, seq_lens, nullptr, kv->kc + l * kv->layer_elems,
+                         kv->vc + l * kv->layer_elems, kv->cap));
         TRY(f.attention(2.0 * B * (double)Hq * S * S * 128, pk ? "llm attention (packed)" : "llm attention", [&] {
             if (pk)
                 return launch_attn_tc128(P_(w.qkv), qkv_cols, M, 0, Hq * 128, (Hq + Hkv) * 128, P_(w.attn), Hq * 128, pk->n_seq, pk->max_seq_len,
@@ -222,15 +244,22 @@ static int qwen_score(vqa_handle* h, QwenState& q, const void* pixel_patches, in
         TRY(f.gemm(Gemm(P_(w.xn), Lw.gu_w, P_(w.ff), M, 2 * c.mlp, D).with_epilogue(EPI_GATED_SILU, c.mlp)));
         TRY(f.gemm(Gemm(P_(w.ff), Lw.down_w, P_(w.x), M, D, c.mlp).with_residual(P_(w.x))));
     }
-    // ---------------- last position -> final norm -> lm_head with fused log-softmax gather ----------------
+    return VQA_OK;
+}
+
+// Last prompt position -> final norm (w.lastn); with a repetition penalty, also the bitmap of every prompt's ids (w.pen_bitmap).
+static int qwen_last_position(Forward& f, QwenState& q, const QwenWorkspace& w, const QwenPrompts& in, const QwenPacked* pk,
+                              float repetition_penalty) {
+    const vqa_qwen25vl_config& c = q.cfg;
+    const int B = in.B, S = in.S, D = c.hidden;
+    const int *input_ids = in.input_ids, *seq_lens = in.seq_lens;
+    auto P_ = [&](size_t off) { return f.at(off); };
     if (pk) TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_rows_by_index_kernel, B, 128, 0, P_(w.x), pk->pair_row, P_(w.last), D));
     else    TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_last_rows_kernel, B, 128, 0, P_(w.x), seq_lens, P_(w.last), S, D));
     TRY(f.rmsnorm(P_(w.last), q.final_norm, P_(w.lastn), B, D, c.rms_eps));
-    const int ntiles = LMHEAD_PARTS * ((c.vocab + LMHEAD_BN - 1) / LMHEAD_BN);
     const int pen_words = (c.vocab + 31) / 32;
-    const bool penalise = repetition_penalty != 1.0f;
     uint32_t* bitmap = f.at<uint32_t>(w.pen_bitmap);
-    if (penalise) {
+    if (repetition_penalty != 1.0f) {
         // HF applies RepetitionPenaltyLogitsProcessor over the prompt ids before the scores are returned (generation/utils.py:2762-2770,
         // logits_process.py): one bit per (sample, vocabulary id) that occurs in the sample's prompt.
         auto g = f.group(CAT_OTHER);
@@ -242,6 +271,26 @@ static int qwen_score(vqa_handle* h, QwenState& q, const void* pixel_patches, in
             TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_kernel, (B * S + 255) / 256, 256, 0, input_ids, seq_lens, B, S, c.vocab,
                          bitmap, pen_words));
     }
+    return VQA_OK;
+}
+
+static int qwen_score(vqa_handle* h, QwenState& q, const QwenPrompts& in, const int* answer_ids, float temperature, float repetition_penalty,
+                      float* out_probs, float* out_logprobs, void* workspace, size_t workspace_bytes, cudaStream_t st,
+                      const QwenPacked* pk = nullptr) {
+    const vqa_qwen25vl_config& c = q.cfg;
+    const int B = in.B, D = c.hidden;
+    const QwenWorkspace w = pk ? qwen_plan_rows(c, B, (size_t)pk->total_rows, in.n_patches) : qwen_plan(c, B, in.S, in.n_patches);
+    if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
+    Forward f(h, workspace, st);
+    auto P_ = [&](size_t off) { return f.at(off); };
+    auto F_ = [&](size_t off) { return f.at<float>(off); };
+    TRY(qwen_prefill(f, q, w, in, pk));
+    TRY(qwen_last_position(f, q, w, in, pk, repetition_penalty));
+    // ---------------- lm_head with fused log-softmax gather ----------------
+    const int ntiles = LMHEAD_PARTS * ((c.vocab + LMHEAD_BN - 1) / LMHEAD_BN);
+    const int pen_words = (c.vocab + 31) / 32;
+    const bool penalise = repetition_penalty != 1.0f;
+    const uint32_t* bitmap = f.at<uint32_t>(w.pen_bitmap);
     Gemm lm(P_(w.lastn), q.lm_head, nullptr, B, c.vocab, D);
     lm.lse(answer_ids, F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit));
     lm.lse_scale = 1.0f / temperature;
@@ -272,4 +321,147 @@ static int qwen_topk(vqa_handle* h, QwenState& q, int B, size_t rows, int n_patc
         topk_softmax_kernel<<<B, 256, 0, st>>>(logits, (long long)c.vocab, c.vocab, 1.0f / temperature, penalise ? bitmap : nullptr, pen_words,
                                                repetition_penalty, K, out_ids, out_probs);
     return cuda_status(h, e, "top-k");
+}
+
+// ================================================================================================ greedy generation
+// Workspace of a generation: the scoring plan of the padded prefill (its language-model buffers hold B rows during decode steps; the
+// [B, vocab] logits of a step go to trace_logits), then the K/V cache (capacity seq_len + max_new_tokens per sequence), the decode
+// attention partials, the split-K slices of the decode GEMMs, and the step state.
+struct QwenGenWorkspace {
+    QwenWorkspace w;
+    size_t kcache, vcache, attn_o, attn_ml, splitk, next_ids, pos3, done, n_done, total;
+    int cap, splits, chunk;
+    size_t layer_elems;
+};
+static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S, int n_patches, int max_new, int num_sms) {
+    QwenGenWorkspace g;
+    g.w = qwen_plan(c, B, S, n_patches);
+    Plan pl;
+    pl.off = g.w.total;
+    g.cap = S + max_new;
+    // flash-decoding: enough key splits for two CTAs per SM (at B = 1 the 4 KV heads alone would occupy 4 of 132 SMs), at least 16 keys each.
+    // Fixed by the capacity, not the live lengths, so a step's launch shapes never change.
+    g.splits = std::max(1, std::min((2 * num_sms + B * c.kv_heads - 1) / (B * c.kv_heads), (g.cap + 15) / 16));
+    g.chunk = (g.cap + g.splits - 1) / g.splits;
+    g.layer_elems = (size_t)B * c.kv_heads * g.cap * 128;
+    g.kcache = pl.take((size_t)c.layers * g.layer_elems * 2);
+    g.vcache = pl.take((size_t)c.layers * g.layer_elems * 2);
+    g.attn_o = pl.take((size_t)B * c.heads * g.splits * 128 * 4);
+    g.attn_ml = pl.take((size_t)B * c.heads * g.splits * 2 * 4);
+    const int qkv_cols = (c.heads + 2 * c.kv_heads) * 128;
+    g.splitk = pl.take((size_t)8 * B * std::max(qkv_cols, c.hidden) * 4);      // splitk_slices() cuts at most 8 slices
+    g.next_ids = pl.take((size_t)B * 4);
+    g.pos3 = pl.take((size_t)3 * B * 4);
+    g.done = pl.take((size_t)B * 4);
+    g.n_done = pl.take(4);
+    g.total = pl.off;
+    return g;
+}
+
+// Outputs and constants of a generation, the same for the prefill and every step
+struct QwenGenArgs {
+    const int* seq_lens;     // [B] prompt lengths
+    const int* first_pos;    // [B] mRoPE position of the first generated token (last prompt position + 1)
+    const int* eos_ids; int n_eos;
+    int max_new; float repetition_penalty;
+    int* tokens;             // [B, max_new], -1 after a sequence's last token
+    int* lengths;            // [B] tokens generated so far
+    int* all_done;           // 1 once every sequence has finished
+};
+
+// lm_head on w.lastn into [B, vocab] bf16 logits, then the greedy token of every unfinished sequence and its bookkeeping
+static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g, int B, const QwenGenArgs& a) {
+    const vqa_qwen25vl_config& c = q.cfg;
+    const QwenWorkspace& w = g.w;
+    bf16* logits = f.at(w.trace_logits);
+    // The [B, vocab] bf16 logits are 0.3 MB per sequence against the 1.1 GB lm_head weight (7B) that the GEMM streams either way.
+    TRY(f.gemm(Gemm(f.at(w.lastn), q.lm_head, logits, B, c.vocab, c.hidden), "lm_head"));
+    const bool penalise = a.repetition_penalty != 1.0f;
+    return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, (const bf16*)logits, c.vocab,
+                    penalise ? f.at<uint32_t>(w.pen_bitmap) : nullptr, (c.vocab + 31) / 32, a.repetition_penalty, a.eos_ids, a.n_eos,
+                    a.max_new, a.first_pos, B, a.tokens, a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done,
+                    f.at<int>(g.next_ids), f.at<int>(g.pos3));
+}
+
+// The prefill of vqa_qwen25vl_score over the padded rows, with every layer's K/V stored in the cache, then the first token.
+static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const QwenPrompts& in, const QwenGenArgs& a, void* workspace,
+                                 size_t workspace_bytes, cudaStream_t st) {
+    const QwenGenWorkspace g = qwen_gen_plan(q.cfg, in.B, in.S, in.n_patches, a.max_new, h->num_sms);
+    if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
+    Forward f(h, workspace, st);
+    TRY(f.launch(CAT_OTHER, 0, "generate init", generate_init_kernel, (in.B * a.max_new + 255) / 256, 256, 0, in.B, a.max_new, a.tokens,
+                 a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
+    const QwenKVCache kv{f.at(g.kcache), f.at(g.vcache), g.layer_elems, g.cap};
+    TRY(qwen_prefill(f, q, g.w, in, nullptr, &kv));
+    TRY(qwen_last_position(f, q, g.w, in, nullptr, a.repetition_penalty));
+    return qwen_select_token(f, q, g, in.B, a);
+}
+
+// decode_attn_partial_kernel for G q heads per KV head (the group sizes of the Qwen2.5-VL family: 7B 7, 3B 8, 32B 5, 72B 8)
+template <typename... Args>
+static cudaError_t launch_decode_attn(int G, dim3 grid, cudaStream_t st, Args... args) {
+    switch (G) {
+        case 1: decode_attn_partial_kernel<1><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 2: decode_attn_partial_kernel<2><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 4: decode_attn_partial_kernel<4><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 5: decode_attn_partial_kernel<5><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 7: decode_attn_partial_kernel<7><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 8: decode_attn_partial_kernel<8><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+
+// One decode step: every sequence feeds its last token (finished ones recompute their frozen last step, which writes nothing new).
+// Decode GEMMs have M = B <= 128 rows and stream their weights. At 7B width qkv (N = 4608), o and down (N = 3584) make 36 / 28 / 28
+// of the 128-wide N tiles that splitk_slices() counts, far fewer than 132 SMs, so their K range is split (2, 4 and 4 slices:
+// tools/bench_generate.py measures the step with and without). gate_up (N = 2 x 18944) and the lm_head (N = 152064) already make
+// 296 and 1188 tiles and have no split.
+static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_patches, const QwenGenArgs& a, void* workspace,
+                              size_t workspace_bytes, cudaStream_t st) {
+    const vqa_qwen25vl_config& c = q.cfg;
+    const QwenGenWorkspace g = qwen_gen_plan(c, B, S, n_patches, a.max_new, h->num_sms);
+    if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
+    const QwenWorkspace& w = g.w;
+    Forward f(h, workspace, st);
+    auto P_ = [&](size_t off) { return f.at(off); };
+    auto F_ = [&](size_t off) { return f.at<float>(off); };
+    const int D = c.hidden, Hq = c.heads, Hkv = c.kv_heads, G = Hq / Hkv, qkv_cols = (Hq + 2 * Hkv) * 128;
+    float* skw = F_(g.splitk);
+    auto skinny = [&](Gemm gm) {
+        const int s = splitk_slices(gm.M, gm.N, gm.K, f.nsm);
+        return s > 1 ? gm.split_k(s, skw) : gm;
+    };
+    {
+        auto grp = f.group(CAT_OTHER);
+        TRY(f.launch(CAT_OTHER, 0, "decode embed", gather_rows_by_index_kernel, B, 128, 0, q.embed, f.at<int>(g.next_ids), P_(w.x), D));
+        TRY(f.launch(CAT_OTHER, 0, "decode rope table", rope_table_kernel, (B * 64 + 255) / 256, 256, 0, f.at<int>(g.pos3), B, q.text_axis,
+                     q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1));
+    }
+    const float tscale = 1.0f / sqrtf(128.0f);
+    for (int l = 0; l < c.layers; ++l) {
+        const QwenLlmLayerW& Lw = q.llm[l];
+        TRY(f.rmsnorm(P_(w.x), Lw.ln1, P_(w.xn), B, D, c.rms_eps));
+        TRY(f.gemm(skinny(Gemm(P_(w.xn), Lw.qkv_w, P_(w.qkv), B, qkv_cols, D).with_bias(Lw.qkv_b)), "decode qkv gemm"));
+        TRY(f.launch(CAT_OTHER, 0, "decode rope", rope_inplace_kernel, (unsigned)((B * (Hq + Hkv) * 8 + 255) / 256), 256, 0, P_(w.qkv), qkv_cols,
+                     0, Hq + Hkv, 128, 128, F_(w.cos), F_(w.sin), (long long)B, c.emulate_bf16_rounding));
+        bf16 *kc = f.at(g.kcache) + l * g.layer_elems, *vc = f.at(g.vcache) + l * g.layer_elems;
+        TRY(f.launch(CAT_OTHER, 0, "kv cache append", kv_cache_write_kernel, (unsigned)((B * Hkv * 16 + 255) / 256), 256, 0, P_(w.qkv), qkv_cols,
+                     Hq * 128, (Hq + Hkv) * 128, Hkv, 1, (long long)B, a.seq_lens, (const int*)a.lengths, kc, vc, g.cap));
+        const double kv_bytes = 2.0 * B * Hkv * (double)g.cap * 128 * 2;      // upper bound: the full capacity
+        TRY(f.op(CAT_ATTENTION, 4.0 * B * Hq * (double)g.cap * 128, kv_bytes, 2, "decode attention", [&] {
+            const dim3 grid(g.splits, Hkv, B);
+            cudaError_t e = launch_decode_attn(G, grid, st, P_(w.qkv), qkv_cols, kc, vc, g.cap, a.seq_lens, a.lengths, Hkv, g.chunk, tscale,
+                                               F_(g.attn_o), F_(g.attn_ml));
+            if (e != cudaSuccess) return e;
+            decode_attn_merge_kernel<<<B * Hq, 128, 0, st>>>(F_(g.attn_o), F_(g.attn_ml), g.splits, P_(w.attn), Hq * 128, Hq);
+            return cudaGetLastError();
+        }));
+        TRY(f.gemm(skinny(Gemm(P_(w.attn), Lw.o_w, P_(w.x), B, D, Hq * 128).with_residual(P_(w.x))), "decode o gemm"));
+        TRY(f.rmsnorm(P_(w.x), Lw.ln2, P_(w.xn), B, D, c.rms_eps));
+        TRY(f.gemm(Gemm(P_(w.xn), Lw.gu_w, P_(w.ff), B, 2 * c.mlp, D).with_epilogue(EPI_GATED_SILU, c.mlp), "decode gate_up gemm"));
+        TRY(f.gemm(skinny(Gemm(P_(w.ff), Lw.down_w, P_(w.x), B, D, c.mlp).with_residual(P_(w.x))), "decode down gemm"));
+    }
+    TRY(f.rmsnorm(P_(w.x), q.final_norm, P_(w.lastn), B, D, c.rms_eps));
+    return qwen_select_token(f, q, g, B, a);
 }

@@ -1,0 +1,189 @@
+// Kernels of the Qwen2.5-VL greedy decode loop: the K/V cache write, flash-decoding attention over the cache, and greedy token selection
+// with the per-step bookkeeping. Every step-dependent value (generated lengths, finished flags, next input ids and positions) lives in
+// device memory, so the launches of one decode step take the same arguments at every step and replay from one CUDA graph.
+#pragma once
+#include "ptx.cuh"
+#include "elementwise.cuh"
+
+namespace vqa {
+
+// K/V cache of one layer: K and V each [B, Hkv, cap, 128] bf16 (post-rope K, as HF's DynamicCache stores it).
+// Source: the packed qkv activation [rows, ld] of the layer, K heads at k_col0, V heads at v_col0, row r = b * S + s.
+//   prefill (gen_len == nullptr): rows s < seq_lens[b] go to slot s;
+//   decode  (S == 1):             the one row of sequence b goes to slot seq_lens[b] + gen_len[b] - 1 (the position of the input token).
+// One thread per (row, kv head, 16-byte chunk).
+__global__ void kv_cache_write_kernel(const __nv_bfloat16* __restrict__ qkv, int ld, int k_col0, int v_col0, int Hkv, int S, long long rows,
+                                      const int* __restrict__ seq_lens, const int* __restrict__ gen_len, __nv_bfloat16* __restrict__ kc,
+                                      __nv_bfloat16* __restrict__ vc, int cap) {
+    pdl_launch_dependents();
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= rows * Hkv * 16) return;
+    const int c = (int)(idx & 15), h = (int)((idx >> 4) % Hkv);
+    const long long r = idx / (16LL * Hkv);
+    const int b = (int)(r / S), s = (int)(r % S);
+    int slot;
+    if (gen_len) {
+        slot = seq_lens[b] + gen_len[b] - 1 + s;
+    } else {
+        if (s >= seq_lens[b]) return;
+        slot = s;
+    }
+    const size_t dst = (((size_t)b * Hkv + h) * cap + slot) * 128 + c * 8;
+    const __nv_bfloat16* src = qkv + (size_t)r * ld + h * 128 + c * 8;
+    *reinterpret_cast<uint4*>(kc + dst) = *reinterpret_cast<const uint4*>(src + k_col0);
+    *reinterpret_cast<uint4*>(vc + dst) = *reinterpret_cast<const uint4*>(src + v_col0);
+}
+
+// Decode attention, head_dim 128, causal GQA over the cache (flash-decoding). One query row per q head; sequence b attends to cache
+// slots [0, seq_lens[b] + gen_len[b]) -- the prompt, every generated token before this step's input, and the input itself.
+// grid (splits, Hkv, B), 128 threads: the CTA holds the G q heads of one KV head, so each K/V byte is read once per group, and covers
+// keys [split * chunk, (split + 1) * chunk). Each warp runs an online softmax over every 4th key of the range (lane = 4 dims), the four
+// warps are merged in shared memory, and the CTA writes its unnormalised partial (max, sum, output) for decode_attn_merge_kernel.
+constexpr int DEC_ATTN_WARPS = 4;
+template <int G>
+__global__ void __launch_bounds__(32 * DEC_ATTN_WARPS) decode_attn_partial_kernel(
+        const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16* __restrict__ kc, const __nv_bfloat16* __restrict__ vc, int cap,
+        const int* __restrict__ seq_lens, const int* __restrict__ gen_len, int Hkv, int chunk, float scale, float* __restrict__ part_o,
+        float* __restrict__ part_ml) {
+    pdl_launch_dependents();
+    __shared__ float s_m[DEC_ATTN_WARPS][G], s_l[DEC_ATTN_WARPS][G];
+    __shared__ float s_o[DEC_ATTN_WARPS][G][128];
+    const int sp = blockIdx.x, kh = blockIdx.y, b = blockIdx.z, splits = gridDim.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int len = seq_lens[b] + gen_len[b];
+    const int k0 = sp * chunk, k1 = min(len, k0 + chunk);
+    const int Hq = Hkv * G;
+    float qv[G][4], acc[G][4], m[G], l[G];
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+        const uint2 u = *reinterpret_cast<const uint2*>(q + (size_t)b * ldq + (kh * G + g) * 128 + lane * 4);
+        const float2 a = unpack_bf16x2(u.x), c = unpack_bf16x2(u.y);
+        qv[g][0] = a.x * scale; qv[g][1] = a.y * scale; qv[g][2] = c.x * scale; qv[g][3] = c.y * scale;
+        acc[g][0] = acc[g][1] = acc[g][2] = acc[g][3] = 0.f;
+        m[g] = -INFINITY; l[g] = 0.f;
+    }
+    const size_t base = ((size_t)b * Hkv + kh) * cap * 128 + lane * 4;
+    for (int j = k0 + warp; j < k1; j += DEC_ATTN_WARPS) {
+        const uint2 ku = *reinterpret_cast<const uint2*>(kc + base + (size_t)j * 128);
+        const uint2 vu = *reinterpret_cast<const uint2*>(vc + base + (size_t)j * 128);
+        const float2 k01 = unpack_bf16x2(ku.x), k23 = unpack_bf16x2(ku.y), v01 = unpack_bf16x2(vu.x), v23 = unpack_bf16x2(vu.y);
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+            float s = qv[g][0] * k01.x + qv[g][1] * k01.y + qv[g][2] * k23.x + qv[g][3] * k23.y;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            const float mn = fmaxf(m[g], s);
+            const float c = __expf(m[g] - mn), p = __expf(s - mn);
+            l[g] = l[g] * c + p;
+            acc[g][0] = acc[g][0] * c + p * v01.x; acc[g][1] = acc[g][1] * c + p * v01.y;
+            acc[g][2] = acc[g][2] * c + p * v23.x; acc[g][3] = acc[g][3] * c + p * v23.y;
+            m[g] = mn;
+        }
+    }
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+        if (lane == 0) { s_m[warp][g] = m[g]; s_l[warp][g] = l[g]; }
+        *reinterpret_cast<float4*>(&s_o[warp][g][lane * 4]) = make_float4(acc[g][0], acc[g][1], acc[g][2], acc[g][3]);
+    }
+    __syncthreads();
+    const int d = threadIdx.x;     // 128 threads = 128 output dims
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+        float M = -INFINITY;
+#pragma unroll
+        for (int w = 0; w < DEC_ATTN_WARPS; ++w) M = fmaxf(M, s_m[w][g]);
+        float L = 0.f, O = 0.f;
+#pragma unroll
+        for (int w = 0; w < DEC_ATTN_WARPS; ++w) {
+            const float e = s_m[w][g] == -INFINITY ? 0.f : __expf(s_m[w][g] - M);
+            L += s_l[w][g] * e;
+            O += s_o[w][g][d] * e;
+        }
+        const size_t row = ((size_t)b * Hq + kh * G + g) * splits + sp;
+        part_o[row * 128 + d] = O;
+        if (d == 0) { part_ml[row * 2] = M; part_ml[row * 2 + 1] = L; }
+    }
+}
+
+// out[b, h * 128 + d] = bf16(sum_s o_s[d] e^(m_s - M) / sum_s l_s e^(m_s - M)) over the splits of (b, h). grid B * Hq, 128 threads.
+__global__ void decode_attn_merge_kernel(const float* __restrict__ part_o, const float* __restrict__ part_ml, int splits,
+                                         __nv_bfloat16* __restrict__ out, int ldo, int Hq) {
+    pdl_launch_dependents();
+    const int bh = blockIdx.x, b = bh / Hq, h = bh % Hq, d = threadIdx.x;
+    const float* ml = part_ml + (size_t)bh * splits * 2;
+    float M = -INFINITY;
+    for (int s = 0; s < splits; ++s) M = fmaxf(M, ml[2 * s]);
+    float L = 0.f, O = 0.f;
+    for (int s = 0; s < splits; ++s) {
+        const float ms = ml[2 * s];
+        if (ms == -INFINITY) continue;
+        const float e = __expf(ms - M);
+        L += ml[2 * s + 1] * e;
+        O += part_o[((size_t)bh * splits + s) * 128 + d] * e;
+    }
+    out[(size_t)b * ldo + h * 128 + d] = __float2bfloat16_rn(O / L);
+}
+
+// Generation state at the start of a prefill: nothing generated, nothing finished, output ids -1.
+__global__ void generate_init_kernel(int B, int max_new, int* __restrict__ tokens, int* __restrict__ lengths, int* __restrict__ done,
+                                     int* __restrict__ n_done, int* __restrict__ all_done) {
+    pdl_launch_dependents();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    for (int k = i; k < B * max_new; k += gridDim.x * blockDim.x) tokens[k] = -1;
+    if (i < B) { lengths[i] = 0; done[i] = 0; }
+    if (i == 0) { *n_done = 0; *all_done = 0; }
+}
+
+// Greedy token selection and the per-token bookkeeping, one block per sequence. The processed logit of id n is HF's: the bf16 lm_head
+// output cast to fp32, then RepetitionPenaltyLogitsProcessor when a penalty bitmap is given (every prompt id and every generated id);
+// the token is the arg-max, ties to the lowest id (torch.argmax). A sequence that is not finished appends the token to tokens[b],
+// sets its penalty bit, advances lengths[b], and stores the next step's input id and (t, h, w) position (all three axes advance
+// together after the prompt: first_pos[b] + index of the token). It finishes on an EOS id or at max_new tokens; the block that
+// finishes the last sequence raises *all_done. A finished sequence is left untouched.
+constexpr int SELECT_THREADS = 1024;
+__global__ void __launch_bounds__(SELECT_THREADS) greedy_select_kernel(
+        const __nv_bfloat16* __restrict__ logits, int V, uint32_t* __restrict__ pen_bitmap, int pen_words, float penalty,
+        const int* __restrict__ eos_ids, int n_eos, int max_new, const int* __restrict__ first_pos, int B, int* __restrict__ tokens,
+        int* __restrict__ lengths, int* __restrict__ done, int* __restrict__ n_done, int* __restrict__ all_done, int* __restrict__ next_ids,
+        int* __restrict__ pos3) {
+    pdl_launch_dependents();
+    __shared__ float s_v[SELECT_THREADS / 32];
+    __shared__ int s_i[SELECT_THREADS / 32];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    if (done[b]) return;
+    const __nv_bfloat16* lr = logits + (size_t)b * V;
+    const uint32_t* pb = pen_bitmap ? pen_bitmap + (size_t)b * pen_words : nullptr;
+    float best = -INFINITY;
+    int bid = 0x7fffffff;
+    for (int n = tid; n < V; n += SELECT_THREADS) {
+        float x = __bfloat162float(lr[n]);
+        if (pb && ((pb[n >> 5] >> (n & 31)) & 1u)) x = x < 0.f ? x * penalty : __fdiv_rn(x, penalty);
+        if (x > best || bid == 0x7fffffff) { best = x; bid = n; }      // ids rise along the scan: strict > keeps the lowest of equals
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bid, o);
+        if (ov > best || (ov == best && oi < bid)) { best = ov; bid = oi; }
+    }
+    if ((tid & 31) == 0) { s_v[tid >> 5] = best; s_i[tid >> 5] = bid; }
+    __syncthreads();
+    if (tid != 0) return;
+    for (int w = 1; w < SELECT_THREADS / 32; ++w)
+        if (s_v[w] > best || (s_v[w] == best && s_i[w] < bid)) { best = s_v[w]; bid = s_i[w]; }
+    const int tok = bid, t = lengths[b];
+    tokens[(size_t)b * max_new + t] = tok;
+    lengths[b] = t + 1;
+    if (pen_bitmap) pen_bitmap[(size_t)b * pen_words + (tok >> 5)] |= 1u << (tok & 31);
+    next_ids[b] = tok;
+    const int p = first_pos[b] + t;
+    pos3[b] = p; pos3[B + b] = p; pos3[2 * B + b] = p;
+    bool fin = t + 1 >= max_new;
+    for (int e = 0; e < n_eos; ++e) fin |= tok == eos_ids[e];
+    if (fin) {
+        done[b] = 1;
+        if (atomicAdd(n_done, 1) + 1 == B) *all_done = 1;
+    }
+}
+
+}  // namespace vqa

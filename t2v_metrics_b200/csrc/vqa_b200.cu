@@ -288,9 +288,9 @@ extern "C" int vqa_qwen25vl_score(vqa_handle* h, const void* pixel_patches, int3
         return fail(h, VQA_ERR_INVALID_ARG, "bad size / temperature / repetition penalty");
     if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
     if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
-    return qwen_score(h, *h->qwen, pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows,
-                      max_window_len, cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index, position_ids, answer_ids, batch,
-                      seq_len, temperature, repetition_penalty, out_probs, out_logprobs, workspace, workspace_bytes,
+    const QwenPrompts in{pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows, max_window_len,
+                         cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index, position_ids, batch, seq_len};
+    return qwen_score(h, *h->qwen, in, answer_ids, temperature, repetition_penalty, out_probs, out_logprobs, workspace, workspace_bytes,
                       reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -333,10 +333,59 @@ extern "C" int vqa_qwen25vl_score_packed(vqa_handle* h, const void* pixel_patche
     QwenPacked pk;
     pk.total_rows = total_rows; pk.n_seq = n_seq; pk.max_seq_len = max_seq_len; pk.max_prompt_len = max_prompt_len;
     pk.cu_seqlens = cu_seqlens; pk.kv_prefix = kv_prefix; pk.pair_row = pair_row; pk.pair_seq = pair_seq;
-    return qwen_score(h, *h->qwen, pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows,
-                      max_window_len, cu_frames, n_frames, max_frame_len, input_ids, nullptr, feat_index, position_ids, answer_ids, n_prompts,
-                      total_rows, temperature, repetition_penalty, out_probs, out_logprobs, workspace, workspace_bytes,
+    const QwenPrompts in{pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows, max_window_len,
+                         cu_frames, n_frames, max_frame_len, input_ids, nullptr, feat_index, position_ids, n_prompts, total_rows};
+    return qwen_score(h, *h->qwen, in, answer_ids, temperature, repetition_penalty, out_probs, out_logprobs, workspace, workspace_bytes,
                       reinterpret_cast<cudaStream_t>(stream), &pk);
+}
+
+// ------------------------------------------------------------------------------------------------ Qwen2.5-VL greedy generation
+static int qwen_gen_check(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, const QwenGenArgs& a, const void* workspace) {
+    if (!h || h->kind != 1) return fail(h, VQA_ERR_INVALID_ARG, "not a Qwen2.5-VL handle");
+    if (!h->finalized) return fail(h, VQA_ERR_MISSING_WEIGHT, "vqa_finalize_weights has not succeeded");
+    if (!a.seq_lens || !a.first_pos || (a.n_eos > 0 && !a.eos_ids) || !a.tokens || !a.lengths || !a.all_done || !workspace)
+        return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    if (batch <= 0 || batch > 128 || seq_len <= 0 || n_patches <= 0 || a.max_new <= 0 || a.n_eos < 0 || !(a.repetition_penalty > 0.f))
+        return fail(h, VQA_ERR_INVALID_ARG, "bad size / repetition penalty (1 <= batch <= 128, max_new_tokens >= 1)");
+    const int G = h->qwen->cfg.heads / h->qwen->cfg.kv_heads;
+    if (G != 1 && G != 2 && G != 4 && G != 5 && G != 7 && G != 8)
+        return fail(h, VQA_ERR_UNSUPPORTED, "decode attention supports 1, 2, 4, 5, 7 or 8 query heads per KV head");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+    return VQA_OK;
+}
+
+extern "C" size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, int32_t max_new_tokens) {
+    if (!h || h->kind != 1 || batch <= 0 || seq_len <= 0 || n_patches <= 0 || max_new_tokens <= 0) return 0;
+    return qwen_gen_plan(h->qwen->cfg, batch, seq_len, n_patches, max_new_tokens, h->num_sms).total;
+}
+
+extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
+                                             const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
+                                             const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
+                                             int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
+                                             const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
+                                             int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
+                                             float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                             void* workspace, size_t workspace_bytes, void* stream) {
+    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done};
+    if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
+    if (!pixel_patches || !vis_pos_hw || !window_index || !reverse_index || !cu_window || !cu_frames || !input_ids || !feat_index || !position_ids)
+        return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    const int unit = h->qwen->cfg.spatial_merge * h->qwen->cfg.spatial_merge;
+    if (n_patches % unit || n_windows <= 0 || n_frames <= 0) return fail(h, VQA_ERR_INVALID_ARG, "bad vision sizes");
+    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
+    const QwenPrompts in{pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows, max_window_len,
+                         cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index, position_ids, batch, seq_len};
+    return qwen_generate_prefill(h, *h->qwen, in, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vqa_qwen25vl_generate_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
+                                          int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
+                                          int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes,
+                                          void* stream) {
+    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done};
+    if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
+    return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ kernel-level ABI

@@ -738,3 +738,106 @@ class QwenVLEngine:
         ans = torch.as_tensor(list(map(int, answer_ids)), dtype=torch.int32).to(dev)
         return self.score_tensors(pixel_patches.to(dev), grid_thw, d["input_ids"], d["seq_lens"], d["feat_index"], d["position_ids"],
                                   ans, temperature, repetition_penalty=repetition_penalty)
+
+    # ------------------------------------------------------------------------------------------ greedy generation
+    MAX_GEN_GRAPHS = 8
+
+    def generate_begin(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
+                       repetition_penalty: float = 1.0, second_per_grid_ts=None) -> dict:
+        """The prefill of a greedy generation (vqa_qwen25vl_generate_prefill): vision tower, padded prompt prefill into the K/V cache, first
+        token. Returns the generation state that generate_step() advances: device tensors `tokens` [B, max_new_tokens] (-1 after a prompt's
+        last token), `lengths` [B] and `all_done` [1], all owned by the state of this call shape."""
+        from . import qwen_host
+        cfg, dev = self.cfg, self.device
+        B = len(prompts)
+        img = list(image_of_sample) if image_of_sample is not None else list(range(B))
+        idx = qwen_host.build_batch_indices([list(map(int, p)) for p in prompts], [tuple(map(int, g)) for g in grid_thw], img,
+                                            cfg.image_token_id, cfg.spatial_merge_size, cfg.tokens_per_second,
+                                            video_token_id=cfg.video_token_id, second_per_grid_ts=second_per_grid_ts)
+        first = qwen_host.first_generated_positions(idx)
+        vi = self.vision_indices(grid_thw)
+        pixel_patches = pixel_patches.to(dev).contiguous()
+        assert pixel_patches.shape == (vi["n_patches"], cfg.patch_dim) and pixel_patches.dtype in (torch.float32, torch.bfloat16)
+        S, max_new = int(idx["input_ids"].shape[1]), int(max_new_tokens)
+        eos = [int(e) for e in eos_ids]
+        need = int(self.lib.vqa_qwen25vl_generate_workspace_bytes(self._h, B, S, vi["n_patches"], max_new))
+        if need == 0:
+            raise ValueError(f"bad generation size: batch {B}, prompt length {S}, max_new_tokens {max_new}")
+        gens = self.__dict__.setdefault("_gen_states", {})
+        ws = getattr(self, "_gen_workspace", None)
+        if ws is None or ws.numel() < need:
+            gens.clear()                         # captured step graphs point into the old workspace
+            self._gen_workspace = None
+            self._gen_workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+        key = (B, S, vi["n_patches"], max_new, float(repetition_penalty), len(eos))
+        st = gens.get(key)
+        if st is None:
+            i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
+            st = gens[key] = dict(B=B, S=S, n_patches=vi["n_patches"], max_new=max_new, penalty=float(repetition_penalty), n_eos=len(eos),
+                                  seq_lens=i32(B), first=i32(B), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new), lengths=i32(B),
+                                  all_done=i32(1), graph=None)
+            while len(gens) > self.MAX_GEN_GRAPHS:
+                gens.pop(next(iter(gens)))
+        st["seq_lens"].copy_(idx["seq_lens"], non_blocking=True)
+        st["first"].copy_(first, non_blocking=True)
+        if eos:
+            st["eos"].copy_(torch.as_tensor(eos, dtype=torch.int32), non_blocking=True)
+        d = {k: v.to(dev) for k, v in idx.items()}
+        pdt = _lib.VQA_DTYPE_F32 if pixel_patches.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
+
+        def prefill():
+            with torch.cuda.device(dev):
+                rc = self.lib.vqa_qwen25vl_generate_prefill(
+                    self._h, _ptr(pixel_patches), pdt, vi["n_patches"], _ptr(vi["vis_pos_hw"]), _ptr(vi["window_index"]), _ptr(vi["reverse_index"]),
+                    _ptr(vi["cu_window"]), vi["n_windows"], vi["max_window"], _ptr(vi["cu_frames"]), vi["n_frames"], vi["max_frame"],
+                    _ptr(d["input_ids"]), _ptr(st["seq_lens"]), _ptr(d["feat_index"]), _ptr(d["position_ids"]), _ptr(st["first"]), B, S,
+                    _ptr(st["eos"]), len(eos), max_new, float(repetition_penalty), _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]),
+                    _ptr(self._gen_workspace), self._gen_workspace.numel(), _stream_ptr(dev))
+            _check(rc, self._h, "vqa_qwen25vl_generate_prefill")
+        st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
+        prefill()
+        return st
+
+    def generate_step(self, st: dict):
+        """One decode step of the generation `st` (vqa_qwen25vl_generate_step), launched directly."""
+        with torch.cuda.device(self.device):
+            rc = self.lib.vqa_qwen25vl_generate_step(self._h, _ptr(st["seq_lens"]), _ptr(st["first"]), st["B"], st["S"], st["n_patches"],
+                                                     _ptr(st["eos"]), st["n_eos"], st["max_new"], st["penalty"], _ptr(st["tokens"]),
+                                                     _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(self._gen_workspace),
+                                                     self._gen_workspace.numel(), _stream_ptr(self.device))
+        _check(rc, self._h, "vqa_qwen25vl_generate_step")
+
+    def generate_prompts(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
+                         repetition_penalty: float = 1.0, second_per_grid_ts=None, use_graph: bool = True, check_every: int = 16):
+        """Greedy generation (HF generate(do_sample=False)) for a batch of prompts (1-D id lists, one image- or video-token run each, as in
+        score_prompts): one prefill, then decode steps replayed from a CUDA graph captured once per (batch, prompt length, max_new_tokens).
+        The host reads the all-finished flag through pinned memory every `check_every` steps and never synchronises in between.
+        Returns each prompt's generated ids, the EOS id included when one ended it."""
+        st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
+                                 second_per_grid_ts)
+        flag = self.__dict__.get("_gen_flag")
+        if flag is None:
+            flag = self._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+        ev = torch.cuda.Event()
+
+        def finished() -> bool:
+            flag.copy_(st["all_done"], non_blocking=True)
+            ev.record()
+            ev.synchronize()
+            return bool(flag[0])
+
+        for step in range(1, st["max_new"]):
+            if (step - 1) % check_every == 0 and finished():
+                break
+            if not use_graph:
+                self.generate_step(st)
+            elif st["graph"] is None:
+                self.generate_step(st)           # the first step runs directly (module loading, kernel attributes), then is captured
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    self.generate_step(st)
+                st["graph"] = graph
+            else:
+                st["graph"].replay()
+        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
+        return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]

@@ -133,6 +133,45 @@ class Qwen2VLModel(VQAScoreModel):
                       f"{[(a['token_text'], round(a['probability'], 6)) for a in alternatives]}")
         return probs, traces
 
+    def _eos_ids(self) -> List[int]:
+        """generation_config.json's eos_token_id beside the checkpoint (an id or a list), else the tokenizer's."""
+        from ...checkpoint import generation_config_value
+        spec = QWEN2_VL_MODELS[self.model_name]
+        eos = generation_config_value(self._checkpoint or spec["model"]["path"], "eos_token_id", None)
+        if eos is None:
+            eos = getattr(self.tokenizer, "eos_token_id", None)
+        if eos is None:
+            return []
+        return [int(e) for e in eos] if isinstance(eos, (list, tuple)) else [int(eos)]
+
+    @torch.no_grad()
+    def generate(self, images: List[str], texts: List[str], fps=None, max_new_tokens: int = 2048, temperature: float = 0.0,
+                 do_sample: Optional[bool] = None, top_p: float = 0.9, eos_token_ids: Optional[List[int]] = None) -> List[str]:
+        """Greedy text generation, the reference's Qwen2VLModel.generate (qwen2vl_model.py:495-563) with its default temperature 0: per
+        sample, the chat prompt of the raw text and the image, generate(do_sample=False) under the checkpoint's repetition penalty, the
+        prompt cut off, decoded with skip_special_tokens and stripped. Here the whole batch is one prefill and one decode loop on the
+        device; identical images are encoded once. Sampling (temperature > 0 or do_sample=True, top-p) is not implemented."""
+        assert len(images) == len(texts), "Number of images/videos and texts must match"
+        if do_sample is None:
+            do_sample = temperature > 0
+        if do_sample or temperature > 0:
+            raise NotImplementedError("only greedy decoding is supported (temperature=0.0, do_sample=False); top-p sampling is not implemented")
+        uniq: Dict[str, int] = {}
+        index = [uniq.setdefault(p, len(uniq)) for p in images]
+        patches, grids = self.load_images(list(uniq.keys()))
+        unit = self.cfg.spatial_merge_size ** 2
+        cache = self.__dict__.setdefault("_prompt_cache", {})
+        if len(cache) > 65536:
+            cache.clear()
+        prompts = []
+        for text, img in zip(texts, index):
+            t, gh, gw = grids[img]
+            prompts.append(build_prompt_ids(self.tokenizer, text, t * gh * gw // unit, self.cfg.image_token_id, cache))
+        eos = self._eos_ids() if eos_token_ids is None else [int(e) for e in eos_token_ids]
+        ids = self.engine.generate_prompts(patches, grids, prompts, max_new_tokens, eos, image_of_sample=index,
+                                           repetition_penalty=self.repetition_penalty)
+        return [self.tokenizer.decode(x, skip_special_tokens=True, clean_up_tokenization_spaces=False).strip() for x in ids]
+
     @torch.no_grad()
     def forward(self, images: List[str], texts: List[str], fps=None, question_template: str = default_question_template,
                 answer_template: str = default_answer_template, max_new_tokens: int = 1, temperature: float = 1.0,

@@ -136,6 +136,19 @@ def build_batch_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequence
     return dict(input_ids=ids, seq_lens=lens, feat_index=feat, position_ids=pos.reshape(3, B * S).contiguous())
 
 
+def first_generated_positions(idx) -> torch.Tensor:
+    """mRoPE position of the first generated token of every prompt of `build_batch_indices(...)`: the position of the prompt's last token
+    + 1; generated token t sits at that + t on all three axes. transformers' generate() advances the last prompt position ids by one per
+    step (modeling_qwen2_5_vl.py:1576-1612, generation/utils.py), which is below max(prompt positions) + 1 when a video's temporal index
+    exceeds the text positions. The chat template ends every prompt with text, where the three axes agree. [B] int32."""
+    B, S = idx["input_ids"].shape
+    pos = idx["position_ids"].view(3, B, S)
+    last = pos[:, torch.arange(B), idx["seq_lens"].long() - 1]                       # [3, B]
+    if not bool((last == last[0]).all()):
+        raise ValueError("generation needs prompts that end with a text token")
+    return (last[0] + 1).to(torch.int32)
+
+
 def build_packed_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequence[int]], image_of_sample: Sequence[int],
                          image_token_id: int, merge: int, tokens_per_second: int, video_token_id: Optional[int] = None,
                          second_per_grid_ts: Optional[Sequence[float]] = None):
