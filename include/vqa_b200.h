@@ -141,6 +141,28 @@ int vqa_clipt5_score(vqa_handle* h, const void* pixels, int32_t pixel_dtype, int
                      const int32_t* labels, int32_t batch, int32_t text_len, int32_t label_len, float* out_scores,
                      float* out_logprobs, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- CLIP-FlanT5 greedy generation (HF T5ForConditionalGeneration.generate(inputs_embeds=<spliced prompt>, do_sample=False, num_beams=1))
+ * One prefill, then one decode step per further token, all on the caller's stream. The prefill runs the encoder pass of vqa_clipt5_score
+ * (same inputs, no labels) and keeps its output in the workspace, then feeds the decoder start token and selects the first token. A step
+ * feeds each prompt's last token through the decoder, appending every layer's self-attention K/V row to a cache inside the workspace
+ * (capacity max_new_tokens per prompt), and selects the next one. Selection: arg-max of the bf16 lm_head logits cast to fp32, ties to the
+ * lowest id; no logits processors. A prompt finishes after emitting one of eos_ids (which is kept in its output) or max_new_tokens tokens;
+ * later steps leave it unchanged. Needs cross_attention_mode 0.
+ *   eos_ids [n_eos]         DEVICE; n_eos may be 0
+ *   out_tokens [batch, max_new_tokens]  generated ids, -1 after a prompt's last one; out_lengths [batch] tokens generated so far;
+ *   all_done [1]            1 once every prompt has finished
+ * Every step-dependent value lives in device memory: the step takes the same arguments every time, so one CUDA graph of it can be
+ * replayed for every token. The prefill and the steps must use the same workspace, sizes and pointers. batch <= 128,
+ * max_new_tokens <= 2048. */
+size_t vqa_clipt5_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, int32_t max_new_tokens);
+int vqa_clipt5_generate_prefill(vqa_handle* h, const void* pixels, int32_t pixel_dtype, int32_t n_images, const int32_t* image_index,
+                                const int32_t* input_ids, const int32_t* text_lens, int32_t batch, int32_t text_len, const int32_t* eos_ids,
+                                int32_t n_eos, int32_t max_new_tokens, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                void* workspace, size_t workspace_bytes, void* stream);
+int vqa_clipt5_generate_step(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, const int32_t* eos_ids, int32_t n_eos,
+                             int32_t max_new_tokens, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace,
+                             size_t workspace_bytes, void* stream);
+
 /* ---- Qwen2.5-VL (replaces Qwen2VLModel.forward's per-sample generate(max_new_tokens=1, output_scores=True) +
  * softmax(scores / T)[answer_id], t2v_metrics/models/vqascore_models/qwen2vl_model.py:160-167,190-289) ---- */
 int vqa_create_qwen25vl(const vqa_qwen25vl_config* cfg, int device, vqa_handle** out);

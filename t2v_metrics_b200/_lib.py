@@ -22,6 +22,7 @@ ABI_SYMBOLS = [
     "vqa_qwen25vl_topk", "vqa_op_gemm_bf16_normfuse",
     "vqa_qwen25vl_packed_workspace_bytes", "vqa_qwen25vl_score_packed", "vqa_debug_max_active_clusters", "vqa_op_attention_d128_ex", "vqa_op_gemm_bf16_grouped", "vqa_op_gemm_bf16_splitk",
     "vqa_qwen25vl_generate_workspace_bytes", "vqa_qwen25vl_generate_prefill", "vqa_qwen25vl_generate_step",
+    "vqa_clipt5_generate_workspace_bytes", "vqa_clipt5_generate_prefill", "vqa_clipt5_generate_step",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -128,6 +129,12 @@ def load() -> C.CDLL:
     lib.vqa_qwen25vl_generate_prefill.restype = C.c_int
     lib.vqa_qwen25vl_generate_step.argtypes = [vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, vp, vp, vp, vp, C.c_size_t, vp]
     lib.vqa_qwen25vl_generate_step.restype = C.c_int
+    lib.vqa_clipt5_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
+    lib.vqa_clipt5_generate_workspace_bytes.restype = C.c_size_t
+    lib.vqa_clipt5_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.vqa_clipt5_generate_prefill.restype = C.c_int
+    lib.vqa_clipt5_generate_step.argtypes = [vp, i32, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.vqa_clipt5_generate_step.restype = C.c_int
     lib.vqa_clip_preprocess_workspace_bytes.argtypes = [C.POINTER(i32), C.POINTER(i32), i32, i32, i32]
     lib.vqa_clip_preprocess_workspace_bytes.restype = C.c_size_t
     lib.vqa_clip_preprocess.argtypes = [vp, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, C.POINTER(C.c_uint8),

@@ -4,7 +4,9 @@
 #include "host.cuh"
 #include "attention.cuh"
 #include "attention_sm90.cuh"
-#include "qwen_kernels.cuh"   // cast_f32_bf16_kernel
+#include "qwen_kernels.cuh"   // cast_f32_bf16_kernel, gather_rows_by_index_kernel
+#include "qwen_decode.cuh"    // generate_init_kernel, greedy_select_kernel
+#include "t5_decode.cuh"
 
 static int clipt5_finalize(vqa_handle* h) {
     const vqa_clipt5_config& c = h->cfg;
@@ -163,17 +165,23 @@ __global__ void __launch_bounds__(256) row_ssq_kernel(const bf16* __restrict__ x
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-// Arguments as vqa_clipt5_score, already validated.
-static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int n_images, const int* image_index, const int* input_ids,
-                        const int* text_lens, const int* labels, int B, int L, int T, float* out_scores, float* out_logprobs, void* workspace,
-                        size_t workspace_bytes, cudaStream_t st) {
+// The image and prompt inputs of one encoder pass (see vqa_clipt5_score)
+struct ClipT5Prompts {
+    const void* pixels; int pixel_dtype, n_images;
+    const int *image_index, *input_ids, *text_lens;
+    int B, L;
+};
+
+// Vision tower, projector, multimodal splice, T5 encoder and its final norm into w.xn (prompt lengths in w.seq_lens), and for the absorbed
+// cross-attention the transposed encoder output in w.xt: everything a decoder pass reads of the prompts.
+static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Prompts& in) {
+    vqa_handle* h = f.h;
     const vqa_clipt5_config& c = h->cfg;
-    const ClipT5Workspace w = plan_workspace(h, B, n_images, L, T);
-    if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
-    Forward f(h, workspace, st);
+    cudaStream_t st = f.st;
+    const void* pixels = in.pixels;
+    const int pixel_dtype = in.pixel_dtype, n_images = in.n_images, B = in.B, L = in.L;
+    const int *image_index = in.image_index, *input_ids = in.input_ids, *text_lens = in.text_lens;
     auto P_ = [&](size_t off) { return f.at(off); };
-    const int rnd = c.emulate_bf16_rounding & VQA_FLAG_ROUND_DECODER;
     const bool round_attn = (c.emulate_bf16_rounding & VQA_FLAG_ROUND_ATTN_SCORES) != 0;
     const bool fuse_norms = (c.emulate_bf16_rounding & VQA_FLAG_FUSE_NORMS) != 0;
 
@@ -182,7 +190,7 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
     const int Dv = c.vit_hidden, Dm = c.d_model, H = c.n_heads, inner = H * 64, Hv = c.vit_heads;
     const int Mp = n_images * P, Mv = n_images * (P + 1);
     const int S = L - 1 + P;
-    const int M = B * S, Md = B * T;
+    const int M = B * S;
 
     // Precision of the vision tower's residual stream: the reference runs CLIPVisionModel under torch.autocast(bf16). nn.LayerNorm is on
     // autocast's fp32 list, so pre_layrnorm hands the encoder an fp32 tensor, every `residual + hidden_states` (modeling_clip.py:371,
@@ -292,16 +300,64 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
     if (c.cross_attention_mode == 0)
         TRY(f.launch(CAT_OTHER, 0, "encoder transpose", transpose_bsd_kernel, dim3((Sp + 31) / 32, (Dm + 31) / 32, B), dim3(32, 8), 0,
                      P_(w.xn), P_(w.xt), S, Dm, Sp));
+    return VQA_OK;
+}
+
+// Absorbed cross-attention of the B * T decoder rows in w.dq against the encoder output (w.xn, w.xt) into w.dattn (exact in real arithmetic;
+// 30x fewer FLOPs than projecting the S encoder rows because only T rows per pair attend):
+//   q.(Wk x_s) = (Wk^T q).x_s          sum_s p_s (Wv x_s) = Wv (sum_s p_s x_s)
+static int clipt5_absorbed_cross_attention(Forward& f, const ClipT5Workspace& w, const T5DecLayerW& Lw, int B, int T, int S) {
+    const vqa_clipt5_config& c = f.h->cfg;
+    auto P_ = [&](size_t off) { return f.at(off); };
+    const int Dm = c.d_model, H = c.n_heads, inner = H * 64, Md = B * T, TH = T * H, Sp = (S + 7) / 8 * 8;
+    // (1) q~[b,t,h,:] = Wk[h]^T q[b,t,h,:]   -- per head: [B*T, 64] x ckT[:, h*64:(h+1)*64]^T -> rows (b*T+t)*H + h
+    Gemm g1(P_(w.dq), Lw.ckT, P_(w.qt), Md, Dm, 64);
+    g1.lda = inner; g1.ldw = inner; g1.ldc = H * Dm;
+    TRY(f.gemm(g1.batched(BatchSpec{H, 0, 64, 0, 64, (long long)Dm, Md, inner, Dm, inner}, Dm >= 256 ? 2561 : 1281), "batched gemm"));
+    // (2) scores[b,(t,h),s] = q~[b,(t,h),:] . x[b,s,:]   -- per pair: [T*H, d] x [S, d]^T
+    Gemm g2(P_(w.qt), P_(w.xn), P_(w.csc), TH, Sp, Dm);
+    TRY(f.gemm(g2.batched(BatchSpec{B, TH, 0, S, 0, (long long)TH * Sp, (long long)B * TH, Dm, (long long)B * S, Dm}, 1281), "batched gemm"));
+    TRY(f.launch(CAT_ATTENTION, 0, "cross softmax", cross_softmax_kernel, (B * TH + 7) / 8, 256, 0, P_(w.csc), (const int*)f.at<int>(w.seq_lens),
+                 TH, B * TH, S, Sp));
+    // (3) ctx[b,(t,h),:] = sum_s p[b,(t,h),s] x[b,s,:]   -- per pair: [T*H, Sp] x (x[b]^T)[d, Sp]^T
+    Gemm g3(P_(w.csc), P_(w.xt), P_(w.cctx), TH, Dm, Sp);
+    TRY(f.gemm(g3.batched(BatchSpec{B, TH, 0, Dm, 0, (long long)TH * Dm, (long long)B * TH, Sp, (long long)B * Dm, Sp}, Dm >= 256 ? 2561 : 1281),
+               "batched gemm"));
+    // (4) o[b,t,h,:] = Wv[h] ctx[b,t,h,:]   -- per head: [B*T, d] (cols h*d..) x Wv[h*64:(h+1)*64, :]^T -> cols h*64..
+    Gemm g4(P_(w.cctx), Lw.ckv + (size_t)inner * Dm, P_(w.dattn), Md, 64, Dm);
+    g4.lda = H * Dm; g4.ldc = inner;
+    return f.gemm(g4.batched(BatchSpec{H, 0, Dm, 64, 0, 64, Md, (long long)H * Dm, inner, Dm}, 641), "batched gemm");
+}
+
+// Decoder store-GEMMs: M = B*T rows against 4096-row weights -> split-K when that fills the SMs, else the plain path
+static Gemm decoder_split_k(const Forward& f, const ClipT5Workspace& w, Gemm g) {
+    const int sl = splitk_slices(g.M, g.N, g.K, f.nsm);
+    if (sl > 1 && (size_t)sl * g.M * g.N * 4 <= w.splitk_bytes) g.split_k(sl, f.at<float>(w.splitk));
+    return g;
+}
+
+// Arguments as vqa_clipt5_score, already validated.
+static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int n_images, const int* image_index, const int* input_ids,
+                        const int* text_lens, const int* labels, int B, int L, int T, float* out_scores, float* out_logprobs, void* workspace,
+                        size_t workspace_bytes, cudaStream_t st) {
+    const vqa_clipt5_config& c = h->cfg;
+    const ClipT5Workspace w = plan_workspace(h, B, n_images, L, T);
+    if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+    Forward f(h, workspace, st);
+    auto P_ = [&](size_t off) { return f.at(off); };
+    const int rnd = c.emulate_bf16_rounding & VQA_FLAG_ROUND_DECODER;
+    const int P = (c.image_size / c.patch_size) * (c.image_size / c.patch_size);
+    const int Dm = c.d_model, H = c.n_heads, inner = H * 64;
+    const int S = L - 1 + P;
+    const int M = B * S, Md = B * T;
+    TRY(clipt5_encode(f, w, ClipT5Prompts{pixels, pixel_dtype, n_images, image_index, input_ids, text_lens, B, L}));
+    int* seq_lens = f.at<int>(w.seq_lens);
 
     // ---------------- T5 decoder (T target rows per pair) ----------------
     TRY(f.launch(CAT_OTHER, 0, "decoder embed", decoder_embed_kernel, Md, 128, 0, labels, h->shared, P_(w.y), T, Dm, c.decoder_start_id,
                  c.pad_token_id));
-    // decoder store-GEMMs: M = B*T rows against 4096-row weights -> split-K when that fills the SMs, else the plain path
-    auto dec = [&](Gemm g) {
-        const int sl = splitk_slices(g.M, g.N, g.K, f.nsm);
-        if (sl > 1 && (size_t)sl * g.M * g.N * 4 <= w.splitk_bytes) g.split_k(sl, f.at<float>(w.splitk));
-        return g;
-    };
+    auto dec = [&](Gemm g) { return decoder_split_k(f, w, g); };
     for (int l = 0; l < c.dec_layers; ++l) {
         const T5DecLayerW& Lw = h->dec[l];
         // self-attention
@@ -318,25 +374,7 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
             TRY(f.launch(CAT_ATTENTION, 4.0 * B * (double)H * T * S * 64, "cross attention", t5_cross_attn_kernel<8>, B * H, 128, 0, P_(w.dq),
                          P_(w.ckv), P_(w.dattn), seq_lens, 2 * inner, B, T, S, H, rnd));
         } else {
-            // absorbed association (exact in real arithmetic; 30x fewer FLOPs because only T rows per pair attend):
-            //   q.(Wk x_s) = (Wk^T q).x_s          sum_s p_s (Wv x_s) = Wv (sum_s p_s x_s)
-            const int TH = T * H;
-            // (1) q~[b,t,h,:] = Wk[h]^T q[b,t,h,:]   -- per head: [B*T, 64] x ckT[:, h*64:(h+1)*64]^T -> rows (b*T+t)*H + h
-            Gemm g1(P_(w.dq), Lw.ckT, P_(w.qt), Md, Dm, 64);
-            g1.lda = inner; g1.ldw = inner; g1.ldc = H * Dm;
-            TRY(f.gemm(g1.batched(BatchSpec{H, 0, 64, 0, 64, (long long)Dm, Md, inner, Dm, inner}, Dm >= 256 ? 2561 : 1281), "batched gemm"));
-            // (2) scores[b,(t,h),s] = q~[b,(t,h),:] . x[b,s,:]   -- per pair: [T*H, d] x [S, d]^T
-            Gemm g2(P_(w.qt), P_(w.xn), P_(w.csc), TH, Sp, Dm);
-            TRY(f.gemm(g2.batched(BatchSpec{B, TH, 0, S, 0, (long long)TH * Sp, (long long)B * TH, Dm, (long long)B * S, Dm}, 1281), "batched gemm"));
-            TRY(f.launch(CAT_ATTENTION, 0, "cross softmax", cross_softmax_kernel, (B * TH + 7) / 8, 256, 0, P_(w.csc), seq_lens, TH, B * TH, S, Sp));
-            // (3) ctx[b,(t,h),:] = sum_s p[b,(t,h),s] x[b,s,:]   -- per pair: [T*H, Sp] x (x[b]^T)[d, Sp]^T
-            Gemm g3(P_(w.csc), P_(w.xt), P_(w.cctx), TH, Dm, Sp);
-            TRY(f.gemm(g3.batched(BatchSpec{B, TH, 0, Dm, 0, (long long)TH * Dm, (long long)B * TH, Sp, (long long)B * Dm, Sp}, Dm >= 256 ? 2561 : 1281),
-                       "batched gemm"));
-            // (4) o[b,t,h,:] = Wv[h] ctx[b,t,h,:]   -- per head: [B*T, d] (cols h*d..) x Wv[h*64:(h+1)*64, :]^T -> cols h*64..
-            Gemm g4(P_(w.cctx), Lw.ckv + (size_t)inner * Dm, P_(w.dattn), Md, 64, Dm);
-            g4.lda = H * Dm; g4.ldc = inner;
-            TRY(f.gemm(g4.batched(BatchSpec{H, 0, Dm, 64, 0, 64, Md, (long long)H * Dm, inner, Dm}, 641), "batched gemm"));
+            TRY(clipt5_absorbed_cross_attention(f, w, Lw, B, T, S));
         }
         TRY(f.gemm(dec(Gemm(P_(w.dattn), Lw.co, P_(w.y), Md, Dm, inner).with_residual(P_(w.y)))));
         // gated FFN
@@ -355,4 +393,113 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
     TRY(f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, lse_max, lse_sum, label_logit, labels, out_scores,
                  out_logprobs, B, T, ntiles));
     return VQA_OK;
+}
+
+// ================================================================================================ greedy generation
+// Workspace of a generation: the scoring plan at T = 1 (its decoder buffers hold the B rows of a step, its split-K slices are sized for
+// them, and the encoder output and prompt lengths stay in it for every step), then the self-attention K/V cache (capacity max_new_tokens
+// per sequence: the start token and the first max_new_tokens - 1 generated tokens are the inputs), the [B, vocab] bf16 logits of a step,
+// and the step state.
+struct ClipT5GenWorkspace {
+    ClipT5Workspace w;
+    size_t kcache, vcache, logits, next_ids, done, n_done, total;
+    size_t layer_elems;
+    int cap;
+};
+static ClipT5GenWorkspace clipt5_gen_plan(const vqa_handle* h, int B, int n_images, int L, int max_new) {
+    const vqa_clipt5_config& c = h->cfg;
+    ClipT5GenWorkspace g;
+    g.w = plan_workspace(h, B, n_images, L, 1);
+    Plan pl;
+    pl.off = g.w.total;
+    g.cap = max_new;
+    g.layer_elems = (size_t)B * c.n_heads * g.cap * 64;
+    g.kcache = pl.take((size_t)c.dec_layers * g.layer_elems * 2);
+    g.vcache = pl.take((size_t)c.dec_layers * g.layer_elems * 2);
+    g.logits = pl.take((size_t)B * c.vocab * 2);
+    g.next_ids = pl.take((size_t)B * 4);
+    g.done = pl.take((size_t)B * 4);
+    g.n_done = pl.take(4);
+    g.total = pl.off;
+    return g;
+}
+
+// Outputs and constants of a generation, the same for the prefill and every step
+struct ClipT5GenArgs {
+    const int* eos_ids; int n_eos;
+    int max_new;
+    int* tokens;             // [B, max_new], -1 after a sequence's last token
+    int* lengths;            // [B] tokens generated so far
+    int* all_done;           // 1 once every sequence has finished
+};
+
+constexpr int T5_DEC_ATTN_WARPS = 4;
+
+// One decoder position per sequence: the start token (first) or the last selected token (next_ids), through every decoder layer with
+// its self-attention K/V appended to the cache, then the final norm, the lm_head into [B, vocab] bf16 logits, and the greedy token of
+// every unfinished sequence. Finished sequences recompute their frozen last position, which changes nothing they output.
+static int clipt5_decode_step(Forward& f, const ClipT5GenWorkspace& g, int B, int S, const ClipT5GenArgs& a, bool first) {
+    vqa_handle* h = f.h;
+    const vqa_clipt5_config& c = h->cfg;
+    const ClipT5Workspace& w = g.w;
+    auto P_ = [&](size_t off) { return f.at(off); };
+    const int rnd = c.emulate_bf16_rounding & VQA_FLAG_ROUND_DECODER;
+    const int Dm = c.d_model, H = c.n_heads, inner = H * 64;
+    int* next_ids = f.at<int>(g.next_ids);
+    if (first)    // decoder_embed_kernel at T = 1 embeds the start token and reads no labels
+        TRY(f.launch(CAT_OTHER, 0, "decoder embed", decoder_embed_kernel, B, 128, 0, (const int*)nullptr, h->shared, P_(w.y), 1, Dm,
+                     c.decoder_start_id, c.pad_token_id));
+    else
+        TRY(f.launch(CAT_OTHER, 0, "decoder embed", gather_rows_by_index_kernel, B, 128, 0, h->shared, (const int*)next_ids, P_(w.y), Dm));
+    auto dec = [&](Gemm gm) { return decoder_split_k(f, w, gm); };
+    for (int l = 0; l < c.dec_layers; ++l) {
+        const T5DecLayerW& Lw = h->dec[l];
+        bf16 *kc = f.at(g.kcache) + l * g.layer_elems, *vc = f.at(g.vcache) + l * g.layer_elems;
+        TRY(f.rmsnorm(P_(w.y), Lw.ln0, P_(w.yn), B, Dm, c.t5_ln_eps));
+        TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.qkv, P_(w.dqkv), B, 3 * inner, Dm))));
+        TRY(f.launch(CAT_OTHER, 0, "kv cache append", t5_kv_cache_append_kernel, (B * H * 8 + 255) / 256, 256, 0, (const bf16*)P_(w.dqkv), B, H,
+                     (const int*)a.lengths, kc, vc, g.cap));
+        TRY(f.launch(CAT_ATTENTION, 4.0 * B * (double)H * g.cap * 64, "decoder self attention (cached)", t5_decode_self_attn_kernel,
+                     (B * H + T5_DEC_ATTN_WARPS - 1) / T5_DEC_ATTN_WARPS, 32 * T5_DEC_ATTN_WARPS, T5_DEC_ATTN_WARPS * g.cap * sizeof(float),
+                     (const bf16*)P_(w.dqkv), (const bf16*)kc, (const bf16*)vc, g.cap, (const int*)a.lengths, P_(w.dattn), h->dec_rel,
+                     (const int*)h->lut_unidir, c.rel_max_distance, B, H, rnd));
+        TRY(f.gemm(dec(Gemm(P_(w.dattn), Lw.o, P_(w.y), B, Dm, inner).with_residual(P_(w.y)))));
+        TRY(f.rmsnorm(P_(w.y), Lw.ln1, P_(w.yn), B, Dm, c.t5_ln_eps));
+        TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.cq, P_(w.dq), B, inner, Dm))));
+        TRY(clipt5_absorbed_cross_attention(f, w, Lw, B, 1, S));
+        TRY(f.gemm(dec(Gemm(P_(w.dattn), Lw.co, P_(w.y), B, Dm, inner).with_residual(P_(w.y)))));
+        TRY(f.rmsnorm(P_(w.y), Lw.ln2, P_(w.yn), B, Dm, c.t5_ln_eps));
+        TRY(f.gemm(Gemm(P_(w.yn), Lw.wi, P_(w.dff), B, 2 * c.d_ff, Dm).with_epilogue(EPI_GATED_GELU, c.d_ff)));
+        TRY(f.gemm(dec(Gemm(P_(w.dff), Lw.wo, P_(w.y), B, Dm, c.d_ff).with_residual(P_(w.y)))));
+    }
+    TRY(f.rmsnorm(P_(w.y), h->dec_final_ln, P_(w.yn), B, Dm, c.t5_ln_eps));
+    // The [B, vocab] bf16 logits are 64 KB per sequence against the 263 MB lm_head weight (xxl) that the GEMM streams either way.
+    bf16* logits = f.at(g.logits);
+    TRY(f.gemm(Gemm(P_(w.yn), h->lm_head, logits, B, c.vocab, Dm), "lm_head"));
+    return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, (const bf16*)logits, c.vocab, (uint32_t*)nullptr,
+                    0, 1.0f, a.eos_ids, a.n_eos, a.max_new, (const int*)nullptr, B, a.tokens, a.lengths, f.at<int>(g.done),
+                    f.at<int>(g.n_done), a.all_done, next_ids, (int*)nullptr);
+}
+
+// Encoder pass of vqa_clipt5_score, the generation state reset, then the first decoder position (the start token) and the first token.
+static int clipt5_generate_prefill(vqa_handle* h, const ClipT5Prompts& in, const ClipT5GenArgs& a, void* workspace, size_t workspace_bytes,
+                                   cudaStream_t st) {
+    const ClipT5GenWorkspace g = clipt5_gen_plan(h, in.B, in.n_images, in.L, a.max_new);
+    if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
+    Forward f(h, workspace, st);
+    TRY(clipt5_encode(f, g.w, in));
+    TRY(f.launch(CAT_OTHER, 0, "generate init", generate_init_kernel, (in.B * a.max_new + 255) / 256, 256, 0, in.B, a.max_new, a.tokens,
+                 a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
+    const int P = (h->cfg.image_size / h->cfg.patch_size) * (h->cfg.image_size / h->cfg.patch_size);
+    return clipt5_decode_step(f, g, in.B, in.L - 1 + P, a, true);
+}
+
+// One decode step: every sequence feeds its last selected token.
+static int clipt5_generate_step(vqa_handle* h, int B, int n_images, int L, const ClipT5GenArgs& a, void* workspace, size_t workspace_bytes,
+                                cudaStream_t st) {
+    const ClipT5GenWorkspace g = clipt5_gen_plan(h, B, n_images, L, a.max_new);
+    if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
+    Forward f(h, workspace, st);
+    const int P = (h->cfg.image_size / h->cfg.patch_size) * (h->cfg.image_size / h->cfg.patch_size);
+    return clipt5_decode_step(f, g, B, L - 1 + P, a, false);
 }

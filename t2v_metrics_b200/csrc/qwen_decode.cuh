@@ -137,9 +137,10 @@ __global__ void generate_init_kernel(int B, int max_new, int* __restrict__ token
 // Greedy token selection and the per-token bookkeeping, one block per sequence. The processed logit of id n is HF's: the bf16 lm_head
 // output cast to fp32, then RepetitionPenaltyLogitsProcessor when a penalty bitmap is given (every prompt id and every generated id);
 // the token is the arg-max, ties to the lowest id (torch.argmax). A sequence that is not finished appends the token to tokens[b],
-// sets its penalty bit, advances lengths[b], and stores the next step's input id and (t, h, w) position (all three axes advance
-// together after the prompt: first_pos[b] + index of the token). It finishes on an EOS id or at max_new tokens; the block that
-// finishes the last sequence raises *all_done. A finished sequence is left untouched.
+// sets its penalty bit, advances lengths[b], and stores the next step's input id and, when pos3 is given, its (t, h, w) position (all
+// three axes advance together after the prompt: first_pos[b] + index of the token; the T5 decoder passes nullptr for both and has no
+// positions to keep). It finishes on an EOS id or at max_new tokens; the block that finishes the last sequence raises *all_done. A finished
+// sequence is left untouched.
 constexpr int SELECT_THREADS = 1024;
 __global__ void __launch_bounds__(SELECT_THREADS) greedy_select_kernel(
         const __nv_bfloat16* __restrict__ logits, int V, uint32_t* __restrict__ pen_bitmap, int pen_words, float penalty,
@@ -176,8 +177,10 @@ __global__ void __launch_bounds__(SELECT_THREADS) greedy_select_kernel(
     lengths[b] = t + 1;
     if (pen_bitmap) pen_bitmap[(size_t)b * pen_words + (tok >> 5)] |= 1u << (tok & 31);
     next_ids[b] = tok;
-    const int p = first_pos[b] + t;
-    pos3[b] = p; pos3[B + b] = p; pos3[2 * B + b] = p;
+    if (pos3) {
+        const int p = first_pos[b] + t;
+        pos3[b] = p; pos3[B + b] = p; pos3[2 * B + b] = p;
+    }
     bool fin = t + 1 >= max_new;
     for (int e = 0; e < n_eos; ++e) fin |= tok == eos_ids[e];
     if (fin) {

@@ -122,6 +122,45 @@ extern "C" int vqa_clipt5_score(vqa_handle* h, const void* pixels, int32_t pixel
                         workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
+// ------------------------------------------------------------------------------------------------ CLIP-FlanT5 greedy generation
+static int clipt5_gen_check(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, const ClipT5GenArgs& a, const void* workspace) {
+    if (!h || h->kind != 0) return fail(h, VQA_ERR_INVALID_ARG, "not a CLIP-FlanT5 handle");
+    if (!h->finalized) return fail(h, VQA_ERR_MISSING_WEIGHT, "vqa_finalize_weights has not succeeded");
+    if ((a.n_eos > 0 && !a.eos_ids) || !a.tokens || !a.lengths || !a.all_done || !workspace) return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    if (batch <= 0 || batch > 128 || n_images <= 0 || text_len <= 0 || a.max_new <= 0 || a.max_new > 2048 || a.n_eos < 0)
+        return fail(h, VQA_ERR_INVALID_ARG, "bad size (1 <= batch <= 128, 1 <= max_new_tokens <= 2048)");
+    if (h->cfg.cross_attention_mode != 0)
+        return fail(h, VQA_ERR_UNSUPPORTED, "generation needs the absorbed cross-attention (cross_attention_mode = 0)");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+    return VQA_OK;
+}
+
+extern "C" size_t vqa_clipt5_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, int32_t max_new_tokens) {
+    if (!h || h->kind != 0 || batch <= 0 || n_images <= 0 || text_len <= 0 || max_new_tokens <= 0) return 0;
+    return clipt5_gen_plan(h, batch, n_images, text_len, max_new_tokens).total;
+}
+
+extern "C" int vqa_clipt5_generate_prefill(vqa_handle* h, const void* pixels, int32_t pixel_dtype, int32_t n_images, const int32_t* image_index,
+                                           const int32_t* input_ids, const int32_t* text_lens, int32_t batch, int32_t text_len,
+                                           const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, int32_t* out_tokens,
+                                           int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes, void* stream) {
+    const ClipT5GenArgs a{eos_ids, n_eos, max_new_tokens, out_tokens, out_lengths, all_done};
+    if (int rc = clipt5_gen_check(h, batch, n_images, text_len, a, workspace)) return rc;
+    if (!pixels || !input_ids || !text_lens) return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    if (!image_index && n_images != batch) return fail(h, VQA_ERR_INVALID_ARG, "image_index == NULL requires n_images == batch");
+    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
+    const ClipT5Prompts in{pixels, pixel_dtype, n_images, image_index, input_ids, text_lens, batch, text_len};
+    return clipt5_generate_prefill(h, in, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vqa_clipt5_generate_step(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, const int32_t* eos_ids, int32_t n_eos,
+                                        int32_t max_new_tokens, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
+    const ClipT5GenArgs a{eos_ids, n_eos, max_new_tokens, out_tokens, out_lengths, all_done};
+    if (int rc = clipt5_gen_check(h, batch, n_images, text_len, a, workspace)) return rc;
+    return clipt5_generate_step(h, batch, n_images, text_len, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
 // Byte offsets inside the caller's workspace of the tensors a parity investigation wants to look at after a call has completed.
 extern "C" int vqa_clipt5_debug_layout(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, int32_t label_len,
                                        size_t* offsets, int32_t n) {

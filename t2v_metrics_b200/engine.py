@@ -288,6 +288,101 @@ class ClipT5Engine:
         names = ("gemm", "attention", "norm", "other")
         return {n: (float(ms[i]), float(fl[i]), int(sc[i]), float(by[i])) for i, n in enumerate(names)}
 
+    # ------------------------------------------------------------------------------------------ greedy generation
+    MAX_GEN_GRAPHS = 8
+
+    def generate_begin(self, pixel_values: torch.Tensor, input_ids: torch.Tensor, text_lens: torch.Tensor, max_new_tokens: int,
+                       eos_ids: Sequence[int], image_index: Optional[torch.Tensor] = None) -> dict:
+        """The prefill of a greedy generation (vqa_clipt5_generate_prefill): the encoder pass of score_tensors over the same inputs (no
+        labels), then the decoder start token and the first token. Returns the generation state that generate_step() advances: device
+        tensors `tokens` [B, max_new_tokens] (-1 after a prompt's last token), `lengths` [B] and `all_done` [1], all owned by the state of
+        this call shape. The generation workspace is separate from the scoring one, so scoring graphs are never invalidated by it."""
+        dev = self.device
+        assert pixel_values.is_cuda and pixel_values.dim() == 4 and pixel_values.is_contiguous()
+        assert pixel_values.dtype in (torch.float32, torch.bfloat16)
+        for t in (input_ids, text_lens):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+        B, L = input_ids.shape
+        NI = pixel_values.shape[0]
+        if image_index is not None:
+            assert image_index.is_cuda and image_index.dtype == torch.int32 and image_index.shape == (B,)
+        max_new = int(max_new_tokens)
+        eos = [int(e) for e in eos_ids]
+        need = int(self.lib.vqa_clipt5_generate_workspace_bytes(self._h, B, NI, L, max_new))
+        if need == 0:
+            raise ValueError(f"bad generation size: batch {B}, images {NI}, prompt length {L}, max_new_tokens {max_new}")
+        gens = self.__dict__.setdefault("_gen_states", collections.OrderedDict())
+        ws = getattr(self, "_gen_workspace", None)
+        if ws is None or ws.numel() < need:
+            gens.clear()                         # captured step graphs point into the old workspace
+            self._gen_workspace = None
+            self._gen_workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+        key = (B, NI, L, max_new, len(eos))
+        st = gens.get(key)
+        if st is None:
+            i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
+            st = gens[key] = dict(B=B, NI=NI, L=L, max_new=max_new, n_eos=len(eos), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new),
+                                  lengths=i32(B), all_done=i32(1), graph=None)
+            while len(gens) > self.MAX_GEN_GRAPHS:
+                gens.popitem(last=False)         # least recently used shape first
+        gens.move_to_end(key)
+        if eos:
+            st["eos"].copy_(torch.as_tensor(eos, dtype=torch.int32), non_blocking=True)
+        pdt = _lib.VQA_DTYPE_F32 if pixel_values.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
+
+        def prefill():
+            with torch.cuda.device(dev):
+                rc = self.lib.vqa_clipt5_generate_prefill(self._h, _ptr(pixel_values), pdt, NI, _ptr(image_index), _ptr(input_ids),
+                                                          _ptr(text_lens), B, L, _ptr(st["eos"]), len(eos), max_new, _ptr(st["tokens"]),
+                                                          _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(self._gen_workspace),
+                                                          self._gen_workspace.numel(), _stream_ptr(dev))
+            _check(rc, self._h, "vqa_clipt5_generate_prefill")
+        st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
+        prefill()
+        return st
+
+    def generate_step(self, st: dict):
+        """One decode step of the generation `st` (vqa_clipt5_generate_step), launched directly."""
+        with torch.cuda.device(self.device):
+            rc = self.lib.vqa_clipt5_generate_step(self._h, st["B"], st["NI"], st["L"], _ptr(st["eos"]), st["n_eos"], st["max_new"],
+                                                   _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(self._gen_workspace),
+                                                   self._gen_workspace.numel(), _stream_ptr(self.device))
+        _check(rc, self._h, "vqa_clipt5_generate_step")
+
+    def generate_tensors(self, pixel_values: torch.Tensor, input_ids: torch.Tensor, text_lens: torch.Tensor, max_new_tokens: int,
+                         eos_ids: Sequence[int], image_index: Optional[torch.Tensor] = None, use_graph: bool = True, check_every: int = 16):
+        """Greedy generation (HF generate(do_sample=False, num_beams=1)) for a batch of prompts laid out as for score_tensors: one prefill,
+        then decode steps replayed from a CUDA graph captured once per (batch, images, prompt length, max_new_tokens) and kept for the
+        MAX_GEN_GRAPHS most recently used shapes. The host reads the all-finished flag through pinned memory every `check_every` steps and
+        never synchronises in between. Returns each prompt's generated ids, the EOS id included when one ended it."""
+        st = self.generate_begin(pixel_values, input_ids, text_lens, max_new_tokens, eos_ids, image_index)
+        flag = self.__dict__.get("_gen_flag")
+        if flag is None:
+            flag = self._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+        ev = torch.cuda.Event()
+
+        def finished() -> bool:
+            flag.copy_(st["all_done"], non_blocking=True)
+            ev.record()
+            ev.synchronize()
+            return bool(flag[0])
+
+        for step in range(1, st["max_new"]):
+            if (step - 1) % check_every == 0 and finished():
+                break
+            if not use_graph:
+                self.generate_step(st)
+            elif st["graph"] is None:
+                self.generate_step(st)           # the first step runs directly (module loading, kernel attributes), then is captured
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    self.generate_step(st)
+                st["graph"] = graph
+            else:
+                st["graph"].replay()
+        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
+        return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]
+
 
 # ------------------------------------------------------------------------------------------------ single-kernel ops
 class ops:

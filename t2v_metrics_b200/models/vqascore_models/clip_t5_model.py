@@ -40,6 +40,19 @@ def format_answer(answer: str, conversation_style: str = "t5_chat") -> str:
     return answer
 
 
+def prompt_token_ids(tokenizer, questions: List[str], context_len: int, vocab: int, cache: dict) -> List[List[int]]:
+    """t5_tokenizer_image_token of each formatted prompt, truncated to context_len. The splice kernel replaces exactly ONE image slot per
+    prompt and embeds every other id: a caption that itself contains the literal "<image>" would add a second slot (t5_tokenizer_image_token
+    splits on it), and an id outside the vocabulary would index past the embedding table. Refuse both on the host."""
+    ids = [t5_tokenizer_image_token(q, tokenizer, chunk_cache=cache)[:context_len] for q in questions]
+    for q, row in zip(questions, ids):
+        if sum(1 for t in row if t == IMAGE_TOKEN_INDEX) != 1:
+            raise ValueError(f"each prompt must contain exactly one {DEFAULT_IMAGE_TOKEN!r} placeholder (the caption must not contain it): {q!r}")
+        if any((t < 0 and t != IMAGE_TOKEN_INDEX) or t >= vocab for t in row):
+            raise ValueError("token id outside [0, vocab)")
+    return ids
+
+
 class CLIPT5Model(VQAScoreModel):
     """VQAScore with CLIP-FlanT5 on the H100 engine."""
     video_mode = "concat"
@@ -103,21 +116,19 @@ class CLIPT5Model(VQAScoreModel):
         raw = [torch.from_numpy(np.ascontiguousarray(np.asarray(self.image_loader(p).convert("RGB"), dtype=np.uint8))) for p in image]
         return clip_preprocess_u8(raw, self.cfg.image_size, self.engine.device, pad=self.image_aspect_ratio == "pad")
 
+    def _prompt_ids(self, questions: List[str]) -> List[List[int]]:
+        cache = self.__dict__.setdefault("_chunk_cache", {})
+        if len(cache) > 65536:
+            cache.clear()
+        return prompt_token_ids(self.tokenizer, questions, self.context_len, self.cfg.vocab, cache)
+
     def _tokenize(self, questions: List[str], answers: List[str]):
         cache = self.__dict__.setdefault("_chunk_cache", {})
         if len(cache) > 65536:
             cache.clear()
-        ids = [t5_tokenizer_image_token(q, self.tokenizer, chunk_cache=cache)[: self.context_len] for q in questions]
+        ids = prompt_token_ids(self.tokenizer, questions, self.context_len, self.cfg.vocab, cache)
         labs = [t5_tokenizer_image_token(a, self.tokenizer, chunk_cache=cache)[: self.context_len] for a in answers]
         pad = getattr(self.tokenizer, "pad_token_id", 0) or 0
-        # The splice kernel replaces exactly ONE image slot per prompt and embeds every other id: a caption that itself contains the
-        # literal "<image>" would add a second slot (t5_tokenizer_image_token splits on it), and an id outside the vocabulary would index
-        # past the embedding table. Refuse both on the host.
-        for q, row in zip(questions, ids):
-            if sum(1 for t in row if t == IMAGE_TOKEN_INDEX) != 1:
-                raise ValueError(f"each prompt must contain exactly one {DEFAULT_IMAGE_TOKEN!r} placeholder (the caption must not contain it): {q!r}")
-            if any((t < 0 and t != IMAGE_TOKEN_INDEX) or t >= self.cfg.vocab for t in row):
-                raise ValueError("token id outside [0, vocab)")
         for row in labs:
             if any(t < 0 or t >= self.cfg.vocab for t in row):
                 raise ValueError(f"answer token id outside [0, vocab) (answers must not contain {DEFAULT_IMAGE_TOKEN!r})")
@@ -132,6 +143,61 @@ class CLIPT5Model(VQAScoreModel):
             labels[i, : len(b)] = torch.tensor(b, dtype=torch.int32)
             lens[i] = len(a)
         return input_ids, lens, labels
+
+    # ---- generation ----------------------------------------------------------------------------------------------
+    GENERATE_MAX_PAIRS = 64
+
+    def _eos_ids(self) -> List[int]:
+        """generation_config.json's eos_token_id beside the checkpoint (an id or a list), else the tokenizer's."""
+        from ...checkpoint import generation_config_value
+        spec = CLIP_T5_MODELS[self.model_name]
+        eos = generation_config_value(self._checkpoint or spec["model"]["path"], "eos_token_id", None)
+        if eos is None:
+            eos = getattr(self.tokenizer, "eos_token_id", None)
+        if eos is None:
+            return []
+        return [int(e) for e in eos] if isinstance(eos, (list, tuple)) else [int(eos)]
+
+    @torch.no_grad()
+    def generate(self, images: List[str], texts: List[str], max_new_tokens: int = 256, temperature: float = 0.0,
+                 do_sample: Optional[bool] = None, eos_token_ids: Optional[List[int]] = None) -> List[str]:
+        """Greedy text generation with CLIP-FlanT5 (V_3.0_README.md:316-325: `model.generate(images=..., texts=...) -> List[str]`).
+
+        Per sample the prompt is format_question(text) -- the raw text, no question template -- through t5_tokenizer_image_token,
+        truncated to context_len, i.e. the scoring path's prompt; identical image paths are encoded once. Decoding is HF
+        T5ForConditionalGeneration.generate(inputs_embeds=<spliced prompt>, attention_mask=<its mask>, do_sample=False, num_beams=1): the
+        decoder starts from decoder_start_id, each token is the arg-max of the fp32-cast bf16 logits over the whole vocabulary (ties to
+        the lowest id) with no logits processors (FlanT5's generation config has no repetition penalty), and a sample stops on an EOS id
+        (kept, then dropped by the decode) or after max_new_tokens tokens. EOS ids come from generation_config.json beside the checkpoint,
+        else the tokenizer; `eos_token_ids=` overrides both. Output: tokenizer.decode(ids, skip_special_tokens=True).strip().
+
+        The v3.0 wrapper's default length is not recoverable from the reference; 256 is this implementation's choice and sizes the K/V
+        cache (393 KB per sample per token at xxl width). The batch runs as one encoder pass and one decode loop on the device, in calls of
+        at most GENERATE_MAX_PAIRS pairs. Sampling (temperature > 0 or do_sample=True) is not implemented."""
+        assert len(images) == len(texts), "Number of images and texts must match"
+        if do_sample is None:
+            do_sample = temperature > 0
+        if do_sample or temperature > 0:
+            raise NotImplementedError("only greedy decoding is supported (temperature=0.0, do_sample=False)")
+        prompts = self._prompt_ids([format_question(t, self.conversational_style) for t in texts])
+        eos = self._eos_ids() if eos_token_ids is None else [int(e) for e in eos_token_ids]
+        out: List[str] = []
+        for lo in range(0, len(images), self.GENERATE_MAX_PAIRS):
+            chunk_images, chunk_prompts = images[lo:lo + self.GENERATE_MAX_PAIRS], prompts[lo:lo + self.GENERATE_MAX_PAIRS]
+            uniq: Dict[str, int] = {}
+            index = [uniq.setdefault(p, len(uniq)) for p in chunk_images]
+            pixels = self.load_images(list(uniq.keys()))
+            dev = self.engine.device
+            L = max(map(len, chunk_prompts))
+            pad = getattr(self.tokenizer, "pad_token_id", 0) or 0
+            input_ids = torch.full((len(chunk_prompts), L), pad, dtype=torch.int32)
+            for i, row in enumerate(chunk_prompts):
+                input_ids[i, :len(row)] = torch.tensor(row, dtype=torch.int32)
+            lens = torch.tensor([len(r) for r in chunk_prompts], dtype=torch.int32)
+            image_index = torch.tensor(index, dtype=torch.int32).to(dev) if len(uniq) != len(chunk_images) else None
+            ids = self.engine.generate_tensors(pixels, input_ids.to(dev), lens.to(dev), max_new_tokens, eos, image_index=image_index)
+            out.extend(self.tokenizer.decode(x, skip_special_tokens=True).strip() for x in ids)
+        return out
 
     # ---- scoring -------------------------------------------------------------------------------------------------
     @torch.no_grad()
