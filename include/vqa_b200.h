@@ -252,6 +252,35 @@ int vqa_qwen25vl_generate_step(vqa_handle* h, const int32_t* seq_lens, const int
                                int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
                                int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Qwen2.5-VL scoring over a greedy rollout (reference Qwen2VLModel.forward / forward_with_trace with max_new_tokens > 1,
+ * qwen2vl_model.py:169-493: generate(do_sample=False, output_scores=True), then softmax(scores[s] / T)[answer id] at chosen steps) ----
+ * vqa_qwen25vl_generate_prefill / _step with one more kernel per token, between the lm_head and the selection: for every step s of every
+ * unfinished prompt b, the log-softmax of the step's processed scores (bf16 logits -> fp32 -> repetition penalty over the prompt and the
+ * tokens generated before s -> / temperature), over the whole vocabulary, at each of the prompt's answer ids. The temperature only
+ * affects these probabilities; the tokens are those of vqa_qwen25vl_generate_*, bit for bit. Same workspace
+ * (vqa_qwen25vl_generate_workspace_bytes) and the same rules for it.
+ *   answer_ids [batch, n_max]   DEVICE, prompt b's ids in its first answer_counts[b] entries (no cap on n_max)
+ *   answer_counts [batch]       DEVICE
+ *   out_logp [batch, max_new_tokens, n_max]          fp32, [b, s, j] = log p(s, answer_ids[b, j]); entries of steps a prompt did not
+ *                                                    generate and of j >= answer_counts[b] are not written
+ *   out_topk_ids / out_topk_probs [batch, max_new_tokens, top_k]  with 0 < top_k <= 8: the step's top_k ids (ties to the lower id) and
+ *                                                    probabilities; may be NULL when top_k == 0
+ * The outputs are caller-owned; a step takes the same arguments every time (one CUDA graph replays every token). */
+int vqa_qwen25vl_rollout_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches, const int32_t* vis_pos_hw,
+                                 const int32_t* window_index, const int32_t* reverse_index, const int32_t* cu_window, int32_t n_windows,
+                                 int32_t max_window_len, const int32_t* cu_frames, int32_t n_frames, int32_t max_frame_len,
+                                 const int32_t* input_ids, const int32_t* seq_lens, const int32_t* feat_index, const int32_t* position_ids,
+                                 const int32_t* first_position, int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos,
+                                 int32_t max_new_tokens, float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                 const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, float temperature, int32_t top_k,
+                                 float* out_logp, int32_t* out_topk_ids, float* out_topk_probs, void* workspace, size_t workspace_bytes,
+                                 void* stream);
+int vqa_qwen25vl_rollout_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
+                              int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
+                              int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, const int32_t* answer_ids,
+                              const int32_t* answer_counts, int32_t n_max, float temperature, int32_t top_k, float* out_logp,
+                              int32_t* out_topk_ids, float* out_topk_probs, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Number of kernels the last vqa_clipt5_score call launched (for bench.py's gpu_launches). */
 int64_t vqa_last_launch_count(vqa_handle* h);
 
@@ -342,6 +371,13 @@ int vqa_op_gemm_bf16_normfuse(const void* A, int32_t lda, const void* W, int32_t
  * scratch: DEVICE float, >= 4*M*ceil(N/128) + M floats. */
 int vqa_op_lmhead_logprob(const void* H, int32_t ldh, const void* W, int32_t ldw, int32_t M, int32_t N, int32_t K,
                           const int32_t* labels, float* logprob, float* scratch, void* stream);
+
+/* The per-step kernel of vqa_qwen25vl_rollout_* on caller-given bf16 logits [batch, V]: for every b with done[b] == 0, row lengths[b] of
+ * out_logp [batch, max_new, n_max] (and of out_topk_ids / out_topk_probs [batch, max_new, top_k] when top_k > 0), under the penalty
+ * bitmap pen_bitmap [batch, ceil(V / 32)] (NULL = none) and the temperature. All pointers DEVICE. */
+int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t V, const uint32_t* pen_bitmap, float repetition_penalty, float temperature,
+                          const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, int32_t max_new, const int32_t* lengths,
+                          const int32_t* done, int32_t top_k, float* out_logp, int32_t* out_topk_ids, float* out_topk_probs, void* stream);
 
 /* Bidirectional attention, head_dim 64, packed qkv [B*S, 3*H*64] -> out [B*S, H*64].
  * bias_table: DEVICE float [H, 2S-1] (index key - query + S - 1) or NULL; seq_lens DEVICE int32 [B] or NULL.

@@ -23,6 +23,7 @@ ABI_SYMBOLS = [
     "vqa_qwen25vl_packed_workspace_bytes", "vqa_qwen25vl_score_packed", "vqa_debug_max_active_clusters", "vqa_op_attention_d128_ex", "vqa_op_gemm_bf16_grouped", "vqa_op_gemm_bf16_splitk",
     "vqa_qwen25vl_generate_workspace_bytes", "vqa_qwen25vl_generate_prefill", "vqa_qwen25vl_generate_step",
     "vqa_clipt5_generate_workspace_bytes", "vqa_clipt5_generate_prefill", "vqa_clipt5_generate_step",
+    "vqa_qwen25vl_rollout_prefill", "vqa_qwen25vl_rollout_step", "vqa_op_answer_logprob",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -129,6 +130,13 @@ def load() -> C.CDLL:
     lib.vqa_qwen25vl_generate_prefill.restype = C.c_int
     lib.vqa_qwen25vl_generate_step.argtypes = [vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, vp, vp, vp, vp, C.c_size_t, vp]
     lib.vqa_qwen25vl_generate_step.restype = C.c_int
+    rollout = [vp, vp, i32, f32, i32, vp, vp, vp]          # answer ids, counts, n_max, temperature, top_k, logp, top-k ids, top-k probs
+    lib.vqa_qwen25vl_rollout_prefill.argtypes = list(lib.vqa_qwen25vl_generate_prefill.argtypes[:-3]) + rollout + [vp, C.c_size_t, vp]
+    lib.vqa_qwen25vl_rollout_prefill.restype = C.c_int
+    lib.vqa_qwen25vl_rollout_step.argtypes = list(lib.vqa_qwen25vl_generate_step.argtypes[:-3]) + rollout + [vp, C.c_size_t, vp]
+    lib.vqa_qwen25vl_rollout_step.restype = C.c_int
+    lib.vqa_op_answer_logprob.argtypes = [vp, i32, i32, vp, f32, f32, vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, vp]
+    lib.vqa_op_answer_logprob.restype = C.c_int
     lib.vqa_clipt5_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
     lib.vqa_clipt5_generate_workspace_bytes.restype = C.c_size_t
     lib.vqa_clipt5_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]

@@ -358,6 +358,16 @@ static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S
     return g;
 }
 
+// Scoring hook of a rollout: the answer log-probabilities (and optionally the top-k) of every step, see answer_logprob_kernel
+struct QwenAnswerScore {
+    const int* answer_ids;       // [B, n_max]
+    const int* answer_counts;    // [B]
+    int n_max; float temperature; int top_k;
+    float* logp;                 // [B, max_new, n_max]
+    int* topk_ids;               // [B, max_new, top_k] (top_k > 0)
+    float* topk_probs;           // [B, max_new, top_k] (top_k > 0)
+};
+
 // Outputs and constants of a generation, the same for the prefill and every step
 struct QwenGenArgs {
     const int* seq_lens;     // [B] prompt lengths
@@ -367,9 +377,11 @@ struct QwenGenArgs {
     int* tokens;             // [B, max_new], -1 after a sequence's last token
     int* lengths;            // [B] tokens generated so far
     int* all_done;           // 1 once every sequence has finished
+    const QwenAnswerScore* score = nullptr;      // rollout scoring: one more launch per token, before the selection
 };
 
-// lm_head on w.lastn into [B, vocab] bf16 logits, then the greedy token of every unfinished sequence and its bookkeeping
+// lm_head on w.lastn into [B, vocab] bf16 logits, then (rollout scoring) the answer log-probabilities of this step, then the greedy token
+// of every unfinished sequence and its bookkeeping
 static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g, int B, const QwenGenArgs& a) {
     const vqa_qwen25vl_config& c = q.cfg;
     const QwenWorkspace& w = g.w;
@@ -377,6 +389,11 @@ static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g
     // The [B, vocab] bf16 logits are 0.3 MB per sequence against the 1.1 GB lm_head weight (7B) that the GEMM streams either way.
     TRY(f.gemm(Gemm(f.at(w.lastn), q.lm_head, logits, B, c.vocab, c.hidden), "lm_head"));
     const bool penalise = a.repetition_penalty != 1.0f;
+    if (const QwenAnswerScore* s = a.score)
+        TRY(f.launch(CAT_OTHER, 0, "answer logprob", answer_logprob_kernel, B, ANSWER_THREADS, 0, (const bf16*)logits, c.vocab,
+                     penalise ? (const uint32_t*)f.at<uint32_t>(w.pen_bitmap) : nullptr, (c.vocab + 31) / 32, a.repetition_penalty,
+                     1.0f / s->temperature, s->answer_ids, s->answer_counts, s->n_max, a.max_new, (const int*)a.lengths,
+                     (const int*)f.at<int>(g.done), s->top_k, s->logp, s->topk_ids, s->topk_probs));
     return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, (const bf16*)logits, c.vocab,
                     penalise ? f.at<uint32_t>(w.pen_bitmap) : nullptr, (c.vocab + 31) / 32, a.repetition_penalty, a.eos_ids, a.n_eos,
                     a.max_new, a.first_pos, B, a.tokens, a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done,

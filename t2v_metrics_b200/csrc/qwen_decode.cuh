@@ -189,4 +189,111 @@ __global__ void __launch_bounds__(SELECT_THREADS) greedy_select_kernel(
     }
 }
 
+// Answer log-probabilities of one generation step (the scores a rollout is scored on), one block per sequence, launched between the
+// lm_head and greedy_select_kernel so the penalty bitmap is still the one this step's token was chosen under. The processed score of id n
+// is that of the scoring path and topk_softmax_kernel: bf16 logit -> fp32 -> repetition penalty (bitmap) -> * inv_temp; over the full
+// vocabulary, logp(n) = score(n) - max - log(sum exp(score - max)). With t = lengths[b] (the step's index), writes
+// out_logp[b, t, j] = logp(answer_ids[b, j]) for j < answer_counts[b] (other entries untouched), and with top_k > 0 the top_k most probable
+// ids and their probabilities to out_topk_ids / out_topk_probs[b, t, :] (ties to the lower id). A finished sequence returns at once.
+// Each thread reads 8 logits (and their penalty words) before it consumes them, so a thread has 8 loads in flight.
+constexpr int ANSWER_THREADS = 256, ANSWER_UNROLL = 8, ANSWER_TOPK_MAX = 8;
+__global__ void __launch_bounds__(ANSWER_THREADS) answer_logprob_kernel(
+        const __nv_bfloat16* __restrict__ logits, int V, const uint32_t* __restrict__ pen_bitmap, int pen_words, float penalty, float inv_temp,
+        const int* __restrict__ answer_ids, const int* __restrict__ answer_counts, int n_max, int max_new, const int* __restrict__ lengths,
+        const int* __restrict__ done, int top_k, float* __restrict__ out_logp, int* __restrict__ out_topk_ids, float* __restrict__ out_topk_probs) {
+    pdl_launch_dependents();
+    __shared__ float s_val[ANSWER_THREADS * ANSWER_TOPK_MAX];
+    __shared__ int s_idx[ANSWER_THREADS * ANSWER_TOPK_MAX];
+    __shared__ float s_red[2][ANSWER_THREADS / 32];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    if (done[b]) return;
+    const __nv_bfloat16* lr = logits + (size_t)b * V;
+    const uint32_t* pb = pen_bitmap ? pen_bitmap + (size_t)b * pen_words : nullptr;
+    auto processed = [&](float x, uint32_t word, int n) {
+        if ((word >> (n & 31)) & 1u) x = x < 0.f ? x * penalty : __fdiv_rn(x, penalty);
+        return x * inv_temp;
+    };
+    float tv[ANSWER_TOPK_MAX];
+    int ti[ANSWER_TOPK_MAX];
+#pragma unroll
+    for (int i = 0; i < ANSWER_TOPK_MAX; ++i) { tv[i] = -INFINITY; ti[i] = -1; }
+    float mx = -INFINITY, sm = 0.f;
+    for (int base = 0; base < V; base += ANSWER_THREADS * ANSWER_UNROLL) {
+        float x[ANSWER_UNROLL];
+        uint32_t w[ANSWER_UNROLL];
+#pragma unroll
+        for (int u = 0; u < ANSWER_UNROLL; ++u) {
+            const int n = base + u * ANSWER_THREADS + tid;
+            x[u] = n < V ? __bfloat162float(lr[n]) : 0.f;
+            w[u] = (pb && n < V) ? pb[n >> 5] : 0u;
+        }
+#pragma unroll
+        for (int u = 0; u < ANSWER_UNROLL; ++u) {
+            const int n = base + u * ANSWER_THREADS + tid;      // ids rise along a thread's scan
+            if (n >= V) break;
+            const float v = processed(x[u], w[u], n);
+            if (v > mx) { sm = sm * __expf(mx - v) + 1.f; mx = v; } else { sm += __expf(v - mx); }
+            if (top_k > 0 && v > tv[ANSWER_TOPK_MAX - 1]) {     // sorted insert; strict > keeps the lower id first among equals
+                int pos = ANSWER_TOPK_MAX - 1;
+#pragma unroll
+                for (int i = ANSWER_TOPK_MAX - 2; i >= 0; --i)
+                    if (v > tv[i]) { tv[i + 1] = tv[i]; ti[i + 1] = ti[i]; pos = i; }
+                tv[pos] = v; ti[pos] = n;
+            }
+        }
+    }
+    // block-wide max and sum of exps
+    float bm = mx;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) bm = fmaxf(bm, __shfl_xor_sync(0xffffffffu, bm, o));
+    if ((tid & 31) == 0) s_red[0][tid >> 5] = bm;
+    __syncthreads();
+    bm = s_red[0][0];
+#pragma unroll
+    for (int i = 1; i < ANSWER_THREADS / 32; ++i) bm = fmaxf(bm, s_red[0][i]);
+    float bs = (mx == -INFINITY) ? 0.f : sm * __expf(mx - bm);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) bs += __shfl_xor_sync(0xffffffffu, bs, o);
+    if ((tid & 31) == 0) s_red[1][tid >> 5] = bs;
+    if (top_k > 0) {
+#pragma unroll
+        for (int i = 0; i < ANSWER_TOPK_MAX; ++i) { s_val[tid * ANSWER_TOPK_MAX + i] = tv[i]; s_idx[tid * ANSWER_TOPK_MAX + i] = ti[i]; }
+    }
+    __syncthreads();
+    float total = 0.f;
+#pragma unroll
+    for (int i = 0; i < ANSWER_THREADS / 32; ++i) total += s_red[1][i];
+    const float lse = bm + logf(total);
+    const int t = lengths[b];
+    const size_t row = (size_t)b * max_new + t;
+    const int cnt = min(answer_counts[b], n_max);
+    for (int j = tid; j < cnt; j += ANSWER_THREADS) {
+        const int id = answer_ids[(size_t)b * n_max + j];
+        out_logp[row * n_max + j] = (id >= 0 && id < V) ? processed(__bfloat162float(lr[id]), pb ? pb[id >> 5] : 0u, id) - lse : -INFINITY;
+    }
+    if (top_k <= 0 || tid >= 32) return;
+    // warp 0 picks the top_k of the 256 sorted lists: highest score, lower id on equal scores
+    for (int k = 0; k < top_k; ++k) {
+        float best = -INFINITY;
+        int bpos = -1, bid = 0x7fffffff;
+        for (int j = tid; j < ANSWER_THREADS * ANSWER_TOPK_MAX; j += 32) {
+            const float v = s_val[j];
+            const int id = s_idx[j];
+            if (id >= 0 && (v > best || (v == best && id < bid))) { best = v; bpos = j; bid = id; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+            const int op = __shfl_xor_sync(0xffffffffu, bpos, o), oid = __shfl_xor_sync(0xffffffffu, bid, o);
+            if (ov > best || (ov == best && oid < bid)) { best = ov; bpos = op; bid = oid; }
+        }
+        if (tid == 0) {
+            out_topk_ids[row * top_k + k] = bpos >= 0 ? bid : -1;
+            out_topk_probs[row * top_k + k] = bpos >= 0 ? __expf(best - bm) / total : 0.f;
+            if (bpos >= 0) s_idx[bpos] = -1;      // remove the winner
+        }
+        __syncwarp();
+    }
+}
+
 }  // namespace vqa

@@ -398,15 +398,16 @@ extern "C" size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t b
     return qwen_gen_plan(h->qwen->cfg, batch, seq_len, n_patches, max_new_tokens, h->num_sms).total;
 }
 
-extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
-                                             const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
-                                             const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
-                                             int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
-                                             const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
-                                             int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
-                                             float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
-                                             void* workspace, size_t workspace_bytes, void* stream) {
-    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done};
+// vqa_qwen25vl_generate_prefill, and with `score` vqa_qwen25vl_rollout_prefill
+static int vqa_qwen25vl_generate_prefill_impl(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
+                                              const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
+                                              const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
+                                              int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
+                                              const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
+                                              int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
+                                              float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                              const QwenAnswerScore* score, void* workspace, size_t workspace_bytes, void* stream) {
+    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done, score};
     if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
     if (!pixel_patches || !vis_pos_hw || !window_index || !reverse_index || !cu_window || !cu_frames || !input_ids || !feat_index || !position_ids)
         return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
@@ -418,11 +419,63 @@ extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const void* pixel_pa
     return qwen_generate_prefill(h, *h->qwen, in, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
+extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
+                                             const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
+                                             const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
+                                             int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
+                                             const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
+                                             int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
+                                             float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                             void* workspace, size_t workspace_bytes, void* stream) {
+    return vqa_qwen25vl_generate_prefill_impl(h, pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window,
+                                              n_windows, max_window_len, cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index,
+                                              position_ids, first_position, batch, seq_len, eos_ids, n_eos, max_new_tokens,
+                                              repetition_penalty, out_tokens, out_lengths, all_done, nullptr, workspace, workspace_bytes, stream);
+}
+
 extern "C" int vqa_qwen25vl_generate_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
                                           int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
                                           int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes,
                                           void* stream) {
     const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done};
+    if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
+    return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
+static int qwen_rollout_check(vqa_handle* h, const QwenAnswerScore& s) {
+    if (!s.answer_ids || !s.answer_counts || !s.logp || (s.top_k > 0 && (!s.topk_ids || !s.topk_probs)))
+        return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    if (s.n_max <= 0 || !(s.temperature > 0.f) || s.top_k < 0 || s.top_k > ANSWER_TOPK_MAX)
+        return fail(h, VQA_ERR_INVALID_ARG, "bad answer size / temperature / top_k (n_max >= 1, temperature > 0, 0 <= top_k <= 8)");
+    return VQA_OK;
+}
+
+extern "C" int vqa_qwen25vl_rollout_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
+                                            const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
+                                            const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
+                                            int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
+                                            const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
+                                            int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
+                                            float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                            const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, float temperature,
+                                            int32_t top_k, float* out_logp, int32_t* out_topk_ids, float* out_topk_probs, void* workspace,
+                                            size_t workspace_bytes, void* stream) {
+    const QwenAnswerScore s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
+    if (int rc = qwen_rollout_check(h, s)) return rc;
+    return vqa_qwen25vl_generate_prefill_impl(h, pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window,
+                                              n_windows, max_window_len, cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index,
+                                              position_ids, first_position, batch, seq_len, eos_ids, n_eos, max_new_tokens,
+                                              repetition_penalty, out_tokens, out_lengths, all_done, &s, workspace, workspace_bytes, stream);
+}
+
+extern "C" int vqa_qwen25vl_rollout_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
+                                         int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
+                                         int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, const int32_t* answer_ids,
+                                         const int32_t* answer_counts, int32_t n_max, float temperature, int32_t top_k, float* out_logp,
+                                         int32_t* out_topk_ids, float* out_topk_probs, void* workspace, size_t workspace_bytes, void* stream) {
+    const QwenAnswerScore s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
+    if (int rc = qwen_rollout_check(h, s)) return rc;
+    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done, &s};
     if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
     return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
@@ -517,6 +570,19 @@ extern "C" int vqa_op_lmhead_logprob(const void* Hs, int32_t ldh, const void* W,
     lse_finalize_kernel<<<(M + 3) / 4, 128, 0, st>>>(lse_max, lse_sum, label_logit, labels, lse_max /*scratch scores*/,
                                                     logprob, M, 1, ntiles);
     return cuda_status(nullptr, cudaGetLastError(), "lse finalize");
+}
+
+extern "C" int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t V, const uint32_t* pen_bitmap, float repetition_penalty,
+                                     float temperature, const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, int32_t max_new,
+                                     const int32_t* lengths, const int32_t* done, int32_t top_k, float* out_logp, int32_t* out_topk_ids,
+                                     float* out_topk_probs, void* stream) {
+    if (!logits || !lengths || !done || batch <= 0 || V <= 0 || max_new <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad answer logprob argument");
+    const QwenAnswerScore s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
+    if (int rc = qwen_rollout_check(nullptr, s)) return rc;
+    answer_logprob_kernel<<<batch, ANSWER_THREADS, 0, (cudaStream_t)stream>>>(
+        (const bf16*)logits, V, pen_bitmap, (V + 31) / 32, repetition_penalty, 1.0f / temperature, answer_ids, answer_counts, n_max, max_new,
+        lengths, done, top_k, out_logp, out_topk_ids, out_topk_probs);
+    return cuda_status(nullptr, cudaGetLastError(), "answer logprob launch");
 }
 
 extern "C" int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32_t H, const int32_t* seq_lens,

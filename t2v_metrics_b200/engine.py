@@ -453,6 +453,28 @@ class ops:
         return out
 
     @staticmethod
+    def answer_logprob(logits: torch.Tensor, answer_ids: torch.Tensor, answer_counts: torch.Tensor, lengths: torch.Tensor, done: torch.Tensor,
+                       max_new: int, temperature: float = 1.0, penalty_bitmap=None, repetition_penalty: float = 1.0, top_k: int = 0,
+                       out_logp=None, out_topk_ids=None, out_topk_probs=None):
+        """The per-step kernel of a scored rollout on given bf16 logits [B, V] (int32 answer_ids [B, n_max], answer_counts / lengths /
+        done [B]; penalty_bitmap int32 [B, ceil(V / 32)] or None). Writes row lengths[b] of out_logp [B, max_new, n_max] and, with
+        top_k > 0, of out_topk_ids / out_topk_probs [B, max_new, top_k]; returns the three outputs (allocated NaN / -1 when not given)."""
+        lib = _lib.load()
+        B, V = logits.shape
+        n_max = answer_ids.shape[1]
+        dev = logits.device
+        if out_logp is None:
+            out_logp = torch.full((B, max_new, n_max), float("nan"), dtype=torch.float32, device=dev)
+        if top_k > 0 and out_topk_ids is None:
+            out_topk_ids = torch.full((B, max_new, top_k), -1, dtype=torch.int32, device=dev)
+            out_topk_probs = torch.full((B, max_new, top_k), float("nan"), dtype=torch.float32, device=dev)
+        rc = lib.vqa_op_answer_logprob(_ptr(logits), B, V, _ptr(penalty_bitmap), float(repetition_penalty), float(temperature), _ptr(answer_ids),
+                                       _ptr(answer_counts), n_max, max_new, _ptr(lengths), _ptr(done), top_k, _ptr(out_logp), _ptr(out_topk_ids),
+                                       _ptr(out_topk_probs), _stream_ptr(dev))
+        _check(rc, None, "vqa_op_answer_logprob")
+        return out_logp, out_topk_ids, out_topk_probs
+
+    @staticmethod
     def norm(x: torch.Tensor, gamma: torch.Tensor, beta=None, eps=1e-6):
         lib = _lib.load()
         y = torch.empty_like(x)
@@ -837,11 +859,18 @@ class QwenVLEngine:
     # ------------------------------------------------------------------------------------------ greedy generation
     MAX_GEN_GRAPHS = 8
 
+    def generate_workspace_bytes(self, batch: int, seq_len: int, n_patches: int, max_new_tokens: int) -> int:
+        """Device bytes of one generation or scored rollout (vqa_qwen25vl_generate_workspace_bytes); 0 for invalid sizes."""
+        return int(self.lib.vqa_qwen25vl_generate_workspace_bytes(self._h, batch, seq_len, n_patches, max_new_tokens))
+
     def generate_begin(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
-                       repetition_penalty: float = 1.0, second_per_grid_ts=None) -> dict:
+                       repetition_penalty: float = 1.0, second_per_grid_ts=None, score: Optional[dict] = None) -> dict:
         """The prefill of a greedy generation (vqa_qwen25vl_generate_prefill): vision tower, padded prompt prefill into the K/V cache, first
         token. Returns the generation state that generate_step() advances: device tensors `tokens` [B, max_new_tokens] (-1 after a prompt's
-        last token), `lengths` [B] and `all_done` [1], all owned by the state of this call shape."""
+        last token), `lengths` [B] and `all_done` [1], all owned by the state of this call shape.
+        score = dict(answer_ids=[ids per prompt], temperature=T, top_k=k) makes it a scored rollout (vqa_qwen25vl_rollout_prefill): the
+        state also holds `logp` [B, max_new_tokens, n_max] (NaN where nothing was written) and, with k > 0, `topk_ids` / `topk_probs`
+        [B, max_new_tokens, k]."""
         from . import qwen_host
         cfg, dev = self.cfg, self.device
         B = len(prompts)
@@ -865,42 +894,76 @@ class QwenVLEngine:
             self._gen_workspace = None
             self._gen_workspace = torch.empty(need, dtype=torch.uint8, device=dev)
         key = (B, S, vi["n_patches"], max_new, float(repetition_penalty), len(eos))
+        if score is not None:
+            answers = [[int(t) for t in a] for a in score["answer_ids"]]
+            if len(answers) != B or not all(answers):
+                raise ValueError("rollout scoring needs one non-empty answer id list per prompt")
+            n_max, temp, top_k = max(len(a) for a in answers), float(score.get("temperature", 1.0)), int(score.get("top_k", 0))
+            key += ("rollout", n_max, temp, top_k)
         st = gens.get(key)
         if st is None:
             i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
             st = gens[key] = dict(B=B, S=S, n_patches=vi["n_patches"], max_new=max_new, penalty=float(repetition_penalty), n_eos=len(eos),
                                   seq_lens=i32(B), first=i32(B), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new), lengths=i32(B),
-                                  all_done=i32(1), graph=None)
+                                  all_done=i32(1), graph=None, score=None)
+            if score is not None:
+                st["score"] = dict(n_max=n_max, temperature=temp, top_k=top_k, answer_ids=i32(B, n_max), counts=i32(B),
+                                   logp=torch.empty(B, max_new, n_max, dtype=torch.float32, device=dev),
+                                   topk_ids=i32(B, max_new, top_k) if top_k > 0 else None,
+                                   topk_probs=torch.empty(B, max_new, top_k, dtype=torch.float32, device=dev) if top_k > 0 else None)
             while len(gens) > self.MAX_GEN_GRAPHS:
                 gens.pop(next(iter(gens)))
         st["seq_lens"].copy_(idx["seq_lens"], non_blocking=True)
         st["first"].copy_(first, non_blocking=True)
         if eos:
             st["eos"].copy_(torch.as_tensor(eos, dtype=torch.int32), non_blocking=True)
+        sc = st["score"]
+        if sc is not None:
+            ans = torch.full((B, sc["n_max"]), -1, dtype=torch.int32)
+            for b, a in enumerate(answers):
+                ans[b, :len(a)] = torch.as_tensor(a, dtype=torch.int32)
+            sc["answer_ids"].copy_(ans, non_blocking=True)
+            sc["counts"].copy_(torch.as_tensor([len(a) for a in answers], dtype=torch.int32), non_blocking=True)
+            sc["logp"].fill_(float("nan"))
+            if sc["top_k"] > 0:
+                sc["topk_ids"].fill_(-1)
+                sc["topk_probs"].fill_(float("nan"))
         d = {k: v.to(dev) for k, v in idx.items()}
         pdt = _lib.VQA_DTYPE_F32 if pixel_patches.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
 
         def prefill():
-            with torch.cuda.device(dev):
-                rc = self.lib.vqa_qwen25vl_generate_prefill(
-                    self._h, _ptr(pixel_patches), pdt, vi["n_patches"], _ptr(vi["vis_pos_hw"]), _ptr(vi["window_index"]), _ptr(vi["reverse_index"]),
+            args = [self._h, _ptr(pixel_patches), pdt, vi["n_patches"], _ptr(vi["vis_pos_hw"]), _ptr(vi["window_index"]), _ptr(vi["reverse_index"]),
                     _ptr(vi["cu_window"]), vi["n_windows"], vi["max_window"], _ptr(vi["cu_frames"]), vi["n_frames"], vi["max_frame"],
                     _ptr(d["input_ids"]), _ptr(st["seq_lens"]), _ptr(d["feat_index"]), _ptr(d["position_ids"]), _ptr(st["first"]), B, S,
-                    _ptr(st["eos"]), len(eos), max_new, float(repetition_penalty), _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]),
-                    _ptr(self._gen_workspace), self._gen_workspace.numel(), _stream_ptr(dev))
-            _check(rc, self._h, "vqa_qwen25vl_generate_prefill")
+                    _ptr(st["eos"]), len(eos), max_new, float(repetition_penalty), _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"])]
+            fn, name = self.lib.vqa_qwen25vl_generate_prefill, "vqa_qwen25vl_generate_prefill"
+            if sc is not None:
+                args += self._rollout_args(sc)
+                fn, name = self.lib.vqa_qwen25vl_rollout_prefill, "vqa_qwen25vl_rollout_prefill"
+            with torch.cuda.device(dev):
+                rc = fn(*args, _ptr(self._gen_workspace), self._gen_workspace.numel(), _stream_ptr(dev))
+            _check(rc, self._h, name)
         st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
         prefill()
         return st
 
+    @staticmethod
+    def _rollout_args(sc: dict) -> list:
+        return [_ptr(sc["answer_ids"]), _ptr(sc["counts"]), sc["n_max"], sc["temperature"], sc["top_k"], _ptr(sc["logp"]),
+                _ptr(sc["topk_ids"]), _ptr(sc["topk_probs"])]
+
     def generate_step(self, st: dict):
-        """One decode step of the generation `st` (vqa_qwen25vl_generate_step), launched directly."""
+        """One decode step of the generation `st` (vqa_qwen25vl_generate_step, or vqa_qwen25vl_rollout_step for a scored rollout),
+        launched directly."""
+        args = [self._h, _ptr(st["seq_lens"]), _ptr(st["first"]), st["B"], st["S"], st["n_patches"], _ptr(st["eos"]), st["n_eos"],
+                st["max_new"], st["penalty"], _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"])]
+        fn, name = self.lib.vqa_qwen25vl_generate_step, "vqa_qwen25vl_generate_step"
+        if st["score"] is not None:
+            args += self._rollout_args(st["score"])
+            fn, name = self.lib.vqa_qwen25vl_rollout_step, "vqa_qwen25vl_rollout_step"
         with torch.cuda.device(self.device):
-            rc = self.lib.vqa_qwen25vl_generate_step(self._h, _ptr(st["seq_lens"]), _ptr(st["first"]), st["B"], st["S"], st["n_patches"],
-                                                     _ptr(st["eos"]), st["n_eos"], st["max_new"], st["penalty"], _ptr(st["tokens"]),
-                                                     _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(self._gen_workspace),
-                                                     self._gen_workspace.numel(), _stream_ptr(self.device))
-        _check(rc, self._h, "vqa_qwen25vl_generate_step")
+            rc = fn(*args, _ptr(self._gen_workspace), self._gen_workspace.numel(), _stream_ptr(self.device))
+        _check(rc, self._h, name)
 
     def generate_prompts(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
                          repetition_penalty: float = 1.0, second_per_grid_ts=None, use_graph: bool = True, check_every: int = 16):
@@ -910,6 +973,30 @@ class QwenVLEngine:
         Returns each prompt's generated ids, the EOS id included when one ended it."""
         st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
                                  second_per_grid_ts)
+        self._decode_loop(st, use_graph, check_every)
+        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
+        return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]
+
+    def rollout_scores(self, pixel_patches, grid_thw, prompts, answer_ids, max_new_tokens: int, eos_ids: Sequence[int],
+                       temperature: float = 1.0, repetition_penalty: float = 1.0, top_k: int = 0, image_of_sample=None,
+                       second_per_grid_ts=None, use_graph: bool = True, check_every: int = 16) -> dict:
+        """A greedy rollout scored at every step: generate_prompts' decode loop (same tokens, bit for bit) plus, at each step s of each
+        prompt b, log softmax(processed scores / temperature) at each of the prompt's answer ids (answer_ids: one id list per prompt) -- the
+        per-step probabilities the reference's forward / forward_with_trace read from generate(output_scores=True) (qwen2vl_model.py:160-167).
+        With top_k > 0 (<= 8) also the step's top_k ids and probabilities. The temperature never changes a token.
+        Returns CPU tensors: dict(tokens=[ids per prompt], lengths [B], logp [B, max_new_tokens, n_max] (NaN beyond a prompt's length or its
+        answer), topk_ids / topk_probs [B, max_new_tokens, top_k] or None)."""
+        st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
+                                 second_per_grid_ts, score=dict(answer_ids=answer_ids, temperature=temperature, top_k=top_k))
+        self._decode_loop(st, use_graph, check_every)
+        sc = st["score"]
+        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
+        cpu = lambda t: None if t is None else t.cpu()
+        return dict(tokens=[tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])], lengths=lengths, logp=cpu(sc["logp"]),
+                    topk_ids=cpu(sc["topk_ids"]), topk_probs=cpu(sc["topk_probs"]))
+
+    def _decode_loop(self, st: dict, use_graph: bool, check_every: int):
+        """Decode steps after generate_begin until every prompt has finished: a CUDA graph of the step captured once per state, replayed."""
         flag = self.__dict__.get("_gen_flag")
         if flag is None:
             flag = self._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)
@@ -934,5 +1021,3 @@ class QwenVLEngine:
                 st["graph"] = graph
             else:
                 st["graph"].replay()
-        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
-        return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]

@@ -4,6 +4,9 @@ Same plugin contract as the reference's `Qwen2VLModel` (t2v_metrics/models/vqasc
 attributes, `forward(images, texts, question_template, answer_template, temperature) -> CPU fp32 Tensor[n]` with
 score = softmax(last-position logits / temperature)[first answer token]. The reference loops over samples and calls
 `generate(max_new_tokens=1)`; here the whole batch is ONE prefill in libvqa_b200.so and identical images are encoded once.
+With `max_new_tokens = k > 1`, `forward` and `forward_with_trace` score the answer tokens on a greedy rollout of k tokens, as the
+reference does with one `generate(max_new_tokens=k, output_scores=True)` per sample (qwen2vl_model.py:239-289, :381-487): here the
+pairs run as batched rollouts on the GPU decode loop, with the answer probabilities of every step computed on the device.
 Video inputs (decord / qwen_vl_utils frame sampling) are outside this engine's scope and raise.
 """
 from __future__ import annotations
@@ -29,6 +32,15 @@ QWEN_VL_UTILS_MIN_PIXELS = 4 * 28 * 28
 QWEN_VL_UTILS_MAX_PIXELS = 16384 * 28 * 28
 
 
+def _require_rollout_engine(plugin) -> None:
+    """max_new_tokens > 1 is scored on a greedy rollout, which only the device engine's scored decode loop (QwenVLEngine.rollout_scores)
+    runs. A plugin without such an engine (none loaded, or an engine object without scored rollouts) refuses before any image is read or
+    any kernel launched."""
+    if not callable(getattr(getattr(plugin, "engine", None), "rollout_scores", None)):
+        raise NotImplementedError("max_new_tokens > 1 needs an engine with scored greedy rollouts (QwenVLEngine.rollout_scores), and this "
+                                  "plugin has none; without it only the single-prefill scoring of max_new_tokens=1 exists")
+
+
 def _generation_config_penalty(checkpoint_path: str) -> float:
     """repetition_penalty of the generation_config.json stored beside the checkpoint (what `from_pretrained` would attach to
     `model.generation_config` in the reference, qwen2vl_model.py:116-130); 1.0 when there is none."""
@@ -40,6 +52,11 @@ class Qwen2VLModel(VQAScoreModel):
     video_mode = "direct"
     allows_image = True
     supports_trace = True
+    # Scoring with max_new_tokens > 1 runs batched rollouts of at most this many pairs, halved until one chunk's generation workspace
+    # (prefill activations of the padded prompts + K/V cache of prompt and rollout, vqa_qwen25vl_generate_workspace_bytes) fits the
+    # budget: large `max_pixels` images make prompts of thousands of tokens.
+    ROLLOUT_MAX_PAIRS = 32
+    ROLLOUT_WORKSPACE_BUDGET = 8 << 30
 
     def __init__(self, model_name="qwen2.5-vl-7b", device="cuda", cache_dir=HF_CACHE_DIR, tokenizer=None,
                  state_dict: Optional[Dict[str, torch.Tensor]] = None, config: Optional[Qwen25VLConfig] = None,
@@ -111,6 +128,10 @@ class Qwen2VLModel(VQAScoreModel):
         `score_position` "start" and "end" coincide. The alternatives come from a top-k pass over the last position's logits
         (engine.topk_last) under the same temperature / repetition penalty as the score."""
         assert score_position in ("start", "end"), f"score_position must be 'start' or 'end', got '{score_position}'"
+        if max_new_tokens != 1:
+            _require_rollout_engine(self)
+            return self._trace_rollout(images, texts, question_template, answer_template, max_new_tokens, temperature, score_position, debug,
+                                       repetition_penalty)
         probs = self.forward(images, texts, fps=fps, question_template=question_template, answer_template=answer_template,
                              max_new_tokens=max_new_tokens, temperature=temperature, debug=False, repetition_penalty=repetition_penalty)
         pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
@@ -143,6 +164,89 @@ class Qwen2VLModel(VQAScoreModel):
         if eos is None:
             return []
         return [int(e) for e in eos] if isinstance(eos, (list, tuple)) else [int(eos)]
+
+    def _rollout(self, images: List[str], texts: List[str], question_template: str, answer_template: str, max_new_tokens: int,
+                 temperature: float, repetition_penalty: float, mode: str, top_k: int) -> List[dict]:
+        """Scored greedy rollouts of max_new_tokens for every (image, text) pair: the scoring prompt, generate(do_sample=False) under the
+        repetition penalty and the EOS ids of generation, and per step the log-probability of every answer token
+        (engine.rollout_scores), then the reference's step selection (qwen_host.rollout_answer_score, `mode` "forward", "start" or "end").
+        Identical images are encoded once per chunk; a chunk holds at most ROLLOUT_MAX_PAIRS pairs and fewer when its generation workspace
+        would exceed ROLLOUT_WORKSPACE_BUDGET. Returns one rollout_answer_score dict per pair, with `tokens`, `answer_ids` and, with
+        top_k > 0, the per-step `topk_ids` / `topk_probs` [max_new_tokens, top_k] added."""
+        from ... import qwen_host
+        if max_new_tokens < 1:
+            raise ValueError("max_new_tokens must be at least 1")
+        questions = [question_template.format(t) for t in texts]
+        answers = [answer_template.format(t) for t in texts]
+        uniq: Dict[str, int] = {}
+        index = [uniq.setdefault(p, len(uniq)) for p in images]
+        patches, grids = self.load_images(list(uniq.keys()))
+        unit = self.cfg.spatial_merge_size ** 2
+        cache = self.__dict__.setdefault("_prompt_cache", {})
+        if len(cache) > 65536:
+            cache.clear()
+        prompts, answer_ids = [], []
+        for q, a, img in zip(questions, answers, index):
+            t, gh, gw = grids[img]
+            prompts.append(build_prompt_ids(self.tokenizer, q, t * gh * gw // unit, self.cfg.image_token_id, cache))
+            ids = cache.get(("answer", a))
+            if ids is None:
+                ids = cache[("answer", a)] = tuple(self.tokenizer.encode(a, add_special_tokens=False))
+            if not ids:
+                raise ValueError("empty answer")
+            answer_ids.append(list(ids))
+        eos = self._eos_ids()
+        special = {getattr(self.tokenizer, n, None) for n in ("eos_token_id", "bos_token_id", "pad_token_id")} - {None}
+        sizes = [t * h * w for t, h, w in grids]
+        offs = [0]
+        for s in sizes:
+            offs.append(offs[-1] + s)
+        chunk = min(self.ROLLOUT_MAX_PAIRS, len(prompts))
+        seq_len = max(len(p) for p in prompts)
+        while chunk > 1 and self.engine.generate_workspace_bytes(chunk, seq_len, min(offs[-1], chunk * max(sizes)),
+                                                                 max_new_tokens) > self.ROLLOUT_WORKSPACE_BUDGET:
+            chunk = (chunk + 1) // 2
+        results = []
+        for c0 in range(0, len(prompts), chunk):
+            sel = list(range(c0, min(len(prompts), c0 + chunk)))
+            imgs = sorted({index[i] for i in sel})
+            local = {g: j for j, g in enumerate(imgs)}
+            pix = patches if len(imgs) == len(grids) else torch.cat([patches[offs[g]:offs[g + 1]] for g in imgs])
+            out = self.engine.rollout_scores(pix, [grids[g] for g in imgs], [prompts[i] for i in sel], [answer_ids[i] for i in sel],
+                                             max_new_tokens, eos, temperature=temperature, repetition_penalty=repetition_penalty,
+                                             top_k=top_k, image_of_sample=[local[index[i]] for i in sel])
+            for b, i in enumerate(sel):
+                r = qwen_host.rollout_answer_score(out["tokens"][b], out["logp"][b], answer_ids[i], special, mode)
+                r.update(tokens=out["tokens"][b], answer_ids=answer_ids[i])
+                if top_k > 0:
+                    r.update(topk_ids=out["topk_ids"][b], topk_probs=out["topk_probs"][b])
+                results.append(r)
+        return results
+
+    def _trace_rollout(self, images, texts, question_template, answer_template, max_new_tokens, temperature, score_position, debug,
+                       repetition_penalty):
+        """forward_with_trace for max_new_tokens > 1 (reference qwen2vl_model.py:381-487): scored rollouts, answer tokens placed at the
+        start or the end of the generation, and the reference's trace dictionary per sample."""
+        pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
+        results = self._rollout(images, texts, question_template, answer_template, max_new_tokens, temperature, pen, score_position, 5)
+        one = lambda t: self.tokenizer.decode([int(t)])
+        traces = []
+        for b, r in enumerate(results):
+            toks, start, n = r["tokens"], r["start"], r["n"]
+            details = []
+            for i, s in enumerate(r["steps"]):
+                alts = [dict(token_id=int(t), token_text=one(t), probability=float(p))
+                        for t, p in zip(r["topk_ids"][s].tolist(), r["topk_probs"][s].tolist())]
+                details.append(dict(position=s, expected_token_id=r["answer_ids"][i], expected_token_text=one(r["answer_ids"][i]),
+                                    probability=r["probs"][i], top_alternatives=alts))
+            traces.append(dict(generated_text=self.tokenizer.decode(toks, skip_special_tokens=True), generated_length=len(toks),
+                               score_position=score_position, score_start_idx=start, scored_indices=list(r["steps"]),
+                               scored_tokens_text=self.tokenizer.decode(toks[start:start + n], skip_special_tokens=True),
+                               probability=r["score"], token_details=details))
+            if debug:
+                print(f"sample {b}: generated {traces[-1]['generated_text']!r} ({len(toks)} tokens); scored steps {r['steps']}; "
+                      f"probabilities {[round(p, 6) for p in r['probs']]}; geometric mean {r['score']:.6f}")
+        return torch.tensor([r["score"] for r in results], dtype=torch.float32), traces
 
     @torch.no_grad()
     def generate(self, images: List[str], texts: List[str], fps=None, max_new_tokens: int = 2048, temperature: float = 0.0,
@@ -178,9 +282,12 @@ class Qwen2VLModel(VQAScoreModel):
                 debug: bool = False, repetition_penalty: Optional[float] = None) -> torch.Tensor:
         assert len(images) == len(texts), "Number of images/videos and texts must match"
         if max_new_tokens != 1:
-            # With max_new_tokens = k > 1 the reference scores answer token i on the logits of generation step len(scores) - n + i, i.e.
-            # conditioned on its own GREEDY continuation (qwen2vl_model.py:259-289) -- a decode loop, not the single prefill this engine runs.
-            raise NotImplementedError("the engine scores the first generated position only (max_new_tokens=1, the reference default)")
+            # the reference scores answer token i on the scores of step len(scores) - n + i (- 1 after a trailing special token) of its own
+            # greedy continuation (qwen2vl_model.py:239-289): a scored rollout on the decode loop
+            _require_rollout_engine(self)
+            pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
+            return torch.tensor([r["score"] for r in self._rollout(images, texts, question_template, answer_template, max_new_tokens,
+                                                                    temperature, pen, "forward", 0)], dtype=torch.float32)
         questions = [question_template.format(t) for t in texts]
         answers = [answer_template.format(t) for t in texts]
         uniq: Dict[str, int] = {}

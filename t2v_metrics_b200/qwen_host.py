@@ -149,6 +149,45 @@ def first_generated_positions(idx) -> torch.Tensor:
     return (last[0] + 1).to(torch.int32)
 
 
+def rollout_answer_score(tokens: Sequence[int], logp: torch.Tensor, answer_ids: Sequence[int], special_ids, mode: str = "forward") -> dict:
+    """Which steps of a greedy rollout score which answer tokens, and the score: the reference's rule (qwen2vl_model.py), restated.
+    tokens: the L generated ids of one sample (a stopping EOS included); logp: fp32 [>= L, >= len(answer_ids)], logp[s, j] = log p(s,
+    answer_ids[j]) (engine.rollout_scores); special_ids: the tokenizer's {eos, bos, pad} ids (not the stop list); mode: "forward"
+    (Qwen2VLModel.forward, :239-289), "start" or "end" (forward_with_trace's score_position, :381-416).
+      * forward: a last token in special_ids sets offset 1 and n = min(n, L - 1) (n <= 0 raises); then n = min(n, L); answer token i is
+        scored at step L - n + i - offset.
+      * end: the same special-token rule; start = max(0, L - n - offset); n = min(n, L - start); n <= 0 raises.
+      * start: start = 0, n = min(n, L).
+    p_i = exp(logp) in fp32; score = (prod_i p_i) ** (1 / n) over Python floats. Returns dict(score, start, steps, n, probs). No device work."""
+    L, n = len(tokens), len(answer_ids)
+    if L < 1 or n < 1:
+        raise ValueError("a rollout of at least one token and a non-empty answer are needed")
+    offset = 0
+    if mode in ("forward", "end") and int(tokens[-1]) in special_ids:
+        offset, n = 1, min(n, L - 1)                                       # :247-257, :392-400
+        if n <= 0 and mode == "forward":
+            raise ValueError("No content tokens to score after removing special tokens")
+    if mode == "forward":
+        n = min(n, L)                                                      # :259-263
+        start = L - n - offset                                             # :267 position -(n - i + offset)
+    elif mode == "end":
+        start = max(0, L - n - offset)                                     # :403-406
+        n = min(n, L - start)                                              # :408-413
+    elif mode == "start":
+        start = 0                                                          # :382-384
+        n = min(n, L - start)
+    else:
+        raise ValueError(f"mode must be 'forward', 'start' or 'end', got {mode!r}")
+    if n <= 0:
+        raise ValueError("No tokens available to score at the specified position")      # :415-416
+    steps = list(range(start, start + n))
+    probs = [float(torch.exp(logp[s, i].float())) for i, s in enumerate(steps)]
+    joint = 1.0
+    for p in probs:
+        joint *= p
+    return dict(score=joint ** (1.0 / n), start=start, steps=steps, n=n, probs=probs)
+
+
 def build_packed_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequence[int]], image_of_sample: Sequence[int],
                          image_token_id: int, merge: int, tokens_per_second: int, video_token_id: Optional[int] = None,
                          second_per_grid_ts: Optional[Sequence[float]] = None):
