@@ -350,7 +350,9 @@ int32_t vqa_resample_table(int32_t in_size, int32_t out_size, int32_t first, int
 /* ---- kernel-level entry points (used by tests/ and bench.py to exercise single kernels through the same ABI) ---- */
 
 /* C[M,N] = epilogue(A[M,K] . W[N,K]^T); all DEVICE bf16 row-major. epilogue: 0 store, 1 quick_gelu, 2 gelu(erf),
- * 3 gated gelu_new (W = [gate; up] with `gate_up_offset` rows between them, C is [M, N/2]), 5 relu.
+ * 3 gated gelu_new, 5 relu, 6 gated silu (C = bf16(bf16(silu(bf16(gate + b_gate))) * bf16(up + b_up)), the Qwen2.5-VL MLPs). The gated
+ * epilogues 3 and 6 read W = [gate; up] with the up block `gate_up_offset` rows below the gate block (gate_up_offset + N/2 <= w_rows;
+ * the bias is laid out the same way) and write C [M, N/2]; N/2 must be a multiple of 8.
  * bias [N] / residual [M, ldr] may be NULL. variant: 0 auto, else (BLOCK_N * 10 + rows / 128): 2561, 1281, 641, 321 are 128-row tiles
  * with BLOCK_N = 256 / 128 / 64 / 32. The two-CTA codes 2562 and 1282 of earlier hardware are still accepted and are aliases of 2561 and
  * 1281 (sm_90a has no CTA-pair MMA). Any other value is rejected. */
@@ -378,6 +380,48 @@ int vqa_op_lmhead_logprob(const void* H, int32_t ldh, const void* W, int32_t ldw
 int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t V, const uint32_t* pen_bitmap, float repetition_penalty, float temperature,
                           const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, int32_t max_new, const int32_t* lengths,
                           const int32_t* done, int32_t top_k, float* out_logp, int32_t* out_topk_ids, float* out_topk_probs, void* stream);
+
+/* The Qwen2.5-VL K/V cache write: the K and V heads (kv_heads x 128 columns at k_col0 / v_col0) of the packed rows qkv [B * S, ld] go to
+ * kc / vc [B, kv_heads, cap, 128]. gen_len == NULL (prefill): row s of sequence b goes to slot s when s < seq_lens[b], padded rows are not
+ * written (S <= cap). gen_len given (decode, S == 1): the row of sequence b goes to slot seq_lens[b] + gen_len[b] - 1. All DEVICE; ld,
+ * k_col0, v_col0 multiples of 8, pointers 16-byte aligned. */
+int vqa_op_kv_cache_write(const void* qkv, int32_t ld, int32_t k_col0, int32_t v_col0, int32_t kv_heads, int32_t B, int32_t S,
+                          const int32_t* seq_lens, const int32_t* gen_len, void* kc, void* vc, int32_t cap, void* stream);
+
+/* The decode-step attention of vqa_qwen25vl_generate_step (head_dim 128, flash-decoding): query row b (q heads at q + b * ldq + h * 128)
+ * attends to cache slots [0, seq_lens[b] + gen_len[b]) of kc / vc [B, kv_heads, cap, 128], KV head h / (q_heads / kv_heads);
+ * out[b * ldo + h * 128 + d] bf16. q_heads / kv_heads in {1, 2, 4, 5, 7, 8} (else VQA_ERR_UNSUPPORTED). The keys are cut into `splits`
+ * ranges of ceil(cap / splits) slots (splits == 0: the generation's rule, returned in *splits_out; splits <= cap), merged by a second kernel;
+ * workspace DEVICE >= B * q_heads * splits * 130 floats. ldq / ldo multiples of 4, q and caches 8-byte aligned. */
+int vqa_op_decode_attention_d128(const void* q, int32_t ldq, const void* kc, const void* vc, int32_t cap, const int32_t* seq_lens,
+                                 const int32_t* gen_len, int32_t B, int32_t q_heads, int32_t kv_heads, float scale, int32_t splits,
+                                 void* workspace, size_t workspace_bytes, int32_t* splits_out, void* out, int32_t ldo, void* stream);
+
+/* The token selection of the greedy generations on caller-owned state (all DEVICE): for every b with done[b] == 0, the arg-max (ties to the
+ * lowest id) of the bf16 logits [B, V] cast to fp32, under HF's repetition penalty on the ids set in pen_bitmap [B, ceil(V / 32)] (NULL = no
+ * penalty); the token goes to tokens[b, lengths[b]] and next_ids[b], its bit is set, lengths[b] advances, and with first_pos [B] / pos3 [3, B]
+ * (both NULL or both given) pos3[:, b] = first_pos[b] + index of the token. A sequence finishes on one of eos_ids [n_eos] or at max_new
+ * tokens: done[b] = 1, ++n_done, and the one that finishes the last of the B raises *all_done. */
+int vqa_op_greedy_select(const void* logits, int32_t B, int32_t V, uint32_t* pen_bitmap, float repetition_penalty, const int32_t* eos_ids,
+                         int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
+                         int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, void* stream);
+
+/* Host-only (no GPU needed): T5's relative-position buckets (T5Attention._relative_position_bucket) of rel = -max_distance .. max_distance,
+ * out[rel + max_distance], HOST int32 [2 * max_distance + 1] -- the table vqa_create_clipt5 builds for the encoder (bidirectional = 1) and
+ * the decoder (0). */
+int vqa_t5_bucket_lut(int32_t bidirectional, int32_t num_buckets, int32_t max_distance, int32_t* out);
+
+/* The CLIP-FlanT5 scoring path's decoder self-attention (head_dim 64, causal, unidirectional buckets, no scale) over T <= 256 target rows:
+ * packed qkv [B * T, 3 * H * 64] -> out [B * T, H * 64]. rel_emb [num_buckets, H] bf16, bucket_lut DEVICE int32 [2 * max_distance + 1]
+ * (vqa_t5_bucket_lut). round_scores != 0: bf16 scores before and after the bias add, as the reference's eager attention forms them. */
+int vqa_op_t5_decoder_self_attn(const void* qkv, void* out, const void* rel_emb, const int32_t* bucket_lut, int32_t max_distance, int32_t B,
+                                int32_t T, int32_t H, int32_t round_scores, void* stream);
+
+/* One cached decoder self-attention layer of vqa_clipt5_generate_step: the step's row qkv [B, 3 * H * 64] of sequence b sits at position
+ * t = min(lengths[b], cap - 1); its K / V go to slot t of kc / vc [B, H, cap, 64] (cap <= 2048), then it attends to slots 0..t.
+ * out [B, H * 64]; rel_emb / bucket_lut / round_scores as vqa_op_t5_decoder_self_attn. qkv and caches 16-byte aligned. */
+int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, int32_t cap, const int32_t* lengths, void* out, const void* rel_emb,
+                               const int32_t* bucket_lut, int32_t max_distance, int32_t B, int32_t H, int32_t round_scores, void* stream);
 
 /* Bidirectional attention, head_dim 64, packed qkv [B*S, 3*H*64] -> out [B*S, H*64].
  * bias_table: DEVICE float [H, 2S-1] (index key - query + S - 1) or NULL; seq_lens DEVICE int32 [B] or NULL.

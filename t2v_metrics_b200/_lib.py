@@ -24,6 +24,8 @@ ABI_SYMBOLS = [
     "vqa_qwen25vl_generate_workspace_bytes", "vqa_qwen25vl_generate_prefill", "vqa_qwen25vl_generate_step",
     "vqa_clipt5_generate_workspace_bytes", "vqa_clipt5_generate_prefill", "vqa_clipt5_generate_step",
     "vqa_qwen25vl_rollout_prefill", "vqa_qwen25vl_rollout_step", "vqa_op_answer_logprob",
+    "vqa_op_kv_cache_write", "vqa_op_decode_attention_d128", "vqa_op_greedy_select", "vqa_t5_bucket_lut", "vqa_op_t5_decoder_self_attn",
+    "vqa_op_t5_decode_self_attn",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -137,6 +139,19 @@ def load() -> C.CDLL:
     lib.vqa_qwen25vl_rollout_step.restype = C.c_int
     lib.vqa_op_answer_logprob.argtypes = [vp, i32, i32, vp, f32, f32, vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, vp]
     lib.vqa_op_answer_logprob.restype = C.c_int
+    lib.vqa_op_kv_cache_write.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, i32, vp]
+    lib.vqa_op_kv_cache_write.restype = C.c_int
+    lib.vqa_op_decode_attention_d128.argtypes = [vp, i32, vp, vp, i32, vp, vp, i32, i32, i32, f32, i32, vp, C.c_size_t, C.POINTER(i32), vp,
+                                                 i32, vp]
+    lib.vqa_op_decode_attention_d128.restype = C.c_int
+    lib.vqa_op_greedy_select.argtypes = [vp, i32, i32, vp, f32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.vqa_op_greedy_select.restype = C.c_int
+    lib.vqa_t5_bucket_lut.argtypes = [i32, i32, i32, C.POINTER(i32)]
+    lib.vqa_t5_bucket_lut.restype = C.c_int
+    lib.vqa_op_t5_decoder_self_attn.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    lib.vqa_op_t5_decoder_self_attn.restype = C.c_int
+    lib.vqa_op_t5_decode_self_attn.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.vqa_op_t5_decode_self_attn.restype = C.c_int
     lib.vqa_clipt5_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
     lib.vqa_clipt5_generate_workspace_bytes.restype = C.c_size_t
     lib.vqa_clipt5_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]

@@ -333,15 +333,23 @@ struct QwenGenWorkspace {
     int cap, splits, chunk;
     size_t layer_elems;
 };
+
+// Key splits of decode_attn_partial_kernel over a cache of `cap` slots: enough for two CTAs per SM (at B = 1 the 4 KV heads alone would
+// occupy 4 of 132 SMs), at least 16 keys each. Fixed by the capacity, not the live lengths, so a step's launch shapes never change.
+static int decode_attn_splits(int B, int kv_heads, int cap, int num_sms) {
+    return std::max(1, std::min((2 * num_sms + B * kv_heads - 1) / (B * kv_heads), (cap + 15) / 16));
+}
+
+// the group sizes (q heads per KV head) launch_decode_attn instantiates
+static bool decode_attn_group_supported(int G) { return G == 1 || G == 2 || G == 4 || G == 5 || G == 7 || G == 8; }
+
 static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S, int n_patches, int max_new, int num_sms) {
     QwenGenWorkspace g;
     g.w = qwen_plan(c, B, S, n_patches);
     Plan pl;
     pl.off = g.w.total;
     g.cap = S + max_new;
-    // flash-decoding: enough key splits for two CTAs per SM (at B = 1 the 4 KV heads alone would occupy 4 of 132 SMs), at least 16 keys each.
-    // Fixed by the capacity, not the live lengths, so a step's launch shapes never change.
-    g.splits = std::max(1, std::min((2 * num_sms + B * c.kv_heads - 1) / (B * c.kv_heads), (g.cap + 15) / 16));
+    g.splits = decode_attn_splits(B, c.kv_heads, g.cap, num_sms);
     g.chunk = (g.cap + g.splits - 1) / g.splits;
     g.layer_elems = (size_t)B * c.kv_heads * g.cap * 128;
     g.kcache = pl.take((size_t)c.layers * g.layer_elems * 2);

@@ -28,6 +28,16 @@ static int host_rel_bucket(int rel, bool bidirectional, int num_buckets, int max
     return bucket + large;
 }
 
+// Host-only: the bucket of every clamped relative position rel in [-max_distance, max_distance], out[rel + max_distance] -- the table
+// the attention kernels index (buckets saturate at |rel| = max_distance, so the clamp loses nothing).
+extern "C" int vqa_t5_bucket_lut(int32_t bidirectional, int32_t num_buckets, int32_t max_distance, int32_t* out) {
+    const int max_exact = bidirectional ? num_buckets / 4 : num_buckets / 2;
+    if (!out || num_buckets < 4 || max_distance <= max_exact || max_distance > (1 << 20))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "bad bucket table request (num_buckets >= 4, exact range < max_distance <= 2^20)");
+    for (int r = -max_distance; r <= max_distance; ++r) out[r + max_distance] = host_rel_bucket(r, bidirectional != 0, num_buckets, max_distance);
+    return VQA_OK;
+}
+
 extern "C" int vqa_create_clipt5(const vqa_clipt5_config* cfg, int device, vqa_handle** out) {
     if (!cfg || !out) return fail(nullptr, VQA_ERR_INVALID_ARG, "null argument");
     if (cfg->vit_hidden % cfg->vit_heads || cfg->vit_hidden / cfg->vit_heads != 64)
@@ -56,9 +66,9 @@ extern "C" int vqa_create_clipt5(const vqa_clipt5_config* cfg, int device, vqa_h
     // bucket LUTs
     const int md = cfg->rel_max_distance;
     std::vector<int> lb(2 * md + 1), lu(2 * md + 1);
-    for (int r = -md; r <= md; ++r) {
-        lb[r + md] = host_rel_bucket(r, true, cfg->rel_buckets, md);
-        lu[r + md] = host_rel_bucket(r, false, cfg->rel_buckets, md);
+    if (vqa_t5_bucket_lut(1, cfg->rel_buckets, md, lb.data()) != VQA_OK || vqa_t5_bucket_lut(0, cfg->rel_buckets, md, lu.data()) != VQA_OK) {
+        delete h;
+        return VQA_ERR_INVALID_ARG;
     }
     if (cudaMalloc(&h->lut_bidir, lb.size() * 4) != cudaSuccess || cudaMalloc(&h->lut_unidir, lu.size() * 4) != cudaSuccess ||
         cudaMemcpy(h->lut_bidir, lb.data(), lb.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
@@ -386,8 +396,7 @@ static int qwen_gen_check(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t
         return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
     if (batch <= 0 || batch > 128 || seq_len <= 0 || n_patches <= 0 || a.max_new <= 0 || a.n_eos < 0 || !(a.repetition_penalty > 0.f))
         return fail(h, VQA_ERR_INVALID_ARG, "bad size / repetition penalty (1 <= batch <= 128, max_new_tokens >= 1)");
-    const int G = h->qwen->cfg.heads / h->qwen->cfg.kv_heads;
-    if (G != 1 && G != 2 && G != 4 && G != 5 && G != 7 && G != 8)
+    if (!decode_attn_group_supported(h->qwen->cfg.heads / h->qwen->cfg.kv_heads))
         return fail(h, VQA_ERR_UNSUPPORTED, "decode attention supports 1, 2, 4, 5, 7 or 8 query heads per KV head");
     if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
     return VQA_OK;
@@ -499,11 +508,21 @@ static Gemm abi_gemm(const void* A, int lda, const void* W, int ldw, int w_rows,
     return g;
 }
 
+// A gated epilogue stores its N / 2 output columns 8 at a time and reads the up block `gate_up_offset` rows below the gate block.
+static int check_gated(int epilogue, int N, int w_rows, int gate_up_offset) {
+    if (!epi_is_gated(epilogue)) return VQA_OK;
+    if ((N / 2) % 8) return fail(nullptr, VQA_ERR_INVALID_ARG, "gated gemm: N / 2 must be a multiple of 8");
+    if (gate_up_offset < 0 || (long long)gate_up_offset + N / 2 > w_rows)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "gated gemm: the up block [gate_up_offset, gate_up_offset + N / 2) must lie inside w_rows");
+    return VQA_OK;
+}
+
 extern "C" int vqa_op_gemm_bf16(const void* A, int32_t lda, const void* W, int32_t ldw, int32_t w_rows, void* C,
                                 int32_t ldc, int32_t M, int32_t N, int32_t K, const void* bias, const void* residual,
                                 int32_t ldr, int32_t epilogue, int32_t gate_up_offset, int32_t variant, void* stream) {
     if (!A || !W || !C || M <= 0 || N <= 0 || K <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad gemm argument");
     if (lda % 8 || ldw % 8 || ldc % 8 || N % 8 || K % 8) return fail(nullptr, VQA_ERR_INVALID_ARG, "gemm: ld/N/K must be multiples of 8");
+    if (int rc = check_gated(epilogue, N, w_rows, gate_up_offset)) return rc;
     Gemm g = abi_gemm(A, lda, W, ldw, w_rows, C, ldc, M, N, K);
     g.bias = (const bf16*)bias; g.residual = residual; g.ldr = ldr; g.epi = epilogue; g.gate_up_offset = gate_up_offset; g.variant = variant;
     return cuda_status(nullptr, run_gemm(g, device_sms(), (cudaStream_t)stream), "gemm launch");
@@ -546,6 +565,7 @@ extern "C" int vqa_op_gemm_bf16_normfuse(const void* A, int32_t lda, const void*
     if (!A || !W || !C || M <= 0 || N <= 0 || K <= 0 || stride <= 0 || stride % 4 || norm_dim <= 0)
         return fail(nullptr, VQA_ERR_INVALID_ARG, "bad gemm argument");
     if (lda % 8 || ldw % 8 || ldc % 8 || N % 8 || K % 8) return fail(nullptr, VQA_ERR_INVALID_ARG, "gemm: ld/N/K must be multiples of 8");
+    if (int rc = check_gated(epilogue, N, w_rows, gate_up_offset)) return rc;
     const int variant = pick_variant(M, N, epilogue);
     const int parts = ssq_parts_for(variant, epi_is_gated(epilogue) ? N / 2 : N);
     if (parts_out) *parts_out = parts;
@@ -583,6 +603,107 @@ extern "C" int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t 
         (const bf16*)logits, V, pen_bitmap, (V + 31) / 32, repetition_penalty, 1.0f / temperature, answer_ids, answer_counts, n_max, max_new,
         lengths, done, top_k, out_logp, out_topk_ids, out_topk_probs);
     return cuda_status(nullptr, cudaGetLastError(), "answer logprob launch");
+}
+
+static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// kv_cache_write_kernel: the 16-byte chunks of the K and V heads of every row go to their cache slot.
+extern "C" int vqa_op_kv_cache_write(const void* qkv, int32_t ld, int32_t k_col0, int32_t v_col0, int32_t kv_heads, int32_t B, int32_t S,
+                                     const int32_t* seq_lens, const int32_t* gen_len, void* kc, void* vc, int32_t cap, void* stream) {
+    if (!qkv || !seq_lens || !kc || !vc) return fail(nullptr, VQA_ERR_INVALID_ARG, "kv cache write: null pointer");
+    if (kv_heads <= 0 || B <= 0 || S <= 0 || cap <= 0 || S > cap || (gen_len && S != 1) || k_col0 < 0 || v_col0 < 0 ||
+        ld < std::max(k_col0, v_col0) + kv_heads * 128)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "kv cache write: bad size (S <= cap, S == 1 in decode mode, heads inside ld)");
+    if (ld % 8 || k_col0 % 8 || v_col0 % 8 || !aligned(qkv, 16) || !aligned(kc, 16) || !aligned(vc, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "kv cache write: ld, column offsets and pointers must be 16-byte aligned");
+    const long long rows = (long long)B * S;
+    kv_cache_write_kernel<<<(unsigned)((rows * kv_heads * 16 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        (const bf16*)qkv, ld, k_col0, v_col0, kv_heads, S, rows, seq_lens, gen_len, (bf16*)kc, (bf16*)vc, cap);
+    return cuda_status(nullptr, cudaGetLastError(), "kv cache write launch");
+}
+
+// decode_attn_partial_kernel over `splits` key ranges of the cache, then decode_attn_merge_kernel; the fp32 partials live in `workspace`.
+extern "C" int vqa_op_decode_attention_d128(const void* q, int32_t ldq, const void* kc, const void* vc, int32_t cap, const int32_t* seq_lens,
+                                            const int32_t* gen_len, int32_t B, int32_t q_heads, int32_t kv_heads, float scale, int32_t splits,
+                                            void* workspace, size_t workspace_bytes, int32_t* splits_out, void* out, int32_t ldo, void* stream) {
+    if (!q || !kc || !vc || !seq_lens || !gen_len || !out) return fail(nullptr, VQA_ERR_INVALID_ARG, "decode attention: null pointer");
+    if (B <= 0 || q_heads <= 0 || kv_heads <= 0 || cap <= 0 || splits < 0 || q_heads % kv_heads)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "decode attention: bad size (q_heads a multiple of kv_heads)");
+    const int G = q_heads / kv_heads;
+    if (!decode_attn_group_supported(G))
+        return fail(nullptr, VQA_ERR_UNSUPPORTED, "decode attention supports 1, 2, 4, 5, 7 or 8 query heads per KV head");
+    if (ldq < q_heads * 128 || ldo < q_heads * 128 || ldq % 4 || ldo % 4 || !aligned(q, 8) || !aligned(kc, 8) || !aligned(vc, 8) ||
+        !aligned(out, 2))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "decode attention: ldq / ldo must cover the q heads and be multiples of 4, q / caches 8-byte aligned");
+    if (splits == 0) splits = decode_attn_splits(B, kv_heads, cap, device_sms());
+    if (splits_out) *splits_out = splits;
+    if (splits > cap) return fail(nullptr, VQA_ERR_INVALID_ARG, "decode attention: more splits than cache slots");
+    const size_t rows = (size_t)B * q_heads * splits;
+    if (!workspace || !aligned(workspace, 4) || workspace_bytes < rows * 130 * 4)
+        return fail(nullptr, VQA_ERR_WORKSPACE, "decode attention: workspace smaller than B * q_heads * splits * 130 floats");
+    float* part_o = static_cast<float*>(workspace);
+    float* part_ml = part_o + rows * 128;
+    const int chunk = (cap + splits - 1) / splits;
+    cudaStream_t st = (cudaStream_t)stream;
+    cudaError_t e = launch_decode_attn(G, dim3(splits, kv_heads, B), st, (const bf16*)q, ldq, (const bf16*)kc, (const bf16*)vc, cap, seq_lens,
+                                       gen_len, kv_heads, chunk, scale, part_o, part_ml);
+    if (e == cudaSuccess) {
+        decode_attn_merge_kernel<<<B * q_heads, 128, 0, st>>>(part_o, part_ml, splits, (bf16*)out, ldo, q_heads);
+        e = cudaGetLastError();
+    }
+    return cuda_status(nullptr, e, "decode attention launch");
+}
+
+// greedy_select_kernel on caller-owned generation state.
+extern "C" int vqa_op_greedy_select(const void* logits, int32_t B, int32_t V, uint32_t* pen_bitmap, float repetition_penalty, const int32_t* eos_ids,
+                                    int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
+                                    int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, void* stream) {
+    if (!logits || !tokens || !lengths || !done || !n_done || !all_done || !next_ids || (n_eos > 0 && !eos_ids) || (!first_pos != !pos3))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "greedy select: null pointer (first_pos and pos3 are given together or not at all)");
+    if (B <= 0 || V <= 0 || max_new <= 0 || n_eos < 0 || !(repetition_penalty > 0.f))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "greedy select: bad size / repetition penalty");
+    greedy_select_kernel<<<B, SELECT_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, V, pen_bitmap, (V + 31) / 32, repetition_penalty,
+                                                                         eos_ids, n_eos, max_new, first_pos, B, tokens, lengths, done, n_done,
+                                                                         all_done, next_ids, pos3);
+    return cuda_status(nullptr, cudaGetLastError(), "greedy select launch");
+}
+
+static int check_t5_self_attn(const void* qkv, const void* out, const void* rel_emb, const int32_t* bucket_lut, int max_distance, int B, int H) {
+    if (!qkv || !out || !rel_emb || !bucket_lut) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 self attention: null pointer");
+    if (B <= 0 || H <= 0 || max_distance <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 self attention: bad size");
+    if (!aligned(qkv, 4) || !aligned(out, 4)) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 self attention: qkv / out must be 4-byte aligned");
+    return VQA_OK;
+}
+
+// t5_decoder_self_attn_kernel (the scoring path's decoder self-attention over T target rows), launched as vqa_clipt5_score does.
+extern "C" int vqa_op_t5_decoder_self_attn(const void* qkv, void* out, const void* rel_emb, const int32_t* bucket_lut, int32_t max_distance, int32_t B,
+                                           int32_t T, int32_t H, int32_t round_scores, void* stream) {
+    if (int rc = check_t5_self_attn(qkv, out, rel_emb, bucket_lut, max_distance, B, H)) return rc;
+    if (T <= 0 || T > 256) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 decoder self attention: 1 <= T <= 256");
+    t5_decoder_self_attn_kernel<<<(B * H * T + 3) / 4, 128, 4 * T * sizeof(float), (cudaStream_t)stream>>>(
+        (const bf16*)qkv, (bf16*)out, (const bf16*)rel_emb, bucket_lut, max_distance, B, T, H, round_scores);
+    return cuda_status(nullptr, cudaGetLastError(), "t5 decoder self attention launch");
+}
+
+// One cached decoder self-attention layer of a generation step: t5_kv_cache_append_kernel, then t5_decode_self_attn_kernel.
+extern "C" int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, int32_t cap, const int32_t* lengths, void* out, const void* rel_emb,
+                                          const int32_t* bucket_lut, int32_t max_distance, int32_t B, int32_t H, int32_t round_scores, void* stream) {
+    if (int rc = check_t5_self_attn(qkv, out, rel_emb, bucket_lut, max_distance, B, H)) return rc;
+    if (!kc || !vc || !lengths) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 decode self attention: null pointer");
+    if (cap <= 0 || cap > 2048) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 decode self attention: 1 <= cap <= 2048");
+    if (!aligned(qkv, 16) || !aligned(kc, 16) || !aligned(vc, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 decode self attention: qkv and caches must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    t5_kv_cache_append_kernel<<<(B * H * 8 + 255) / 256, 256, 0, st>>>((const bf16*)qkv, B, H, lengths, (bf16*)kc, (bf16*)vc, cap);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        t5_decode_self_attn_kernel<<<(B * H + T5_DEC_ATTN_WARPS - 1) / T5_DEC_ATTN_WARPS, 32 * T5_DEC_ATTN_WARPS,
+                                     T5_DEC_ATTN_WARPS * cap * sizeof(float), st>>>((const bf16*)qkv, (const bf16*)kc, (const bf16*)vc, cap, lengths,
+                                                                                    (bf16*)out, (const bf16*)rel_emb, bucket_lut, max_distance, B,
+                                                                                    H, round_scores);
+        e = cudaGetLastError();
+    }
+    return cuda_status(nullptr, e, "t5 decode self attention launch");
 }
 
 extern "C" int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32_t H, const int32_t* seq_lens,

@@ -388,7 +388,8 @@ class ClipT5Engine:
 class ops:
     """Kernel-level calls through the same C ABI (used by tests and bench.py's roofline probe)."""
 
-    EPI = dict(store=0, quick_gelu=1, gelu=2, gated_gelu=3, relu=5)
+    EPI = dict(store=0, quick_gelu=1, gelu=2, gated_gelu=3, relu=5, gated_silu=6)
+    GATED = (3, 6)          # W = [gate; up] `gate_up_offset` rows apart, C has N / 2 columns
 
     @staticmethod
     def gemm(a: torch.Tensor, w: torch.Tensor, bias=None, residual=None, epilogue="store", variant=0, out=None,
@@ -397,12 +398,13 @@ class ops:
         M, K = a.shape
         n_rows = w.shape[0]
         epi = ops.EPI[epilogue]
-        n_out = n_rows // 2 if epi == 3 else n_rows
+        gated = epi in ops.GATED
+        n_out = n_rows // 2 if gated else n_rows
         if out is None:
             out = torch.empty(M, n_out, dtype=torch.bfloat16, device=a.device)
         rc = lib.vqa_op_gemm_bf16(_ptr(a), a.stride(0), _ptr(w), w.stride(0), n_rows, _ptr(out), out.stride(0), M, n_rows,
                                   K, _ptr(bias), _ptr(residual), residual.stride(0) if residual is not None else 0, epi,
-                                  gate_up_offset if epi == 3 else 0, variant, _stream_ptr(a.device))
+                                  gate_up_offset if gated else 0, variant, _stream_ptr(a.device))
         _check(rc, None, "vqa_op_gemm_bf16")
         return out
 
@@ -415,14 +417,15 @@ class ops:
         M, K = a.shape
         n_rows = w.shape[0]
         epi = ops.EPI[epilogue]
-        n_out = n_rows // 2 if epi == 3 else n_rows
+        gated = epi in ops.GATED
+        n_out = n_rows // 2 if gated else n_rows
         if out is None:
             out = torch.empty(M, n_out, dtype=torch.bfloat16, device=a.device)
         buf = ssq_in if ssq_in is not None else ssq_out
         parts = C.c_int32(0)
         rc = lib.vqa_op_gemm_bf16_normfuse(_ptr(a), a.stride(0), _ptr(w), w.stride(0), n_rows, _ptr(out), out.stride(0), M, n_rows, K,
                                            _ptr(residual), residual.stride(0) if residual is not None else 0, epi,
-                                           gate_up_offset if epi == 3 else 0, _ptr(ssq_in), _ptr(ssq_out), buf.shape[1], norm_dim or K, float(eps),
+                                           gate_up_offset if gated else 0, _ptr(ssq_in), _ptr(ssq_out), buf.shape[1], norm_dim or K, float(eps),
                                            C.byref(parts), _stream_ptr(a.device))
         _check(rc, None, "vqa_op_gemm_bf16_normfuse")
         return out, int(parts.value)
@@ -473,6 +476,88 @@ class ops:
                                        _ptr(out_topk_probs), _stream_ptr(dev))
         _check(rc, None, "vqa_op_answer_logprob")
         return out_logp, out_topk_ids, out_topk_probs
+
+    @staticmethod
+    def kv_cache_write(qkv: torch.Tensor, k_col0: int, v_col0: int, kv_heads: int, S: int, seq_lens: torch.Tensor, kc: torch.Tensor,
+                       vc: torch.Tensor, gen_len=None):
+        """The Qwen2.5-VL K/V cache write on packed rows qkv [B * S, ld] into kc / vc [B, kv_heads, cap, 128] (in place). gen_len None:
+        prefill, row s < seq_lens[b] to slot s; gen_len int32 [B] (S == 1): decode, to slot seq_lens[b] + gen_len[b] - 1."""
+        lib = _lib.load()
+        B, cap = kc.shape[0], kc.shape[2]
+        rc = lib.vqa_op_kv_cache_write(_ptr(qkv), qkv.stride(0), k_col0, v_col0, kv_heads, B, S, _ptr(seq_lens), _ptr(gen_len), _ptr(kc), _ptr(vc),
+                                       cap, _stream_ptr(qkv.device))
+        _check(rc, None, "vqa_op_kv_cache_write")
+
+    @staticmethod
+    def decode_attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, seq_lens: torch.Tensor, gen_len: torch.Tensor, q_heads: int,
+                         scale: float, splits: int = 0, out=None):
+        """Flash-decoding attention of query rows q [B, >= q_heads * 128] (row stride q.stride(0)) over kc / vc [B, kv_heads, cap, 128],
+        sequence b over slots [0, seq_lens[b] + gen_len[b]). splits == 0: the generation's rule. Returns (out [B, q_heads * 128] or the given
+        out, splits used)."""
+        lib = _lib.load()
+        B, kv_heads, cap = kc.shape[0], kc.shape[1], kc.shape[2]
+        if out is None:
+            out = torch.empty(B, q_heads * 128, dtype=torch.bfloat16, device=q.device)
+        used = C.c_int32(0)
+        args = (_ptr(q), q.stride(0), _ptr(kc), _ptr(vc), cap, _ptr(seq_lens), _ptr(gen_len), B, q_heads, kv_heads, float(scale), splits)
+        if splits == 0:      # a call without workspace stops at the workspace check and returns the rule's split count
+            rc = lib.vqa_op_decode_attention_d128(*args, None, 0, C.byref(used), _ptr(out), out.stride(0), _stream_ptr(q.device))
+            if rc != -4:     # VQA_ERR_WORKSPACE is the expected answer; anything else is an argument error
+                _check(rc or -1, None, "vqa_op_decode_attention_d128")
+            splits = used.value
+        ws = torch.empty(max(1, B * q_heads * splits * 130), dtype=torch.float32, device=q.device)
+        rc = lib.vqa_op_decode_attention_d128(*args[:-1], splits, _ptr(ws), ws.numel() * 4, C.byref(used), _ptr(out), out.stride(0),
+                                              _stream_ptr(q.device))
+        _check(rc, None, "vqa_op_decode_attention_d128")
+        return out, int(used.value)
+
+    @staticmethod
+    def greedy_select(logits: torch.Tensor, tokens: torch.Tensor, lengths: torch.Tensor, done: torch.Tensor, n_done: torch.Tensor,
+                      all_done: torch.Tensor, next_ids: torch.Tensor, eos_ids=None, pen_bitmap=None, repetition_penalty: float = 1.0,
+                      first_pos=None, pos3=None):
+        """One greedy selection step on bf16 logits [B, V] and the caller's int32 state (in place): tokens [B, max_new], lengths / done /
+        next_ids [B], n_done / all_done [1], pen_bitmap [B, ceil(V / 32)] or None, first_pos [B] and pos3 [3, B] or both None."""
+        lib = _lib.load()
+        B, V = logits.shape
+        n_eos = eos_ids.numel() if eos_ids is not None else 0
+        rc = lib.vqa_op_greedy_select(_ptr(logits), B, V, _ptr(pen_bitmap), float(repetition_penalty), _ptr(eos_ids), n_eos, tokens.shape[1],
+                                      _ptr(first_pos), _ptr(tokens), _ptr(lengths), _ptr(done), _ptr(n_done), _ptr(all_done), _ptr(next_ids),
+                                      _ptr(pos3), _stream_ptr(logits.device))
+        _check(rc, None, "vqa_op_greedy_select")
+
+    @staticmethod
+    def t5_bucket_lut(bidirectional: bool, num_buckets: int, max_distance: int) -> torch.Tensor:
+        """The engine's relative-position bucket table (host): int32 [2 * max_distance + 1], entry rel + max_distance."""
+        lib = _lib.load()
+        out = torch.empty(2 * max_distance + 1, dtype=torch.int32)
+        rc = lib.vqa_t5_bucket_lut(1 if bidirectional else 0, num_buckets, max_distance, C.cast(out.data_ptr(), C.POINTER(C.c_int32)))
+        _check(rc, None, "vqa_t5_bucket_lut")
+        return out
+
+    @staticmethod
+    def t5_decoder_self_attn(qkv: torch.Tensor, B: int, T: int, H: int, rel_emb: torch.Tensor, bucket_lut: torch.Tensor, max_distance: int,
+                             round_scores: bool = False):
+        """The scoring path's T5 decoder self-attention: qkv [B * T, 3 * H * 64] -> [B * T, H * 64]; bucket_lut on the device."""
+        lib = _lib.load()
+        out = torch.empty(B * T, H * 64, dtype=torch.bfloat16, device=qkv.device)
+        rc = lib.vqa_op_t5_decoder_self_attn(_ptr(qkv), _ptr(out), _ptr(rel_emb), _ptr(bucket_lut), max_distance, B, T, H, 1 if round_scores else 0,
+                                             _stream_ptr(qkv.device))
+        _check(rc, None, "vqa_op_t5_decoder_self_attn")
+        return out
+
+    @staticmethod
+    def t5_decode_self_attn(qkv: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, lengths: torch.Tensor, rel_emb: torch.Tensor,
+                            bucket_lut: torch.Tensor, max_distance: int, round_scores: bool = False, out=None):
+        """One cached T5 decoder self-attention layer of a generation step: the row qkv [B, 3 * H * 64] of sequence b is appended to
+        kc / vc [B, H, cap, 64] at min(lengths[b], cap - 1) (in place) and attends to the slots up to it. Returns out [B, H * 64]."""
+        lib = _lib.load()
+        B, H, cap = kc.shape[0], kc.shape[1], kc.shape[2]
+        if out is None:
+            out = torch.empty(B, H * 64, dtype=torch.bfloat16, device=qkv.device)
+        rc = lib.vqa_op_t5_decode_self_attn(_ptr(qkv), _ptr(kc), _ptr(vc), cap, _ptr(lengths), _ptr(out), _ptr(rel_emb), _ptr(bucket_lut),
+                                            max_distance, B, H, 1 if round_scores else 0, _stream_ptr(qkv.device))
+        _check(rc, None, "vqa_op_t5_decode_self_attn")
+        return out
 
     @staticmethod
     def norm(x: torch.Tensor, gamma: torch.Tensor, beta=None, eps=1e-6):

@@ -16,9 +16,13 @@ def ops():
 
 def ref_gemm(a, w, bias=None, residual=None, epilogue="store", gate_off=0):
     acc = a.float() @ w.float().t()
-    if epilogue == "gated_gelu":
+    if epilogue in ("gated_gelu", "gated_silu"):
+        if bias is not None:            # [gate bias | up bias], gate_off apart like the weight rows
+            acc = acc + bias.float()
         g = acc[:, :gate_off].bfloat16().float()
         u = acc[:, gate_off:].bfloat16().float()
+        if epilogue == "gated_silu":    # Qwen2MLP: act_fn(gate_proj(x)) * up_proj(x), every op a bf16 tensor
+            return (torch.nn.functional.silu(g).bfloat16().float() * u).bfloat16()
         return (torch.nn.functional.gelu(g, approximate="tanh").bfloat16().float() * u).bfloat16()
     if bias is not None:
         acc = acc + bias.float()
@@ -58,7 +62,7 @@ def test_gemm_store_bias_residual(ops, variant, shape):
 
 
 @pytest.mark.parametrize("variant", [2562, 2561, 1281, 641, 0])
-@pytest.mark.parametrize("epi", ["quick_gelu", "gelu", "relu", "gated_gelu"])
+@pytest.mark.parametrize("epi", ["quick_gelu", "gelu", "relu", "gated_gelu", "gated_silu"])
 def test_gemm_fused_epilogues(ops, variant, epi):
     torch.manual_seed(2)
     M, N, K = 700, 1024, 512
@@ -67,6 +71,24 @@ def test_gemm_fused_epilogues(ops, variant, epi):
     bias = None if epi == "gated_gelu" else (torch.randn(N, device="cuda") * 0.1).bfloat16()
     c = ops.gemm(a, w, bias=bias, epilogue=epi, variant=variant, gate_up_offset=N // 2)
     close(c, ref_gemm(a, w, bias, None, epi, N // 2), epi)
+
+
+@pytest.mark.parametrize("with_bias", [False, True])
+@pytest.mark.parametrize("M", [1, 7, 128])
+def test_gemm_gated_silu_decode_rows(ops, M, with_bias):
+    """The gated-SiLU GEMM at decode-step row counts (M = B <= 128) with the padded vision-MLP width (2 x 3456, up block 3456 rows below
+    the gate block) and the tower's gate / up biases."""
+    torch.manual_seed(13)
+    N, K = 2 * 3456, 1280
+    a = torch.randn(M, K, device="cuda").bfloat16()
+    w = (torch.randn(N, K, device="cuda") * K ** -0.5).bfloat16()
+    bias = (torch.randn(N, device="cuda") * 0.5).bfloat16() if with_bias else None
+    c = ops.gemm(a, w, bias=bias, epilogue="gated_silu", gate_up_offset=N // 2)
+    assert c.shape == (M, N // 2)
+    ref = ref_gemm(a, w, bias, None, "gated_silu", N // 2)
+    close(c, ref, (M, with_bias))
+    if with_bias:       # the bias does move the result: a kernel that dropped it (or read the up bias at the gate offset) would fail
+        assert float((ref_gemm(a, w, None, None, "gated_silu", N // 2).float() - ref.float()).abs().max()) > 0.5
 
 
 @pytest.mark.parametrize("M,N,K,splits", [(128, 4096, 4096, 0), (2, 4096, 10240, 0), (100, 1024, 2048, 4), (7, 512, 4096, 8)])
