@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Kernel-level measurements through the C ABI (run on the GPU box).
 
-  python tools/bench_kernels.py attn            # head_dim-64 attention: T5 encoder shape and CLIP shape, CUDA-event timing
+  python tools/bench_kernels.py attn [--dump DIR]   # head_dim-64 attention: T5 encoder shape and CLIP shape, both rounding modes,
+                                                    # CUDA-event timing; --dump writes the outputs (raw bf16) to DIR
   python tools/bench_kernels.py gemm-time       # the four T5-encoder GEMM shapes under a list of tile schedules, CUDA-event timing
   python tools/bench_kernels.py gemm-ncu        # same launches once each, in a fixed order, for `ncu --metrics dram__bytes_*`
   python tools/bench_kernels.py gemm-list       # prints that order (shape, group_rows, chunk_rows) as JSON
@@ -28,26 +29,38 @@ def time_ms(fn, iters=20, warm=3):
     return e0.elapsed_time(e1) / iters
 
 
-def attn():
+def attn(dump_dir=None):
+    """Both rounding modes at each shape. useful: 4 * 64 * H * sum(len_b^2) FLOP; tiles128: the same with every sequence padded to whole
+    128-row tiles (what a kernel that runs every query and key tile in full executes). dump_dir: the outputs as raw bf16 bytes, so that
+    two builds can be compared byte for byte."""
+    import numpy as np
     from t2v_metrics_b200.engine import ops
     out = {}
-    torch.manual_seed(0)
     for name, (B, S, H, bias, scale) in dict(t5_enc=(64, 672, 64, True, 1.0), t5_enc_ragged=(64, 672, 64, True, 1.0),
                                              clip=(64, 577, 16, False, 0.125)).items():
+        torch.manual_seed(0)
         qkv = (torch.randn(B * S, 3 * H * 64, device="cuda") * (0.5 if bias else 1.0)).bfloat16()
         table = None
         if bias:
             rel = torch.arange(-(S - 1), S, device="cuda").clamp(-128, 128) + 128
             table = (torch.randn(H, 257, device="cuda")).bfloat16().float()[:, rel].contiguous()
         lens = torch.randint(639, 673, (B,), device="cuda", dtype=torch.int32) if "ragged" in name else None
-        rnd = os.environ.get("ATTN_ROUND", "1") == "1"
-        fn = lambda: ops.attention(qkv, B, S, H, seq_lens=lens, bias_table=table, scale=scale, bias_const_from=128 if bias else 0, round_scores=rnd)
-        ms = time_ms(fn)
-        o = fn()
-        torch.cuda.synchronize()
-        flops = 4.0 * B * H * S * S * 64
-        out[name] = dict(ms=round(ms, 4), tflops=round(flops / ms / 1e9, 1), checksum=float(o.float().abs().sum()))
-    print(json.dumps(dict(kernel="attn_wgmma_kernel d64", **out)))
+        L = lens.double().cpu() if lens is not None else torch.full((B,), float(S), dtype=torch.float64)
+        useful = 4.0 * 64 * H * float((L * L).sum())
+        tiles = 4.0 * 64 * H * float(((torch.ceil(L / 128) * 128) ** 2).sum())
+        for rnd in (False, True):
+            fn = lambda: ops.attention(qkv, B, S, H, seq_lens=lens, bias_table=table, scale=scale, bias_const_from=128 if bias else 0,
+                                       round_scores=rnd)
+            ms = time_ms(fn)
+            o = fn()
+            torch.cuda.synchronize()
+            key = f"{name}_round{int(rnd)}"
+            out[key] = dict(ms=round(ms, 4), tflops_useful=round(useful / ms / 1e9, 1), tflops_tiles128=round(tiles / ms / 1e9, 1),
+                            checksum=float(o.float().abs().sum()))
+            if dump_dir:
+                os.makedirs(dump_dir, exist_ok=True)
+                np.save(os.path.join(dump_dir, key + ".npy"), o.view(torch.int16).cpu().numpy())
+    print(json.dumps(dict(kernel="attn64_ws_kernel", **out)))
 
 
 def _t5_attn_inputs(B=64, S=672, H=64):
@@ -146,7 +159,7 @@ def gemm(mode):
 if __name__ == "__main__":
     cmd = sys.argv[1]
     if cmd == "attn":
-        attn()
+        attn(sys.argv[sys.argv.index("--dump") + 1] if "--dump" in sys.argv else None)
     elif cmd == "attn-one":
         attn_one()
     elif cmd == "attn128":
