@@ -459,6 +459,49 @@ int vqa_op_gemm_bf16_splitk(const void* A, int32_t lda, const void* W, int32_t l
 int vqa_op_gemm_bf16_grouped(const void* A, int32_t lda, const void* W, int32_t ldw, int32_t w_rows, void* C, int32_t ldc, int32_t M, int32_t N,
                              int32_t K, const void* bias, int32_t group_in, int32_t group_out, int32_t variant, void* stream);
 
+/* The CLIP tower's residual GEMMs (out_proj, fc2 under autocast): fp32 C[M, ldc] += bf16(A . W^T + bias) in place, the Linear's output rounded
+ * to bf16 once and added to the fp32 stream unrounded. A / W bf16 as vqa_op_gemm_bf16 (lda, ldw, N, K multiples of 8, lda / ldw >= K);
+ * C DEVICE float, ldc a multiple of 4 and >= N; bias [N] bf16 or NULL; variant as vqa_op_gemm_bf16. */
+int vqa_op_gemm_bf16_f32acc(const void* A, int32_t lda, const void* W, int32_t ldw, int32_t w_rows, float* C, int32_t ldc, int32_t M, int32_t N,
+                            int32_t K, const void* bias, int32_t variant, void* stream);
+
+/* `nb` GEMMs of one shape in one launch, plain store epilogue: batch b computes C[b * c_stride + m * ldc + n] = bf16(sum_k A[m + b * a_row_off,
+ * k + b * a_k_off] . W[n + b * w_row_off, k + b * w_k_off]) for m < M, n < N, k < K. A is read as an [a_rows, a_cols] matrix (row stride lda)
+ * and W as [w_rows, w_cols] (ldw); rows past those extents read as zero, so a batch's last A or W rows may run past them (the absorbed
+ * cross-attention's score GEMM reads Sp - S rows past the encoder output in its last batch). Accepted when every batch's first row lies
+ * inside its operand's rows ((nb - 1) * a_row_off < a_rows, (nb - 1) * w_row_off < w_rows) and its K columns inside its columns
+ * ((nb - 1) * a_k_off + K <= a_cols, likewise W); lda, ldw, ldc, N, K, c_stride multiples of 8, a_cols <= lda, w_cols <= ldw, ldc >= N,
+ * offsets >= 0, A / W / C 16-byte aligned; else VQA_ERR_INVALID_ARG. variant as vqa_op_gemm_bf16. */
+int vqa_op_gemm_bf16_batched(const void* A, int32_t lda, const void* W, int32_t ldw, void* C, int32_t ldc, int32_t M, int32_t N, int32_t K,
+                             int32_t nb, int32_t a_row_off, int32_t a_k_off, int32_t w_row_off, int32_t w_k_off, int64_t c_stride,
+                             int64_t a_rows, int64_t a_cols, int64_t w_rows, int64_t w_cols, int32_t variant, void* stream);
+
+/* One CLIP-FlanT5 decoder layer's cross-attention (head_dim 64, no scale, zero bias, encoder padding mask) as vqa_clipt5_score runs it:
+ * decoder queries q [B * T, H * 64] against the encoder output x [B * S, d_model], pair b attending to its first seq_lens[b] rows
+ * (1 <= seq_lens[b] <= S), into out [B * T, H * 64]. wkT = Wk^T [d_model, H * 64], wkv = [Wk; Wv] [2 * H * 64, d_model]. All DEVICE,
+ * 16-byte aligned.
+ *   mode 0 (cross_attention_mode 0, the absorbed association; round_scores unused, wkv's V half only): the encoder transpose, then
+ *     q~ = Wk^T q, bf16 scores q~ . x, their masked fp32 softmax as bf16 P, ctx = P . x, out = Wv ctx. Workspace layout, each buffer
+ *     starting at the next multiple of 256 bytes: xt [B, d_model, Sp] (Sp = S rounded up to 8; columns [S, Sp) zero) | q~ [B * T * H,
+ *     d_model] (row (b * T + t) * H + h) | csc [B * T * H + 256, Sp] (row as q~: P, zero for keys >= seq_lens[b]) | ctx [B * T * H, d_model].
+ *   mode 1 (the reference association, T <= 8 else VQA_ERR_UNSUPPORTED; wkT unused): kv = x . wkv^T [B * S, 2 * H * 64] in the workspace,
+ *     then the flash-style kernel; round_scores != 0 rounds the scores to bf16 before the softmax.
+ * workspace DEVICE, 256-byte aligned; *workspace_needed (HOST, optional) receives the bytes the call needs, also when it returns
+ * VQA_ERR_WORKSPACE. */
+int vqa_op_t5_cross_attention(const void* q, const void* x, const int32_t* seq_lens, const void* wkT, const void* wkv, void* out, int32_t B,
+                              int32_t T, int32_t S, int32_t H, int32_t d_model, int32_t mode, int32_t round_scores, void* workspace,
+                              size_t workspace_bytes, size_t* workspace_needed, void* stream);
+
+/* nn.LayerNorm of the CLIP tower's fp32 residual stream (fp32 statistics): x DEVICE float [rows, D] -> y bf16 [rows, D]; gamma / beta bf16 [D].
+ * D in {256, 512, 768, 1024} (else VQA_ERR_UNSUPPORTED); pointers 16-byte aligned. */
+int vqa_op_layernorm_f32(const float* x, const void* gamma, const void* beta, void* y, int32_t rows, int32_t D, float eps, void* stream);
+
+/* CLIP embeddings + pre_layrnorm: row t of image i is e = bf16(cls + pos[0]) for t = 0, bf16(patch[i * P + t - 1] + pos[t]) otherwise (the
+ * reference adds in bf16), then LayerNorm(e) with fp32 statistics into y DEVICE float [n_images * (P + 1), D]. patch bf16 [n_images * P, D],
+ * cls [D], pos [P + 1, D], gamma / beta [D]. D in {256, 1024} (else VQA_ERR_UNSUPPORTED); pointers 16-byte aligned. */
+int vqa_op_clip_embed_ln(const void* patch, const void* cls, const void* pos, const void* gamma, const void* beta, float* y, int32_t n_images,
+                         int32_t P, int32_t D, float eps, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -25,7 +25,8 @@ ABI_SYMBOLS = [
     "vqa_clipt5_generate_workspace_bytes", "vqa_clipt5_generate_prefill", "vqa_clipt5_generate_step",
     "vqa_qwen25vl_rollout_prefill", "vqa_qwen25vl_rollout_step", "vqa_op_answer_logprob",
     "vqa_op_kv_cache_write", "vqa_op_decode_attention_d128", "vqa_op_greedy_select", "vqa_t5_bucket_lut", "vqa_op_t5_decoder_self_attn",
-    "vqa_op_t5_decode_self_attn",
+    "vqa_op_t5_decode_self_attn", "vqa_op_gemm_bf16_f32acc", "vqa_op_gemm_bf16_batched", "vqa_op_t5_cross_attention", "vqa_op_layernorm_f32",
+    "vqa_op_clip_embed_ln",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -152,6 +153,16 @@ def load() -> C.CDLL:
     lib.vqa_op_t5_decoder_self_attn.restype = C.c_int
     lib.vqa_op_t5_decode_self_attn.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.vqa_op_t5_decode_self_attn.restype = C.c_int
+    lib.vqa_op_gemm_bf16_f32acc.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, vp, i32, vp]
+    lib.vqa_op_gemm_bf16_f32acc.restype = C.c_int
+    lib.vqa_op_gemm_bf16_batched.argtypes = [vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i64, i64, i64, i64, i64, i32, vp]
+    lib.vqa_op_gemm_bf16_batched.restype = C.c_int
+    lib.vqa_op_t5_cross_attention.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t), vp]
+    lib.vqa_op_t5_cross_attention.restype = C.c_int
+    lib.vqa_op_layernorm_f32.argtypes = [vp, vp, vp, vp, i32, i32, f32, vp]
+    lib.vqa_op_layernorm_f32.restype = C.c_int
+    lib.vqa_op_clip_embed_ln.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp]
+    lib.vqa_op_clip_embed_ln.restype = C.c_int
     lib.vqa_clipt5_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
     lib.vqa_clipt5_generate_workspace_bytes.restype = C.c_size_t
     lib.vqa_clipt5_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]

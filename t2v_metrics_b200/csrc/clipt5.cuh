@@ -76,6 +76,19 @@ struct ClipT5Workspace {
     size_t total;
 };
 static int ssq_stride(int d_model) { return (d_model / 32 + 3) / 4 * 4; }
+
+// Buffers of the absorbed cross-attention (clipt5_absorbed_cross_attention), taken in this order from `pl`: the transposed encoder output
+// xt [B, Dm, Sp], q~ [B * T * H, Dm], the scores / probabilities csc [B * T * H (+ 256 spare rows), Sp] and the context sums ctx [B * T * H, Dm].
+struct CrossAttnBuffers { size_t xt, qt, csc, ctx; };
+static CrossAttnBuffers take_cross_attn_buffers(Plan& pl, size_t B, size_t T, size_t S, size_t H, size_t Dm) {
+    const size_t Sp = (S + 7) / 8 * 8, TH = T * H;
+    CrossAttnBuffers b;
+    b.xt = pl.take(B * Dm * Sp * 2);
+    b.qt = pl.take(B * TH * Dm * 2);
+    b.csc = pl.take((B * TH + 256) * Sp * 2);
+    b.ctx = pl.take(B * TH * Dm * 2);
+    return b;
+}
 static ClipT5Workspace plan_workspace(const vqa_handle* h, int B, int NI, int L, int T) {
     const vqa_clipt5_config& c = h->cfg;
     const int P = (c.image_size / c.patch_size) * (c.image_size / c.patch_size);
@@ -105,14 +118,10 @@ static ClipT5Workspace plan_workspace(const vqa_handle* h, int B, int NI, int L,
     w.ssq_b = pl.take(M * (size_t)ssq_stride(c.d_model) * 4);
     w.bias_table = pl.take((size_t)c.n_heads * (2 * S - 1) * 4);
     w.seq_lens = pl.take((size_t)B * 4);
-    const size_t Sp = (size_t)(S + 7) / 8 * 8;
-    const size_t TH = (size_t)T * c.n_heads;
     if (c.cross_attention_mode == 0) {
         w.ckv = 0;
-        w.xt = pl.take((size_t)B * c.d_model * Sp * 2);
-        w.qt = pl.take((size_t)B * TH * c.d_model * 2);
-        w.csc = pl.take(((size_t)B * TH + 256) * Sp * 2);
-        w.cctx = pl.take((size_t)B * TH * c.d_model * 2);
+        const CrossAttnBuffers xb = take_cross_attn_buffers(pl, B, T, S, c.n_heads, c.d_model);
+        w.xt = xb.xt; w.qt = xb.qt; w.csc = xb.csc; w.cctx = xb.ctx;
     } else {
         w.ckv = pl.take(M * 2 * inner * 2);
         w.xt = w.qt = w.csc = w.cctx = 0;
@@ -165,6 +174,14 @@ __global__ void __launch_bounds__(256) row_ssq_kernel(const bf16* __restrict__ x
 }
 
 // ------------------------------------------------------------------------------------------------ forward
+// Encoder output x [B * S, Dm] -> xt [B, Dm, Sp] (Sp = S rounded up to 8, columns [S, Sp) zero): the K-major operand of GEMM (3) of the
+// absorbed cross-attention.
+static int clipt5_transpose_encoder(Forward& f, const bf16* x, bf16* xt, int B, int S, int Dm) {
+    const int Sp = (S + 7) / 8 * 8;
+    return f.launch(CAT_OTHER, 0, "encoder transpose", transpose_bsd_kernel, dim3((Sp + 31) / 32, (Dm + 31) / 32, B), dim3(32, 8), 0, x, xt, S,
+                    Dm, Sp);
+}
+
 // The image and prompt inputs of one encoder pass (see vqa_clipt5_score)
 struct ClipT5Prompts {
     const void* pixels; int pixel_dtype, n_images;
@@ -296,37 +313,56 @@ static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Promp
         }
     }
     TRY(f.rmsnorm(P_(w.x), h->enc_final_ln, P_(w.xn), M, Dm, c.t5_ln_eps));  // encoder output lives in xn from here on
-    const int Sp = (S + 7) / 8 * 8;
-    if (c.cross_attention_mode == 0)
-        TRY(f.launch(CAT_OTHER, 0, "encoder transpose", transpose_bsd_kernel, dim3((Sp + 31) / 32, (Dm + 31) / 32, B), dim3(32, 8), 0,
-                     P_(w.xn), P_(w.xt), S, Dm, Sp));
+    if (c.cross_attention_mode == 0) TRY(clipt5_transpose_encoder(f, P_(w.xn), P_(w.xt), B, S, Dm));
     return VQA_OK;
 }
 
-// Absorbed cross-attention of the B * T decoder rows in w.dq against the encoder output (w.xn, w.xt) into w.dattn (exact in real arithmetic;
-// 30x fewer FLOPs than projecting the S encoder rows because only T rows per pair attend):
+// Absorbed cross-attention of the B * T decoder rows q [B * T, H * 64] against the encoder output x [B * S, Dm] (and its transpose xt from
+// clipt5_transpose_encoder) into out [B * T, H * 64] (exact in real arithmetic; 30x fewer FLOPs than projecting the S encoder rows because
+// only T rows per pair attend):
 //   q.(Wk x_s) = (Wk^T q).x_s          sum_s p_s (Wv x_s) = Wv (sum_s p_s x_s)
-static int clipt5_absorbed_cross_attention(Forward& f, const ClipT5Workspace& w, const T5DecLayerW& Lw, int B, int T, int S) {
-    const vqa_clipt5_config& c = f.h->cfg;
-    auto P_ = [&](size_t off) { return f.at(off); };
-    const int Dm = c.d_model, H = c.n_heads, inner = H * 64, Md = B * T, TH = T * H, Sp = (S + 7) / 8 * 8;
+// The scoring pass, every generation step and vqa_op_t5_cross_attention run this sequence.
+struct AbsorbedCrossAttn {
+    const bf16 *q, *x, *xt;
+    const int* seq_lens;          // [B] encoder rows each pair attends to (<= S)
+    const bf16 *wkT, *wv;         // Wk^T [Dm, H * 64]; Wv [H * 64, Dm] (the V half of the layer's k|v weight)
+    bf16 *qt, *csc, *ctx, *out;   // CrossAttnBuffers
+    int B, T, S, H, Dm;
+};
+static int clipt5_absorbed_cross_attention(Forward& f, const AbsorbedCrossAttn& a) {
+    const int B = a.B, S = a.S, Dm = a.Dm, H = a.H, inner = H * 64, Md = B * a.T, TH = a.T * H, Sp = (S + 7) / 8 * 8;
     // (1) q~[b,t,h,:] = Wk[h]^T q[b,t,h,:]   -- per head: [B*T, 64] x ckT[:, h*64:(h+1)*64]^T -> rows (b*T+t)*H + h
-    Gemm g1(P_(w.dq), Lw.ckT, P_(w.qt), Md, Dm, 64);
+    Gemm g1(a.q, a.wkT, a.qt, Md, Dm, 64);
     g1.lda = inner; g1.ldw = inner; g1.ldc = H * Dm;
     TRY(f.gemm(g1.batched(BatchSpec{H, 0, 64, 0, 64, (long long)Dm, Md, inner, Dm, inner}, Dm >= 256 ? 2561 : 1281), "batched gemm"));
     // (2) scores[b,(t,h),s] = q~[b,(t,h),:] . x[b,s,:]   -- per pair: [T*H, d] x [S, d]^T
-    Gemm g2(P_(w.qt), P_(w.xn), P_(w.csc), TH, Sp, Dm);
+    Gemm g2(a.qt, a.x, a.csc, TH, Sp, Dm);
     TRY(f.gemm(g2.batched(BatchSpec{B, TH, 0, S, 0, (long long)TH * Sp, (long long)B * TH, Dm, (long long)B * S, Dm}, 1281), "batched gemm"));
-    TRY(f.launch(CAT_ATTENTION, 0, "cross softmax", cross_softmax_kernel, (B * TH + 7) / 8, 256, 0, P_(w.csc), (const int*)f.at<int>(w.seq_lens),
-                 TH, B * TH, S, Sp));
+    TRY(f.launch(CAT_ATTENTION, 0, "cross softmax", cross_softmax_kernel, (B * TH + 7) / 8, 256, 0, a.csc, a.seq_lens, TH, B * TH, S, Sp));
     // (3) ctx[b,(t,h),:] = sum_s p[b,(t,h),s] x[b,s,:]   -- per pair: [T*H, Sp] x (x[b]^T)[d, Sp]^T
-    Gemm g3(P_(w.csc), P_(w.xt), P_(w.cctx), TH, Dm, Sp);
+    Gemm g3(a.csc, a.xt, a.ctx, TH, Dm, Sp);
     TRY(f.gemm(g3.batched(BatchSpec{B, TH, 0, Dm, 0, (long long)TH * Dm, (long long)B * TH, Sp, (long long)B * Dm, Sp}, Dm >= 256 ? 2561 : 1281),
                "batched gemm"));
     // (4) o[b,t,h,:] = Wv[h] ctx[b,t,h,:]   -- per head: [B*T, d] (cols h*d..) x Wv[h*64:(h+1)*64, :]^T -> cols h*64..
-    Gemm g4(P_(w.cctx), Lw.ckv + (size_t)inner * Dm, P_(w.dattn), Md, 64, Dm);
+    Gemm g4(a.ctx, a.wv, a.out, Md, 64, Dm);
     g4.lda = H * Dm; g4.ldc = inner;
     return f.gemm(g4.batched(BatchSpec{H, 0, Dm, 64, 0, 64, Md, (long long)H * Dm, inner, Dm}, 641), "batched gemm");
+}
+static int clipt5_absorbed_cross_attention(Forward& f, const ClipT5Workspace& w, const T5DecLayerW& Lw, int B, int T, int S) {
+    const vqa_clipt5_config& c = f.h->cfg;
+    return clipt5_absorbed_cross_attention(f, AbsorbedCrossAttn{f.at(w.dq), f.at(w.xn), f.at(w.xt), f.at<int>(w.seq_lens), Lw.ckT,
+                                                                Lw.ckv + (size_t)c.n_heads * 64 * c.d_model, f.at(w.qt), f.at(w.csc),
+                                                                f.at(w.cctx), f.at(w.dattn), B, T, S, c.n_heads, c.d_model});
+}
+
+// Reference association (cross_attention_mode 1): K/V projection of all S encoder rows (modeling_t5.py:297-299) into kv [B * S, 2 * H * 64],
+// then t5_cross_attn_kernel (T <= 8). round_scores: bf16 scores before the softmax.
+static int clipt5_reference_cross_attention(Forward& f, const bf16* q, const bf16* x, const bf16* wkv, bf16* kv, bf16* out, const int* seq_lens,
+                                            int B, int T, int S, int H, int Dm, int round_scores) {
+    const int inner = H * 64;
+    TRY(f.gemm(Gemm(x, wkv, kv, B * S, 2 * inner, Dm)));
+    return f.launch(CAT_ATTENTION, 4.0 * B * (double)H * T * S * 64, "cross attention", t5_cross_attn_kernel<8>, B * H, 128, 0, q, (const bf16*)kv,
+                    out, seq_lens, 2 * inner, B, T, S, H, round_scores);
 }
 
 // Decoder store-GEMMs: M = B*T rows against 4096-row weights -> split-K when that fills the SMs, else the plain path
@@ -350,7 +386,7 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
     const int P = (c.image_size / c.patch_size) * (c.image_size / c.patch_size);
     const int Dm = c.d_model, H = c.n_heads, inner = H * 64;
     const int S = L - 1 + P;
-    const int M = B * S, Md = B * T;
+    const int Md = B * T;
     TRY(clipt5_encode(f, w, ClipT5Prompts{pixels, pixel_dtype, n_images, image_index, input_ids, text_lens, B, L}));
     int* seq_lens = f.at<int>(w.seq_lens);
 
@@ -369,10 +405,7 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
         TRY(f.rmsnorm(P_(w.y), Lw.ln1, P_(w.yn), Md, Dm, c.t5_ln_eps));
         TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.cq, P_(w.dq), Md, inner, Dm))));
         if (c.cross_attention_mode != 0) {
-            // reference association: K/V projection of all S encoder rows in every layer (modeling_t5.py:297-299)
-            TRY(f.gemm(Gemm(P_(w.xn), Lw.ckv, P_(w.ckv), M, 2 * inner, Dm)));
-            TRY(f.launch(CAT_ATTENTION, 4.0 * B * (double)H * T * S * 64, "cross attention", t5_cross_attn_kernel<8>, B * H, 128, 0, P_(w.dq),
-                         P_(w.ckv), P_(w.dattn), seq_lens, 2 * inner, B, T, S, H, rnd));
+            TRY(clipt5_reference_cross_attention(f, P_(w.dq), P_(w.xn), Lw.ckv, P_(w.ckv), P_(w.dattn), seq_lens, B, T, S, H, Dm, rnd));
         } else {
             TRY(clipt5_absorbed_cross_attention(f, w, Lw, B, T, S));
         }

@@ -743,6 +743,108 @@ extern "C" int vqa_op_norm(const void* x, const void* gamma, const void* beta, v
     return cuda_status(nullptr, e, "norm launch");
 }
 
+// ------------------------------------------------------------------------------------------------ kernel-level ABI: the CLIP-FlanT5 scoring path
+static bool gemm_variant_known(int v) { return v == 0 || v == 2561 || v == 2562 || v == 1281 || v == 1282 || v == 641 || v == 321; }
+
+// The CLIP tower's residual GEMMs (out_proj, fc2): fp32 C[M, ldc] += bf16(A W^T + bias), in place.
+extern "C" int vqa_op_gemm_bf16_f32acc(const void* A, int32_t lda, const void* W, int32_t ldw, int32_t w_rows, float* C, int32_t ldc, int32_t M,
+                                       int32_t N, int32_t K, const void* bias, int32_t variant, void* stream) {
+    if (!A || !W || !C || M <= 0 || N <= 0 || K <= 0 || w_rows <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32-accumulate gemm: bad argument");
+    if (lda % 8 || ldw % 8 || N % 8 || K % 8 || ldc % 4 || lda < K || ldw < K || ldc < N)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32-accumulate gemm: lda / ldw / N / K multiples of 8 and >= K, ldc a multiple of 4 and >= N");
+    if (!aligned(A, 16) || !aligned(W, 16) || !aligned(C, 16) || !aligned(bias, 8))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32-accumulate gemm: A / W / C 16-byte aligned, bias 8-byte aligned");
+    if (!gemm_variant_known(variant)) return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32-accumulate gemm: unknown tile variant");
+    Gemm g = abi_gemm(A, lda, W, ldw, w_rows, C, ldc, M, N, K);
+    g.bias = (const bf16*)bias; g.variant = variant;
+    return cuda_status(nullptr, run_gemm(g.accumulate_f32(), device_sms(), (cudaStream_t)stream), "gemm launch");
+}
+
+// `nb` GEMMs of one shape in one launch (BatchSpec), plain store epilogue. See include/vqa_b200.h for the acceptance rule.
+extern "C" int vqa_op_gemm_bf16_batched(const void* A, int32_t lda, const void* W, int32_t ldw, void* C, int32_t ldc, int32_t M, int32_t N, int32_t K,
+                                        int32_t nb, int32_t a_row_off, int32_t a_k_off, int32_t w_row_off, int32_t w_k_off, int64_t c_stride,
+                                        int64_t a_rows, int64_t a_cols, int64_t w_rows, int64_t w_cols, int32_t variant, void* stream) {
+    if (!A || !W || !C || M <= 0 || N <= 0 || K <= 0 || nb <= 0 || a_rows <= 0 || a_cols <= 0 || w_rows <= 0 || w_cols <= 0 ||
+        a_row_off < 0 || a_k_off < 0 || w_row_off < 0 || w_k_off < 0 || c_stride < 0)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: bad argument");
+    if (lda % 8 || ldw % 8 || ldc % 8 || N % 8 || K % 8 || c_stride % 8 || a_cols > lda || w_cols > ldw || ldc < N || a_rows > INT32_MAX ||
+        w_rows > INT32_MAX)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: ld / N / K / c_stride multiples of 8, extents inside the leading dimensions, ldc >= N");
+    if (!aligned(A, 16) || !aligned(W, 16) || !aligned(C, 16)) return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: A / W / C 16-byte aligned");
+    const long long last = nb - 1;
+    if (last * a_row_off >= a_rows || last * w_row_off >= w_rows || last * a_k_off + K > a_cols || last * w_k_off + K > w_cols)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: every batch's first A / W row and its K columns must lie inside the extents");
+    if (!gemm_variant_known(variant)) return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: unknown tile variant");
+    Gemm g = abi_gemm(A, lda, W, ldw, (int)w_rows, C, ldc, M, N, K);
+    g.batched(BatchSpec{nb, a_row_off, a_k_off, w_row_off, w_k_off, c_stride, a_rows, a_cols, w_rows, w_cols}, variant);
+    return cuda_status(nullptr, run_gemm(g, device_sms(), (cudaStream_t)stream), "gemm launch");
+}
+
+// One decoder layer's cross-attention as vqa_clipt5_score runs it: mode 0 the absorbed sequence (the encoder transpose, then
+// clipt5_absorbed_cross_attention), mode 1 the reference association (clipt5_reference_cross_attention).
+extern "C" int vqa_op_t5_cross_attention(const void* q, const void* x, const int32_t* seq_lens, const void* wkT, const void* wkv, void* out,
+                                         int32_t B, int32_t T, int32_t S, int32_t H, int32_t d_model, int32_t mode, int32_t round_scores,
+                                         void* workspace, size_t workspace_bytes, size_t* workspace_needed, void* stream) {
+    if (!q || !x || !seq_lens || !wkv || !out || (mode == 0 && !wkT)) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 cross attention: null pointer");
+    if (B <= 0 || T <= 0 || S <= 0 || H <= 0 || d_model <= 0 || d_model % 8 || (mode != 0 && mode != 1))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 cross attention: bad size (d_model a multiple of 8) or mode (0 or 1)");
+    if (mode == 1 && T > 8) return fail(nullptr, VQA_ERR_UNSUPPORTED, "t5 cross attention: the reference association takes T <= 8");
+    if (!aligned(q, 16) || !aligned(x, 16) || !aligned(wkT, 16) || !aligned(wkv, 16) || !aligned(out, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 cross attention: q / x / weights / out must be 16-byte aligned");
+    const int inner = H * 64;
+    Plan pl;
+    CrossAttnBuffers xb{};
+    size_t kv = 0;
+    if (mode == 0) xb = take_cross_attn_buffers(pl, B, T, S, H, d_model);
+    else kv = pl.take((size_t)B * S * 2 * inner * 2);
+    if (workspace_needed) *workspace_needed = pl.off;
+    if (!workspace || workspace_bytes < pl.off) return fail(nullptr, VQA_ERR_WORKSPACE, "t5 cross attention: workspace too small");
+    if (!aligned(workspace, 256)) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 cross attention: workspace must be 256-byte aligned");
+    vqa_handle launcher;        // a Forward needs a handle; this one only collects the launch count and the error text
+    launcher.num_sms = device_sms();
+    Forward f(&launcher, workspace, (cudaStream_t)stream);
+    int rc;
+    if (mode == 0) {
+        rc = clipt5_transpose_encoder(f, (const bf16*)x, f.at(xb.xt), B, S, d_model);
+        if (rc == VQA_OK)
+            rc = clipt5_absorbed_cross_attention(f, AbsorbedCrossAttn{(const bf16*)q, (const bf16*)x, f.at(xb.xt), seq_lens, (const bf16*)wkT,
+                                                                      (const bf16*)wkv + (size_t)inner * d_model, f.at(xb.qt), f.at(xb.csc),
+                                                                      f.at(xb.ctx), (bf16*)out, B, T, S, H, d_model});
+    } else {
+        rc = clipt5_reference_cross_attention(f, (const bf16*)q, (const bf16*)x, (const bf16*)wkv, f.at(kv), (bf16*)out, seq_lens, B, T, S, H,
+                                              d_model, round_scores);
+    }
+    return rc == VQA_OK ? VQA_OK : fail(nullptr, rc, launcher.err);
+}
+
+// LayerNorm of the CLIP tower's fp32 residual stream: x fp32 [rows, D] -> y bf16 [rows, D].
+extern "C" int vqa_op_layernorm_f32(const float* x, const void* gamma, const void* beta, void* y, int32_t rows, int32_t D, float eps, void* stream) {
+    if (!x || !gamma || !beta || !y || rows <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32 layernorm: bad argument");
+    if (D != 256 && D != 512 && D != 768 && D != 1024) return fail(nullptr, VQA_ERR_UNSUPPORTED, "fp32 layernorm: D must be 256, 512, 768 or 1024");
+    if (!aligned(x, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32 layernorm: pointers must be 16-byte aligned");
+    return cuda_status(nullptr, run_layernorm_f32(x, (const bf16*)gamma, (const bf16*)beta, (bf16*)y, rows, D, eps, (cudaStream_t)stream),
+                       "layernorm launch");
+}
+
+// The CLIP embeddings and pre_layrnorm as vqa_clipt5_score launches them: patch rows [n_images * P, D] -> fp32 y [n_images * (P + 1), D].
+extern "C" int vqa_op_clip_embed_ln(const void* patch, const void* cls, const void* pos, const void* gamma, const void* beta, float* y,
+                                    int32_t n_images, int32_t P, int32_t D, float eps, void* stream) {
+    if (!patch || !cls || !pos || !gamma || !beta || !y || n_images <= 0 || P <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "clip embed: bad argument");
+    if (D != 256 && D != 1024) return fail(nullptr, VQA_ERR_UNSUPPORTED, "clip embed: D must be 256 or 1024");
+    if (!aligned(patch, 16) || !aligned(cls, 16) || !aligned(pos, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "clip embed: pointers must be 16-byte aligned");
+    const int rows = n_images * (P + 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (D == 1024)
+        clip_embed_ln_kernel<1024><<<(rows + 7) / 8, 256, 0, st>>>((const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma,
+                                                                   (const bf16*)beta, y, n_images, P, eps);
+    else
+        clip_embed_ln_kernel<256><<<(rows + 7) / 8, 256, 0, st>>>((const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma,
+                                                                  (const bf16*)beta, y, n_images, P, eps);
+    return cuda_status(nullptr, cudaGetLastError(), "clip embed launch");
+}
+
 // ---------------------------------------------------------------------------------------------- image pre-processing (SURVEY 8(f)2)
 extern "C" size_t vqa_clip_preprocess_workspace_bytes(const int32_t* heights, const int32_t* widths, int32_t n_images,
                                                       int32_t out_size, int32_t pad_to_square) {

@@ -568,6 +568,73 @@ class ops:
         _check(rc, None, "vqa_op_norm")
         return y
 
+    @staticmethod
+    def gemm_f32acc(a: torch.Tensor, w: torch.Tensor, c: torch.Tensor, bias=None, variant=0):
+        """The CLIP tower's residual GEMM: fp32 c[M, N] += bf16(a . w^T + bias), in place (row stride c.stride(0))."""
+        lib = _lib.load()
+        M, K = a.shape
+        N = w.shape[0]
+        rc = lib.vqa_op_gemm_bf16_f32acc(_ptr(a), a.stride(0), _ptr(w), w.stride(0), N, _ptr(c), c.stride(0), M, N, K, _ptr(bias), variant,
+                                         _stream_ptr(a.device))
+        _check(rc, None, "vqa_op_gemm_bf16_f32acc")
+        return c
+
+    @staticmethod
+    def gemm_batched(a: torch.Tensor, w: torch.Tensor, c: torch.Tensor, M: int, N: int, K: int, nb: int, a_off=(0, 0), w_off=(0, 0),
+                     c_stride: int = 0, a_extent=None, w_extent=None, variant: int = 0):
+        """`nb` store-GEMMs in one launch (see vqa_op_gemm_bf16_batched): batch b reads a at (row, k) + b * a_off, w at (row, k) + b * w_off
+        and writes c.flatten()[b * c_stride + m * c.stride(0) + n]. a_extent / w_extent (rows, cols) default to the tensors' shapes."""
+        lib = _lib.load()
+        a_rows, a_cols = a_extent or a.shape
+        w_rows, w_cols = w_extent or w.shape
+        rc = lib.vqa_op_gemm_bf16_batched(_ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(c), c.stride(0), M, N, K, nb, a_off[0], a_off[1],
+                                          w_off[0], w_off[1], c_stride, a_rows, a_cols, w_rows, w_cols, variant, _stream_ptr(a.device))
+        _check(rc, None, "vqa_op_gemm_bf16_batched")
+        return c
+
+    @staticmethod
+    def t5_cross_attention(q: torch.Tensor, x: torch.Tensor, seq_lens: torch.Tensor, wkT, wkv: torch.Tensor, B: int, T: int, S: int, H: int,
+                           mode: int = 0, round_scores: bool = False, out=None, workspace=None):
+        """One CLIP-FlanT5 decoder cross-attention layer (see vqa_op_t5_cross_attention): mode 0 absorbed, mode 1 the reference association.
+        Returns (out [B * T, H * 64], the uint8 workspace, whose mode-0 layout the header documents)."""
+        lib = _lib.load()
+        Dm = x.shape[1]
+        if out is None:
+            out = torch.empty(B * T, H * 64, dtype=torch.bfloat16, device=q.device)
+        need = C.c_size_t(0)
+        args = (_ptr(q), _ptr(x), _ptr(seq_lens), _ptr(wkT), _ptr(wkv), _ptr(out), B, T, S, H, Dm, mode, 1 if round_scores else 0)
+        if workspace is None:   # a call without workspace stops at the workspace check and returns the size
+            rc = lib.vqa_op_t5_cross_attention(*args, None, 0, C.byref(need), _stream_ptr(q.device))
+            if rc != -4:
+                _check(rc or -1, None, "vqa_op_t5_cross_attention")
+            workspace = torch.empty(need.value, dtype=torch.uint8, device=q.device)
+        rc = lib.vqa_op_t5_cross_attention(*args, _ptr(workspace), workspace.numel(), C.byref(need), _stream_ptr(q.device))
+        _check(rc, None, "vqa_op_t5_cross_attention")
+        return out, workspace
+
+    @staticmethod
+    def layernorm_f32(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5, out=None):
+        """LayerNorm of an fp32 [rows, D] stream into bf16 (the CLIP tower's ln1 / ln2)."""
+        lib = _lib.load()
+        if out is None:
+            out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+        rc = lib.vqa_op_layernorm_f32(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), x.shape[0], x.shape[1], float(eps), _stream_ptr(x.device))
+        _check(rc, None, "vqa_op_layernorm_f32")
+        return out
+
+    @staticmethod
+    def clip_embed_ln(patch: torch.Tensor, cls: torch.Tensor, pos: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, n_images: int,
+                      eps: float = 1e-5, out=None):
+        """CLIP embeddings + pre_layrnorm: patch rows [n_images * P, D] -> fp32 [n_images * (P + 1), D]."""
+        lib = _lib.load()
+        P, D = patch.shape[0] // n_images, patch.shape[1]
+        if out is None:
+            out = torch.empty(n_images * (P + 1), D, dtype=torch.float32, device=patch.device)
+        rc = lib.vqa_op_clip_embed_ln(_ptr(patch), _ptr(cls), _ptr(pos), _ptr(gamma), _ptr(beta), _ptr(out), n_images, P, D, float(eps),
+                                      _stream_ptr(patch.device))
+        _check(rc, None, "vqa_op_clip_embed_ln")
+        return out
+
 
 # ------------------------------------------------------------------------------------------------ image pre-processing
 class _PinnedRing:
