@@ -341,6 +341,24 @@ int vqa_qwen_preprocess(const void* src, const int64_t* offsets, const int32_t* 
                         const float* stdv, void* out, int32_t out_dtype, void* workspace, size_t workspace_bytes, void* host_staging,
                         void* stream);
 
+/* Qwen2.5-VL still images and decoded video frame stacks in one launch: each frame goes through the still-image path above
+ * (qwen_vl_utils fetch_video on a list of frames runs fetch_image on each), then Qwen2VLVideoProcessor._preprocess with
+ * do_resize=False (video_processing_qwen2_vl.py:228-275): frames 2k and 2k+1 fill temporal slots 0 and 1 of temporal group k's patch
+ * rows, and an odd last frame fills both (the processor's padding with copies of the last frame; no second read of the source).
+ *   n_frames / heights / widths / is_video   HOST arrays [n_items]; all frames of an item share its size. is_video[i] == 0: a still
+ *              image (n_frames[i] must be 1), its frame written to every temporal slot, grid (1, gh, gw); else a video of
+ *              ceil(n_frames / temporal_patch) temporal groups. A 1-frame video has the pixels of a still but is a video grid.
+ *   frame_offsets  HOST [sum n_frames]: byte offset in `src` of every frame (HWC uint8 RGB), item by item.
+ * vqa_qwen_preprocess_video_plan is host-only: grid_thw [n_items][3], total_patches = rows of `out`, workspace_bytes = device scratch.
+ * out: DEVICE [total_patches, 3*temporal_patch*patch^2], item i's rows after those of items < i. At most 65535 frames per call. */
+int vqa_qwen_preprocess_video_plan(const int32_t* n_frames, const int32_t* heights, const int32_t* widths, const int32_t* is_video,
+                                   int32_t n_items, int32_t patch, int32_t temporal_patch, int32_t merge, int64_t min_pixels,
+                                   int64_t max_pixels, int32_t* grid_thw, int64_t* total_patches, size_t* workspace_bytes);
+int vqa_qwen_preprocess_video(const void* src, const int64_t* frame_offsets, const int32_t* n_frames, const int32_t* heights,
+                              const int32_t* widths, const int32_t* is_video, int32_t n_items, int32_t patch, int32_t temporal_patch,
+                              int32_t merge, int64_t min_pixels, int64_t max_pixels, const float* mean, const float* stdv, void* out,
+                              int32_t out_dtype, void* workspace, size_t workspace_bytes, void* host_staging, void* stream);
+
 /* Host-only helper (no GPU needed): the 22-bit fixed-point bicubic tap table of one resize axis (in_size -> out_size, output
  * pixels [first, first + count)), exactly as vqa_clip_preprocess builds it after Pillow's precompute_coeffs /
  * normalize_coeffs_8bpc. bounds [count][2] = (first source index, taps used); kk [count][ksize]; returns ksize (0 = bad

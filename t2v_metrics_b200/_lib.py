@@ -26,7 +26,7 @@ ABI_SYMBOLS = [
     "vqa_qwen25vl_rollout_prefill", "vqa_qwen25vl_rollout_step", "vqa_op_answer_logprob",
     "vqa_op_kv_cache_write", "vqa_op_decode_attention_d128", "vqa_op_greedy_select", "vqa_t5_bucket_lut", "vqa_op_t5_decoder_self_attn",
     "vqa_op_t5_decode_self_attn", "vqa_op_gemm_bf16_f32acc", "vqa_op_gemm_bf16_batched", "vqa_op_t5_cross_attention", "vqa_op_layernorm_f32",
-    "vqa_op_clip_embed_ln",
+    "vqa_op_clip_embed_ln", "vqa_qwen_preprocess_video_plan", "vqa_qwen_preprocess_video",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -180,6 +180,12 @@ def load() -> C.CDLL:
     lib.vqa_qwen_preprocess.argtypes = [vp, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, i32, i64, i64,
                                         C.POINTER(C.c_float), C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
     lib.vqa_qwen_preprocess.restype = C.c_int
+    lib.vqa_qwen_preprocess_video_plan.argtypes = [C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, i32, i64, i64,
+                                                   C.POINTER(i32), C.POINTER(i64), C.POINTER(C.c_size_t)]
+    lib.vqa_qwen_preprocess_video_plan.restype = C.c_int
+    lib.vqa_qwen_preprocess_video.argtypes = [vp, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, i32,
+                                              i32, i64, i64, C.POINTER(C.c_float), C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
+    lib.vqa_qwen_preprocess_video.restype = C.c_int
     lib.vqa_clipt5_debug_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(C.c_size_t), i32]
     lib.vqa_clipt5_debug_layout.restype = C.c_int
     lib.vqa_qwen25vl_debug_layout.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_size_t), i32]

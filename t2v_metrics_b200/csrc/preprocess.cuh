@@ -43,6 +43,7 @@ struct PreImage {            // one per image, lives in the workspace (device) a
     long long out_off;       // element offset of this image's output inside `out`
     int x_lo4, span4;        // groups of 4 canvas columns [x_lo4, x_lo4 + span4) the horizontal tap words touch
     int chunk_groups;        // groups of 4 canvas rows staged per pass (1 or 2)
+    int t0, nt;              // PRE_QWEN_PATCHES: temporal slots [t0, t0 + nt) of its patch rows this frame fills
 };
 
 enum PreLayout { PRE_CHW = 0, PRE_QWEN_PATCHES = 1 };
@@ -154,7 +155,8 @@ __device__ __forceinline__ unsigned pre_finish(unsigned a0, unsigned a1, int a2)
 
 // LAYOUT PRE_CHW: out[c][y][x] per image ([3, out_h, out_w]). PRE_QWEN_PATCHES: the Qwen2-VL processor's patch rows
 // (image_processing_qwen2_vl.py:191-220): row ((by * gw/m + bx) * m + iy) * m + ix for the 14x14 patch at grid (by*m+iy, bx*m+ix),
-// column (c * temporal + t) * ps*ps + py * ps + px, the still frame written to every temporal slot t.
+// column (c * temporal + t) * ps*ps + py * ps + px, the frame written to temporal slots t in [t0, t0 + nt): every slot for a still
+// image, its own slot for a video frame (video_processing_qwen2_vl.py:255-272), and the remaining slots for the last frame of a stack.
 template <typename OUT, int LAYOUT>
 __global__ void __launch_bounds__(PRE_THREADS)
 image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restrict__ images, const int* __restrict__ tables,
@@ -302,7 +304,7 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
                 OUT* q = dst + row * (size_t)(3 * geom.temporal * pp) + py * ps + px_;
 #pragma unroll
                 for (int c = 0; c < 3; ++c)
-                    for (int t = 0; t < geom.temporal; ++t) {
+                    for (int t = im.t0; t < im.t0 + im.nt; ++t) {
                         if constexpr (sizeof(OUT) == 4) q[(size_t)(c * geom.temporal + t) * pp] = v[c];
                         else q[(size_t)(c * geom.temporal + t) * pp] = __float2bfloat16_rn(v[c]);
                     }
@@ -421,34 +423,61 @@ inline bool pre_smart_resize(int height, int width, int factor, long long min_pi
     return true;
 }
 
-// Qwen still images: smart_resize, plain bicubic resize of the whole image (no canvas, no crop), patch-row output; image i's rows
-// start at sum_{j<i} gh_j * gw_j. grid_hw[i] = (gh, gw) in patches.
-inline bool pre_plan_qwen(const int32_t* heights, const int32_t* widths, const int64_t* offsets, int n, int patch, int merge, int temporal,
-                          long long min_pixels, long long max_pixels, PrePlan& plan, int32_t* grid_hw, long long* total_rows) {
+// Qwen still images and frame stacks: one smart_resize per item (all frames of a stack share their size, so they share one set of
+// tables), plain bicubic resize of the whole frame (no canvas, no crop), patch-row output. Item i has n_frames[i] frames at byte
+// offsets frame_offsets[f0 .. f0 + n_frames[i]) of `src`; a still (is_video[i] == 0, one frame) fills every temporal slot of its rows,
+// a video's frame f fills slot f % temporal of the rows of temporal group f / temporal, and its last frame also fills the slots after
+// its own (the processor pads the stack with copies of the last frame, video_processing_qwen2_vl.py:245-249). Item i's rows start at
+// sum_{j<i} t_j * gh_j * gw_j; grid_thw[i] = (t, gh, gw) with t = 1 for a still and ceil(n_frames / temporal) for a video.
+inline bool pre_plan_qwen_video(const int32_t* n_frames, const int32_t* heights, const int32_t* widths, const int32_t* is_video,
+                                const int64_t* frame_offsets, int n, int patch, int merge, int temporal, long long min_pixels,
+                                long long max_pixels, PrePlan& plan, int32_t* grid_thw, long long* total_rows) {
     std::vector<PreTableKey> cache;
     cache.reserve(n);
-    plan.images.resize(n);
+    plan.images.clear();
     long long rows = 0;
     const long long row_elems = 3LL * temporal * patch * patch;
     for (int i = 0; i < n; ++i) {
-        const int h = heights[i], w = widths[i];
+        const int h = heights[i], w = widths[i], nf = n_frames[i];
         if (h <= 0 || w <= 0) { plan.error = "image with non-positive size"; return false; }
+        if (nf <= 0 || (!is_video[i] && nf != 1)) { plan.error = "a video needs at least one frame and a still image exactly one"; return false; }
         int rh, rw;
         if (!pre_smart_resize(h, w, patch * merge, min_pixels, max_pixels, rh, rw)) {
             plan.error = "absolute aspect ratio must be smaller than 200";
             return false;
         }
-        PreImage& im = plan.images[i];
-        im.src_off = offsets[i]; im.h = h; im.w = w;
-        im.canvas_h = h; im.canvas_w = w; im.paste_x = im.paste_y = 0;
         const PreTableKey* k = pre_tables(plan, cache, h, w, rh, rw, 0, 0, rh, rw);
         if (!k) return false;
-        pre_finish_image(plan, im, *k);
-        im.out_off = rows * row_elems;
-        if (grid_hw) { grid_hw[2 * i] = rh / patch; grid_hw[2 * i + 1] = rw / patch; }
-        rows += (long long)(rh / patch) * (rw / patch);
+        const long long frame_rows = (long long)(rh / patch) * (rw / patch);
+        const int gt = is_video[i] ? (nf + temporal - 1) / temporal : 1;
+        for (int f = 0; f < nf; ++f) {
+            PreImage im{};
+            im.src_off = frame_offsets[f]; im.h = h; im.w = w;
+            im.canvas_h = h; im.canvas_w = w;
+            pre_finish_image(plan, im, *k);
+            im.out_off = (rows + (long long)(f / temporal) * frame_rows) * row_elems;
+            im.t0 = is_video[i] ? f % temporal : 0;
+            im.nt = f + 1 < nf ? 1 : temporal - im.t0;
+            plan.images.push_back(im);
+        }
+        frame_offsets += nf;
+        if (grid_thw) { grid_thw[3 * i] = gt; grid_thw[3 * i + 1] = rh / patch; grid_thw[3 * i + 2] = rw / patch; }
+        rows += gt * frame_rows;
     }
     if (total_rows) *total_rows = rows;
+    return true;
+}
+
+// Qwen still images only: image i's rows start at sum_{j<i} gh_j * gw_j. grid_hw[i] = (gh, gw) in patches.
+inline bool pre_plan_qwen(const int32_t* heights, const int32_t* widths, const int64_t* offsets, int n, int patch, int merge, int temporal,
+                          long long min_pixels, long long max_pixels, PrePlan& plan, int32_t* grid_hw, long long* total_rows) {
+    const std::vector<int32_t> one(n, 1), still(n, 0);
+    std::vector<int32_t> thw(3 * (size_t)n);
+    if (!pre_plan_qwen_video(one.data(), heights, widths, still.data(), offsets, n, patch, merge, temporal, min_pixels, max_pixels, plan,
+                             thw.data(), total_rows))
+        return false;
+    if (grid_hw)
+        for (int i = 0; i < n; ++i) { grid_hw[2 * i] = thw[3 * i + 1]; grid_hw[2 * i + 1] = thw[3 * i + 2]; }
     return true;
 }
 

@@ -944,6 +944,53 @@ extern "C" int vqa_qwen_preprocess(const void* src, const int64_t* offsets, cons
                                         workspace, workspace_bytes, host_staging, reinterpret_cast<cudaStream_t>(stream));
 }
 
+static int qwen_video_args(const int32_t* n_frames, const int32_t* heights, const int32_t* widths, const int32_t* is_video, int32_t n_items,
+                           int32_t patch, int32_t temporal_patch, int32_t merge, int64_t min_pixels, int64_t max_pixels, int64_t* frames) {
+    if (!n_frames || !heights || !widths || !is_video || n_items <= 0 || patch <= 0 || merge <= 0 || temporal_patch <= 0 || min_pixels <= 0 ||
+        max_pixels < min_pixels)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "bad argument");
+    int64_t total = 0;
+    for (int i = 0; i < n_items; ++i) total += n_frames[i] > 0 ? n_frames[i] : 0;
+    if (total > 65535) return fail(nullptr, VQA_ERR_INVALID_ARG, "more than 65535 frames in one call");     // gridDim.y of the launch
+    *frames = total;
+    return VQA_OK;
+}
+
+extern "C" int vqa_qwen_preprocess_video_plan(const int32_t* n_frames, const int32_t* heights, const int32_t* widths, const int32_t* is_video,
+                                              int32_t n_items, int32_t patch, int32_t temporal_patch, int32_t merge, int64_t min_pixels,
+                                              int64_t max_pixels, int32_t* grid_thw, int64_t* total_patches, size_t* workspace_bytes) {
+    int64_t frames = 0;
+    if (int rc = qwen_video_args(n_frames, heights, widths, is_video, n_items, patch, temporal_patch, merge, min_pixels, max_pixels, &frames))
+        return rc;
+    PrePlan plan;
+    std::vector<int64_t> off(frames, 0);
+    long long rows = 0;
+    if (!pre_plan_qwen_video(n_frames, heights, widths, is_video, off.data(), n_items, patch, merge, temporal_patch, min_pixels, max_pixels,
+                             plan, grid_thw, &rows))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, plan.error);
+    if (total_patches) *total_patches = rows;
+    if (workspace_bytes) *workspace_bytes = plan.bytes();
+    return VQA_OK;
+}
+
+extern "C" int vqa_qwen_preprocess_video(const void* src, const int64_t* frame_offsets, const int32_t* n_frames, const int32_t* heights,
+                                         const int32_t* widths, const int32_t* is_video, int32_t n_items, int32_t patch, int32_t temporal_patch,
+                                         int32_t merge, int64_t min_pixels, int64_t max_pixels, const float* mean, const float* stdv, void* out,
+                                         int32_t out_dtype, void* workspace, size_t workspace_bytes, void* host_staging, void* stream) {
+    if (!src || !frame_offsets || !mean || !stdv || !out || !workspace) return fail(nullptr, VQA_ERR_INVALID_ARG, "null pointer");
+    int64_t frames = 0;
+    if (int rc = qwen_video_args(n_frames, heights, widths, is_video, n_items, patch, temporal_patch, merge, min_pixels, max_pixels, &frames))
+        return rc;
+    if (out_dtype != VQA_DTYPE_F32 && out_dtype != VQA_DTYPE_BF16) return fail(nullptr, VQA_ERR_INVALID_ARG, "out_dtype must be f32 or bf16");
+    PrePlan plan;
+    if (!pre_plan_qwen_video(n_frames, heights, widths, is_video, frame_offsets, n_items, patch, merge, temporal_patch, min_pixels, max_pixels,
+                             plan, nullptr, nullptr))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, plan.error);
+    const uint8_t no_bg[3] = {0, 0, 0};
+    return pre_launch<PRE_QWEN_PATCHES>(plan, src, (int)plan.images.size(), no_bg, mean, stdv, PrePatchGeom{patch, merge, temporal_patch}, out,
+                                        out_dtype, workspace, workspace_bytes, host_staging, reinterpret_cast<cudaStream_t>(stream));
+}
+
 // Host-only: the fixed-point tap table of one resize axis, exactly as vqa_clip_preprocess builds it (for CPU tests of the host logic).
 // bounds: [count][2] (first source index, taps used), kk: [count][ksize] with ksize = return value (call with kk = NULL to size it).
 extern "C" int32_t vqa_resample_table(int32_t in_size, int32_t out_size, int32_t first, int32_t count, int32_t* bounds, int32_t* kk) {

@@ -776,6 +776,55 @@ def qwen_preprocess_u8(images: Sequence[torch.Tensor], device, patch: int = 14, 
     return out, grids
 
 
+def qwen_preprocess_video_u8(items: Sequence[torch.Tensor], device, patch: int = 14, temporal_patch: int = 2, merge: int = 2,
+                             min_pixels: int = 56 * 56, max_pixels: int = 14 * 14 * 4 * 1280, mean=CLIP_MEAN, std=CLIP_STD,
+                             out_dtype: torch.dtype = torch.float32):
+    """Decoded still images (uint8 [h, w, 3]) and video frame stacks (uint8 [n, h, w, 3]), host or device, in any mix -> (pixel_patches
+    [sum t*gh*gw, 3*temporal*patch^2] on the device, [(t, gh, gw), ...]) by ONE kernel launch (vqa_qwen_preprocess_video): every frame
+    gets the still-image pre-processing of qwen_preprocess_u8, and a stack's frames fill consecutive temporal slots of its patch rows, the
+    last frame repeated into the slots a count that is not a multiple of temporal_patch leaves -- bit-identical to
+    models/vqascore_models/qwen_utils.qwen_video_to_patches. A still keeps grid t = 1 and the rows of qwen_preprocess_u8."""
+    lib = _lib.load()
+    dev = torch.device(device)
+    n = len(items)
+    assert n > 0
+    nf, hs, ws, vid, offs, total = [], [], [], [], [], 0
+    for it in items:
+        assert it.dtype == torch.uint8 and it.dim() in (3, 4) and it.shape[-1] == 3, "items must be uint8 [h, w, 3] or [n, h, w, 3]"
+        frames = int(it.shape[0]) if it.dim() == 4 else 1
+        nf.append(frames); hs.append(int(it.shape[-3])); ws.append(int(it.shape[-2])); vid.append(int(it.dim() == 4))
+        step = hs[-1] * ws[-1] * 3
+        offs.extend(total + f * step for f in range(frames))
+        total += int(it.numel())
+    i32 = lambda v: (C.c_int32 * n)(*v)
+    NF, H, W, V = i32(nf), i32(hs), i32(ws), i32(vid)
+    grid = (C.c_int32 * (3 * n))()
+    rows, need = C.c_int64(0), C.c_size_t(0)
+    _check(lib.vqa_qwen_preprocess_video_plan(NF, H, W, V, n, patch, temporal_patch, merge, min_pixels, max_pixels, grid, C.byref(rows),
+                                              C.byref(need)), None, "vqa_qwen_preprocess_video_plan")
+    if all(it.is_cuda for it in items):
+        src = items[0].contiguous().view(-1) if n == 1 else torch.cat([it.contiguous().view(-1) for it in items])
+    else:
+        stage = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+        o = 0
+        for it in items:
+            stage[o:o + it.numel()] = it.contiguous().view(-1)
+            o += it.numel()
+        src = stage.to(dev, non_blocking=True)
+    out = torch.empty(int(rows.value), 3 * temporal_patch * patch * patch, dtype=out_dtype, device=dev)
+    wsb = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=dev)
+    ring = _staging(dev)
+    stage_buf = ring.acquire(wsb.numel())
+    with torch.cuda.device(dev):
+        rc = lib.vqa_qwen_preprocess_video(_ptr(src), (C.c_int64 * len(offs))(*offs), NF, H, W, V, n, patch, temporal_patch, merge, min_pixels,
+                                           max_pixels, (C.c_float * 3)(*mean), (C.c_float * 3)(*std), _ptr(out),
+                                           _lib.VQA_DTYPE_F32 if out_dtype == torch.float32 else _lib.VQA_DTYPE_BF16, _ptr(wsb), wsb.numel(),
+                                           stage_buf.data_ptr(), _stream_ptr(dev))
+    ring.release(dev)
+    _check(rc, None, "vqa_qwen_preprocess_video")
+    return out, [tuple(int(grid[3 * i + k]) for k in range(3)) for i in range(n)]
+
+
 # ================================================================================================ Qwen2.5-VL
 def convert_qwen_state_dict(sd: Dict[str, torch.Tensor], cfg, device) -> Dict[str, torch.Tensor]:
     """HF `Qwen2_5_VLForConditionalGeneration` names -> the engine's fused bf16 layout:
@@ -1010,6 +1059,10 @@ class QwenVLEngine:
 
     # ------------------------------------------------------------------------------------------ greedy generation
     MAX_GEN_GRAPHS = 8
+
+    def score_workspace_bytes(self, batch: int, seq_len: int, n_patches: int) -> int:
+        """Device bytes of one padded scoring prefill (vqa_qwen25vl_workspace_bytes), the most score_prompts needs; 0 for invalid sizes."""
+        return int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, batch, seq_len, n_patches))
 
     def generate_workspace_bytes(self, batch: int, seq_len: int, n_patches: int, max_new_tokens: int) -> int:
         """Device bytes of one generation or scored rollout (vqa_qwen25vl_generate_workspace_bytes); 0 for invalid sizes."""

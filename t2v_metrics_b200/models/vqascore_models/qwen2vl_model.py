@@ -7,7 +7,10 @@ score = softmax(last-position logits / temperature)[first answer token]. The ref
 With `max_new_tokens = k > 1`, `forward` and `forward_with_trace` score the answer tokens on a greedy rollout of k tokens, as the
 reference does with one `generate(max_new_tokens=k, output_scores=True)` per sample (qwen2vl_model.py:239-289, :381-487): here the
 pairs run as batched rollouts on the GPU decode loop, with the answer probabilities of every step computed on the device.
-Video inputs (decord / qwen_vl_utils frame sampling) are outside this engine's scope and raise.
+Videos arrive as decoded frame stacks: a 4-D `.npy` [n, h, w, 3] is scored as a video, as the reference's decoder-free path does
+(qwen2vl_model.py:145-153, a list of frames as `{"type": "video"}`), with its frames pre-processed on the device in the same launch as the
+still images of the call, video tokens in the prompt and the processor's `second_per_grid_ts`. Stills and videos mix freely in one call.
+Video files (.mp4, .avi, .mov, .mkv: decoding and fps frame sampling) are outside this engine's scope and raise.
 """
 from __future__ import annotations
 
@@ -30,6 +33,43 @@ QWEN2_VL_MODELS: Dict[str, dict] = {name: dict(model=dict(path=spec["weights"]),
 # its source and exposed as constructor arguments (`min_pixels=`, `max_pixels=`) for other versions.
 QWEN_VL_UTILS_MIN_PIXELS = 4 * 28 * 28
 QWEN_VL_UTILS_MAX_PIXELS = 16384 * 28 * 28
+
+# A frame stack reaches the processor as a list of frames, whose VideoMetadata has fps None, and `VideoMetadata.sampled_fps` is then
+# `self.fps or 24` (transformers 5.5.0 video_utils.py:108-111). Qwen2_5_VLProcessor divides temporal_patch_size by it
+# (processing_qwen2_5_vl.py:103-113), so a stack's second_per_grid_ts is temporal_patch_size / 24 whatever `fps` the caller passes, and
+# the temporal rope step tokens_per_second * int(2 / 24) is 0 (modeling_qwen2_5_vl.py:1019, :1120).
+HF_FRAME_LIST_FPS = 24
+
+_VIDEO_FILES = (".mp4", ".avi", ".mov", ".mkv")
+
+
+def _is_frame_stack(path: str) -> bool:
+    """A 4-D .npy is a decoded video; only its header is read."""
+    import numpy as np
+    return path.lower().endswith(".npy") and np.load(path, mmap_mode="r").ndim == 4
+
+
+def _chunks(n_pairs: int, max_pairs: int, budget: int, workspace_bytes, seq_len: int, sizes: List[int]) -> List[List[int]]:
+    """Pairs in order, in chunks of at most max_pairs, halved while one chunk's workspace_bytes(pairs, seq_len, patch rows) exceeds the
+    budget (a chunk's patch rows are bounded by all of them and by pairs x the largest item)."""
+    chunk = min(max_pairs, n_pairs)
+    while chunk > 1 and workspace_bytes(chunk, seq_len, min(sum(sizes), chunk * max(sizes))) > budget:
+        chunk = (chunk + 1) // 2
+    return [list(range(c0, min(n_pairs, c0 + chunk))) for c0 in range(0, n_pairs, chunk)]
+
+
+def _subset(patches: torch.Tensor, grids, index: List[int], sel: List[int]):
+    """The patch rows and grids of the items the pairs `sel` use, each once, and each pair's item in that subset."""
+    items = sorted({index[i] for i in sel})
+    local = {g: j for j, g in enumerate(items)}
+    if len(items) == len(grids):
+        pix = patches
+    else:
+        offs = [0]
+        for t, h, w in grids:
+            offs.append(offs[-1] + t * h * w)
+        pix = torch.cat([patches[offs[g]:offs[g + 1]] for g in items])
+    return pix, items, [local[index[i]] for i in sel]
 
 
 def _require_rollout_engine(plugin) -> None:
@@ -57,6 +97,10 @@ class Qwen2VLModel(VQAScoreModel):
     # budget: large `max_pixels` images make prompts of thousands of tokens.
     ROLLOUT_MAX_PAIRS = 32
     ROLLOUT_WORKSPACE_BUDGET = 8 << 30
+    # A video makes a prompt of thousands of tokens: a single-prefill scoring or `generate` call with a video is split, by the same halving
+    # rule, into engine calls whose workspace (score_workspace_bytes / generate_workspace_bytes) fits this budget. Calls with still images
+    # only run as one engine call, as they always have.
+    VIDEO_WORKSPACE_BUDGET = 8 << 30
 
     def __init__(self, model_name="qwen2.5-vl-7b", device="cuda", cache_dir=HF_CACHE_DIR, tokenizer=None,
                  state_dict: Optional[Dict[str, torch.Tensor]] = None, config: Optional[Qwen25VLConfig] = None,
@@ -94,30 +138,63 @@ class Qwen2VLModel(VQAScoreModel):
         self._state_dict = None
 
     def load_images(self, image: List[str]):
-        """-> (patches fp32 [sum P, 1176] on the device, [(1, gh, gw), ...])"""
-        if any(p[-4:].lower() in (".mp4", ".avi", ".mov", ".mkv") for p in image):
-            raise NotImplementedError("video inputs are outside the engine's hot-path scope")
-        # PIL decode on the host, everything else (smart_resize, PIL-exact bicubic, normalise, frame duplication, merge-order patch
-        # rows) in ONE device kernel -- bit-identical to qwen_utils.qwen_image_to_patches, the CPU path the reference runs per image
+        """-> (patches fp32 [sum P, 1176] on the device, [(t, gh, gw), ...]): t = 1 for a still image, ceil(n / 2) for a 4-D .npy stack
+        of n frames (a video)."""
+        if any(p[-4:].lower() in _VIDEO_FILES for p in image):
+            raise NotImplementedError("video files need decoding, which is outside the engine's scope: pass the decoded frames as a 4-D "
+                                      ".npy [n, h, w, 3]")
+        # PIL decode on the host, everything else (smart_resize, PIL-exact bicubic, normalise, frame duplication or pairing, merge-order
+        # patch rows) in ONE device kernel -- bit-identical to qwen_utils.qwen_image_to_patches / qwen_video_to_patches, the CPU paths
+        # the reference runs per image / per video
         import numpy as np
         from PIL import Image
-        from ...engine import qwen_preprocess_u8
-        raw = []
+        from ...engine import qwen_preprocess_u8, qwen_preprocess_video_u8
+        raw, video = [], False
         for p in image:
             if p.lower().endswith(".npy"):
-                # the reference's Qwen path takes the array as RGB, no channel flip (qwen2vl_model.py:146-153); 4-D arrays are frame stacks
+                # the reference's Qwen path takes the array as RGB, no channel flip (qwen2vl_model.py:146-153); a 4-D array is a frame
+                # stack, each frame Image.fromarray(frame.astype('uint8'), 'RGB'), scored as a video
                 arr = np.load(p)
                 if arr.ndim == 4:
-                    raise NotImplementedError("4-D .npy frame stacks are video inputs: outside the engine's hot-path scope")
-                if arr.ndim != 3:
+                    arr = np.stack([np.asarray(Image.fromarray(f.astype("uint8"), "RGB"), dtype=np.uint8) for f in arr])
+                    video = True
+                elif arr.ndim == 3:
+                    arr = np.asarray(Image.fromarray(arr.astype("uint8"), "RGB"), dtype=np.uint8)
+                else:
                     raise ValueError(f"Unexpected shape for NumPy array in {p}")
-                arr = np.asarray(Image.fromarray(arr.astype("uint8"), "RGB"), dtype=np.uint8)
             else:
                 with Image.open(p) as im:
                     arr = np.asarray(im.convert("RGB"), dtype=np.uint8)
             raw.append(torch.from_numpy(np.ascontiguousarray(arr)))
-        return qwen_preprocess_u8(raw, self.engine.device, self.cfg.patch_size, self.cfg.temporal_patch_size, self.cfg.spatial_merge_size,
-                                  min_pixels=self.min_pixels, max_pixels=self.max_pixels)
+        pre = qwen_preprocess_video_u8 if video else qwen_preprocess_u8
+        return pre(raw, self.engine.device, self.cfg.patch_size, self.cfg.temporal_patch_size, self.cfg.spatial_merge_size,
+                   min_pixels=self.min_pixels, max_pixels=self.max_pixels)
+
+    def _vision(self, images: List[str]):
+        """Identical paths encoded once: -> (item of every pair, patches, grids, per-item prompt token id, per-item second_per_grid_ts
+        or None when there is no video)."""
+        uniq: Dict[str, int] = {}
+        index = [uniq.setdefault(p, len(uniq)) for p in images]
+        paths = list(uniq.keys())
+        patches, grids = self.load_images(paths)
+        video = [_is_frame_stack(p) for p in paths]
+        tokens = [self.cfg.video_token_id if v else self.cfg.image_token_id for v in video]
+        spg = [self.cfg.temporal_patch_size / HF_FRAME_LIST_FPS if v else 1.0 for v in video] if any(video) else None
+        return index, patches, grids, tokens, spg
+
+    def _memo(self) -> dict:
+        cache = self.__dict__.setdefault("_prompt_cache", {})
+        if len(cache) > 65536:
+            cache.clear()
+        return cache
+
+    def _answer_ids(self, answer: str, cache: dict) -> tuple:
+        ids = cache.get(("answer", answer))
+        if ids is None:
+            ids = cache[("answer", answer)] = tuple(self.tokenizer.encode(answer, add_special_tokens=False))
+        if not ids:
+            raise ValueError("empty answer")
+        return ids
 
     @torch.no_grad()
     def forward_with_trace(self, images: List[str], texts: List[str], fps=None, question_template: str = default_question_template,
@@ -132,15 +209,12 @@ class Qwen2VLModel(VQAScoreModel):
             _require_rollout_engine(self)
             return self._trace_rollout(images, texts, question_template, answer_template, max_new_tokens, temperature, score_position, debug,
                                        repetition_penalty)
-        probs = self.forward(images, texts, fps=fps, question_template=question_template, answer_template=answer_template,
-                             max_new_tokens=max_new_tokens, temperature=temperature, debug=False, repetition_penalty=repetition_penalty)
-        pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
-        ids, top_p = self.engine.topk_last(5, temperature=temperature, repetition_penalty=pen)
-        ids, top_p = ids.cpu().tolist(), top_p.cpu().tolist()
+        assert len(images) == len(texts), "Number of images/videos and texts must match"
+        probs, answer_ids, ids, top_p = self._score(images, texts, question_template, answer_template, temperature, repetition_penalty, 5)
         dec = lambda t: self.tokenizer.decode([t]) if hasattr(self.tokenizer, "decode") else str(t)
         special = {getattr(self.tokenizer, n, None) for n in ("eos_token_id", "bos_token_id", "pad_token_id")} - {None}
         traces = []
-        for b, (p, answer_id) in enumerate(zip(probs.tolist(), self._last_answer_ids)):
+        for b, (p, answer_id) in enumerate(zip(probs.tolist(), answer_ids)):
             generated = ids[b][0]                                   # generate(max_new_tokens=1, do_sample=False) emits the arg-max
             if generated in special:
                 # the reference drops a trailing special token and then has nothing left to score (qwen2vl_model.py:395-419)
@@ -178,43 +252,25 @@ class Qwen2VLModel(VQAScoreModel):
             raise ValueError("max_new_tokens must be at least 1")
         questions = [question_template.format(t) for t in texts]
         answers = [answer_template.format(t) for t in texts]
-        uniq: Dict[str, int] = {}
-        index = [uniq.setdefault(p, len(uniq)) for p in images]
-        patches, grids = self.load_images(list(uniq.keys()))
+        index, patches, grids, tokens, spg = self._vision(images)
         unit = self.cfg.spatial_merge_size ** 2
-        cache = self.__dict__.setdefault("_prompt_cache", {})
-        if len(cache) > 65536:
-            cache.clear()
+        cache = self._memo()
         prompts, answer_ids = [], []
         for q, a, img in zip(questions, answers, index):
             t, gh, gw = grids[img]
-            prompts.append(build_prompt_ids(self.tokenizer, q, t * gh * gw // unit, self.cfg.image_token_id, cache))
-            ids = cache.get(("answer", a))
-            if ids is None:
-                ids = cache[("answer", a)] = tuple(self.tokenizer.encode(a, add_special_tokens=False))
-            if not ids:
-                raise ValueError("empty answer")
-            answer_ids.append(list(ids))
+            prompts.append(build_prompt_ids(self.tokenizer, q, t * gh * gw // unit, tokens[img], cache))
+            answer_ids.append(list(self._answer_ids(a, cache)))
         eos = self._eos_ids()
         special = {getattr(self.tokenizer, n, None) for n in ("eos_token_id", "bos_token_id", "pad_token_id")} - {None}
-        sizes = [t * h * w for t, h, w in grids]
-        offs = [0]
-        for s in sizes:
-            offs.append(offs[-1] + s)
-        chunk = min(self.ROLLOUT_MAX_PAIRS, len(prompts))
-        seq_len = max(len(p) for p in prompts)
-        while chunk > 1 and self.engine.generate_workspace_bytes(chunk, seq_len, min(offs[-1], chunk * max(sizes)),
-                                                                 max_new_tokens) > self.ROLLOUT_WORKSPACE_BUDGET:
-            chunk = (chunk + 1) // 2
+        ws = lambda b, s, p: self.engine.generate_workspace_bytes(b, s, p, max_new_tokens)
         results = []
-        for c0 in range(0, len(prompts), chunk):
-            sel = list(range(c0, min(len(prompts), c0 + chunk)))
-            imgs = sorted({index[i] for i in sel})
-            local = {g: j for j, g in enumerate(imgs)}
-            pix = patches if len(imgs) == len(grids) else torch.cat([patches[offs[g]:offs[g + 1]] for g in imgs])
-            out = self.engine.rollout_scores(pix, [grids[g] for g in imgs], [prompts[i] for i in sel], [answer_ids[i] for i in sel],
+        for sel in _chunks(len(prompts), self.ROLLOUT_MAX_PAIRS, self.ROLLOUT_WORKSPACE_BUDGET, ws, max(len(p) for p in prompts),
+                           [t * h * w for t, h, w in grids]):
+            pix, items, local = _subset(patches, grids, index, sel)
+            video = {} if spg is None else dict(second_per_grid_ts=[spg[g] for g in items])
+            out = self.engine.rollout_scores(pix, [grids[g] for g in items], [prompts[i] for i in sel], [answer_ids[i] for i in sel],
                                              max_new_tokens, eos, temperature=temperature, repetition_penalty=repetition_penalty,
-                                             top_k=top_k, image_of_sample=[local[index[i]] for i in sel])
+                                             top_k=top_k, image_of_sample=local, **video)
             for b, i in enumerate(sel):
                 r = qwen_host.rollout_answer_score(out["tokens"][b], out["logp"][b], answer_ids[i], special, mode)
                 r.update(tokens=out["tokens"][b], answer_ids=answer_ids[i])
@@ -254,32 +310,72 @@ class Qwen2VLModel(VQAScoreModel):
         """Greedy text generation, the reference's Qwen2VLModel.generate (qwen2vl_model.py:495-563) with its default temperature 0: per
         sample, the chat prompt of the raw text and the image, generate(do_sample=False) under the checkpoint's repetition penalty, the
         prompt cut off, decoded with skip_special_tokens and stripped. Here the whole batch is one prefill and one decode loop on the
-        device; identical images are encoded once. Sampling (temperature > 0 or do_sample=True, top-p) is not implemented."""
+        device (a call with a video: as few as fit VIDEO_WORKSPACE_BUDGET); identical paths are encoded once. `fps` does not change the
+        output for a .npy frame stack (see HF_FRAME_LIST_FPS). Sampling (temperature > 0 or do_sample=True, top-p) is not implemented."""
         assert len(images) == len(texts), "Number of images/videos and texts must match"
         if do_sample is None:
             do_sample = temperature > 0
         if do_sample or temperature > 0:
             raise NotImplementedError("only greedy decoding is supported (temperature=0.0, do_sample=False); top-p sampling is not implemented")
-        uniq: Dict[str, int] = {}
-        index = [uniq.setdefault(p, len(uniq)) for p in images]
-        patches, grids = self.load_images(list(uniq.keys()))
+        index, patches, grids, tokens, spg = self._vision(images)
         unit = self.cfg.spatial_merge_size ** 2
-        cache = self.__dict__.setdefault("_prompt_cache", {})
-        if len(cache) > 65536:
-            cache.clear()
+        cache = self._memo()
         prompts = []
         for text, img in zip(texts, index):
             t, gh, gw = grids[img]
-            prompts.append(build_prompt_ids(self.tokenizer, text, t * gh * gw // unit, self.cfg.image_token_id, cache))
+            prompts.append(build_prompt_ids(self.tokenizer, text, t * gh * gw // unit, tokens[img], cache))
         eos = self._eos_ids() if eos_token_ids is None else [int(e) for e in eos_token_ids]
-        ids = self.engine.generate_prompts(patches, grids, prompts, max_new_tokens, eos, image_of_sample=index,
-                                           repetition_penalty=self.repetition_penalty)
+        ws = lambda b, s, p: self.engine.generate_workspace_bytes(b, s, p, max_new_tokens)
+        ids = []
+        for sel in self._prefill_chunks(prompts, grids, spg, ws):
+            pix, items, local = _subset(patches, grids, index, sel)
+            video = {} if spg is None else dict(second_per_grid_ts=[spg[g] for g in items])
+            ids += self.engine.generate_prompts(pix, [grids[g] for g in items], [prompts[i] for i in sel], max_new_tokens, eos,
+                                                image_of_sample=local, repetition_penalty=self.repetition_penalty, **video)
         return [self.tokenizer.decode(x, skip_special_tokens=True, clean_up_tokenization_spaces=False).strip() for x in ids]
+
+    def _prefill_chunks(self, prompts, grids, spg, workspace_bytes) -> List[List[int]]:
+        """All pairs in one engine call without a video (spg None); with one, chunks under VIDEO_WORKSPACE_BUDGET."""
+        if spg is None:
+            return [list(range(len(prompts)))]
+        return _chunks(len(prompts), len(prompts), self.VIDEO_WORKSPACE_BUDGET, workspace_bytes, max(len(p) for p in prompts),
+                       [t * h * w for t, h, w in grids])
+
+    def _score(self, images, texts, question_template, answer_template, temperature, repetition_penalty, top_k):
+        """Single-prefill scores of the first answer token -> (probs fp32 CPU [n], answer ids, and with top_k > 0 the top-k ids / probs of
+        the last position as lists, else None, None)."""
+        questions = [question_template.format(t) for t in texts]
+        answers = [answer_template.format(t) for t in texts]
+        index, patches, grids, tokens, spg = self._vision(images)
+        unit = self.cfg.spatial_merge_size ** 2
+        prompts, answer_ids = [], []
+        cache = self._memo()
+        for q, a, img in zip(questions, answers, index):
+            t, gh, gw = grids[img]
+            prompts.append(build_prompt_ids(self.tokenizer, q, t * gh * gw // unit, tokens[img], cache))
+            # one generated position => the reference truncates a multi-token answer to its first token ("Generated 1 tokens but need n,
+            # adjusting", qwen2vl_model.py:259-263) and the geometric mean over one token is that token's probability
+            answer_ids.append(self._answer_ids(a, cache)[0])
+        pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
+        probs, top_ids, top_p = [], [], []
+        for sel in self._prefill_chunks(prompts, grids, spg, lambda b, s, p: self.engine.score_workspace_bytes(b, s, p)):
+            pix, items, local = _subset(patches, grids, index, sel)
+            video = {} if spg is None else dict(second_per_grid_ts=[spg[g] for g in items])
+            probs.append(self.engine.score_prompts(pix, [grids[g] for g in items], [prompts[i] for i in sel], [answer_ids[i] for i in sel],
+                                                   image_of_sample=local, temperature=temperature, repetition_penalty=pen, **video).float().cpu())
+            if top_k:
+                ids, p = self.engine.topk_last(top_k, temperature=temperature, repetition_penalty=pen)
+                top_ids += ids.cpu().tolist()
+                top_p += p.cpu().tolist()
+        return torch.cat(probs), answer_ids, (top_ids if top_k else None), (top_p if top_k else None)
 
     @torch.no_grad()
     def forward(self, images: List[str], texts: List[str], fps=None, question_template: str = default_question_template,
                 answer_template: str = default_answer_template, max_new_tokens: int = 1, temperature: float = 1.0,
                 debug: bool = False, repetition_penalty: Optional[float] = None) -> torch.Tensor:
+        """Scores of (image or video, text) pairs. A 4-D .npy is a video; `fps` is accepted and does not change its score, as in the
+        reference on transformers 5.5.0, whose processor takes a frame list's rate to be 24 fps whatever is passed (HF_FRAME_LIST_FPS).
+        A call with a video runs as few single-prefill engine calls as fit VIDEO_WORKSPACE_BUDGET; one with still images only, as one."""
         assert len(images) == len(texts), "Number of images/videos and texts must match"
         if max_new_tokens != 1:
             # the reference scores answer token i on the scores of step len(scores) - n + i (- 1 after a trailing special token) of its own
@@ -288,28 +384,4 @@ class Qwen2VLModel(VQAScoreModel):
             pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
             return torch.tensor([r["score"] for r in self._rollout(images, texts, question_template, answer_template, max_new_tokens,
                                                                     temperature, pen, "forward", 0)], dtype=torch.float32)
-        questions = [question_template.format(t) for t in texts]
-        answers = [answer_template.format(t) for t in texts]
-        uniq: Dict[str, int] = {}
-        index = [uniq.setdefault(p, len(uniq)) for p in images]
-        patches, grids = self.load_images(list(uniq.keys()))
-        unit = self.cfg.spatial_merge_size ** 2
-        prompts, answer_ids = [], []
-        cache = self.__dict__.setdefault("_prompt_cache", {})
-        if len(cache) > 65536:
-            cache.clear()
-        for q, a, img in zip(questions, answers, index):
-            t, gh, gw = grids[img]
-            prompts.append(build_prompt_ids(self.tokenizer, q, t * gh * gw // unit, self.cfg.image_token_id, cache))
-            ids = cache.get(("answer", a))
-            if ids is None:
-                ids = cache[("answer", a)] = tuple(self.tokenizer.encode(a, add_special_tokens=False))
-            if not ids:
-                raise ValueError("empty answer")
-            # one generated position => the reference truncates a multi-token answer to its first token ("Generated 1 tokens but need n,
-            # adjusting", qwen2vl_model.py:259-263) and the geometric mean over one token is that token's probability
-            answer_ids.append(ids[0])
-        self._last_answer_ids = list(answer_ids)
-        probs = self.engine.score_prompts(patches, grids, prompts, answer_ids, image_of_sample=index, temperature=temperature,
-                                          repetition_penalty=self.repetition_penalty if repetition_penalty is None else repetition_penalty)
-        return probs.float().cpu()
+        return self._score(images, texts, question_template, answer_template, temperature, repetition_penalty, 0)[0]
