@@ -4,9 +4,14 @@
 //     tile-by-tile from HBM/L2 by TMA into a 128B-swizzled shared-memory ring;
 //   * CTA tile 128 x BLOCK_N: warpgroup 0 is the TMA producer, warpgroups 1 and 2 each own 64 rows of the tile and accumulate
 //     them in registers with wgmma (m64 x BLOCK_N x k16, both operands read from shared memory);
-//   * the epilogue stages 64-column slices of the accumulators through shared memory so that one thread owns one row's 32
-//     consecutive columns, and applies the fused epilogue (bias / activation / gated-GELU / residual add / online log-sum-exp for
-//     the lm_head) before the only write to HBM. The producer keeps loading the next tile's operands meanwhile.
+//   * dense bf16 outputs (TMA_EPI): each consumer thread applies the fused epilogue (bias / activation / gated GELU or SiLU / residual
+//     add) to the accumulator columns it holds, writes the bf16 results into a 128B-swizzled 64-row box with stmatrix, and a thread of
+//     warpgroup 0 stores the box with TMA. That thread also TMA-loads the bf16 residual of each box ahead of the consumers, so the
+//     consumers start the next tile's main loop without waiting on HBM in either direction;
+//   * the other launches (fp32 C, split-K partials, batched GEMMs, scattered column groups, RMSNorm partial sums, the lm_head's online
+//     log-sum-exp) stage 64-column fp32 slices of the accumulators through shared memory so that one thread owns one row's 32
+//     consecutive columns before the only write to HBM.
+//   The producer keeps loading the next tile's operands during either epilogue.
 //
 // Replaces the cuBLAS bf16 GEMMs that the reference reaches through nn.Linear
 // (transformers/models/t5/modeling_t5.py:109-111,178-181; transformers/models/clip/modeling_clip.py:296-299,344-345).
@@ -89,10 +94,11 @@ struct GemmConfig {
     static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
     static constexpr int NUM_THREADS = 384;       // warpgroup 0: TMA; warpgroups 1, 2: wgmma + epilogue
-    // epilogue staging: per consumer warpgroup 64 rows x EPI_COLS fp32 accumulators, rows padded by 4 floats (conflict-free float4 reads)
+    // epilogue staging area, the same size on both epilogue paths: per consumer warpgroup either one 64 x EPI_COLS fp32 slice of the
+    // accumulators (staged path; 16-byte chunks XOR-swizzled by row, see stg_index), or two bf16 output boxes of 64 rows x <= 64 columns
+    // (TMA-store path)
     static constexpr int EPI_COLS = BLOCK_N >= 64 ? 64 : 32;
-    static constexpr int EPI_LD = EPI_COLS + 4;
-    static constexpr int EPI_BYTES = 2 * 64 * EPI_LD * 4;
+    static constexpr int EPI_BYTES = 2 * 64 * EPI_COLS * 4;
     // one thread per (row, 32-column half of a staged slice): LSE_PARTS partial results per row and tile
     static constexpr int LSE_PARTS = EPI_COLS / 32;
     static constexpr int SMEM_LIMIT = 227 * 1024;  // H100: dynamic shared memory per block
@@ -102,8 +108,21 @@ struct GemmConfig {
     static_assert(BLOCK_N >= 32 && BLOCK_N <= 256 && (BLOCK_N & (BLOCK_N - 1)) == 0, "BLOCK_N must be 32..256, pow2");
     static_assert(B_HALF_ROWS % 8 == 0, "B half tile must hold whole 8-row swizzle atoms");
     static_assert(STAGES >= 3, "pipeline too shallow");
+    // the main loop keeps one wgmma group in flight, which holds two slots: a fourth stage gives the 256-wide tile's producer two k blocks of look-ahead
+    static_assert(BLOCK_N != 256 || STAGES == 4, "the 256-wide tile runs a four-stage ring on both epilogue paths");
     static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory");
+    // staged path: float index of (row r, column c) of a warpgroup's fp32 slice. Chunk c / 4 of row r sits at chunk (c / 4) ^ s(r) with
+    // s(r) = 2 (r % 4) + (r / 4) % 2: the float2 writes in accumulator layout (rows r..r+3 of 8-aligned groups, two adjacent chunks per row)
+    // and the float4 row reads (8 consecutive rows, one chunk) are both free of bank conflicts.
+    __device__ static __forceinline__ int stg_index(int r, int c) {
+        return r * EPI_COLS + ((((c >> 2) ^ (((r & 3) << 1) | ((r >> 2) & 1)))) << 2) + (c & 3);
+    }
 };
+
+// TMA-store epilogue: columns of one bf16 output box (64 rows per consumer warpgroup). Gated epilogues write BLOCK_N / 2 columns per tile.
+__host__ __device__ constexpr int gemm_out_box_cols(int block_n, int epi) {
+    return (epi_is_gated(epi) ? block_n / 2 : block_n) >= 64 ? 64 : 32;
+}
 
 __device__ __forceinline__ float act_quick_gelu(float x) { return __fdividef(x, 1.0f + __expf(-1.702f * x)); }
 __device__ __forceinline__ float act_silu(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
@@ -140,36 +159,62 @@ __device__ __forceinline__ void static_for_impl(F&& f) {
 template <int N, typename F>
 __device__ __forceinline__ void static_for(F&& f) { static_for_impl<0, N>(f); }
 
-template <int BLOCK_N, int EPI>
+// TMA_EPI: the TMA-store epilogue (dense bf16 C, not batched); tmap_c maps C as [M, n_out] with row stride ldc, tmap_r the bf16 residual
+// the same way (both boxes of 64 rows x gemm_out_box_cols). Otherwise the staged epilogue, which serves EPI_STORE and EPI_LSE only, and
+// the two maps are not read.
+template <int BLOCK_N, int EPI, bool TMA_EPI>
 __global__ void __launch_bounds__(384, 1)
 gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                      const GemmParams p) {
+                      const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r, const GemmParams p) {
     using Cfg = GemmConfig<BLOCK_N>;
     static_assert(!epi_is_gated(EPI) || BLOCK_N >= 64, "gated epilogue pairs two >=32-column half tiles");
+    static_assert(TMA_EPI ? EPI != EPI_LSE : (EPI == EPI_STORE || EPI == EPI_LSE), "the staged epilogue serves plain stores and the lm_head");
     pdl_launch_dependents();
     constexpr int STAGES = Cfg::STAGES;
     constexpr int BLOCK_M = Cfg::BLOCK_M;
     constexpr int BLOCK_K = Cfg::BLOCK_K;
-    constexpr int EPI_LD = Cfg::EPI_LD;
+    constexpr int OUT_TILE_COLS = epi_is_gated(EPI) ? BLOCK_N / 2 : BLOCK_N;
+    constexpr int BOX_COLS = gemm_out_box_cols(BLOCK_N, EPI);
+    constexpr int BOX_ROW_BYTES = BOX_COLS * 2;                  // 128 B (SWIZZLE_128B) or 64 B (SWIZZLE_64B)
+    constexpr int BOX_BYTES = 64 * BOX_ROW_BYTES;
+    constexpr int NBOX = OUT_TILE_COLS / BOX_COLS;               // boxes per consumer warpgroup and tile
+    static_assert(4 * BOX_BYTES <= Cfg::EPI_BYTES, "two boxes per consumer warpgroup fit the staging area");
+    static_assert((2 * STAGES + 8) * 8 <= 256, "mbarriers fit their 256 bytes");
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;                                      // [STAGES][128 x 64 bf16]
     uint8_t* smem_b = smem + STAGES * Cfg::A_STAGE_BYTES;        // [STAGES][BLOCK_N x 64 bf16]
-    float* smem_epi = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);   // [2][64][EPI_LD]
+    uint8_t* smem_epi = smem + STAGES * Cfg::STAGE_BYTES;        // staged: [2][64][EPI_COLS] fp32; TMA store: [2 warpgroups][2][BOX_BYTES]
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::EPI_BYTES);
     uint64_t* full_bar = bars;                 // [STAGES]
     uint64_t* empty_bar = bars + STAGES;       // [STAGES]
+    // TMA-store epilogue, box buffer i = 2 * (consumer warpgroup) + (box count & 1):
+    //   box_free[i]  (count 1)  buffer i may be written: holds the box's residual (expect_tx) or its previous store has read it (plain arrive)
+    //   box_ready[i] (count 4)  each consumer warp has written its rows of the box into buffer i
+    uint64_t* box_free = bars + 2 * STAGES;    // [4]
+    uint64_t* box_ready = bars + 2 * STAGES + 4;   // [4]
 
     const uint32_t wg = threadIdx.x >> 7;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_b);
+        if constexpr (TMA_EPI) {
+            tma_prefetch_desc(&tmap_c);
+            tma_prefetch_desc(&tmap_r);
+        }
 #pragma unroll
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);    // the producer's expect_tx
             mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
+        }
+        if constexpr (TMA_EPI) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                mbar_init(&box_free[i], 1);
+                mbar_init(&box_ready[i], 4);
+            }
         }
         fence_barrier_init();
     }
@@ -232,23 +277,87 @@ gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
                 }
             }
         }
+        if constexpr (TMA_EPI) {
+            // ===================== box thread of consumer warpgroup cw (lane 0 of warp 1 + cw) =====================
+            // Walks the same tiles as its consumer warpgroup; box q (q = 0, 1, ... over all of them) uses buffer b = q & 1 for the
+            // u = q >> 1 th time. Protocol of buffer b (both barriers complete one phase per use, so use u waits on parity u & 1):
+            //   box thread, box q:  if q >= 2: wait box_ready[b] (parity of use u - 1), TMA-store box q - 2, wait until the store
+            //                       has read the buffer; then complete box_free[b] for use u -- with the residual's expect_tx and its
+            //                       TMA load, or with a plain arrive when there is nothing to load;
+            //   consumers,  box q:  wait box_free[b] (parity u & 1), read the residual, write the results in place, fence.proxy.async,
+            //                       one arrive per warp on box_ready[b].
+            // box_free[b] for use u + 1 needs box_ready[b] of use u, which needs box_free[b] of use u: neither barrier can run a phase
+            // ahead of the wait that reads it. After the last box the thread stores the (up to) two pending boxes and waits for all of
+            // its stores to complete before the CTA exits.
+            if (threadIdx.x == 32 || threadIdx.x == 64) {
+                const int cw = (int)(threadIdx.x >> 5) - 1;
+                const int n_out = epi_is_gated(EPI) ? p.N / 2 : p.N;
+                const bool load_residual = !epi_is_gated(EPI) && p.residual != nullptr;
+                uint8_t* buf = smem_epi + cw * 2 * BOX_BYTES;
+                uint64_t* free_bar = box_free + cw * 2;
+                uint64_t* ready_bar = box_ready + cw * 2;
+                auto store_box = [&](int q, int c0, int r0) {
+                    mbar_wait(&ready_bar[q & 1], (uint32_t)(q >> 1) & 1u);
+                    if (r0 < p.M && c0 < n_out) {   // a box wholly outside C is not stored
+                        tma_store_2d(&tmap_c, buf + (q & 1) * BOX_BYTES, c0, r0);
+                        bulk_commit_group();
+                        bulk_wait_group_read<0>();
+                    }
+                };
+                int q = 0;
+                int c0_1 = 0, r0_1 = 0, c0_2 = 0, r0_2 = 0;   // boxes q - 1 and q - 2
+                for (int t = worker; t < num_tiles; t += num_workers) {
+                    int batch, m_blk, n_blk;
+                    tile_coords(t, batch, m_blk, n_blk);
+                    const int r0 = m_blk * BLOCK_M + cw * 64;
+                    for (int s = 0; s < NBOX; ++s, ++q) {
+                        const int c0 = n_blk * OUT_TILE_COLS + s * BOX_COLS;
+                        if (q >= 2) store_box(q - 2, c0_2, r0_2);
+                        if (load_residual && r0 < p.M && c0 < n_out) {
+                            mbar_arrive_expect_tx(&free_bar[q & 1], BOX_BYTES);
+                            tma_load_2d(buf + (q & 1) * BOX_BYTES, &tmap_r, &free_bar[q & 1], c0, r0);
+                        } else {
+                            mbar_arrive(&free_bar[q & 1]);
+                        }
+                        c0_2 = c0_1; r0_2 = r0_1; c0_1 = c0; r0_1 = r0;
+                    }
+                }
+                if (q >= 2) store_box(q - 2, c0_2, r0_2);
+                if (q >= 1) store_box(q - 1, c0_1, r0_1);
+                bulk_wait_group<0>();
+            }
+        }
     } else {
         // ===================== consumers: wgmma main loop, then the epilogue of the tile =====================
         regs_alloc<232>();
         const int cw = (int)wg - 1;                  // rows [64 cw, 64 cw + 64) of every tile
         const int tid = (int)threadIdx.x - 128 * (int)wg;
         const int lane = tid & 31;
-        float* stg = smem_epi + cw * 64 * EPI_LD;
+        float* stg = reinterpret_cast<float*>(smem_epi) + cw * 64 * Cfg::EPI_COLS;
         // accumulator fragment of this thread: rows fr and fr + 8, columns 8j + fc + {0, 1}
         const int fr = (tid >> 5) * 16 + (lane >> 2);
         const int fc = (lane & 3) * 2;
-        // epilogue ownership: row er of the warpgroup's 64, 32-column half esub of each staged slice
+        // staged epilogue ownership: row er of the warpgroup's 64, 32-column half esub of each staged slice
         const int er = tid & 63;
         const int esub = tid >> 6;
-        constexpr int OUT_TILE_COLS = epi_is_gated(EPI) ? BLOCK_N / 2 : BLOCK_N;
-        // staged slices per tile: EPI_COLS accumulator columns, or (gated) 32 gate + the matching 32 up columns
-        constexpr int NSLICE = epi_is_gated(EPI) ? OUT_TILE_COLS / 32 : BLOCK_N / Cfg::EPI_COLS;
+        constexpr int NSLICE = BLOCK_N / Cfg::EPI_COLS;   // staged slices per tile
         const bool e_active = esub < Cfg::LSE_PARTS;
+        // TMA-store epilogue: this lane's row address in the x4 matrix moves (matrix i = lane / 8: rows +8 (i & 1), 8-column chunk +(i >> 1))
+        const int mx_row = (tid >> 5) * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+        const int mx_chunk = lane >> 4;
+        uint8_t* box_buf = smem_epi + cw * 2 * BOX_BYTES;
+        int box_q = 0;                               // boxes this warpgroup has written (see the box thread's protocol)
+        // fused RMSNorm of the A rows (consumer side): rsqrt(mean of squares + eps) of row m
+        auto row_scale_of = [&](int m) {
+            if (!p.ssq_in || m >= p.M) return 1.0f;
+            const float* sp = p.ssq_in + (size_t)m * p.ssq_in_parts;
+            float ssum = 0.f;
+            for (int i = 0; i < p.ssq_in_parts; i += 4) {
+                const float4 v4 = __ldg(reinterpret_cast<const float4*>(sp + i));
+                ssum += (v4.x + v4.y) + (v4.z + v4.w);
+            }
+            return rsqrtf(ssum * p.ssq_inv_dim + p.ssq_eps);
+        };
         float acc[BLOCK_N / 2];
         int stage = 0;
         uint32_t phase = 0;
@@ -277,70 +386,34 @@ gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
             fence_regs(acc);
             if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
-            // ---------------- epilogue
-            const long long c_off = (long long)batch * p.c_batch_stride;
-            const int m = m_blk * BLOCK_M + cw * 64 + er;
-            const bool row_ok = m < p.M;
-            float row_scale = 1.0f;     // fused RMSNorm of the A rows (consumer side)
-            if (p.ssq_in && row_ok) {
-                const float* sp = p.ssq_in + (size_t)m * p.ssq_in_parts;
-                float ssum = 0.f;
-                for (int i = 0; i < p.ssq_in_parts; i += 4) {
-                    const float4 v4 = __ldg(reinterpret_cast<const float4*>(sp + i));
-                    ssum += (v4.x + v4.y) + (v4.z + v4.w);
-                }
-                row_scale = rsqrtf(ssum * p.ssq_inv_dim + p.ssq_eps);
-            }
-            // accumulator columns [src, src + 8 * n8) -> staging columns [dst, ...) of this warpgroup's 64 rows
-            auto stage_out = [&](auto src_c, int dst, auto n8_c) {
-                constexpr int src = decltype(src_c)::value;
-                constexpr int n8 = decltype(n8_c)::value;
-#pragma unroll
-                for (int j = 0; j < n8; ++j) {
-                    const int b = (src / 8 + j) * 4;
-                    *reinterpret_cast<float2*>(stg + fr * EPI_LD + dst + 8 * j + fc) = make_float2(acc[b], acc[b + 1]);
-                    *reinterpret_cast<float2*>(stg + (fr + 8) * EPI_LD + dst + 8 * j + fc) = make_float2(acc[b + 2], acc[b + 3]);
-                }
-            };
-            auto load_row = [&](int col, auto n_c, uint32_t* v) {
-                constexpr int n = decltype(n_c)::value;
-#pragma unroll
-                for (int i = 0; i < n; i += 4) {
-                    const float4 f = *reinterpret_cast<const float4*>(stg + er * EPI_LD + col + i);
-                    v[i] = __float_as_uint(f.x); v[i + 1] = __float_as_uint(f.y); v[i + 2] = __float_as_uint(f.z); v[i + 3] = __float_as_uint(f.w);
-                }
-            };
-            float run_max = -INFINITY, run_sum = 0.f;   // EPI_LSE
-            float ssq_acc = 0.f;                        // producer side of the fused RMSNorm: sum of squares of the bf16 values this thread stores
-            const int label = (EPI == EPI_LSE && row_ok) ? p.labels[m] : -1;
-            static_for<NSLICE>([&](auto s_c) {
-                constexpr int s = decltype(s_c)::value;
-                named_bar_sync(1 + cw, 128);            // the previous slice has been read
-                if constexpr (epi_is_gated(EPI)) {
-                    stage_out(std::integral_constant<int, s * 32>{}, 0, std::integral_constant<int, 4>{});
-                    stage_out(std::integral_constant<int, OUT_TILE_COLS + s * 32>{}, 32, std::integral_constant<int, 4>{});
-                } else {
-                    stage_out(std::integral_constant<int, s * Cfg::EPI_COLS>{}, 0, std::integral_constant<int, Cfg::EPI_COLS / 8>{});
-                }
-                named_bar_sync(1 + cw, 128);
-                if (!e_active) return;
-                if constexpr (epi_is_gated(EPI)) {
-                    // this thread: output columns [s * 32 + 16 esub, + 16) of the tile
-                    uint32_t g[16], u[16];
-                    load_row(esub * 16, std::integral_constant<int, 16>{}, g);
-                    load_row(32 + esub * 16, std::integral_constant<int, 16>{}, u);
-                    const int n_out0 = n_blk * OUT_TILE_COLS + s * 32 + esub * 16;
-                    if (row_ok) {
-                        __nv_bfloat16* crow = p.C + c_off + (size_t)m * p.ldc + n_out0;
-#pragma unroll
-                        for (int j = 0; j < 2; ++j) {
-                            uint32_t w[4];
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                float g0 = __uint_as_float(g[j * 8 + 2 * e]) * row_scale, g1 = __uint_as_float(g[j * 8 + 2 * e + 1]) * row_scale;
-                                float u0 = __uint_as_float(u[j * 8 + 2 * e]) * row_scale, u1 = __uint_as_float(u[j * 8 + 2 * e + 1]) * row_scale;
+            if constexpr (TMA_EPI) {
+                // ---------------- TMA-store epilogue: the math in the accumulator layout, bf16 results into the box buffers
+                const int m0 = m_blk * BLOCK_M + cw * 64 + fr;
+                const float rs[2] = {row_scale_of(m0), row_scale_of(m0 + 8)};
+                static_for<NBOX>([&](auto s_c) {
+                    constexpr int s = decltype(s_c)::value;
+                    const int b = box_q & 1;
+                    uint8_t* box = box_buf + b * BOX_BYTES;
+                    mbar_wait(&box_free[cw * 2 + b], (uint32_t)(box_q >> 1) & 1u);
+                    static_for<BOX_COLS / 16>([&](auto t_c) {
+                        constexpr int t = decltype(t_c)::value;
+                        // swizzled address of (row mx_row, 16-byte chunk 2t + mx_chunk): the box's 16-byte chunk c of row r sits at chunk
+                        // c ^ ((row byte offset / 128) % (BOX_ROW_BYTES / 16)), the pattern TMA's 128B / 64B swizzle reads and writes
+                        const uint32_t off = (uint32_t)(mx_row * BOX_ROW_BYTES + (2 * t + mx_chunk) * 16);
+                        const uint32_t addr = smem_u32(box) + (off ^ (((off >> 7) & (BOX_ROW_BYTES / 16 - 1)) << 4));
+                        uint32_t v[4] = {0u, 0u, 0u, 0u};
+                        if (!epi_is_gated(EPI) && p.residual) ldmatrix_x4(addr, v);   // the TMA-loaded residual of the same elements
+                        static_for<4>([&](auto k_c) {
+                            constexpr int k = decltype(k_c)::value;
+                            constexpr int jo = s * (BOX_COLS / 8) + 2 * t + (k >> 1);   // output 8-column chunk of the tile
+                            constexpr int h = k & 1;                                   // row fr + 8h
+                            constexpr int ia = 4 * jo + 2 * h;                         // acc index of the pair's first column
+                            const int n = n_blk * OUT_TILE_COLS + 8 * jo + fc;        // output column of the pair
+                            if constexpr (epi_is_gated(EPI)) {
+                                // gate column n at acc[ia], its up column (BLOCK_N / 2 accumulator columns further) at acc[ia + BLOCK_N / 4]
+                                float g0 = acc[ia] * rs[h], g1 = acc[ia + 1] * rs[h];
+                                float u0 = acc[ia + BLOCK_N / 4] * rs[h], u1 = acc[ia + BLOCK_N / 4 + 1] * rs[h];
                                 if (p.bias) {   // [gate bias | up bias], `gate_up_offset` apart like the weight rows
-                                    const int n = n_out0 + j * 8 + 2 * e;
                                     if (n < p.N / 2) {
                                         const float2 bg = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.bias + n));
                                         const float2 bu = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.bias + p.gate_up_offset + n));
@@ -358,13 +431,68 @@ gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
                                     h0 = bf16_round(act_silu(g0)) * u0;
                                     h1 = bf16_round(act_silu(g1)) * u1;
                                 }
-                                w[e] = pack_bf16x2(h0, h1);
+                                v[k] = pack_bf16x2(h0, h1);
+                            } else {
+                                float f0 = acc[ia] * rs[h], f1 = acc[ia + 1] * rs[h];
+                                const float2 bb = (p.bias && n < p.N) ? unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)))
+                                                                      : make_float2(0.f, 0.f);
+                                f0 += bb.x; f1 += bb.y;
+                                float y[2] = {bf16_round(f0), bf16_round(f1)};   // the Linear's bf16 output in the reference
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    if constexpr (EPI == EPI_QUICK_GELU) y[e] = act_quick_gelu_bf16_ops(y[e]);
+                                    if constexpr (EPI == EPI_GELU_ERF) y[e] = act_gelu_erf(y[e]);
+                                    if constexpr (EPI == EPI_RELU) y[e] = fmaxf(y[e], 0.f);
+                                }
+                                const float2 r = unpack_bf16x2(v[k]);   // zero without a residual
+                                f0 = y[0]; f1 = y[1];
+                                f0 += r.x; f1 += r.y;
+                                v[k] = pack_bf16x2(f0, f1);
                             }
-                            if (n_out0 + j * 8 < p.N / 2)
-                                *reinterpret_cast<uint4*>(crow + j * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-                        }
-                    }
-                } else {
+                        });
+                        stmatrix_x4(addr, v);
+                    });
+                    fence_proxy_async_shared();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&box_ready[cw * 2 + b]);
+                    ++box_q;
+                });
+                continue;
+            }
+            // ---------------- staged epilogue
+            const long long c_off = (long long)batch * p.c_batch_stride;
+            const int m = m_blk * BLOCK_M + cw * 64 + er;
+            const bool row_ok = m < p.M;
+            const float row_scale = row_scale_of(m);
+            // accumulator columns [src, src + 8 * n8) -> staging columns [dst, ...) of this warpgroup's 64 rows
+            auto stage_out = [&](auto src_c, int dst, auto n8_c) {
+                constexpr int src = decltype(src_c)::value;
+                constexpr int n8 = decltype(n8_c)::value;
+#pragma unroll
+                for (int j = 0; j < n8; ++j) {
+                    const int b = (src / 8 + j) * 4;
+                    *reinterpret_cast<float2*>(stg + Cfg::stg_index(fr, dst + 8 * j + fc)) = make_float2(acc[b], acc[b + 1]);
+                    *reinterpret_cast<float2*>(stg + Cfg::stg_index(fr + 8, dst + 8 * j + fc)) = make_float2(acc[b + 2], acc[b + 3]);
+                }
+            };
+            auto load_row = [&](int col, auto n_c, uint32_t* v) {
+                constexpr int n = decltype(n_c)::value;
+#pragma unroll
+                for (int i = 0; i < n; i += 4) {
+                    const float4 f = *reinterpret_cast<const float4*>(stg + Cfg::stg_index(er, col + i));
+                    v[i] = __float_as_uint(f.x); v[i + 1] = __float_as_uint(f.y); v[i + 2] = __float_as_uint(f.z); v[i + 3] = __float_as_uint(f.w);
+                }
+            };
+            float run_max = -INFINITY, run_sum = 0.f;   // EPI_LSE
+            float ssq_acc = 0.f;                        // producer side of the fused RMSNorm: sum of squares of the bf16 values this thread stores
+            const int label = (EPI == EPI_LSE && row_ok) ? p.labels[m] : -1;
+            static_for<NSLICE>([&](auto s_c) {
+                constexpr int s = decltype(s_c)::value;
+                named_bar_sync(1 + cw, 128);            // the previous slice has been read
+                stage_out(std::integral_constant<int, s * Cfg::EPI_COLS>{}, 0, std::integral_constant<int, Cfg::EPI_COLS / 8>{});
+                named_bar_sync(1 + cw, 128);
+                if (!e_active) return;
+                {
                     uint32_t v[32];
                     load_row(esub * 32, std::integral_constant<int, 32>{}, v);
                     const int nc = n_blk * BLOCK_N + s * Cfg::EPI_COLS + esub * 32;   // first column of this thread's 32
@@ -439,13 +567,7 @@ gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
                                         f[4] += b2.x; f[5] += b2.y; f[6] += b3.x; f[7] += b3.y;
                                     }
 #pragma unroll
-                                    for (int e = 0; e < 8; ++e) {
-                                        float y = bf16_round(f[e]);   // the Linear's bf16 output in the reference
-                                        if constexpr (EPI == EPI_QUICK_GELU) y = act_quick_gelu_bf16_ops(y);
-                                        if constexpr (EPI == EPI_GELU_ERF) y = act_gelu_erf(y);
-                                        if constexpr (EPI == EPI_RELU) y = fmaxf(y, 0.f);
-                                        f[e] = y;
-                                    }
+                                    for (int e = 0; e < 8; ++e) f[e] = bf16_round(f[e]);   // the Linear's bf16 output in the reference
                                     {
                                         float2 r0 = unpack_bf16x2(rq.x), r1 = unpack_bf16x2(rq.y);
                                         float2 r2 = unpack_bf16x2(rq.z), r3 = unpack_bf16x2(rq.w);
@@ -503,18 +625,18 @@ inline PFN_encodeTiled get_encode_tiled() {
     return fn;
 }
 
-// bf16 row-major [rows, cols] (row stride ld elements) -> 2-D map, box {64 cols, box_rows}, 128B swizzle.
+// bf16 row-major [rows, cols] (row stride ld elements) -> 2-D map, box {box_cols, box_rows}; box_cols 64 (128B swizzle) or 32 (64B swizzle).
 inline bool make_tmap_bf16_2d(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                              uint32_t box_rows) {
+                              uint32_t box_rows, uint32_t box_cols = 64) {
     PFN_encodeTiled enc = get_encode_tiled();
-    if (!enc) return false;
+    if (!enc || (box_cols != 64 && box_cols != 32)) return false;
     cuuint64_t dims[2] = {cols, rows};
     cuuint64_t strides[1] = {ld * 2};
-    cuuint32_t box[2] = {64, box_rows};
+    cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
 }
 
@@ -525,24 +647,27 @@ static int g_gemm_chunk_rows_override = 0;
 // The same (base, shape) pairs come back on every forward (weights and workspace slices are stable), and encoding a CUtensorMap costs
 // a driver call: keep the encoded maps per thread. The map only describes address + extents, so a hit is valid whatever lives there.
 struct TmapKey {
-    const void* base; uint64_t rows, cols, ld; uint32_t box_rows;
-    bool operator==(const TmapKey& o) const { return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows; }
+    const void* base; uint64_t rows, cols, ld; uint32_t box_rows, box_cols;
+    bool operator==(const TmapKey& o) const {
+        return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && box_cols == o.box_cols;
+    }
 };
 struct TmapKeyHash {
     size_t operator()(const TmapKey& k) const {
         uint64_t h = reinterpret_cast<uint64_t>(k.base) * 0x9E3779B97F4A7C15ull;
         h ^= (k.rows + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2));
         h ^= (k.cols * 0xC2B2AE3D27D4EB4Full + (h << 6) + (h >> 2));
-        h ^= (k.ld * 0x165667B19E3779F9ull + k.box_rows + (h << 6) + (h >> 2));
+        h ^= (k.ld * 0x165667B19E3779F9ull + k.box_rows + ((uint64_t)k.box_cols << 32) + (h << 6) + (h >> 2));
         return (size_t)h;
     }
 };
-inline bool tmap_bf16_2d_cached(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
+inline bool tmap_bf16_2d_cached(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+                                uint32_t box_cols = 64) {
     static thread_local std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
-    const TmapKey key{base, rows, cols, ld, box_rows};
+    const TmapKey key{base, rows, cols, ld, box_rows, box_cols};
     auto it = cache.find(key);
     if (it != cache.end()) { memcpy(map, &it->second, sizeof(CUtensorMap)); return true; }
-    if (!make_tmap_bf16_2d(map, base, rows, cols, ld, box_rows)) return false;
+    if (!make_tmap_bf16_2d(map, base, rows, cols, ld, box_rows, box_cols)) return false;
     if (cache.size() > 16384) cache.clear();
     cache.emplace(key, *map);
     return true;
@@ -576,10 +701,12 @@ struct GemmLaunch {
     GemmParams p;
 };
 
-template <int BLOCK_N, int EPI>
+// TMA_EPI: the TMA-store epilogue (dense bf16 C and residual, one batch); C and the residual must start on 16 bytes and have row strides
+// that are multiples of 8 elements.
+template <int BLOCK_N, int EPI, bool TMA_EPI>
 inline cudaError_t launch_gemm_t(const GemmLaunch& g, int num_sms, cudaStream_t stream) {
     using Cfg = GemmConfig<BLOCK_N>;
-    auto kernel = gemm_bf16_sm90_kernel<BLOCK_N, EPI>;
+    auto kernel = gemm_bf16_sm90_kernel<BLOCK_N, EPI, TMA_EPI>;
     static PerDeviceOnce attr;
     {
         cudaError_t e = attr.ensure([&] { return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); });
@@ -592,6 +719,17 @@ inline cudaError_t launch_gemm_t(const GemmLaunch& g, int num_sms, cudaStream_t 
     if (!tmap_bf16_2d_cached(&ta, g.A, a_rows, a_cols, (uint64_t)g.lda, Cfg::BLOCK_M)) return cudaErrorInvalidValue;
     if (!tmap_bf16_2d_cached(&tb, g.W, (uint64_t)g.w_rows, w_cols, (uint64_t)g.ldw, Cfg::B_HALF_ROWS))
         return cudaErrorInvalidValue;
+    CUtensorMap tc = ta, tr = ta;   // not read by the staged epilogue
+    if constexpr (TMA_EPI) {
+        // extents [M, n_out]: the hardware clips the ragged last tiles, and columns n_out .. ldc - 1 are never written
+        const GemmParams& q = g.p;
+        const uint64_t n_out = epi_is_gated(EPI) ? q.N / 2 : q.N;
+        constexpr uint32_t box_cols = gemm_out_box_cols(BLOCK_N, EPI);
+        auto tma_ok = [](const void* ptr, int ld) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && ld > 0 && ld % 8 == 0; };
+        if (g.p.num_batches > 1 || !tma_ok(q.C, q.ldc) || (q.residual && !tma_ok(q.residual, q.ldr))) return cudaErrorInvalidValue;
+        if (!tmap_bf16_2d_cached(&tc, q.C, (uint64_t)q.M, n_out, (uint64_t)q.ldc, 64, box_cols)) return cudaErrorInvalidValue;
+        if (q.residual && !tmap_bf16_2d_cached(&tr, q.residual, (uint64_t)q.M, n_out, (uint64_t)q.ldr, 64, box_cols)) return cudaErrorInvalidValue;
+    }
     GemmParams p = g.p;
     if (p.num_batches < 1) p.num_batches = 1;
     const int rows_per_tile = Cfg::BLOCK_M;
@@ -601,7 +739,8 @@ inline cudaError_t launch_gemm_t(const GemmLaunch& g, int num_sms, cudaStream_t 
     //   * W-stationary: W cut into chunks of <= ~14 MB, small A groups stream past each chunk;
     //   * A-stationary: one chunk (all of W streams), A groups of ~12 MB.
     // Sizes chosen for the H100's 50 MB L2. Measured against other orders at the clip-flant5-xxl encoder shapes (M = 43008, isolated CUDA-event
-    // times, one run; DESIGN.md section 8): best or within 3 % for qkv / o / wo, 7 % behind W-stationary 32 MB chunks for the FFN wi GEMM.
+    // times; DESIGN.md section 8): best or within 3 % for qkv / o / wo; for the FFN wi GEMM, W-stationary 32 MB chunks won one of three runs
+    // against this order and lost the other two, so the order stays.
     // vqa_set_gemm_schedule() / VQA_GEMM_GROUP_ROWS / VQA_GEMM_CHUNK_ROWS override (tuning).
     static const int env_rows = [] { const char* v = getenv("VQA_GEMM_GROUP_ROWS"); return (v && v[0]) ? atoi(v) : 0; }();
     static const int env_chunk = [] { const char* v = getenv("VQA_GEMM_CHUNK_ROWS"); return (v && v[0]) ? atoi(v) : 0; }();
@@ -655,7 +794,7 @@ inline cudaError_t launch_gemm_t(const GemmLaunch& g, int num_sms, cudaStream_t 
     attrs[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attrs;
     cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kernel, ta, tb, p);
+    return cudaLaunchKernelEx(&cfg, kernel, ta, tb, tc, tr, p);
 }
 
 }  // namespace vqa

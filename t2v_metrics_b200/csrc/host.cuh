@@ -92,17 +92,17 @@ static int env_int(const char* name, int dflt) {
 
 // Tile variants are named <BLOCK_N><rows / 128> (ABI values of vqa_op_gemm_bf16 and VQA_GEMM_VARIANT). sm_90a has no CTA-pair MMA, so the
 // two-CTA names 2562 / 1282 select the same 128-row tile as 2561 / 1281.
-template <int EPI>
+template <int EPI, bool TMA_EPI>
 static cudaError_t gemm_dispatch_variant(const GemmLaunch& g, int variant, int num_sms, cudaStream_t st) {
     switch (variant) {
         case 2562:
-        case 2561: return launch_gemm_t<256, EPI>(g, num_sms, st);
+        case 2561: return launch_gemm_t<256, EPI, TMA_EPI>(g, num_sms, st);
         case 1282:
-        case 1281: return launch_gemm_t<128, EPI>(g, num_sms, st);
-        case 641:  return launch_gemm_t<64, EPI>(g, num_sms, st);
+        case 1281: return launch_gemm_t<128, EPI, TMA_EPI>(g, num_sms, st);
+        case 641:  return launch_gemm_t<64, EPI, TMA_EPI>(g, num_sms, st);
         case 321:
             if constexpr (epi_is_gated(EPI)) return cudaErrorInvalidValue;
-            else return launch_gemm_t<32, EPI>(g, num_sms, st);
+            else return launch_gemm_t<32, EPI, TMA_EPI>(g, num_sms, st);
         default:   return cudaErrorInvalidValue;
     }
 }
@@ -251,7 +251,7 @@ static cudaError_t run_gemm(const Gemm& g, int num_sms, cudaStream_t st) {
         if (!g.labels || !g.lse_max || !g.lse_sum || !g.label_logit) return cudaErrorInvalidValue;
         p.lse_max = g.lse_max; p.lse_sum = g.lse_sum; p.labels = g.labels; p.label_logit = g.label_logit; p.lse_scale = g.lse_scale;
         p.penalty_bitmap = g.penalty_bitmap; p.penalty_words = g.penalty_words; p.penalty = g.penalty;
-        return launch_gemm_t<LMHEAD_BN, EPI_LSE>(L, num_sms, st);
+        return launch_gemm_t<LMHEAD_BN, EPI_LSE, false>(L, num_sms, st);
     }
     bf16* C = static_cast<bf16*>(g.C);
     const bf16* residual = static_cast<const bf16*>(g.residual);
@@ -260,7 +260,7 @@ static cudaError_t run_gemm(const Gemm& g, int num_sms, cudaStream_t st) {
         L.a_rows = g.M; L.a_cols = g.K; L.w_cols = g.K;
         p.K = Ks; p.C = reinterpret_cast<bf16*>(g.splitk_ws); p.ldc = g.N; p.c_f32 = 2;
         p.num_batches = g.k_slices; p.a_k_off = Ks; p.w_k_off = Ks; p.c_batch_stride = (long long)g.M * g.N;
-        cudaError_t e = gemm_dispatch_variant<EPI_STORE>(L, 1281, num_sms, st);
+        cudaError_t e = gemm_dispatch_variant<EPI_STORE, false>(L, 1281, num_sms, st);
         if (e != cudaSuccess) return e;
         const long long n = (long long)g.M * (g.N / 8);
         splitk_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g.splitk_ws, g.k_slices, g.M, g.N, g.bias, residual, g.ldr, C, g.ldc);
@@ -286,13 +286,18 @@ static cudaError_t run_gemm(const Gemm& g, int num_sms, cudaStream_t st) {
     p.ssq_inv_dim = nf.inv_dim; p.ssq_eps = nf.eps;
     if (nf.ssq_out && (g.epi != EPI_STORE || g.c_f32)) return cudaErrorInvalidValue;
     const int variant = g.variant ? g.variant : pick_variant(g.M, g.N, g.epi);
+    // Dense bf16 outputs take the TMA-store epilogue. The staged one keeps what a box store cannot do with the same bits: fp32 C, the
+    // batched launches (whose gap rows between batches keep their contents), the scattered column groups and the per-row sums of squares
+    // (their summation order). Those are plain stores; the other epilogues have only the TMA-store path.
+    if (g.batch.nb > 0 || g.c_f32 || g.c_group_in > 0 || nf.ssq_out)
+        return g.epi == EPI_STORE ? gemm_dispatch_variant<EPI_STORE, false>(L, variant, num_sms, st) : cudaErrorInvalidValue;
     switch (g.epi) {
-        case EPI_STORE:      return gemm_dispatch_variant<EPI_STORE>(L, variant, num_sms, st);
-        case EPI_QUICK_GELU: return gemm_dispatch_variant<EPI_QUICK_GELU>(L, variant, num_sms, st);
-        case EPI_GELU_ERF:   return gemm_dispatch_variant<EPI_GELU_ERF>(L, variant, num_sms, st);
-        case EPI_GATED_GELU: return gemm_dispatch_variant<EPI_GATED_GELU>(L, variant, num_sms, st);
-        case EPI_RELU:       return gemm_dispatch_variant<EPI_RELU>(L, variant, num_sms, st);
-        case EPI_GATED_SILU: return gemm_dispatch_variant<EPI_GATED_SILU>(L, variant, num_sms, st);
+        case EPI_STORE:      return gemm_dispatch_variant<EPI_STORE, true>(L, variant, num_sms, st);
+        case EPI_QUICK_GELU: return gemm_dispatch_variant<EPI_QUICK_GELU, true>(L, variant, num_sms, st);
+        case EPI_GELU_ERF:   return gemm_dispatch_variant<EPI_GELU_ERF, true>(L, variant, num_sms, st);
+        case EPI_GATED_GELU: return gemm_dispatch_variant<EPI_GATED_GELU, true>(L, variant, num_sms, st);
+        case EPI_RELU:       return gemm_dispatch_variant<EPI_RELU, true>(L, variant, num_sms, st);
+        case EPI_GATED_SILU: return gemm_dispatch_variant<EPI_GATED_SILU, true>(L, variant, num_sms, st);
         default:             return cudaErrorInvalidValue;
     }
 }

@@ -84,6 +84,33 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* desc, ui
         : "memory");
 }
 
+// 2-D tile store shared -> global, tracked by the issuing thread's bulk async-groups. Elements outside the map's extents are not written.
+__device__ __forceinline__ void tma_store_2d(const void* desc, const void* smem_src, int32_t c0, int32_t c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(desc)),
+                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still READING shared memory (their global writes may still be in flight)
+template <int N> __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups not yet complete
+template <int N> __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// orders this thread's generic-proxy shared-memory writes before later async-proxy (TMA) reads of them
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// Four 8x8 bf16 matrices between registers and shared memory; lanes 8i..8i+7 give the row addresses of matrix i, and register i holds
+// matrix i in the accumulator pair layout (lane l: row l / 4, columns 2 (l % 4) + {0, 1}).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
+                 : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr)
+                 : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma (warpgroup MMA)
 // Shared-memory matrix descriptor of an operand tile stored as rows of 64 bf16 (128 B) with the 128-byte swizzle TMA writes
 // (CU_TENSOR_MAP_SWIZZLE_128B): 8-row atoms of 1024 B. K-major (rows = M or N index): SBO = 1024 B between 8-row atoms, LBO unused.

@@ -211,7 +211,7 @@ extern "C" int vqa_set_gemm_schedule(int32_t group_rows, int32_t chunk_rows) {
 extern "C" int vqa_debug_max_active_clusters(int32_t cluster_size) {
     if (cluster_size < 1 || cluster_size > 16) return VQA_ERR_INVALID_ARG;
     using Cfg = GemmConfig<256>;
-    auto kernel = gemm_bf16_sm90_kernel<256, EPI_STORE>;
+    auto kernel = gemm_bf16_sm90_kernel<256, EPI_STORE, true>;
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess) return VQA_ERR_CUDA;
     if (cluster_size > 8 && cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) return VQA_ERR_CUDA;
     int dev = 0, sms = 0;

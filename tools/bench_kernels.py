@@ -3,7 +3,8 @@
 
   python tools/bench_kernels.py attn [--dump DIR]   # head_dim-64 attention: T5 encoder shape and CLIP shape, both rounding modes,
                                                     # CUDA-event timing; --dump writes the outputs (raw bf16) to DIR
-  python tools/bench_kernels.py gemm-time       # the four T5-encoder GEMM shapes under a list of tile schedules, CUDA-event timing
+  python tools/bench_kernels.py gemm-time [--dump DIR]   # the T5-encoder and CLIP-tower GEMM shapes under a list of tile schedules,
+                                                # CUDA-event timing; --dump writes each shape's output (raw bytes) to DIR
   python tools/bench_kernels.py gemm-ncu        # same launches once each, in a fixed order, for `ncu --metrics dram__bytes_*`
   python tools/bench_kernels.py gemm-list       # prints that order (shape, group_rows, chunk_rows) as JSON
 """
@@ -109,17 +110,28 @@ def attn128():
     print(json.dumps(dict(kernel="attn_wgmma_kernel d128", **res)))
 
 
-SHAPES = dict(   # name: (M, N, K, epilogue, residual)   clip-flant5-xxl encoder layer at B=64, S=672
-    qkv=(43008, 12288, 4096, "store", False),
-    o=(43008, 4096, 4096, "store", True),
-    wi=(43008, 20480, 4096, "gated_gelu", False),
-    wo=(43008, 4096, 10240, "store", True),
+SHAPES = dict(   # name: (M, N, K, epilogue, residual, bias)   residual: None, "bf16" (in the output's place) or "f32" (fp32 stream, in place)
+    # clip-flant5-xxl encoder layer at B=64, S=672
+    qkv=(43008, 12288, 4096, "store", None, False),
+    o=(43008, 4096, 4096, "store", "bf16", False),
+    wi=(43008, 20480, 4096, "gated_gelu", None, False),
+    wo=(43008, 4096, 10240, "store", "bf16", False),
+    # o with twice the K: 2 t(o) - t(o_k8192) is the fixed cost per tile (epilogue, pipeline ramp) that the main loop does not amortise
+    o_k8192=(43008, 4096, 8192, "store", "bf16", False),
+    # CLIP ViT-L/14-336 layer at 64 images x 577 tokens
+    clip_qkv=(36928, 3072, 1024, "store", None, True),
+    clip_out=(36928, 1024, 1024, "store", "f32", True),
+    clip_fc1=(36928, 4096, 1024, "quick_gelu", None, True),
+    clip_fc2=(36928, 1024, 4096, "store", "f32", True),
 )
 SCHEDULES = [(0, 0), (4096, -1), (1024, -1), (512, 2048), (512, 4096), (1024, 3072), (1024, 4096), (1024, 6144), (2048, 4096), (1024, 8192),
              (2048, 2048), (512, 6144)]
 
 
-def gemm(mode):
+def gemm(mode, dump_dir=None):
+    """dump_dir: each shape's output after its last schedule, as raw bytes (bf16 or fp32), so that two builds can be compared byte for byte.
+    The in-place residual shapes restore their residual before every launch, so the dumped output is one GEMM's result."""
+    import numpy as np
     from t2v_metrics_b200 import _lib
     from t2v_metrics_b200.engine import ops
     lib = _lib.load()
@@ -131,18 +143,23 @@ def gemm(mode):
     if os.environ.get("BALLAST_GB"):      # mimic the footprint of the real step (weights + workspace) around the operands
         ballast = torch.empty(int(os.environ["BALLAST_GB"]) << 30, dtype=torch.uint8, device="cuda").fill_(1)
     for name in only:
-        M, N, K, epi, res = SHAPES[name]
+        M, N, K, epi, res, has_bias = SHAPES[name]
         a = (torch.randn(M, K, device="cuda") * 0.5).bfloat16()
         w = (torch.randn(N, K, device="cuda") * K ** -0.5).bfloat16()
         if os.environ.get("ZERO_OPERANDS"):
             a.zero_(); w.zero_()
+        bias = (torch.randn(N, device="cuda") * 0.1).bfloat16() if has_bias else None
         n_out = N // 2 if epi == "gated_gelu" else N
-        c = torch.empty(M, n_out, dtype=torch.bfloat16, device="cuda")
-        r = torch.randn(M, n_out, device="cuda").bfloat16() if res else None
+        if res == "f32":
+            c = torch.randn(M, n_out, device="cuda")
+            fn = lambda: ops.gemm_f32acc(a, w, c, bias=bias)
+        else:
+            c = torch.empty(M, n_out, dtype=torch.bfloat16, device="cuda")
+            r = torch.randn(M, n_out, device="cuda").bfloat16() if res == "bf16" else None
+            fn = lambda: ops.gemm(a, w, bias=bias, residual=r, epilogue=epi, out=c, gate_up_offset=N // 2 if epi == "gated_gelu" else 0)
         flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
         for (g, ch) in scheds:
             lib.vqa_set_gemm_schedule(g, ch)
-            fn = lambda: ops.gemm(a, w, residual=r, epilogue=epi, out=c, gate_up_offset=N // 2 if epi == "gated_gelu" else 0)
             if mode == "ncu":
                 flush.zero_()      # start every measured launch from a cold L2
                 fn()
@@ -150,8 +167,16 @@ def gemm(mode):
             else:
                 ms = time_ms(fn, iters=10, warm=2)
                 rows.append(dict(shape=name, group_rows=g, chunk_rows=ch, ms=round(ms, 4), tflops=round(2.0 * M * N * K / ms / 1e9, 1)))
+        if dump_dir:
+            if res == "f32":   # one accumulation into a fresh copy of the seeded stream
+                torch.manual_seed(1)
+                c.copy_(torch.randn(M, n_out, device="cuda"))
+            fn()
+            torch.cuda.synchronize()
+            os.makedirs(dump_dir, exist_ok=True)
+            np.save(os.path.join(dump_dir, f"gemm_{name}.npy"), c.view(torch.int32 if c.dtype == torch.float32 else torch.int16).cpu().numpy())
         lib.vqa_set_gemm_schedule(0, 0)
-        del a, w, c, r
+        del a, w, c
     if mode != "ncu":
         print(json.dumps(rows))
 
@@ -165,7 +190,7 @@ if __name__ == "__main__":
     elif cmd == "attn128":
         attn128()
     elif cmd == "gemm-time":
-        gemm("time")
+        gemm("time", sys.argv[sys.argv.index("--dump") + 1] if "--dump" in sys.argv else None)
     elif cmd == "gemm-ncu":
         gemm("ncu")
     elif cmd == "gemm-list":
