@@ -387,10 +387,15 @@ int vqa_op_gemm_bf16_normfuse(const void* A, int32_t lda, const void* W, int32_t
                               int32_t K, const void* residual, int32_t ldr, int32_t epilogue, int32_t gate_up_offset, const float* ssq_in,
                               float* ssq_out, int32_t stride, int32_t norm_dim, float eps, int32_t* parts_out, void* stream);
 
-/* Fused lm_head + log-softmax gather: logprob[m] = (h[m].W[label[m]]) - logsumexp_n(h[m].W[n]); logits never stored.
- * scratch: DEVICE float, >= 4*M*ceil(N/128) + M floats. */
-int vqa_op_lmhead_logprob(const void* H, int32_t ldh, const void* W, int32_t ldw, int32_t M, int32_t N, int32_t K,
-                          const int32_t* labels, float* logprob, float* scratch, void* stream);
+/* The lm_head of vqa_qwen25vl_score with its fused log-softmax gather: with x_n = bf16(h[m].W[n]) in fp32, penalised where bit n of row m
+ * of pen_bitmap [M, ceil(N / 32)] is set (x < 0 ? x * repetition_penalty : x / repetition_penalty; pen_bitmap NULL or penalty 1: none) and
+ * divided by the temperature, logprob[m] = x_label[m] - logsumexp_n x_n. Logits are never stored; labels in [0, N). All DEVICE; K, ldh, ldw
+ * multiples of 8 and >= K, H / W 16-byte aligned, temperature and penalty > 0. scratch DEVICE float: lse_max and lse_sum (M x 2 ceil(N / 128)
+ * partials each), the label logits [M] and the scores [M]; *scratch_needed (HOST, optional) receives its size in bytes, also when a smaller
+ * scratch_bytes returns VQA_ERR_WORKSPACE. */
+int vqa_op_lmhead_logprob(const void* H, int32_t ldh, const void* W, int32_t ldw, int32_t M, int32_t N, int32_t K, const int32_t* labels,
+                          float temperature, const uint32_t* pen_bitmap, float repetition_penalty, float* logprob, float* scratch,
+                          size_t scratch_bytes, size_t* scratch_needed, void* stream);
 
 /* The per-step kernel of vqa_qwen25vl_rollout_* on caller-given bf16 logits [batch, V]: for every b with done[b] == 0, row lengths[b] of
  * out_logp [batch, max_new, n_max] (and of out_topk_ids / out_topk_probs [batch, max_new, top_k] when top_k > 0), under the penalty
@@ -454,15 +459,19 @@ int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32
 int vqa_op_norm(const void* x, const void* gamma, const void* beta, void* y, int32_t rows, int32_t D, float eps,
                 void* stream);
 
-/* head_dim-128 attention on a packed buffer [rows, ld]: q heads at q_col0 + h*128, k/v heads at k_col0/v_col0 + (h/kv_group)*128.
- * cu_seqlens [n_seq+1] (variable-length sequences) or NULL with fixed stride S and optional seq_lens [n_seq]. */
+/* head_dim-128 attention on a packed buffer [rows, ld]: q heads at q_col0 + h*128, k/v heads at k_col0/v_col0 + (h/kv_group)*128,
+ * out[row * ldo + h * 128 + d]. cu_seqlens [n_seq+1] (variable-length sequences) or NULL with fixed stride S and optional seq_lens [n_seq]:
+ * then all S rows of every sequence are written, zeros past seq_lens[b], so S >= 1, n_seq * S <= rows and max_len >= S. q_heads a multiple
+ * of kv_group; ld, ldo, the column offsets multiples of 8 with every head inside its row; qkv / out 16-byte aligned; else
+ * VQA_ERR_INVALID_ARG before anything launches. */
 int vqa_op_attention_d128(const void* qkv, int32_t ld, int64_t rows, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out,
                           int32_t ldo, int32_t n_seq, int32_t max_len, int32_t S, int32_t q_heads, int32_t kv_group,
                           const int32_t* cu_seqlens, const int32_t* seq_lens, float scale, int32_t causal, void* stream);
 
 /* vqa_op_attention_d128 in variable-length mode with its extras: kv_prefix [n_seq] (or NULL): sequence b also attends to all rows of sequence
  * kv_prefix[b] >= 0, placed in front of its own keys; pair_sequences: two consecutive sequences (each <= 64 rows) share one 128-row tile under a
- * block-diagonal mask (non-causal only); output head h is written at column h * o_head_stride, first d_out (multiple of 8) head dims only. */
+ * block-diagonal mask (non-causal, no kv_prefix, max_len <= 64); output head h is written at column h * o_head_stride, first d_out (multiple
+ * of 8, <= 128 and <= o_head_stride) head dims only. The other checks are those of vqa_op_attention_d128. */
 int vqa_op_attention_d128_ex(const void* qkv, int32_t ld, int64_t rows, int32_t q_col0, int32_t k_col0, int32_t v_col0, void* out, int32_t ldo,
                              int32_t n_seq, int32_t max_len, int32_t q_heads, int32_t kv_group, const int32_t* cu_seqlens, const int32_t* kv_prefix,
                              float scale, int32_t causal, int32_t pair_sequences, int32_t o_head_stride, int32_t d_out, void* stream);
@@ -519,6 +528,42 @@ int vqa_op_layernorm_f32(const float* x, const void* gamma, const void* beta, vo
  * cls [D], pos [P + 1, D], gamma / beta [D]. D in {256, 1024} (else VQA_ERR_UNSUPPORTED); pointers 16-byte aligned. */
 int vqa_op_clip_embed_ln(const void* patch, const void* cls, const void* pos, const void* gamma, const void* beta, float* y, int32_t n_images,
                          int32_t P, int32_t D, float eps, void* stream);
+
+/* The Qwen2.5-VL scoring path's glue kernels, launched as vqa_qwen25vl_score launches them. All pointers DEVICE. */
+
+/* Rotary embedding (M-RoPE): the tables cos_t / sin_t [rows, 2 * half] float get, for i < half, angle = positions[axis_of_dim[i] * rows + row]
+ * * inv_freq[i] (positions int32 [n_axes, rows], axis_of_dim int32 / inv_freq float [half]) and cos / sin(angle) at columns i and i + half;
+ * then the n_heads heads of x bf16 [rows, ld] at columns col0 + h * head_stride are rotated in place over their first head_dim = 2 * half dims:
+ * x' = x * cos + rotate_half(x) * sin. text_mode != 0: the tables are rounded to bf16 and every product is rounded to bf16 before the sum
+ * (the language model); 0: fp32 throughout (the vision tower). head_dim a multiple of 16 and <= head_stride; ld, col0, head_stride multiples
+ * of 8 with every head inside ld; x and the tables 16-byte aligned. */
+int vqa_op_qwen_rope(const int32_t* positions, int32_t rows, const int32_t* axis_of_dim, const float* inv_freq, int32_t half, float* cos_t,
+                     float* sin_t, void* x, int32_t ld, int32_t col0, int32_t n_heads, int32_t head_stride, int32_t head_dim, int32_t text_mode,
+                     void* stream);
+
+/* Row re-order: dst row r = src row index[r / group] * group + r % group for r < rows (rows a multiple of group), D bf16 columns (a multiple
+ * of 8) per row: the vision tower's window order (group 4 = spatial_merge^2) and its inverse on the merged features (group 1). src / dst
+ * 16-byte aligned. */
+int vqa_op_gather_rows(const void* src, void* dst, const int32_t* index, int32_t rows, int32_t group, int32_t D, void* stream);
+
+/* Embedding splice: row r = b * S + s of out [rows, D] (rows a multiple of S) is feats[feat_index[r]] when feat_index[r] >= 0, else
+ * embed[ids[r]], for s < seq_lens[b]; zero past it (ids and feat_index are not read there). Padded rows: seq_lens [rows / S]; packed rows as
+ * vqa_qwen25vl_score_packed: seq_lens = cu_seqlens + n_seq and S = rows. D a multiple of 8; embed / feats / out 16-byte aligned. */
+int vqa_op_qwen_embed(const int32_t* ids, const int32_t* feat_index, const int32_t* seq_lens, const void* embed, const void* feats, void* out,
+                      int32_t rows, int32_t S, int32_t D, void* stream);
+
+/* Repetition-penalty bitmap: bit id of row b of bitmap uint32 [B, ceil(vocab / 32)] is OR-ed in for every prompt id of pair b with
+ * 0 <= id < vocab (the caller zeroes the bitmap first). cu_seqlens NULL: padded prompts, ids [B, S], row b's first seq_lens[b] ids.
+ * Otherwise packed rows: pair b's prompt is all of sequence kv_prefix[pair_seq[b]] (kv_prefix NULL or the entry < 0: none) followed by
+ * sequence pair_seq[b], at most max_prompt_len ids in all. */
+int vqa_op_token_bitmap(const int32_t* ids, const int32_t* seq_lens, int32_t B, int32_t S, const int32_t* cu_seqlens, const int32_t* kv_prefix,
+                        const int32_t* pair_seq, int32_t max_prompt_len, int32_t vocab, uint32_t* bitmap, void* stream);
+
+/* The trace output of vqa_qwen25vl_topk on caller bf16 logits [B, ldl] (ldl >= V): the K (1..8) most probable ids of each row, ties to the
+ * lower id, into out_ids int32 / out_probs float [B, K], under the penalty bitmap pen_bitmap [B, ceil(V / 32)] (NULL or penalty 1: none)
+ * and softmax(x / temperature) over all V. */
+int vqa_op_topk_softmax(const void* logits, int64_t ldl, int32_t B, int32_t V, float temperature, const uint32_t* pen_bitmap,
+                        float repetition_penalty, int32_t K, int32_t* out_ids, float* out_probs, void* stream);
 
 #ifdef __cplusplus
 }

@@ -27,6 +27,7 @@ ABI_SYMBOLS = [
     "vqa_op_kv_cache_write", "vqa_op_decode_attention_d128", "vqa_op_greedy_select", "vqa_t5_bucket_lut", "vqa_op_t5_decoder_self_attn",
     "vqa_op_t5_decode_self_attn", "vqa_op_gemm_bf16_f32acc", "vqa_op_gemm_bf16_batched", "vqa_op_t5_cross_attention", "vqa_op_layernorm_f32",
     "vqa_op_clip_embed_ln", "vqa_qwen_preprocess_video_plan", "vqa_qwen_preprocess_video",
+    "vqa_op_qwen_rope", "vqa_op_gather_rows", "vqa_op_qwen_embed", "vqa_op_token_bitmap", "vqa_op_topk_softmax",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -102,7 +103,7 @@ def load() -> C.CDLL:
     lib.vqa_op_gemm_bf16_normfuse.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, vp, i32, i32, i32, vp, vp, i32, i32, f32,
                                               C.POINTER(i32), vp]
     lib.vqa_op_gemm_bf16_normfuse.restype = C.c_int
-    lib.vqa_op_lmhead_logprob.argtypes = [vp, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp]
+    lib.vqa_op_lmhead_logprob.argtypes = [vp, i32, vp, i32, i32, i32, i32, vp, f32, vp, f32, vp, vp, C.c_size_t, C.POINTER(C.c_size_t), vp]
     lib.vqa_op_lmhead_logprob.restype = C.c_int
     lib.vqa_op_attention_d64.argtypes = [vp, vp, i32, i32, i32, vp, vp, f32, i32, i32, vp]
     lib.vqa_op_attention_d64.restype = C.c_int
@@ -163,6 +164,16 @@ def load() -> C.CDLL:
     lib.vqa_op_layernorm_f32.restype = C.c_int
     lib.vqa_op_clip_embed_ln.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp]
     lib.vqa_op_clip_embed_ln.restype = C.c_int
+    lib.vqa_op_qwen_rope.argtypes = [vp, i32, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    lib.vqa_op_qwen_rope.restype = C.c_int
+    lib.vqa_op_gather_rows.argtypes = [vp, vp, vp, i32, i32, i32, vp]
+    lib.vqa_op_gather_rows.restype = C.c_int
+    lib.vqa_op_qwen_embed.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]
+    lib.vqa_op_qwen_embed.restype = C.c_int
+    lib.vqa_op_token_bitmap.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, vp]
+    lib.vqa_op_token_bitmap.restype = C.c_int
+    lib.vqa_op_topk_softmax.argtypes = [vp, i64, i32, i32, f32, vp, f32, i32, vp, vp, vp]
+    lib.vqa_op_topk_softmax.restype = C.c_int
     lib.vqa_clipt5_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
     lib.vqa_clipt5_generate_workspace_bytes.restype = C.c_size_t
     lib.vqa_clipt5_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]

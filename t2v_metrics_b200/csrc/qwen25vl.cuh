@@ -168,14 +168,14 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
         else
             TRY(f.copy(P_(w.patches), pixel_patches, n * 2, "pixel copy"));
         // rotary table of the (already window-ordered) patch positions: [h freqs | w freqs] duplicated (:404-409, :487)
-        TRY(f.launch(CAT_OTHER, 0, "vision rope table", rope_table_kernel, (L * (hdv / 2) + 255) / 256, 256, 0, vis_pos_hw, L, q.vis_axis,
+        TRY(f.launch(CAT_OTHER, 0, "vision rope table", rope_table_kernel, rope_table_blocks(L, hdv / 2), GLUE_THREADS, 0, vis_pos_hw, L, q.vis_axis,
                      q.vis_inv_freq, hdv / 2, F_(w.vcos), F_(w.vsin), 0));
     }
     // patch embedding (Conv3d == GEMM), then re-order 2x2 groups into window order (:470-472)
     TRY(f.gemm(Gemm(P_(w.patches), q.patch_w, P_(w.vxn), L, Dv, c.patch_dim)));
     {
         auto g = f.group(CAT_OTHER);
-        TRY(f.launch(CAT_OTHER, 0, "window reorder", gather_rows_kernel, L, 128, 0, P_(w.vxn), P_(w.vx), window_index, unit, Dv));
+        TRY(f.launch(CAT_OTHER, 0, "window reorder", gather_rows_kernel, L, ROW_COPY_THREADS, 0, P_(w.vxn), P_(w.vx), window_index, unit, Dv));
         // the qkv GEMMs write head_dim of every 128-wide head slot; the attention kernel contracts q.k over all 128: zero the rest once
         if (hdv < 128) TRY(f.memset0(P_(w.vqkv), (size_t)L * 3 * Hv * 128 * 2, "vision qkv clear"));
     }
@@ -188,8 +188,7 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
         qkv.ldc = 3 * Hv * 128;
         if (hdv < 128) { qkv.c_group_in = hdv; qkv.c_group_out = 128; }
         TRY(f.gemm(qkv.with_bias(Lw.qkv_b), "vision qkv gemm"));
-        const long long nthr = (long long)L * 2 * Hv * (hdv / 16);
-        TRY(f.launch(CAT_OTHER, 0, "vision rope", rope_inplace_kernel, (unsigned)((nthr + 255) / 256), 256, 0, P_(w.vqkv), 3 * Hv * 128, 0, 2 * Hv,
+        TRY(f.launch(CAT_OTHER, 0, "vision rope", rope_inplace_kernel, rope_inplace_blocks(L, 2 * Hv, hdv), GLUE_THREADS, 0, P_(w.vqkv), 3 * Hv * 128, 0, 2 * Hv,
                      128, hdv, F_(w.vcos), F_(w.vsin), L, 0));
         const int nseq = full ? n_frames : n_windows, mlen = full ? max_frame_len : max_window_len;
         static const bool no_pairs = getenv("VQA_ATTN128_NO_PAIRS") != nullptr;     // A/B switch
@@ -209,13 +208,13 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
     TRY(f.gemm(Gemm(P_(w.vfc1), q.fc2_w, P_(w.vfeat), L / unit, c.out_hidden, Dv * unit).with_bias(q.fc2_b)));
     {
         auto g = f.group(CAT_OTHER);
-        TRY(f.launch(CAT_OTHER, 0, "merger reorder", gather_rows_kernel, L / unit, 128, 0, P_(w.vfeat), P_(w.vfeat_orig), reverse_index, 1,
+        TRY(f.launch(CAT_OTHER, 0, "merger reorder", gather_rows_kernel, L / unit, ROW_COPY_THREADS, 0, P_(w.vfeat), P_(w.vfeat_orig), reverse_index, 1,
                      c.out_hidden));
         // ---------------- language model input ----------------
         // packed rows: one "sample" of M rows, all valid (its length is the last entry of cu_seqlens)
-        TRY(f.launch(CAT_OTHER, 0, "llm embed", qwen_embed_kernel, M, 128, 0, input_ids, feat_index, pk ? pk->cu_seqlens + pk->n_seq : seq_lens,
+        TRY(f.launch(CAT_OTHER, 0, "llm embed", qwen_embed_kernel, M, ROW_COPY_THREADS, 0, input_ids, feat_index, pk ? pk->cu_seqlens + pk->n_seq : seq_lens,
                      q.embed, P_(w.vfeat_orig), P_(w.x), pk ? M : S, D));
-        TRY(f.launch(CAT_OTHER, 0, "llm rope table", rope_table_kernel, (M * 64 + 255) / 256, 256, 0, position_ids, M, q.text_axis,
+        TRY(f.launch(CAT_OTHER, 0, "llm rope table", rope_table_kernel, rope_table_blocks(M, 64), GLUE_THREADS, 0, position_ids, M, q.text_axis,
                      q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1));
     }
     const int Hq = c.heads, Hkv = c.kv_heads, qkv_cols = (Hq + 2 * Hkv) * 128;
@@ -225,8 +224,7 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
         TRY(f.rmsnorm(P_(w.x), Lw.ln1, P_(w.xn), M, D, c.rms_eps));
         TRY(f.gemm(Gemm(P_(w.xn), Lw.qkv_w, P_(w.qkv), M, qkv_cols, D).with_bias(Lw.qkv_b)));
         // q heads and k heads are contiguous in the packed buffer -> one launch rotates Hq + Hkv heads
-        const long long nthr = (long long)M * (Hq + Hkv) * 8;
-        TRY(f.launch(CAT_OTHER, 0, "llm rope", rope_inplace_kernel, (unsigned)((nthr + 255) / 256), 256, 0, P_(w.qkv), qkv_cols, 0, Hq + Hkv,
+        TRY(f.launch(CAT_OTHER, 0, "llm rope", rope_inplace_kernel, rope_inplace_blocks(M, Hq + Hkv, 128), GLUE_THREADS, 0, P_(w.qkv), qkv_cols, 0, Hq + Hkv,
                      128, 128, F_(w.cos), F_(w.sin), M, c.emulate_bf16_rounding));
         if (kv)
             TRY(f.launch(CAT_OTHER, 0, "kv cache write", kv_cache_write_kernel, (unsigned)(((long long)M * Hkv * 16 + 255) / 256), 256, 0, P_(w.qkv),
@@ -257,7 +255,7 @@ static int qwen_last_position(Forward& f, QwenState& q, const QwenWorkspace& w, 
     if (pk) TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_rows_by_index_kernel, B, 128, 0, P_(w.x), pk->pair_row, P_(w.last), D));
     else    TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_last_rows_kernel, B, 128, 0, P_(w.x), seq_lens, P_(w.last), S, D));
     TRY(f.rmsnorm(P_(w.last), q.final_norm, P_(w.lastn), B, D, c.rms_eps));
-    const int pen_words = (c.vocab + 31) / 32;
+    const int pen_words = token_bitmap_words(c.vocab);
     uint32_t* bitmap = f.at<uint32_t>(w.pen_bitmap);
     if (repetition_penalty != 1.0f) {
         // HF applies RepetitionPenaltyLogitsProcessor over the prompt ids before the scores are returned (generation/utils.py:2762-2770,
@@ -265,10 +263,10 @@ static int qwen_last_position(Forward& f, QwenState& q, const QwenWorkspace& w, 
         auto g = f.group(CAT_OTHER);
         TRY(f.memset0(bitmap, (size_t)B * pen_words * 4, "penalty bitmap clear"));
         if (pk)
-            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_packed_kernel, dim3((pk->max_prompt_len + 255) / 256, B), 256, 0, input_ids,
+            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_packed_kernel, token_bitmap_packed_grid(pk->max_prompt_len, B), GLUE_THREADS, 0, input_ids,
                          pk->cu_seqlens, pk->kv_prefix, pk->pair_seq, c.vocab, bitmap, pen_words));
         else
-            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_kernel, (B * S + 255) / 256, 256, 0, input_ids, seq_lens, B, S, c.vocab,
+            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_kernel, token_bitmap_blocks(B, S), GLUE_THREADS, 0, input_ids, seq_lens, B, S, c.vocab,
                          bitmap, pen_words));
     }
     return VQA_OK;
@@ -318,7 +316,7 @@ static int qwen_topk(vqa_handle* h, QwenState& q, int B, size_t rows, int n_patc
     const uint32_t* bitmap = reinterpret_cast<const uint32_t*>(ws + w.pen_bitmap);      // built by the scoring call with the same penalty
     cudaError_t e = run_gemm(Gemm(lastn, q.lm_head, logits, B, c.vocab, c.hidden), h->num_sms, st);
     if (e == cudaSuccess)
-        topk_softmax_kernel<<<B, 256, 0, st>>>(logits, (long long)c.vocab, c.vocab, 1.0f / temperature, penalise ? bitmap : nullptr, pen_words,
+        topk_softmax_kernel<<<B, GLUE_THREADS, 0, st>>>(logits, (long long)c.vocab, c.vocab, 1.0f / temperature, penalise ? bitmap : nullptr, pen_words,
                                                repetition_penalty, K, out_ids, out_probs);
     return cuda_status(h, e, "top-k");
 }

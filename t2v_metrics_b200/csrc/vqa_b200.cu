@@ -508,6 +508,8 @@ static Gemm abi_gemm(const void* A, int lda, const void* W, int ldw, int w_rows,
     return g;
 }
 
+static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 // A gated epilogue stores its N / 2 output columns 8 at a time and reads the up block `gate_up_offset` rows below the gate block.
 static int check_gated(int epilogue, int N, int w_rows, int gate_up_offset) {
     if (!epi_is_gated(epilogue)) return VQA_OK;
@@ -576,19 +578,39 @@ extern "C" int vqa_op_gemm_bf16_normfuse(const void* A, int32_t lda, const void*
     return cuda_status(nullptr, run_gemm(g, device_sms(), (cudaStream_t)stream), "gemm launch");
 }
 
-extern "C" int vqa_op_lmhead_logprob(const void* Hs, int32_t ldh, const void* W, int32_t ldw, int32_t M, int32_t N,
-                                     int32_t K, const int32_t* labels, float* logprob, float* scratch, void* stream) {
-    if (!Hs || !W || !labels || !logprob || !scratch) return fail(nullptr, VQA_ERR_INVALID_ARG, "null pointer");
+// Scratch of vqa_op_lmhead_logprob, in floats: lse_max | lse_sum ([M, LMHEAD_PARTS * n tiles] each) | label_logit [M] | scores [M].
+static size_t lmhead_scratch_floats(int M, int N) {
+    const size_t parts = (size_t)LMHEAD_PARTS * ((N + LMHEAD_BN - 1) / LMHEAD_BN);
+    return 2 * (size_t)M * parts + 2 * (size_t)M;
+}
+
+extern "C" int vqa_op_lmhead_logprob(const void* Hs, int32_t ldh, const void* W, int32_t ldw, int32_t M, int32_t N, int32_t K,
+                                     const int32_t* labels, float temperature, const uint32_t* pen_bitmap, float repetition_penalty,
+                                     float* logprob, float* scratch, size_t scratch_bytes, size_t* scratch_needed, void* stream) {
+    if (!Hs || !W || !labels || !logprob) return fail(nullptr, VQA_ERR_INVALID_ARG, "lmhead logprob: null pointer");
+    if (M <= 0 || N <= 0 || K <= 0 || K % 8 || ldh % 8 || ldw % 8 || ldh < K || ldw < K)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "lmhead logprob: bad size (K, ldh, ldw multiples of 8, ldh / ldw >= K)");
+    if (!(temperature > 0.f) || !(repetition_penalty > 0.f))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "lmhead logprob: temperature and repetition penalty must be > 0");
+    if (!aligned(Hs, 16) || !aligned(W, 16) || !aligned(pen_bitmap, 4))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "lmhead logprob: H / W 16-byte aligned, pen_bitmap 4-byte aligned");
+    const size_t need = lmhead_scratch_floats(M, N);
+    if (scratch_needed) *scratch_needed = need * sizeof(float);
+    if (!scratch || !aligned(scratch, 4) || scratch_bytes < need * sizeof(float))
+        return fail(nullptr, VQA_ERR_WORKSPACE, "lmhead logprob: scratch smaller than lmhead_scratch_floats(M, N) floats");
     const int ntiles = LMHEAD_PARTS * ((N + LMHEAD_BN - 1) / LMHEAD_BN);
     float* lse_max = scratch;
-    float* lse_sum = scratch + (size_t)M * ntiles;
-    float* label_logit = scratch + 2 * (size_t)M * ntiles;
+    float* lse_sum = lse_max + (size_t)M * ntiles;
+    float* label_logit = lse_sum + (size_t)M * ntiles;
+    float* scores = label_logit + M;            // one target per row: exp(logprob), not returned
     cudaStream_t st = (cudaStream_t)stream;
+    // the launch of qwen_score's lm_head
     Gemm g = abi_gemm(Hs, ldh, W, ldw, N, nullptr, 0, M, N, K);
-    if (int rc = cuda_status(nullptr, run_gemm(g.lse(labels, lse_max, lse_sum, label_logit), device_sms(), st), "lmhead launch")) return rc;
-    // T = 1: score buffer unused -> reuse finalize with logprobs output only
-    lse_finalize_kernel<<<(M + 3) / 4, 128, 0, st>>>(lse_max, lse_sum, label_logit, labels, lse_max /*scratch scores*/,
-                                                    logprob, M, 1, ntiles);
+    g.lse(labels, lse_max, lse_sum, label_logit);
+    g.lse_scale = 1.0f / temperature;
+    g.penalty_bitmap = repetition_penalty != 1.0f ? pen_bitmap : nullptr; g.penalty_words = token_bitmap_words(N); g.penalty = repetition_penalty;
+    if (int rc = cuda_status(nullptr, run_gemm(g, device_sms(), st), "lmhead launch")) return rc;
+    lse_finalize_kernel<<<(M + 3) / 4, 128, 0, st>>>(lse_max, lse_sum, label_logit, labels, scores, logprob, M, 1, ntiles);
     return cuda_status(nullptr, cudaGetLastError(), "lse finalize");
 }
 
@@ -604,8 +626,6 @@ extern "C" int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t 
         lengths, done, top_k, out_logp, out_topk_ids, out_topk_probs);
     return cuda_status(nullptr, cudaGetLastError(), "answer logprob launch");
 }
-
-static bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
 
 // kv_cache_write_kernel: the 16-byte chunks of the K and V heads of every row go to their cache slot.
 extern "C" int vqa_op_kv_cache_write(const void* qkv, int32_t ld, int32_t k_col0, int32_t v_col0, int32_t kv_heads, int32_t B, int32_t S,
@@ -714,10 +734,33 @@ extern "C" int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32
     return cuda_status(nullptr, e, "attention launch");
 }
 
+// What attn_wgmma_kernel trusts of its arguments: every q / k / v head inside the row of `ld` columns, 16-byte aligned TMA columns and
+// output rows, every output head inside the row of `ldo` columns.
+static int check_attn_d128(const void* qkv, int ld, long long rows, int q_col0, int k_col0, int v_col0, const void* out, int ldo, int n_seq,
+                           int max_len, int q_heads, int kv_group, int o_head_stride, int d_out) {
+    if (!qkv || !out) return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: null pointer");
+    if (rows <= 0 || n_seq <= 0 || max_len <= 0 || q_heads <= 0 || kv_group <= 0 || q_heads % kv_group)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: bad size (q_heads a multiple of kv_group)");
+    if (ld % 8 || ldo % 8 || q_col0 % 8 || k_col0 % 8 || v_col0 % 8 || q_col0 < 0 || k_col0 < 0 || v_col0 < 0 || !aligned(qkv, 16) ||
+        !aligned(out, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: ld, ldo and column offsets multiples of 8, qkv / out 16-byte aligned");
+    const long long kv_cols = (long long)(q_heads / kv_group) * 128;
+    if ((long long)q_col0 + (long long)q_heads * 128 > ld || k_col0 + kv_cols > ld || v_col0 + kv_cols > ld)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: q / k / v heads must lie inside ld");
+    if (d_out < 8 || d_out > 128 || d_out % 8 || o_head_stride % 8 || o_head_stride < d_out ||
+        (long long)(q_heads - 1) * o_head_stride + d_out > ldo)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: 8 <= d_out <= 128 and o_head_stride multiples of 8, output heads inside ldo");
+    return VQA_OK;
+}
+
 extern "C" int vqa_op_attention_d128(const void* qkv, int32_t ld, int64_t rows, int32_t q_col0, int32_t k_col0, int32_t v_col0,
                                      void* out, int32_t ldo, int32_t n_seq, int32_t max_len, int32_t S, int32_t q_heads, int32_t kv_group,
                                      const int32_t* cu_seqlens, const int32_t* seq_lens, float scale, int32_t causal, void* stream) {
-    if (!qkv || !out || n_seq <= 0 || max_len <= 0 || q_heads <= 0 || kv_group <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad attention argument");
+    if (int rc = check_attn_d128(qkv, ld, rows, q_col0, k_col0, v_col0, out, ldo, n_seq, max_len, q_heads, kv_group, 128, 128)) return rc;
+    // fixed stride: the kernel writes all S rows of every sequence (zeros past seq_lens[b]), so they must lie inside `rows` and the grid,
+    // which covers max_len rows per sequence, must reach them
+    if (!cu_seqlens && (S < 1 || (long long)n_seq * S > rows || max_len < S))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: fixed stride needs S >= 1, n_seq * S <= rows and max_len >= S");
     cudaError_t e = launch_attn_tc128((const bf16*)qkv, ld, rows, q_col0, k_col0, v_col0, (bf16*)out, ldo, n_seq, max_len, S, q_heads, kv_group,
                                       cu_seqlens, seq_lens, scale, causal != 0, (cudaStream_t)stream);
     return cuda_status(nullptr, e, "attention d128 launch");
@@ -728,8 +771,11 @@ extern "C" int vqa_op_attention_d128_ex(const void* qkv, int32_t ld, int64_t row
                                         void* out, int32_t ldo, int32_t n_seq, int32_t max_len, int32_t q_heads, int32_t kv_group,
                                         const int32_t* cu_seqlens, const int32_t* kv_prefix, float scale, int32_t causal,
                                         int32_t pair_sequences, int32_t o_head_stride, int32_t d_out, void* stream) {
-    if (!qkv || !out || !cu_seqlens || n_seq <= 0 || max_len <= 0 || q_heads <= 0 || kv_group <= 0)
-        return fail(nullptr, VQA_ERR_INVALID_ARG, "bad attention argument");
+    if (!cu_seqlens) return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: null cu_seqlens");
+    if (int rc = check_attn_d128(qkv, ld, rows, q_col0, k_col0, v_col0, out, ldo, n_seq, max_len, q_heads, kv_group, o_head_stride, d_out))
+        return rc;
+    if (pair_sequences && (max_len > 64 || causal || kv_prefix))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: pair_sequences takes sequences of <= 64 rows, non-causal, without kv_prefix");
     cudaError_t e = launch_attn_tc128((const bf16*)qkv, ld, rows, q_col0, k_col0, v_col0, (bf16*)out, ldo, n_seq, max_len, 0, q_heads, kv_group,
                                       cu_seqlens, nullptr, scale, causal != 0, (cudaStream_t)stream, kv_prefix, pair_sequences != 0, o_head_stride, d_out);
     return cuda_status(nullptr, e, "attention d128 launch");
@@ -843,6 +889,90 @@ extern "C" int vqa_op_clip_embed_ln(const void* patch, const void* cls, const vo
         clip_embed_ln_kernel<256><<<(rows + 7) / 8, 256, 0, st>>>((const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma,
                                                                   (const bf16*)beta, y, n_images, P, eps);
     return cuda_status(nullptr, cudaGetLastError(), "clip embed launch");
+}
+
+// ------------------------------------------------------------------------------------------------ kernel-level ABI: the Qwen2.5-VL scoring path
+// Each entry launches one glue kernel of qwen_prefill / qwen_last_position / qwen_topk with their geometry (qwen_kernels.cuh).
+
+// rope_table_kernel into the caller's tables, then rope_inplace_kernel on n_heads heads of x; text_mode: bf16 table and bf16 products.
+extern "C" int vqa_op_qwen_rope(const int32_t* positions, int32_t rows, const int32_t* axis_of_dim, const float* inv_freq, int32_t half, float* cos_t,
+                                float* sin_t, void* x, int32_t ld, int32_t col0, int32_t n_heads, int32_t head_stride, int32_t head_dim,
+                                int32_t text_mode, void* stream) {
+    if (!positions || !axis_of_dim || !inv_freq || !cos_t || !sin_t || !x) return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen rope: null pointer");
+    if (rows <= 0 || n_heads <= 0 || head_dim <= 0 || head_dim % 16 || head_dim > head_stride || half * 2 != head_dim)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen rope: bad size (head_dim a multiple of 16, <= head_stride, == 2 * half)");
+    if (ld % 8 || col0 % 8 || head_stride % 8 || col0 < 0 || (long long)col0 + (long long)(n_heads - 1) * head_stride + head_dim > ld)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen rope: ld, col0, head_stride multiples of 8, heads inside ld");
+    if (!aligned(x, 16) || !aligned(cos_t, 16) || !aligned(sin_t, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen rope: x and the tables must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int round = text_mode != 0 ? 1 : 0;
+    rope_table_kernel<<<rope_table_blocks(rows, half), GLUE_THREADS, 0, st>>>(positions, rows, axis_of_dim, inv_freq, half, cos_t, sin_t, round);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        rope_inplace_kernel<<<rope_inplace_blocks(rows, n_heads, head_dim), GLUE_THREADS, 0, st>>>((bf16*)x, ld, col0, n_heads, head_stride, head_dim,
+                                                                                                  cos_t, sin_t, rows, round);
+        e = cudaGetLastError();
+    }
+    return cuda_status(nullptr, e, "qwen rope launch");
+}
+
+// gather_rows_kernel: dst row r = src row index[r / group] * group + r % group, for r < rows.
+extern "C" int vqa_op_gather_rows(const void* src, void* dst, const int32_t* index, int32_t rows, int32_t group, int32_t D, void* stream) {
+    if (!src || !dst || !index) return fail(nullptr, VQA_ERR_INVALID_ARG, "gather rows: null pointer");
+    if (rows <= 0 || group <= 0 || rows % group || D <= 0 || D % 8)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "gather rows: bad size (rows a multiple of group, D a multiple of 8)");
+    if (!aligned(src, 16) || !aligned(dst, 16)) return fail(nullptr, VQA_ERR_INVALID_ARG, "gather rows: src / dst must be 16-byte aligned");
+    gather_rows_kernel<<<rows, ROW_COPY_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)src, (bf16*)dst, index, group, D);
+    return cuda_status(nullptr, cudaGetLastError(), "gather rows launch");
+}
+
+// qwen_embed_kernel over `rows` = n * S output rows: row b * S + s < seq_lens[b] takes feats[feat_index] or embed[ids], the rest zero.
+extern "C" int vqa_op_qwen_embed(const int32_t* ids, const int32_t* feat_index, const int32_t* seq_lens, const void* embed, const void* feats, void* out,
+                                 int32_t rows, int32_t S, int32_t D, void* stream) {
+    if (!ids || !feat_index || !seq_lens || !embed || !feats || !out) return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen embed: null pointer");
+    if (rows <= 0 || S <= 0 || rows % S || D <= 0 || D % 8)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen embed: bad size (rows a multiple of S, D a multiple of 8)");
+    if (!aligned(embed, 16) || !aligned(feats, 16) || !aligned(out, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen embed: embed / feats / out must be 16-byte aligned");
+    qwen_embed_kernel<<<rows, ROW_COPY_THREADS, 0, (cudaStream_t)stream>>>(ids, feat_index, seq_lens, (const bf16*)embed, (const bf16*)feats,
+                                                                           (bf16*)out, S, D);
+    return cuda_status(nullptr, cudaGetLastError(), "qwen embed launch");
+}
+
+// The repetition-penalty bitmap: token_bitmap_kernel (cu_seqlens NULL) or token_bitmap_packed_kernel, OR-ed into the caller's bitmap.
+extern "C" int vqa_op_token_bitmap(const int32_t* ids, const int32_t* seq_lens, int32_t B, int32_t S, const int32_t* cu_seqlens, const int32_t* kv_prefix,
+                                   const int32_t* pair_seq, int32_t max_prompt_len, int32_t vocab, uint32_t* bitmap, void* stream) {
+    if (!ids || !bitmap) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: null pointer");
+    if (B <= 0 || vocab <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: bad size");
+    if (!aligned(bitmap, 4)) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: bitmap must be 4-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int words = token_bitmap_words(vocab);
+    if (cu_seqlens) {
+        if (!pair_seq || max_prompt_len <= 0)
+            return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: packed rows need pair_seq and max_prompt_len >= 1");
+        token_bitmap_packed_kernel<<<token_bitmap_packed_grid(max_prompt_len, B), GLUE_THREADS, 0, st>>>(ids, cu_seqlens, kv_prefix, pair_seq, vocab,
+                                                                                                       bitmap, words);
+    } else {
+        if (!seq_lens || S <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: padded rows need seq_lens and S >= 1");
+        token_bitmap_kernel<<<token_bitmap_blocks(B, S), GLUE_THREADS, 0, st>>>(ids, seq_lens, B, S, vocab, bitmap, words);
+    }
+    return cuda_status(nullptr, cudaGetLastError(), "token bitmap launch");
+}
+
+// topk_softmax_kernel (the trace output of qwen_topk) on caller logits [B, ldl].
+extern "C" int vqa_op_topk_softmax(const void* logits, int64_t ldl, int32_t B, int32_t V, float temperature, const uint32_t* pen_bitmap,
+                                   float repetition_penalty, int32_t K, int32_t* out_ids, float* out_probs, void* stream) {
+    if (!logits || !out_ids || !out_probs) return fail(nullptr, VQA_ERR_INVALID_ARG, "top-k softmax: null pointer");
+    if (B <= 0 || V <= 0 || ldl < V || K < 1 || K > TOPK_MAX) return fail(nullptr, VQA_ERR_INVALID_ARG, "top-k softmax: bad size (ldl >= V, 1 <= K <= 8)");
+    if (!(temperature > 0.f) || !(repetition_penalty > 0.f))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "top-k softmax: temperature and repetition penalty must be > 0");
+    if (!aligned(logits, 2) || !aligned(pen_bitmap, 4)) return fail(nullptr, VQA_ERR_INVALID_ARG, "top-k softmax: misaligned logits / bitmap");
+    const bool penalise = repetition_penalty != 1.0f;
+    topk_softmax_kernel<<<B, GLUE_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, (long long)ldl, V, 1.0f / temperature,
+                                                                      penalise ? pen_bitmap : nullptr, token_bitmap_words(V), repetition_penalty, K,
+                                                                      out_ids, out_probs);
+    return cuda_status(nullptr, cudaGetLastError(), "top-k softmax launch");
 }
 
 // ---------------------------------------------------------------------------------------------- image pre-processing (SURVEY 8(f)2)

@@ -431,15 +431,22 @@ class ops:
         return out, int(parts.value)
 
     @staticmethod
-    def lmhead_logprob(h: torch.Tensor, w: torch.Tensor, labels: torch.Tensor):
+    def lmhead_logprob(h: torch.Tensor, w: torch.Tensor, labels: torch.Tensor, temperature: float = 1.0, pen_bitmap=None,
+                       repetition_penalty: float = 1.0):
+        """The Qwen2.5-VL score's lm_head: log softmax(penalised bf16 logits / temperature)[labels] of h [M, K] against w [N, K], without
+        materialising the logits. pen_bitmap int32 [M, ceil(N / 32)] or None. Returns fp32 [M]."""
         lib = _lib.load()
         M, K = h.shape
         N = w.shape[0]
-        ntiles = (N + 127) // 128
-        scratch = torch.empty(4 * M * ntiles + M, dtype=torch.float32, device=h.device)
         out = torch.empty(M, dtype=torch.float32, device=h.device)
-        rc = lib.vqa_op_lmhead_logprob(_ptr(h), h.stride(0), _ptr(w), w.stride(0), M, N, K, _ptr(labels), _ptr(out),
-                                       _ptr(scratch), _stream_ptr(h.device))
+        need = C.c_size_t(0)
+        args = (_ptr(h), h.stride(0), _ptr(w), w.stride(0), M, N, K, _ptr(labels), float(temperature), _ptr(pen_bitmap), float(repetition_penalty),
+                _ptr(out))
+        rc = lib.vqa_op_lmhead_logprob(*args, None, 0, C.byref(need), _stream_ptr(h.device))
+        if rc != -4:        # a call without scratch stops at the scratch check and returns the size
+            _check(rc or -1, None, "vqa_op_lmhead_logprob")
+        scratch = torch.empty((need.value + 3) // 4, dtype=torch.float32, device=h.device)
+        rc = lib.vqa_op_lmhead_logprob(*args, _ptr(scratch), scratch.numel() * 4, None, _stream_ptr(h.device))
         _check(rc, None, "vqa_op_lmhead_logprob")
         return out
 
@@ -634,6 +641,91 @@ class ops:
                                       _stream_ptr(patch.device))
         _check(rc, None, "vqa_op_clip_embed_ln")
         return out
+
+    @staticmethod
+    def attention_d128(qkv: torch.Tensor, out: torch.Tensor, q_col0: int, k_col0: int, v_col0: int, n_seq: int, max_len: int, q_heads: int,
+                       kv_group: int, scale: float, causal: bool, S: int = 0, seq_lens=None, cu_seqlens=None, kv_prefix=None,
+                       pair_sequences: bool = False, o_head_stride: int = 128, d_out: int = 128, rows: Optional[int] = None):
+        """Head-dim-128 attention on packed rows qkv [rows, ld] into out (row stride out.stride(0)), in place: fixed stride S with seq_lens
+        [n_seq] (cu_seqlens None, vqa_op_attention_d128), or variable-length cu_seqlens [n_seq + 1] with the extras of
+        vqa_op_attention_d128_ex. rows defaults to qkv.shape[0]."""
+        lib = _lib.load()
+        rows = qkv.shape[0] if rows is None else rows
+        st = _stream_ptr(qkv.device)
+        if cu_seqlens is None:
+            rc = lib.vqa_op_attention_d128(_ptr(qkv), qkv.stride(0), rows, q_col0, k_col0, v_col0, _ptr(out), out.stride(0), n_seq, max_len, S,
+                                           q_heads, kv_group, None, _ptr(seq_lens), float(scale), 1 if causal else 0, st)
+        else:
+            rc = lib.vqa_op_attention_d128_ex(_ptr(qkv), qkv.stride(0), rows, q_col0, k_col0, v_col0, _ptr(out), out.stride(0), n_seq, max_len,
+                                              q_heads, kv_group, _ptr(cu_seqlens), _ptr(kv_prefix), float(scale), 1 if causal else 0,
+                                              1 if pair_sequences else 0, o_head_stride, d_out, st)
+        _check(rc, None, "vqa_op_attention_d128")
+        return out
+
+    @staticmethod
+    def qwen_rope(positions: torch.Tensor, axis_of_dim: torch.Tensor, inv_freq: torch.Tensor, x: torch.Tensor, col0: int, n_heads: int,
+                  head_stride: int, head_dim: int, text_mode: bool, cos_t=None, sin_t=None):
+        """M-RoPE as the scoring path applies it: tables from positions int32 [n_axes, rows], axis_of_dim int32 / inv_freq fp32 [head_dim / 2]
+        into cos_t / sin_t fp32 [rows, head_dim] (allocated when None), then n_heads heads of x bf16 [rows, ld] rotated in place.
+        Returns (cos_t, sin_t)."""
+        lib = _lib.load()
+        rows = positions.shape[1]
+        if cos_t is None:
+            cos_t = torch.empty(rows, head_dim, dtype=torch.float32, device=x.device)
+            sin_t = torch.empty(rows, head_dim, dtype=torch.float32, device=x.device)
+        rc = lib.vqa_op_qwen_rope(_ptr(positions), rows, _ptr(axis_of_dim), _ptr(inv_freq), head_dim // 2, _ptr(cos_t), _ptr(sin_t), _ptr(x),
+                                  x.stride(0), col0, n_heads, head_stride, head_dim, 1 if text_mode else 0, _stream_ptr(x.device))
+        _check(rc, None, "vqa_op_qwen_rope")
+        return cos_t, sin_t
+
+    @staticmethod
+    def gather_rows(src: torch.Tensor, index: torch.Tensor, group: int, out=None):
+        """out row r = src row index[r / group] * group + r % group, for every row of out (default: src's shape)."""
+        lib = _lib.load()
+        if out is None:
+            out = torch.empty_like(src)
+        rc = lib.vqa_op_gather_rows(_ptr(src), _ptr(out), _ptr(index), out.shape[0], group, out.shape[1], _stream_ptr(src.device))
+        _check(rc, None, "vqa_op_gather_rows")
+        return out
+
+    @staticmethod
+    def qwen_embed(ids: torch.Tensor, feat_index: torch.Tensor, seq_lens: torch.Tensor, embed: torch.Tensor, feats: torch.Tensor, S: int, out=None):
+        """The embedding splice over rows = ids.numel() rows of S (packed rows: seq_lens = cu_seqlens[n_seq:], S = rows). Returns out [rows, D]."""
+        lib = _lib.load()
+        rows, D = ids.numel(), embed.shape[1]
+        if out is None:
+            out = torch.empty(rows, D, dtype=torch.bfloat16, device=embed.device)
+        rc = lib.vqa_op_qwen_embed(_ptr(ids), _ptr(feat_index), _ptr(seq_lens), _ptr(embed), _ptr(feats), _ptr(out), rows, S, D,
+                                   _stream_ptr(embed.device))
+        _check(rc, None, "vqa_op_qwen_embed")
+        return out
+
+    @staticmethod
+    def token_bitmap(ids: torch.Tensor, vocab: int, B: int, seq_lens=None, S: int = 0, cu_seqlens=None, kv_prefix=None, pair_seq=None,
+                     max_prompt_len: int = 0, bitmap=None):
+        """The repetition-penalty bitmap int32 [B, ceil(vocab / 32)] (zeroed here when not given) of padded prompts (seq_lens, S) or packed
+        rows (cu_seqlens, kv_prefix, pair_seq, max_prompt_len)."""
+        lib = _lib.load()
+        if bitmap is None:
+            bitmap = torch.zeros(B, (vocab + 31) // 32, dtype=torch.int32, device=ids.device)
+        rc = lib.vqa_op_token_bitmap(_ptr(ids), _ptr(seq_lens), B, S, _ptr(cu_seqlens), _ptr(kv_prefix), _ptr(pair_seq), max_prompt_len, vocab,
+                                     _ptr(bitmap), _stream_ptr(ids.device))
+        _check(rc, None, "vqa_op_token_bitmap")
+        return bitmap
+
+    @staticmethod
+    def topk_softmax(logits: torch.Tensor, K: int, V: Optional[int] = None, temperature: float = 1.0, pen_bitmap=None,
+                     repetition_penalty: float = 1.0):
+        """The trace top-K of bf16 logits [B, >= V] (row stride logits.stride(0)): (ids int32 [B, K], probabilities fp32 [B, K])."""
+        lib = _lib.load()
+        B = logits.shape[0]
+        V = logits.shape[1] if V is None else V
+        ids = torch.full((B, K), -2, dtype=torch.int32, device=logits.device)
+        probs = torch.full((B, K), float("nan"), dtype=torch.float32, device=logits.device)
+        rc = lib.vqa_op_topk_softmax(_ptr(logits), logits.stride(0), B, V, float(temperature), _ptr(pen_bitmap), float(repetition_penalty), K,
+                                     _ptr(ids), _ptr(probs), _stream_ptr(logits.device))
+        _check(rc, None, "vqa_op_topk_softmax")
+        return ids, probs
 
 
 # ------------------------------------------------------------------------------------------------ image pre-processing

@@ -1,4 +1,5 @@
-"""Qwen2.5-VL path on a real H100: head-dim-128 wgmma attention vs torch, and the engine vs the oracle."""
+"""Qwen2.5-VL path on a real H100: the grouped qkv GEMM and the engine vs the oracle (the head-dim-128 attention has its kernel-level tests
+in test_gpu_qwen_kernels.py)."""
 import dataclasses
 
 import pytest
@@ -16,55 +17,6 @@ def dev():
     if not torch.cuda.is_available():
         pytest.skip("no GPU")
     return torch.device("cuda:0")
-
-
-def attn_d128(qkv, out_cols, n_seq, max_len, S, Hq, group, cu, lens, scale, causal, q0, k0, v0):
-    import ctypes as C
-    from t2v_metrics_b200 import _lib
-    from t2v_metrics_b200.engine import _ptr, _stream_ptr, _check
-    lib = _lib.load()
-    out = torch.zeros(qkv.shape[0], out_cols, dtype=torch.bfloat16, device=qkv.device)
-    rc = lib.vqa_op_attention_d128(_ptr(qkv), qkv.shape[1], qkv.shape[0], q0, k0, v0, _ptr(out), out_cols, n_seq, max_len, S, Hq, group,
-                                   _ptr(cu), _ptr(lens), float(scale), 1 if causal else 0, _stream_ptr(qkv.device))
-    _check(rc, None, "vqa_op_attention_d128")
-    torch.cuda.synchronize()
-    return out
-
-
-@pytest.mark.parametrize("lens", [[64] * 6, [64, 64, 40, 64, 17], [8, 64, 64], [33]])
-def test_window_pairs_and_compact_heads_d128(dev, lens):
-    """Vision-tower windows (<= 64 tokens, modeling_qwen2_5_vl.py get_window_index) two per 128-row tile under a block-diagonal mask, output
-    heads written compactly at their native width (80): must equal the one-window-per-tile launch and the fp32 reference."""
-    import ctypes as C
-    from t2v_metrics_b200 import _lib
-    from t2v_metrics_b200.engine import _ptr, _stream_ptr, _check
-    lib = _lib.load()
-    torch.manual_seed(5)
-    H, hd = 3, 80
-    L = sum(lens)
-    x = torch.zeros(L, 3, H, 128, device=dev)
-    x[..., :hd] = torch.randn(L, 3, H, hd, device=dev) * 0.7
-    x[:, 2, :, hd:] = 7.0                                   # V padding need not be zero: those output columns are never written
-    qkv = x.reshape(L, 3 * H * 128).bfloat16()
-    cu = torch.tensor([0] + torch.tensor(lens).cumsum(0).tolist(), dtype=torch.int32, device=dev)
-    outs = []
-    for pair in (0, 1):
-        out = torch.full((L, H * hd), 3.0, dtype=torch.bfloat16, device=dev)
-        rc = lib.vqa_op_attention_d128_ex(_ptr(qkv), qkv.shape[1], L, 0, H * 128, 2 * H * 128, _ptr(out), H * hd, len(lens), max(lens), H, 1, _ptr(cu),
-                                          None, float(hd ** -0.5), 0, pair, hd, hd, _stream_ptr(qkv.device))
-        _check(rc, None, "vqa_op_attention_d128_ex")
-        torch.cuda.synchronize()
-        outs.append(out.float())
-    xf = qkv.float().view(L, 3, H, 128)[..., :hd]
-    ref = torch.zeros(L, H, hd, device=dev)
-    o = 0
-    for n in lens:
-        q, k, v = (xf[o:o + n, i].transpose(0, 1) for i in range(3))
-        ref[o:o + n] = (torch.softmax(q @ k.transpose(1, 2) * hd ** -0.5, -1) @ v).transpose(0, 1)
-        o += n
-    assert float((outs[0] - ref.reshape(L, H * hd)).abs().max()) < 0.02
-    assert float((outs[1] - ref.reshape(L, H * hd)).abs().max()) < 0.02
-    assert float((outs[1] - outs[0]).abs().max()) < 4e-3        # same keys, same tile: only masked columns differ
 
 
 def test_gemm_grouped_output_columns(dev):
@@ -85,48 +37,6 @@ def test_gemm_grouped_output_columns(dev):
     got = c.float().view(M, G, go)
     assert float((got[..., :gi] - ref).abs().max()) < 0.03
     assert bool((got[..., gi:] == -5.0).all())
-
-
-@pytest.mark.parametrize("B,S,Hq,Hkv", [(3, 320, 4, 2), (2, 130, 2, 1), (1, 64, 28, 4)])
-def test_causal_gqa_attention_d128(dev, B, S, Hq, Hkv):
-    torch.manual_seed(0)
-    cols = (Hq + 2 * Hkv) * 128
-    qkv = (torch.randn(B * S, cols, device=dev) * 0.5).bfloat16()
-    lens = torch.randint(max(1, S // 2), S + 1, (B,), device=dev, dtype=torch.int32)
-    out = attn_d128(qkv, Hq * 128, B, S, S, Hq, Hq // Hkv, None, lens, 128 ** -0.5, True, 0, Hq * 128, (Hq + Hkv) * 128)
-    x = qkv.float().view(B, S, Hq + 2 * Hkv, 128)
-    q, k, v = x[:, :, :Hq], x[:, :, Hq:Hq + Hkv], x[:, :, Hq + Hkv:]
-    k = k.repeat_interleave(Hq // Hkv, dim=2)
-    v = v.repeat_interleave(Hq // Hkv, dim=2)
-    sc = torch.einsum("bqhd,bkhd->bhqk", q, k) * 128 ** -0.5
-    mask = torch.tril(torch.ones(S, S, dtype=torch.bool, device=dev))[None, None] & (torch.arange(S, device=dev)[None, None, None, :] < lens[:, None, None, None])
-    sc = sc.masked_fill(~mask, float("-inf"))
-    ref = torch.einsum("bhqk,bkhd->bqhd", torch.softmax(sc, -1), v).reshape(B * S, Hq * 128)
-    valid = (torch.arange(S, device=dev)[None, :] < lens[:, None]).reshape(-1)
-    assert float((out[valid].float() - ref[valid]).abs().max()) < 0.02
-    assert float(out[~valid].float().abs().max()) == 0.0 if (~valid).any() else True
-
-
-def test_varlen_window_attention_d128_padded_heads(dev):
-    """Vision-tower layout: 80-wide heads zero-padded to 128 columns, variable-length windows via cu_seqlens."""
-    torch.manual_seed(1)
-    H, hd = 4, 80
-    lens = [64, 64, 16, 48, 130, 2]
-    L = sum(lens)
-    cu = torch.tensor([0] + list(torch.tensor(lens).cumsum(0)), dtype=torch.int32, device=dev)
-    x = torch.zeros(L, 3, H, 128, device=dev)
-    x[..., :hd] = torch.randn(L, 3, H, hd, device=dev) * 0.5
-    qkv = x.reshape(L, 3 * H * 128).bfloat16()
-    out = attn_d128(qkv, H * 128, len(lens), max(lens), 0, H, 1, cu, None, hd ** -0.5, False, 0, H * 128, 2 * H * 128)
-    xf = qkv.float().view(L, 3, H, 128)
-    ref = torch.zeros(L, H, 128, device=dev)
-    s = 0
-    for n in lens:
-        q, k, v = (xf[s:s + n, i].transpose(0, 1) for i in range(3))
-        p = torch.softmax(torch.matmul(q, k.transpose(1, 2)) * hd ** -0.5, -1)
-        ref[s:s + n] = torch.matmul(p, v).transpose(0, 1)
-        s += n
-    assert float((out.float() - ref.reshape(L, H * 128)).abs().max()) < 0.02
 
 
 def make_engine(cfg, sd, dev):
