@@ -130,9 +130,11 @@ size_t vqa_clipt5_workspace_bytes(vqa_handle* h, int32_t batch, int32_t n_images
  *   image_index DEVICE int32 [batch] -> which image each pair uses, or NULL for identity (n_images == batch)
  *   input_ids   DEVICE int32 [batch, text_len], image slot = cfg.image_token_id, right-padded with pad_token_id
  *   text_lens   DEVICE int32 [batch] valid ids per row
- *   labels      DEVICE int32 [batch, label_len], -100 = ignored (padding)
- *   out_scores  DEVICE float [batch] : exp(-mean CE)  (v3.0 CLIPT5Model.forward)
- *   out_logprobs DEVICE float [batch, label_len] per-token log-probabilities, or NULL
+ *   labels      DEVICE int32 [batch, label_len] < vocab, -100 = ignored (padding). Every negative label is ignored like -100: it adds
+ *               nothing to the mean and the decoder input after it is pad_token_id
+ *   out_scores  DEVICE float [batch] : exp(-mean CE)  (v3.0 CLIPT5Model.forward); NaN for a pair whose labels are all ignored, as the
+ *               reference's CrossEntropyLoss(reduction='mean') gives over zero targets
+ *   out_logprobs DEVICE float [batch, label_len] per-token log-probabilities (ignored positions are not written), or NULL
  *   workspace   DEVICE, >= vqa_clipt5_workspace_bytes(...)
  *   stream      cudaStream_t
  */
@@ -455,7 +457,9 @@ int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, int32_t cap,
 int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32_t H, const int32_t* seq_lens,
                          const float* bias_table, float scale, int32_t bias_const_from, int32_t round_scores, void* stream);
 
-/* T5LayerNorm / nn.LayerNorm on [rows, D] bf16. beta == NULL selects T5 RMS norm. */
+/* T5LayerNorm / nn.LayerNorm on [rows, D] bf16. beta == NULL selects T5 RMS norm: y = gamma * bf16(x * rsqrt(mean(x^2) + eps)), fp32
+ * statistics; D a multiple of 8 up to 8192. LayerNorm: D in {256, 512, 768, 1024, 1280}. rows >= 1; x, gamma, beta and y 16-byte aligned;
+ * else VQA_ERR_INVALID_ARG before anything launches. */
 int vqa_op_norm(const void* x, const void* gamma, const void* beta, void* y, int32_t rows, int32_t D, float eps,
                 void* stream);
 
@@ -528,6 +532,50 @@ int vqa_op_layernorm_f32(const float* x, const void* gamma, const void* beta, vo
  * cls [D], pos [P + 1, D], gamma / beta [D]. D in {256, 1024} (else VQA_ERR_UNSUPPORTED); pointers 16-byte aligned. */
 int vqa_op_clip_embed_ln(const void* patch, const void* cls, const void* pos, const void* gamma, const void* beta, float* y, int32_t n_images,
                          int32_t P, int32_t D, float eps, void* stream);
+
+/* The CLIP-FlanT5 scoring path's glue kernels, launched as vqa_clipt5_score / vqa_clipt5_generate_* launch them. All pointers DEVICE. */
+
+/* Patch gather for the patch-embedding GEMM: pixels [n_images, 3, image_size, image_size] (pixel_dtype F32 or BF16) -> out bf16
+ * [n_images * P, kpad], P = (image_size / patch)^2, row i * P + py * (image_size / patch) + px, column c * patch^2 + ky * patch + kx holding
+ * bf16(pixel); columns [3 * patch^2, kpad) are +0. kpad a multiple of 8 and >= 3 * patch^2; pixels aligned to their element size, out 16-byte
+ * aligned. */
+int vqa_op_patchify(const void* pixels, int32_t pixel_dtype, int32_t n_images, int32_t image_size, int32_t patch, int32_t kpad, void* out,
+                    void* stream);
+
+/* Multimodal splice into the encoder input out bf16 [B, S, D], S = L - 1 + P, and seq_lens int32 [B]. Row b's first text_lens[b] (1..L)
+ * ids of ids int32 [B, L] are embedded with shared_emb bf16 [vocab, D] (ids in [0, vocab)), except that the first id equal to image_token
+ * is replaced by the P feature rows of image image_index[b] (NULL: image b), rows [img * feat_rows_per_image + feat_row_offset, + P) of
+ * feats bf16 (row stride ldf). seq_lens[b] = text_lens[b] - 1 + P with an image slot, text_lens[b] without; rows past it are +0. D and ldf
+ * multiples of 8, ldf >= D, feat_row_offset + P <= feat_rows_per_image; shared_emb / feats / out 16-byte aligned. */
+int vqa_op_splice_embed(const int32_t* ids, const int32_t* text_lens, const int32_t* image_index, const void* shared_emb, const void* feats,
+                        int32_t ldf, int32_t feat_row_offset, int32_t feat_rows_per_image, void* out, int32_t* seq_lens, int32_t B, int32_t L,
+                        int32_t P, int32_t D, int32_t image_token, void* stream);
+
+/* Decoder input embeddings out bf16 [B * T, D] of shift_right(labels): row (b, 0) is shared_emb[start_id], row (b, t > 0) is
+ * shared_emb[labels[b, t - 1]], or shared_emb[pad_id] for a negative label. labels int32 [B, T] (< vocab), or NULL with T = 1 (the
+ * generation prefill's start token). D a multiple of 8; shared_emb / out 16-byte aligned. */
+int vqa_op_decoder_embed(const int32_t* labels, const void* shared_emb, void* out, int32_t B, int32_t T, int32_t D, int32_t start_id,
+                         int32_t pad_id, void* stream);
+
+/* The T5 encoder's relative-position bias table: table float [H, 2S - 1], table[h, r] = rel_emb[bucket_lut[clamp(r - (S - 1), +-max_distance)
+ * + max_distance], h] with rel_emb bf16 [num_buckets, H] and bucket_lut int32 [2 * max_distance + 1] (vqa_t5_bucket_lut). Past
+ * |r - (S - 1)| >= max_distance every entry of a head and side equals the one at +-max_distance, which the encoder attention relies on
+ * (bias_const_from = max_distance). */
+int vqa_op_t5_bias_table(const void* rel_emb, const int32_t* bucket_lut, int32_t max_distance, float* table, int32_t H, int32_t S,
+                         void* stream);
+
+/* The tail of vqa_clipt5_score: the lm_head of H bf16 [B * T, ldh] against W bf16 [N, ldw] with its fused log-softmax gather of labels int32
+ * [B, T] (< N; negative = ignored), then scores[b] = exp(mean of logprobs[b, t] over the labels of row b) (NaN when all are ignored) and,
+ * unless logprobs is NULL, logprobs float [B * T] = bf16 logit of the label - logsumexp of the bf16 logits (ignored positions not written).
+ * K, ldh, ldw multiples of 8 and >= K; H / W 16-byte aligned. scratch DEVICE float: the layout of vqa_op_lmhead_logprob at M = B * T (the
+ * scores slot unused); *scratch_needed (HOST, optional) receives its size in bytes, also when a smaller scratch_bytes returns
+ * VQA_ERR_WORKSPACE. */
+int vqa_op_lmhead_score(const void* H, int32_t ldh, const void* W, int32_t ldw, int32_t B, int32_t T, int32_t N, int32_t K, const int32_t* labels,
+                        float* scores, float* logprobs, float* scratch, size_t scratch_bytes, size_t* scratch_needed, void* stream);
+
+/* Sum of squares of every row of x bf16 [rows, D] (fp32) into ssq float [rows, stride] at column 0, the seed of the fused-RMSNorm chain
+ * (see vqa_op_gemm_bf16_normfuse); columns 1.. are not written. D a multiple of 8; x 16-byte aligned. */
+int vqa_op_row_ssq(const void* x, float* ssq, int32_t rows, int32_t D, int32_t stride, void* stream);
 
 /* The Qwen2.5-VL scoring path's glue kernels, launched as vqa_qwen25vl_score launches them. All pointers DEVICE. */
 

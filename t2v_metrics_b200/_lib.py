@@ -28,6 +28,7 @@ ABI_SYMBOLS = [
     "vqa_op_t5_decode_self_attn", "vqa_op_gemm_bf16_f32acc", "vqa_op_gemm_bf16_batched", "vqa_op_t5_cross_attention", "vqa_op_layernorm_f32",
     "vqa_op_clip_embed_ln", "vqa_qwen_preprocess_video_plan", "vqa_qwen_preprocess_video",
     "vqa_op_qwen_rope", "vqa_op_gather_rows", "vqa_op_qwen_embed", "vqa_op_token_bitmap", "vqa_op_topk_softmax",
+    "vqa_op_patchify", "vqa_op_splice_embed", "vqa_op_decoder_embed", "vqa_op_t5_bias_table", "vqa_op_lmhead_score", "vqa_op_row_ssq",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -174,6 +175,18 @@ def load() -> C.CDLL:
     lib.vqa_op_token_bitmap.restype = C.c_int
     lib.vqa_op_topk_softmax.argtypes = [vp, i64, i32, i32, f32, vp, f32, i32, vp, vp, vp]
     lib.vqa_op_topk_softmax.restype = C.c_int
+    lib.vqa_op_patchify.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp]
+    lib.vqa_op_patchify.restype = C.c_int
+    lib.vqa_op_splice_embed.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, i32, i32, i32, i32, i32, vp]
+    lib.vqa_op_splice_embed.restype = C.c_int
+    lib.vqa_op_decoder_embed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
+    lib.vqa_op_decoder_embed.restype = C.c_int
+    lib.vqa_op_t5_bias_table.argtypes = [vp, vp, i32, vp, i32, i32, vp]
+    lib.vqa_op_t5_bias_table.restype = C.c_int
+    lib.vqa_op_lmhead_score.argtypes = [vp, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, C.c_size_t, C.POINTER(C.c_size_t), vp]
+    lib.vqa_op_lmhead_score.restype = C.c_int
+    lib.vqa_op_row_ssq.argtypes = [vp, vp, i32, i32, i32, vp]
+    lib.vqa_op_row_ssq.restype = C.c_int
     lib.vqa_clipt5_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
     lib.vqa_clipt5_generate_workspace_bytes.restype = C.c_size_t
     lib.vqa_clipt5_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]

@@ -173,6 +173,55 @@ __global__ void __launch_bounds__(256) row_ssq_kernel(const bf16* __restrict__ x
     if (lane == 0) ssq[(size_t)row * stride] = ss;
 }
 
+// ------------------------------------------------------------------------------------------------ glue launches
+// The launches of the scoring path's glue kernels. The forwards below and the kernel-level entry points (vqa_b200.cu) both call these, so
+// the two cannot launch a kernel with different geometry.
+
+// Pixels [n_images, 3, image_size, image_size] (fp32 or bf16) -> patch rows out [n_images * P, kpad] bf16.
+static int clipt5_patchify(Forward& f, const void* pixels, int pixel_dtype, bf16* out, int n_images, int image_size, int patch, int kpad) {
+    const int rows = n_images * (image_size / patch) * (image_size / patch);
+    if (pixel_dtype == VQA_DTYPE_F32)
+        return f.launch(CAT_OTHER, 0, "patchify", patchify_kernel<float>, rows, 128, 0, reinterpret_cast<const float*>(pixels), out, n_images,
+                        image_size, image_size, patch, kpad);
+    return f.launch(CAT_OTHER, 0, "patchify", patchify_kernel<bf16>, rows, 128, 0, reinterpret_cast<const bf16*>(pixels), out, n_images,
+                    image_size, image_size, patch, kpad);
+}
+
+// Text embeddings and image features -> the encoder input x [B, S = L - 1 + P, D] and seq_lens [B]. Image i's features are rows
+// [i * rows_per_image + row_offset, + P) of feats (row stride ldf).
+static int clipt5_splice(Forward& f, const int* ids, const int* text_lens, const int* image_index, const bf16* shared, const bf16* feats, int ldf,
+                         int row_offset, int rows_per_image, bf16* x, int* seq_lens, int B, int L, int P, int D, int image_token) {
+    const int S = L - 1 + P;
+    return f.launch(CAT_OTHER, 0, "splice", splice_embed_kernel, B * S, 128, 0, ids, text_lens, image_index, shared, feats, ldf, row_offset,
+                    rows_per_image, x, seq_lens, B, L, S, P, D, image_token);
+}
+
+// The encoder's relative-position bias table [H, 2S - 1] fp32 from rel_emb [buckets, H] and the bucket LUT [2 * max_distance + 1].
+static int clipt5_bias_table(Forward& f, const bf16* rel_emb, const int* lut, int max_distance, float* table, int H, int S) {
+    return f.launch(CAT_OTHER, 0, "bias table", bias_table_from_lut_kernel, (H * (2 * S - 1) + 255) / 256, 256, 0, rel_emb, lut, max_distance,
+                    table, H, S);
+}
+
+// Decoder input embeddings y [B * T, D] of shift_right(labels [B, T]); labels NULL with T = 1: the start token (generation prefill).
+static int clipt5_decoder_embed(Forward& f, const int* labels, const bf16* shared, bf16* y, int B, int T, int D, int start_id, int pad_id) {
+    return f.launch(CAT_OTHER, 0, "decoder embed", decoder_embed_kernel, B * T, 128, 0, labels, shared, y, T, D, start_id, pad_id);
+}
+
+// The score's tail: the EPI_LSE lm_head GEMM g (M = B * T rows) with its (max, sum) partials and label logits, then lse_finalize_kernel into
+// scores [B] and, unless NULL, logprobs [B * T].
+static int clipt5_lmhead_score(Forward& f, Gemm g, const int* labels, float* lse_max, float* lse_sum, float* label_logit, float* scores,
+                               float* logprobs, int B, int T) {
+    const int ntiles = LMHEAD_PARTS * ((g.N + LMHEAD_BN - 1) / LMHEAD_BN);
+    TRY(f.gemm(g.lse(labels, lse_max, lse_sum, label_logit), "lm_head"));
+    return f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, (const float*)lse_max, (const float*)lse_sum,
+                    (const float*)label_logit, labels, scores, logprobs, B, T, ntiles);
+}
+
+// Sum of squares of the rows of x [rows, D] into slot 0 of ssq [rows, stride].
+static int clipt5_row_ssq(Forward& f, const bf16* x, float* ssq, int rows, int D, int stride) {
+    return f.launch(CAT_NORM, 0, "row ssq", row_ssq_kernel, (rows + 7) / 8, 256, 0, x, ssq, rows, D, stride);
+}
+
 // ------------------------------------------------------------------------------------------------ forward
 // Encoder output x [B * S, Dm] -> xt [B, Dm, Sp] (Sp = S rounded up to 8, columns [S, Sp) zero): the K-major operand of GEMM (3) of the
 // absorbed cross-attention.
@@ -217,12 +266,7 @@ static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Promp
     float* hv = f.at<float>(w.hv);
 
     // ---------------- vision tower (CLIP ViT, layers 0 .. vit_layers_run-1; hidden_states[-2]) ----------------
-    if (pixel_dtype == VQA_DTYPE_F32)
-        TRY(f.launch(CAT_OTHER, 0, "patchify", patchify_kernel<float>, Mp, 128, 0, reinterpret_cast<const float*>(pixels), P_(w.patches),
-                     n_images, c.image_size, c.image_size, c.patch_size, h->kpad));
-    else
-        TRY(f.launch(CAT_OTHER, 0, "patchify", patchify_kernel<bf16>, Mp, 128, 0, reinterpret_cast<const bf16*>(pixels), P_(w.patches),
-                     n_images, c.image_size, c.image_size, c.patch_size, h->kpad));
+    TRY(clipt5_patchify(f, pixels, pixel_dtype, P_(w.patches), n_images, c.image_size, c.patch_size, h->kpad));
     TRY(f.gemm(Gemm(P_(w.patches), h->patch_w, P_(w.patch_out), Mp, Dv, h->kpad)));
     if (Dv == 1024)
         TRY(f.launch(CAT_NORM, 0, "clip_embed_ln", clip_embed_ln_kernel<1024>, (Mv + 7) / 8, 256, 0, P_(w.patch_out), h->cls, h->pos,
@@ -258,10 +302,9 @@ static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Promp
     {
         auto g = f.group(CAT_OTHER);
         // feature block of an image = P + 1 rows, first patch row = 1 (drop CLS: mm_vision_select_feature='patch')
-        TRY(f.launch(CAT_OTHER, 0, "splice", splice_embed_kernel, B * S, 128, 0, input_ids, text_lens, image_index, h->shared, P_(w.proj2),
-                     Dm, 1, P + 1, P_(w.x), seq_lens, B, L, S, P, Dm, c.image_token_id));
-        TRY(f.launch(CAT_OTHER, 0, "bias table", bias_table_from_lut_kernel, (H * (2 * S - 1) + 255) / 256, 256, 0, h->enc_rel, h->lut_bidir,
-                     c.rel_max_distance, bias_table, H, S));
+        TRY(clipt5_splice(f, input_ids, text_lens, image_index, h->shared, P_(w.proj2), Dm, 1, P + 1, P_(w.x), seq_lens, B, L, P, Dm,
+                          c.image_token_id));
+        TRY(clipt5_bias_table(f, h->enc_rel, h->lut_bidir, c.rel_max_distance, bias_table, H, S));
     }
 
     // ---------------- T5 encoder ----------------
@@ -281,7 +324,7 @@ static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Promp
         auto g = f.group(CAT_NORM);
         TRY(f.memset0(ssq_cur, (size_t)M * stride * 4, "ssq clear"));
         TRY(f.memset0(ssq_nxt, (size_t)M * stride * 4, "ssq clear"));
-        TRY(f.launch(CAT_NORM, 0, "row ssq", row_ssq_kernel, (M + 7) / 8, 256, 0, P_(w.x), ssq_cur, M, Dm, stride));
+        TRY(clipt5_row_ssq(f, P_(w.x), ssq_cur, M, Dm, stride));
     }
     for (int l = 0; l < c.enc_layers; ++l) {
         const T5EncLayerW& Lw = h->enc[l];
@@ -391,8 +434,7 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
     int* seq_lens = f.at<int>(w.seq_lens);
 
     // ---------------- T5 decoder (T target rows per pair) ----------------
-    TRY(f.launch(CAT_OTHER, 0, "decoder embed", decoder_embed_kernel, Md, 128, 0, labels, h->shared, P_(w.y), T, Dm, c.decoder_start_id,
-                 c.pad_token_id));
+    TRY(clipt5_decoder_embed(f, labels, h->shared, P_(w.y), B, T, Dm, c.decoder_start_id, c.pad_token_id));
     auto dec = [&](Gemm g) { return decoder_split_k(f, w, g); };
     for (int l = 0; l < c.dec_layers; ++l) {
         const T5DecLayerW& Lw = h->dec[l];
@@ -418,14 +460,8 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
     TRY(f.rmsnorm(P_(w.y), h->dec_final_ln, P_(w.yn), Md, Dm, c.t5_ln_eps));
 
     // ---------------- lm_head x hidden, fused log-sum-exp + label gather; logits never reach HBM ----------------
-    float* lse_max = f.at<float>(w.lse_max);
-    float* lse_sum = f.at<float>(w.lse_sum);
-    float* label_logit = f.at<float>(w.label_logit);
-    const int ntiles = LMHEAD_PARTS * ((c.vocab + LMHEAD_BN - 1) / LMHEAD_BN);
-    TRY(f.gemm(Gemm(P_(w.yn), h->lm_head, nullptr, Md, c.vocab, Dm).lse(labels, lse_max, lse_sum, label_logit), "lm_head"));
-    TRY(f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, lse_max, lse_sum, label_logit, labels, out_scores,
-                 out_logprobs, B, T, ntiles));
-    return VQA_OK;
+    return clipt5_lmhead_score(f, Gemm(P_(w.yn), h->lm_head, nullptr, Md, c.vocab, Dm), labels, f.at<float>(w.lse_max), f.at<float>(w.lse_sum),
+                               f.at<float>(w.label_logit), out_scores, out_logprobs, B, T);
 }
 
 // ================================================================================================ greedy generation
@@ -480,8 +516,7 @@ static int clipt5_decode_step(Forward& f, const ClipT5GenWorkspace& g, int B, in
     const int Dm = c.d_model, H = c.n_heads, inner = H * 64;
     int* next_ids = f.at<int>(g.next_ids);
     if (first)    // decoder_embed_kernel at T = 1 embeds the start token and reads no labels
-        TRY(f.launch(CAT_OTHER, 0, "decoder embed", decoder_embed_kernel, B, 128, 0, (const int*)nullptr, h->shared, P_(w.y), 1, Dm,
-                     c.decoder_start_id, c.pad_token_id));
+        TRY(clipt5_decoder_embed(f, nullptr, h->shared, P_(w.y), B, 1, Dm, c.decoder_start_id, c.pad_token_id));
     else
         TRY(f.launch(CAT_OTHER, 0, "decoder embed", gather_rows_by_index_kernel, B, 128, 0, h->shared, (const int*)next_ids, P_(w.y), Dm));
     auto dec = [&](Gemm gm) { return decoder_split_k(f, w, gm); };

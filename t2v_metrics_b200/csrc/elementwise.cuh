@@ -330,14 +330,15 @@ __global__ void splice_embed_kernel(const int* __restrict__ ids,          // [B,
 }
 
 // Decoder input embedding: decoder_input_ids = shift_right(labels) (modeling_t5.py:595-614): [start, l0, l1, ...],
-// -100 -> pad. One block per (b, t).
+// -100 -> pad. Every negative label becomes pad, not only -100: lse_finalize_kernel ignores all of them, and no negative id may index
+// shared_emb. One block per (b, t).
 __global__ void decoder_embed_kernel(const int* __restrict__ labels,  // [B, T]
                                      const __nv_bfloat16* __restrict__ shared_emb, __nv_bfloat16* __restrict__ out,
                                      int T, int D, int start_id, int pad_id) {
     pdl_launch_dependents();
     const int b = blockIdx.x / T, t = blockIdx.x % T;
     int id = (t == 0) ? start_id : labels[b * T + t - 1];
-    if (id == -100) id = pad_id;
+    if (id < 0) id = pad_id;
     const uint4* src = reinterpret_cast<const uint4*>(shared_emb + (size_t)id * D);
     uint4* dst = reinterpret_cast<uint4*>(out + (size_t)blockIdx.x * D);
     for (int i = threadIdx.x; i < (D >> 3); i += blockDim.x) dst[i] = src[i];
@@ -358,8 +359,9 @@ __global__ void bias_table_from_lut_kernel(const __nv_bfloat16* __restrict__ rel
 }
 
 // Combine per-tile (max, sumexp) partials and the gathered label logits into the score:
-//   logp[b,t] = logit[label] - logsumexp ; score[b] = exp(mean_t logp[b,t]) over labels != -100
-// (v3.0 CLIPT5Model.forward: (-CrossEntropyLoss(reduction='mean')(logits[k], labels[k])).exp()). One warp per sample.
+//   logp[b,t] = logit[label] - logsumexp ; score[b] = exp(mean_t logp[b,t]) over labels >= 0
+// (v3.0 CLIPT5Model.forward: (-CrossEntropyLoss(reduction='mean')(logits[k], labels[k])).exp()). A sample without a label scores NaN, the
+// 0 / 0 of that mean. logprobs of ignored labels are not written. One warp per sample.
 __global__ void lse_finalize_kernel(const float* __restrict__ lse_max, const float* __restrict__ lse_sum,
                                     const float* __restrict__ label_logit, const int* __restrict__ labels,
                                     float* __restrict__ scores, float* __restrict__ logprobs, int B, int T,
@@ -387,7 +389,7 @@ __global__ void lse_finalize_kernel(const float* __restrict__ lse_max, const flo
         acc += lp;
         ++cnt;
     }
-    if (lane == 0) scores[b] = cnt > 0 ? expf(acc / (float)cnt) : 0.f;
+    if (lane == 0) scores[b] = cnt > 0 ? expf(acc / (float)cnt) : __int_as_float(0x7fc00000);
 }
 
 }  // namespace vqa

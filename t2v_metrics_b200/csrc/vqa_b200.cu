@@ -783,7 +783,12 @@ extern "C" int vqa_op_attention_d128_ex(const void* qkv, int32_t ld, int64_t row
 
 extern "C" int vqa_op_norm(const void* x, const void* gamma, const void* beta, void* y, int32_t rows, int32_t D, float eps,
                            void* stream) {
-    if (!x || !gamma || !y) return fail(nullptr, VQA_ERR_INVALID_ARG, "null pointer");
+    if (!x || !gamma || !y) return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: null pointer");
+    if (rows <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: rows must be >= 1");
+    if (beta ? !(D == 256 || D == 512 || D == 768 || D == 1024 || D == 1280) : (D <= 0 || D % 8 || D > 8192))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: LayerNorm takes D = 256, 512, 768, 1024 or 1280; RMSNorm a multiple of 8 up to 8192");
+    if (!aligned(x, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: x / gamma / beta / y must be 16-byte aligned");
     cudaError_t e = beta ? run_layernorm((const bf16*)x, (const bf16*)gamma, (const bf16*)beta, (bf16*)y, rows, D, eps, (cudaStream_t)stream)
                          : run_rmsnorm((const bf16*)x, (const bf16*)gamma, (bf16*)y, rows, D, eps, (cudaStream_t)stream);
     return cuda_status(nullptr, e, "norm launch");
@@ -889,6 +894,95 @@ extern "C" int vqa_op_clip_embed_ln(const void* patch, const void* cls, const vo
         clip_embed_ln_kernel<256><<<(rows + 7) / 8, 256, 0, st>>>((const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma,
                                                                   (const bf16*)beta, y, n_images, P, eps);
     return cuda_status(nullptr, cudaGetLastError(), "clip embed launch");
+}
+
+// The glue launches of clipt5.cuh on the caller's stream, through a handle of their own that only counts the launches and keeps the error
+// text.
+template <typename Body>
+static int glue_launch(void* stream, Body&& body) {
+    vqa_handle launcher;
+    launcher.num_sms = device_sms();
+    Forward f(&launcher, nullptr, (cudaStream_t)stream);
+    const int rc = body(f);
+    return rc == VQA_OK ? VQA_OK : fail(nullptr, rc, launcher.err);
+}
+
+extern "C" int vqa_op_patchify(const void* pixels, int32_t pixel_dtype, int32_t n_images, int32_t image_size, int32_t patch, int32_t kpad, void* out,
+                               void* stream) {
+    if (!pixels || !out) return fail(nullptr, VQA_ERR_INVALID_ARG, "patchify: null pointer");
+    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(nullptr, VQA_ERR_INVALID_ARG, "patchify: pixels fp32 or bf16");
+    if (n_images <= 0 || patch <= 0 || image_size < patch || kpad % 8 || kpad < 3 * patch * patch)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "patchify: bad size (patch <= image_size, kpad a multiple of 8 and >= 3 * patch^2)");
+    if ((long long)n_images * (image_size / patch) * (image_size / patch) > INT32_MAX)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "patchify: too many patch rows");
+    if (!aligned(pixels, pixel_dtype == VQA_DTYPE_F32 ? 4 : 2) || !aligned(out, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "patchify: pixels aligned to their element size, out 16-byte aligned");
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_patchify(f, pixels, pixel_dtype, (bf16*)out, n_images, image_size, patch, kpad);
+    });
+}
+
+extern "C" int vqa_op_splice_embed(const int32_t* ids, const int32_t* text_lens, const int32_t* image_index, const void* shared_emb, const void* feats,
+                                   int32_t ldf, int32_t feat_row_offset, int32_t feat_rows_per_image, void* out, int32_t* seq_lens, int32_t B, int32_t L,
+                                   int32_t P, int32_t D, int32_t image_token, void* stream) {
+    if (!ids || !text_lens || !shared_emb || !feats || !out || !seq_lens) return fail(nullptr, VQA_ERR_INVALID_ARG, "splice: null pointer");
+    if (B <= 0 || L <= 0 || P <= 0 || D <= 0 || D % 8 || ldf % 8 || ldf < D || feat_row_offset < 0 ||
+        (long long)feat_row_offset + P > feat_rows_per_image || (long long)B * (L - 1 + P) > INT32_MAX)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "splice: bad size (D, ldf multiples of 8, ldf >= D, the P feature rows inside each image's block)");
+    if (!aligned(ids, 4) || !aligned(text_lens, 4) || !aligned(image_index, 4) || !aligned(seq_lens, 4) || !aligned(shared_emb, 16) ||
+        !aligned(feats, 16) || !aligned(out, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "splice: int32 arrays 4-byte aligned, embeddings / features / out 16-byte aligned");
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_splice(f, ids, text_lens, image_index, (const bf16*)shared_emb, (const bf16*)feats, ldf, feat_row_offset, feat_rows_per_image,
+                             (bf16*)out, seq_lens, B, L, P, D, image_token);
+    });
+}
+
+extern "C" int vqa_op_decoder_embed(const int32_t* labels, const void* shared_emb, void* out, int32_t B, int32_t T, int32_t D, int32_t start_id,
+                                    int32_t pad_id, void* stream) {
+    if (!shared_emb || !out || (!labels && T != 1)) return fail(nullptr, VQA_ERR_INVALID_ARG, "decoder embed: null pointer (labels NULL needs T = 1)");
+    if (B <= 0 || T <= 0 || D <= 0 || D % 8 || start_id < 0 || pad_id < 0 || (long long)B * T > INT32_MAX)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "decoder embed: bad size (D a multiple of 8, start / pad ids >= 0)");
+    if (!aligned(labels, 4) || !aligned(shared_emb, 16) || !aligned(out, 16))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "decoder embed: labels 4-byte aligned, embeddings / out 16-byte aligned");
+    return glue_launch(stream, [&](Forward& f) { return clipt5_decoder_embed(f, labels, (const bf16*)shared_emb, (bf16*)out, B, T, D, start_id, pad_id); });
+}
+
+extern "C" int vqa_op_t5_bias_table(const void* rel_emb, const int32_t* bucket_lut, int32_t max_distance, float* table, int32_t H, int32_t S,
+                                    void* stream) {
+    if (!rel_emb || !bucket_lut || !table) return fail(nullptr, VQA_ERR_INVALID_ARG, "bias table: null pointer");
+    if (H <= 0 || S <= 0 || max_distance <= 0 || (long long)H * (2 * (long long)S - 1) > INT32_MAX)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "bias table: bad size");
+    if (!aligned(rel_emb, 2) || !aligned(bucket_lut, 4) || !aligned(table, 4))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "bias table: rel_emb 2-byte, lut / table 4-byte aligned");
+    return glue_launch(stream, [&](Forward& f) { return clipt5_bias_table(f, (const bf16*)rel_emb, bucket_lut, max_distance, table, H, S); });
+}
+
+extern "C" int vqa_op_lmhead_score(const void* Hs, int32_t ldh, const void* W, int32_t ldw, int32_t B, int32_t T, int32_t N, int32_t K,
+                                   const int32_t* labels, float* scores, float* logprobs, float* scratch, size_t scratch_bytes, size_t* scratch_needed,
+                                   void* stream) {
+    if (!Hs || !W || !labels || !scores) return fail(nullptr, VQA_ERR_INVALID_ARG, "lmhead score: null pointer");
+    if (B <= 0 || T <= 0 || N <= 0 || K <= 0 || K % 8 || ldh % 8 || ldw % 8 || ldh < K || ldw < K || (long long)B * T > INT32_MAX)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "lmhead score: bad size (K, ldh, ldw multiples of 8, ldh / ldw >= K)");
+    if (!aligned(Hs, 16) || !aligned(W, 16) || !aligned(labels, 4) || !aligned(scores, 4) || !aligned(logprobs, 4))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "lmhead score: H / W 16-byte aligned, labels / scores / logprobs 4-byte aligned");
+    const int M = B * T;
+    const size_t need = lmhead_scratch_floats(M, N);
+    if (scratch_needed) *scratch_needed = need * sizeof(float);
+    if (!scratch || !aligned(scratch, 4) || scratch_bytes < need * sizeof(float))
+        return fail(nullptr, VQA_ERR_WORKSPACE, "lmhead score: scratch smaller than lmhead_scratch_floats(B * T, N) floats");
+    const size_t parts = (size_t)M * LMHEAD_PARTS * ((N + LMHEAD_BN - 1) / LMHEAD_BN);
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_lmhead_score(f, abi_gemm(Hs, ldh, W, ldw, N, nullptr, 0, M, N, K), labels, scratch, scratch + parts, scratch + 2 * parts, scores,
+                                   logprobs, B, T);
+    });
+}
+
+extern "C" int vqa_op_row_ssq(const void* x, float* ssq, int32_t rows, int32_t D, int32_t stride, void* stream) {
+    if (!x || !ssq) return fail(nullptr, VQA_ERR_INVALID_ARG, "row ssq: null pointer");
+    if (rows <= 0 || D <= 0 || D % 8 || stride <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "row ssq: bad size (D a multiple of 8)");
+    if (!aligned(x, 16) || !aligned(ssq, 4)) return fail(nullptr, VQA_ERR_INVALID_ARG, "row ssq: x 16-byte, ssq 4-byte aligned");
+    return glue_launch(stream, [&](Forward& f) { return clipt5_row_ssq(f, (const bf16*)x, ssq, rows, D, stride); });
 }
 
 // ------------------------------------------------------------------------------------------------ kernel-level ABI: the Qwen2.5-VL scoring path

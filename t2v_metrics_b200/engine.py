@@ -18,6 +18,7 @@ from .config import ClipT5Config
 
 IMAGE_TOKEN_INDEX = -200  # t2v_metrics/constants.py:7
 IGNORE_INDEX = -100       # t2v_metrics/constants.py:6
+ATTN_KEY_TILE = 128       # key rows per tile of the head-dim-128 attention kernel (attention_sm90.cuh)
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -567,13 +568,94 @@ class ops:
         return out
 
     @staticmethod
-    def norm(x: torch.Tensor, gamma: torch.Tensor, beta=None, eps=1e-6):
+    def norm(x: torch.Tensor, gamma: torch.Tensor, beta=None, eps=1e-6, out=None):
         lib = _lib.load()
-        y = torch.empty_like(x)
+        y = torch.empty_like(x) if out is None else out
         rc = lib.vqa_op_norm(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(y), x.shape[0], x.shape[1], float(eps),
                              _stream_ptr(x.device))
         _check(rc, None, "vqa_op_norm")
         return y
+
+    @staticmethod
+    def patchify(pixels: torch.Tensor, patch: int, kpad: int, out=None):
+        """The patch gather of the CLIP tower: pixels [n, 3, S, S] fp32 / bf16 -> bf16 [n * (S / patch)^2, kpad]."""
+        lib = _lib.load()
+        n, S = pixels.shape[0], pixels.shape[2]
+        if out is None:
+            out = torch.empty(n * (S // patch) ** 2, kpad, dtype=torch.bfloat16, device=pixels.device)
+        dt = _lib.VQA_DTYPE_F32 if pixels.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
+        rc = lib.vqa_op_patchify(_ptr(pixels), dt, n, S, patch, kpad, _ptr(out), _stream_ptr(pixels.device))
+        _check(rc, None, "vqa_op_patchify")
+        return out
+
+    @staticmethod
+    def splice_embed(ids: torch.Tensor, text_lens: torch.Tensor, image_index, shared: torch.Tensor, feats: torch.Tensor, P: int,
+                     rows_per_image: int, row_offset: int = 1, image_token: int = -200, out=None, seq_lens=None):
+        """The multimodal splice: ids int32 [B, L], text_lens int32 [B], image_index int32 [B] or None, shared [vocab, D], feats [rows, >= D]
+        (row stride feats.stride(0)), image i's P feature rows from row i * rows_per_image + row_offset. Returns (out [B, L - 1 + P, D],
+        seq_lens int32 [B])."""
+        lib = _lib.load()
+        B, L = ids.shape
+        D = shared.shape[1]
+        if out is None:
+            out = torch.empty(B, L - 1 + P, D, dtype=torch.bfloat16, device=ids.device)
+        if seq_lens is None:
+            seq_lens = torch.empty(B, dtype=torch.int32, device=ids.device)
+        rc = lib.vqa_op_splice_embed(_ptr(ids), _ptr(text_lens), _ptr(image_index), _ptr(shared), _ptr(feats), feats.stride(0), row_offset,
+                                     rows_per_image, _ptr(out), _ptr(seq_lens), B, L, P, D, image_token, _stream_ptr(ids.device))
+        _check(rc, None, "vqa_op_splice_embed")
+        return out, seq_lens
+
+    @staticmethod
+    def decoder_embed(labels, shared: torch.Tensor, B: int, T: int, start_id: int = 0, pad_id: int = 0, out=None):
+        """Decoder input embeddings of shift_right(labels int32 [B, T]) (labels None: T = 1, the start token). Returns [B * T, D]."""
+        lib = _lib.load()
+        D = shared.shape[1]
+        if out is None:
+            out = torch.empty(B * T, D, dtype=torch.bfloat16, device=shared.device)
+        rc = lib.vqa_op_decoder_embed(_ptr(labels), _ptr(shared), _ptr(out), B, T, D, start_id, pad_id, _stream_ptr(shared.device))
+        _check(rc, None, "vqa_op_decoder_embed")
+        return out
+
+    @staticmethod
+    def t5_bias_table(rel_emb: torch.Tensor, bucket_lut: torch.Tensor, max_distance: int, S: int, out=None):
+        """The encoder's relative-position bias table fp32 [H, 2S - 1] from rel_emb bf16 [buckets, H] and a device bucket LUT."""
+        lib = _lib.load()
+        H = rel_emb.shape[1]
+        if out is None:
+            out = torch.empty(H, 2 * S - 1, dtype=torch.float32, device=rel_emb.device)
+        rc = lib.vqa_op_t5_bias_table(_ptr(rel_emb), _ptr(bucket_lut), max_distance, _ptr(out), H, S, _stream_ptr(rel_emb.device))
+        _check(rc, None, "vqa_op_t5_bias_table")
+        return out
+
+    @staticmethod
+    def lmhead_score(h: torch.Tensor, w: torch.Tensor, labels: torch.Tensor, scores=None, logprobs=None):
+        """The CLIP-FlanT5 score's lm_head and finalisation: h [B * T, K] against w [N, K], labels int32 [B, T]. Returns (scores fp32 [B],
+        logprobs fp32 [B * T]); both are allocated NaN-filled when not given, and ignored positions of logprobs keep their value."""
+        lib = _lib.load()
+        B, T = labels.shape
+        N, K = w.shape[0], h.shape[1]
+        if scores is None:
+            scores = torch.full((B,), float("nan"), dtype=torch.float32, device=h.device)
+        if logprobs is None:
+            logprobs = torch.full((B * T,), float("nan"), dtype=torch.float32, device=h.device)
+        need = C.c_size_t(0)
+        args = (_ptr(h), h.stride(0), _ptr(w), w.stride(0), B, T, N, K, _ptr(labels), _ptr(scores), _ptr(logprobs))
+        rc = lib.vqa_op_lmhead_score(*args, None, 0, C.byref(need), _stream_ptr(h.device))
+        if rc != -4:        # a call without scratch stops at the scratch check and returns the size
+            _check(rc or -1, None, "vqa_op_lmhead_score")
+        scratch = torch.empty((need.value + 3) // 4, dtype=torch.float32, device=h.device)
+        rc = lib.vqa_op_lmhead_score(*args, _ptr(scratch), scratch.numel() * 4, None, _stream_ptr(h.device))
+        _check(rc, None, "vqa_op_lmhead_score")
+        return scores, logprobs
+
+    @staticmethod
+    def row_ssq(x: torch.Tensor, ssq: torch.Tensor):
+        """Sum of squares of the rows of x bf16 [rows, D] into column 0 of ssq fp32 [rows, stride] (in place)."""
+        lib = _lib.load()
+        rc = lib.vqa_op_row_ssq(_ptr(x), _ptr(ssq), x.shape[0], x.shape[1], ssq.stride(0), _stream_ptr(x.device))
+        _check(rc, None, "vqa_op_row_ssq")
+        return ssq
 
     @staticmethod
     def gemm_f32acc(a: torch.Tensor, w: torch.Tensor, c: torch.Tensor, bias=None, variant=0):
@@ -1128,7 +1210,8 @@ class QwenVLEngine:
         call. Videos are grids with t > 1 whose prompt run uses cfg.video_token_id (second_per_grid_ts = temporal_patch / fps).
         share_prefix: None = automatically when at least two prompts start with the same [chat prefix + vision run] over the same image
         (the M x N scoring API repeats every image N times, reference score.py:104-106); their prefix then runs through the language
-        model once (KV-prefix sharing, exact under causal attention)."""
+        model once (KV-prefix sharing, exact under causal attention). The shared part is cut to whole key tiles of the attention kernel
+        (ATTN_KEY_TILE rows), so a shared prefill is bit-identical to the unshared one; a prefix shorter than one tile is not shared."""
         from . import qwen_host
         cfg, dev = self.cfg, self.device
         B = len(prompts)
@@ -1136,7 +1219,8 @@ class QwenVLEngine:
         if share_prefix is None or share_prefix:
             pk = qwen_host.build_packed_indices([list(map(int, p)) for p in prompts], [tuple(map(int, g)) for g in grid_thw], img,
                                                 cfg.image_token_id, cfg.spatial_merge_size, cfg.tokens_per_second,
-                                                video_token_id=cfg.video_token_id, second_per_grid_ts=second_per_grid_ts)
+                                                video_token_id=cfg.video_token_id, second_per_grid_ts=second_per_grid_ts,
+                                                align=ATTN_KEY_TILE)
             if pk["n_shared"] > 0 or share_prefix:
                 d = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in pk.items()}
                 ans = torch.as_tensor(list(map(int, answer_ids)), dtype=torch.int32).to(dev)

@@ -190,13 +190,16 @@ def rollout_answer_score(tokens: Sequence[int], logp: torch.Tensor, answer_ids: 
 
 def build_packed_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequence[int]], image_of_sample: Sequence[int],
                          image_token_id: int, merge: int, tokens_per_second: int, video_token_id: Optional[int] = None,
-                         second_per_grid_ts: Optional[Sequence[float]] = None):
+                         second_per_grid_ts: Optional[Sequence[float]] = None, align: int = 1):
     """KV-prefix sharing (SURVEY 8(f)1): prompts that start with the same tokens up to the end of their vision run -- the chat prefix and
     the image's pad tokens, i.e. every text scored against one image (reference score.py:104-106) -- share that prefix as ONE packed
     sequence; each prompt keeps only its remaining tokens as its own sequence. Returns the int32 CPU arrays vqa_qwen25vl_score_packed takes
     plus sizes: dict(input_ids [R], feat_index [R], position_ids [3, R], cu_seqlens [n_seq + 1], kv_prefix [n_seq], pair_row [B],
     pair_seq [B], total_rows, n_seq, max_seq_len, max_prompt_len, n_shared). A prompt whose prefix nobody else uses is stored whole
-    (kv_prefix -1), so the packed form never has more rows than sum(len(prompt))."""
+    (kv_prefix -1), so the packed form never has more rows than sum(len(prompt)).
+    align: the shared prefix is cut to a multiple of `align` tokens (the rest stays in each prompt's own sequence). The engine passes the
+    attention kernel's key tile (128): a prefix of whole key tiles leaves every suffix row's attention bit-identical to the unshared
+    prefill, so sharing a prefix never changes a score."""
     unit = merge * merge
     feat_off = [0]
     for t, h, w in grids:
@@ -206,7 +209,7 @@ def build_packed_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequenc
     cut = []                                    # prefix length of each prompt = index after its last vision token
     for p in prompts:
         last = max((i for i, t in enumerate(p) if t in vis), default=-1)
-        cut.append(last + 1)
+        cut.append((last + 1) // align * align)
     groups = {}
     for b, p in enumerate(prompts):
         if cut[b] > 0 and cut[b] < len(p):
@@ -237,7 +240,7 @@ def build_packed_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequenc
         pos_cache[b0] = positions(b0)
         prefix_seq[key] = len(seqs)
         seqs.append(list(pre)); kvp.append(-1)
-        pos_rows.append(pos_cache[b0][:, :len(pre)]); feat_rows.append(feats(pre, img))
+        pos_rows.append(pos_cache[b0][:, :len(pre)]); feat_rows.append(feats(prompts[b0], img)[:len(pre)])
     pair_seq, pair_last = [], []
     for b, p in enumerate(prompts):
         key = (image_of_sample[b], tuple(p[:cut[b]]))
@@ -251,7 +254,7 @@ def build_packed_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequenc
         pair_seq.append(len(seqs))
         seqs.append(own); kvp.append(pre)
         pos_rows.append(pos[:, start:])
-        feat_rows.append(feats(own, image_of_sample[b]) if pre < 0 else torch.full((len(own),), -1, dtype=torch.int32))
+        feat_rows.append(feats(p, image_of_sample[b])[start:])
     lens = [len(x) for x in seqs]
     cu = torch.zeros(len(seqs) + 1, dtype=torch.int32)
     cu[1:] = torch.as_tensor(lens, dtype=torch.int32).cumsum(0)

@@ -217,3 +217,28 @@ def test_packed_indices_reassemble_every_prompt():
         assert int(pk["pair_row"][b]) == rows[-1]
     assert int(pk["kv_prefix"][int(pk["pair_seq"][-1])]) == -1
     assert pk["max_prompt_len"] == max(map(len, prompts)) and pk["max_seq_len"] == max(cu[i + 1] - cu[i] for i in range(pk["n_seq"]))
+
+
+def test_packed_prefix_is_cut_to_whole_key_tiles():
+    """With align = 128 (the engine's setting) the shared prefix is the longest common run of whole 128-row key tiles, which may end inside
+    the vision run; the suffixes then carry the rest of it, and re-assembly still gives the padded layout exactly."""
+    cfg = qo.Qwen25VLConfig.tiny(**TINY)
+    grids = [(1, 20, 40), (1, 4, 4)]                 # 200 and 4 vision tokens
+    ntok = [t * h * w // 4 for t, h, w in grids]
+    prompts = [[5, 6, 7] + [cfg.image_token_id] * ntok[0] + [9, 10 + k, 11] for k in range(3)]
+    prompts += [[5, 6] + [cfg.image_token_id] * ntok[1] + [9, 12 + k] for k in range(2)]       # prefix shorter than one tile: not shared
+    img = [0, 0, 0, 1, 1]
+    args = (cfg.image_token_id, cfg.spatial_merge_size, cfg.tokens_per_second)
+    pk = qwen_host.build_packed_indices(prompts, grids, img, *args, video_token_id=cfg.video_token_id, align=128)
+    full = qwen_host.build_batch_indices(prompts, grids, img, *args, video_token_id=cfg.video_token_id)
+    S = full["input_ids"].shape[1]
+    cu = pk["cu_seqlens"].tolist()
+    assert pk["n_shared"] == 1 and cu[1] - cu[0] == 128
+    for b, p in enumerate(prompts):
+        sq = int(pk["pair_seq"][b])
+        pre = int(pk["kv_prefix"][sq])
+        assert (pre >= 0) == (b < 3)
+        rows = (list(range(cu[pre], cu[pre + 1])) if pre >= 0 else []) + list(range(cu[sq], cu[sq + 1]))
+        assert pk["input_ids"][rows].tolist() == p
+        assert torch.equal(pk["position_ids"][:, rows], full["position_ids"].view(3, len(prompts), S)[:, b, :len(p)])
+        assert torch.equal(pk["feat_index"][rows], full["feat_index"][b, :len(p)])
