@@ -361,6 +361,27 @@ int vqa_qwen_preprocess_video(const void* src, const int64_t* frame_offsets, con
                               int32_t merge, int64_t min_pixels, int64_t max_pixels, const float* mean, const float* stdv, void* out,
                               int32_t out_dtype, void* workspace, size_t workspace_bytes, void* host_staging, void* stream);
 
+/* Qwen2.5-VL frames sampled from a video FILE: qwen_vl_utils fetch_video resizes them as one tensor with torchvision
+ * resize(BICUBIC, antialias=True) (torch's _upsample_bicubic2d_aa in fp32: the horizontal pass, then the vertical one, each output the
+ * fused multiply-add of its taps in order; then clamp, round half to even, uint8), and the processor runs with do_resize=False. Here both
+ * passes run on the device with torch's own fp32 weights, and the uint8 result goes to the same patch rows as vqa_qwen_preprocess_video
+ * writes for a frame stack. One video is sent in slices of frames: each call takes frames [frame0, frame0 + n_frames) of a video of
+ * total_frames frames and writes their temporal slots.
+ *   first_h / first_v   HOST [out_w] / [out_h]: first input column / row of each output's window; windows inside the frame, rows
+ *                       non-decreasing in the output row.
+ *   weights_h / weights_v  HOST fp32 [out_w][htaps] / [out_h][vtaps]: the taps, zero-padded where a window is shorter.
+ *   src      DEVICE uint8 [n_frames, in_h, in_w, 3] RGB.
+ *   out      DEVICE [total_patches, 3*temporal_patch*patch^2]: the video's patch rows (same layout as vqa_qwen_preprocess_video's).
+ * vqa_qwen_preprocess_video_aa_plan is host-only: total_patches = rows of the whole video, workspace_bytes = device scratch per call. */
+int vqa_qwen_preprocess_video_aa_plan(int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w, const int32_t* first_h, int32_t htaps,
+                                      const int32_t* first_v, int32_t vtaps, int32_t patch, int32_t temporal_patch, int32_t merge,
+                                      int32_t total_frames, int64_t* total_patches, size_t* workspace_bytes);
+int vqa_qwen_preprocess_video_aa(const void* src, int32_t n_frames, int32_t frame0, int32_t total_frames, int32_t in_h, int32_t in_w,
+                                 int32_t out_h, int32_t out_w, const int32_t* first_h, const float* weights_h, int32_t htaps,
+                                 const int32_t* first_v, const float* weights_v, int32_t vtaps, int32_t patch, int32_t temporal_patch,
+                                 int32_t merge, const float* mean, const float* stdv, void* out, int32_t out_dtype, void* workspace,
+                                 size_t workspace_bytes, void* host_staging, void* stream);
+
 /* Host-only helper (no GPU needed): the 22-bit fixed-point bicubic tap table of one resize axis (in_size -> out_size, output
  * pixels [first, first + count)), exactly as vqa_clip_preprocess builds it after Pillow's precompute_coeffs /
  * normalize_coeffs_8bpc. bounds [count][2] = (first source index, taps used); kk [count][ksize]; returns ksize (0 = bad

@@ -29,6 +29,7 @@ ABI_SYMBOLS = [
     "vqa_op_clip_embed_ln", "vqa_qwen_preprocess_video_plan", "vqa_qwen_preprocess_video",
     "vqa_op_qwen_rope", "vqa_op_gather_rows", "vqa_op_qwen_embed", "vqa_op_token_bitmap", "vqa_op_topk_softmax",
     "vqa_op_patchify", "vqa_op_splice_embed", "vqa_op_decoder_embed", "vqa_op_t5_bias_table", "vqa_op_lmhead_score", "vqa_op_row_ssq",
+    "vqa_qwen_preprocess_video_aa_plan", "vqa_qwen_preprocess_video_aa",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -210,6 +211,13 @@ def load() -> C.CDLL:
     lib.vqa_qwen_preprocess_video.argtypes = [vp, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, i32,
                                               i32, i64, i64, C.POINTER(C.c_float), C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
     lib.vqa_qwen_preprocess_video.restype = C.c_int
+    lib.vqa_qwen_preprocess_video_aa_plan.argtypes = [i32, i32, i32, i32, C.POINTER(i32), i32, C.POINTER(i32), i32, i32, i32, i32, i32,
+                                                      C.POINTER(i64), C.POINTER(C.c_size_t)]
+    lib.vqa_qwen_preprocess_video_aa_plan.restype = C.c_int
+    lib.vqa_qwen_preprocess_video_aa.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(C.c_float), i32,
+                                                 C.POINTER(i32), C.POINTER(C.c_float), i32, i32, i32, i32, C.POINTER(C.c_float),
+                                                 C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
+    lib.vqa_qwen_preprocess_video_aa.restype = C.c_int
     lib.vqa_clipt5_debug_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(C.c_size_t), i32]
     lib.vqa_clipt5_debug_layout.restype = C.c_int
     lib.vqa_qwen25vl_debug_layout.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_size_t), i32]

@@ -153,6 +153,32 @@ __device__ __forceinline__ unsigned pre_finish(unsigned a0, unsigned a1, int a2)
     return (unsigned)pre_clip8((int)t);
 }
 
+// out = ((u8 / 255) - mean[c]) / std[c] in fp32 with IEEE division and no fma, as numpy / torch compute it on the host; lut[3][256]
+__device__ __forceinline__ void pre_fill_lut(float* lut, float3 mean, float3 stdv) {
+    for (int i = threadIdx.x; i < 768; i += PRE_THREADS) {
+        const int c = i >> 8;
+        const float mu = c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), sd = c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z);
+        lut[i] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)(i & 255), 255.0f), mu), sd);
+    }
+}
+
+// PRE_QWEN_PATCHES output of pixel (y, x) with channel values v: the Qwen2-VL processor's patch rows (image_processing_qwen2_vl.py:191-220),
+// row ((by * gw/m + bx) * m + iy) * m + ix for the 14x14 patch at grid (by*m+iy, bx*m+ix), column (c * temporal + t) * ps*ps + py * ps + px,
+// written to temporal slots t in [t0, t0 + nt). gwm = patches per row / merge.
+template <typename OUT>
+__device__ __forceinline__ void pre_store_patch(OUT* dst, PrePatchGeom geom, int gwm, int y, int x, const float* v, int t0, int nt) {
+    const int ps = geom.patch, mg = geom.merge, pp = geom.patch * geom.patch;
+    const int gy = y / ps, py = y - gy * ps, gx = x / ps, px_ = x - gx * ps;
+    const size_t row = (((size_t)(gy / mg) * gwm + gx / mg) * mg + gy % mg) * mg + gx % mg;
+    OUT* q = dst + row * (size_t)(3 * geom.temporal * pp) + py * ps + px_;
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+        for (int t = t0; t < t0 + nt; ++t) {
+            if constexpr (sizeof(OUT) == 4) q[(size_t)(c * geom.temporal + t) * pp] = v[c];
+            else q[(size_t)(c * geom.temporal + t) * pp] = __float2bfloat16_rn(v[c]);
+        }
+}
+
 // LAYOUT PRE_CHW: out[c][y][x] per image ([3, out_h, out_w]). PRE_QWEN_PATCHES: the Qwen2-VL processor's patch rows
 // (image_processing_qwen2_vl.py:191-220): row ((by * gw/m + bx) * m + iy) * m + ix for the 14x14 patch at grid (by*m+iy, bx*m+ix),
 // column (c * temporal + t) * ps*ps + py * ps + px, the frame written to temporal slots t in [t0, t0 + nt): every slot for a still
@@ -184,12 +210,7 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
     const unsigned bgc[3] = {background.x, background.y, background.z};
     const int lane_x = threadIdx.x % PRE_XL, grp = threadIdx.x / PRE_XL;
 
-    // out = ((u8 / 255) - mean[c]) / std[c] in fp32 with IEEE division and no fma, as numpy / torch compute it on the host
-    for (int i = threadIdx.x; i < 768; i += PRE_THREADS) {
-        const int c = i >> 8;
-        const float mu = c == 0 ? mean.x : (c == 1 ? mean.y : mean.z), sd = c == 0 ? stdv.x : (c == 1 ? stdv.y : stdv.z);
-        lut[i] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)(i & 255), 255.0f), mu), sd);
-    }
+    pre_fill_lut(lut, mean, stdv);
 
     for (int cg = 0; cg < ng; cg += im.chunk_groups) {
         const int ngc = min(im.chunk_groups, ng - cg);
@@ -269,8 +290,7 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
 
     // ---- vertical pass (ImagingResampleVertical_8bpc) + normalisation
     OUT* dst = out + im.out_off;
-    const int ps = geom.patch, mg = geom.merge, pp = geom.patch * geom.patch;
-    const int gwm = LAYOUT == PRE_QWEN_PATCHES ? out_w / (ps * mg) : 0;
+    const int gwm = LAYOUT == PRE_QWEN_PATCHES ? out_w / (geom.patch * geom.merge) : 0;
     for (int yy = grp; yy < ny; yy += PRE_RG) {
         const int y = y0 + yy;
         const int gs = vstart[y] - g0;
@@ -299,15 +319,7 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
                     else dst[o] = __float2bfloat16_rn(v[c]);
                 }
             } else {
-                const int gy = y / ps, py = y - gy * ps, gx = xx / ps, px_ = xx - gx * ps;
-                const size_t row = (((size_t)(gy / mg) * gwm + gx / mg) * mg + gy % mg) * mg + gx % mg;
-                OUT* q = dst + row * (size_t)(3 * geom.temporal * pp) + py * ps + px_;
-#pragma unroll
-                for (int c = 0; c < 3; ++c)
-                    for (int t = im.t0; t < im.t0 + im.nt; ++t) {
-                        if constexpr (sizeof(OUT) == 4) q[(size_t)(c * geom.temporal + t) * pp] = v[c];
-                        else q[(size_t)(c * geom.temporal + t) * pp] = __float2bfloat16_rn(v[c]);
-                    }
+                pre_store_patch(dst, geom, gwm, y, xx, v, im.t0, im.nt);
             }
         }
     }
@@ -479,6 +491,121 @@ inline bool pre_plan_qwen(const int32_t* heights, const int32_t* widths, const i
     if (grid_hw)
         for (int i = 0; i < n; ++i) { grid_hw[2 * i] = thw[3 * i + 1]; grid_hw[2 * i + 1] = thw[3 * i + 2]; }
     return true;
+}
+
+// ---------------------------------------------------------------------------------------------- torch's antialiased bicubic resize
+// A video FILE reaches the Qwen processor through qwen_vl_utils fetch_video, which resizes the sampled frames as one tensor with
+// torchvision resize(BICUBIC, antialias=True): uint8 -> fp32, torch's _upsample_bicubic2d_aa, clamp to [0, 255], round half to even, uint8.
+// On the CPU that is separable_upsample_generic_Nd_kernel_impl (aten/src/ATen/native/cpu/UpSampleKernel.cpp): the horizontal pass into an
+// fp32 buffer, then the vertical pass, each output t0 * w0 + t1 * w1 + ... accumulated in tap order. This kernel runs the same two fp32
+// passes with fused multiply-adds in that order. The weights are torch's own fp32 values, read off on the host by resizing impulses
+// (engine._aa_bicubic_taps); every output of an axis reads `taps` consecutive inputs from first[i], zero weights padding a shorter
+// window (adding 0 * t leaves an fp32 sum unchanged). The uint8 result then goes through pre_store_patch like a still image's pixels.
+//
+// One CTA = one frame x a tile of tile_rows x PRE_AA_TX output pixels. It runs the horizontal pass for the band of input rows its output
+// rows read (fp32 in shared memory, [3][band_rows][PRE_AA_TX]) and then the vertical pass out of that band.
+constexpr int PRE_AA_TX = 64;
+constexpr int PRE_AA_MAX_SMEM = 96 * 1024;
+
+struct PreAAGeom {
+    int in_h, in_w, out_h, out_w, htaps, vtaps;
+    int tile_rows, band_rows, tiles_x;
+    int frame0, total_frames;    // index in the video of the launch's first frame; frames of the whole video
+};
+
+inline size_t pre_aa_smem_bytes(int band_rows) { return (768 + (size_t)3 * band_rows * PRE_AA_TX) * sizeof(float); }
+
+// tables: first_h[out_w] | first_v[out_h] | fp32 weights_h[out_w][htaps] | fp32 weights_v[out_h][vtaps]. `out` is the video's first patch
+// row; frame f of the launch (frame frame0 + f of the video) fills slot (frame0 + f) % temporal of temporal group (frame0 + f) / temporal,
+// and the video's last frame also the slots after its own (the processor pads with copies of the last frame).
+template <typename OUT>
+__global__ void __launch_bounds__(PRE_THREADS)
+video_resize_aa_kernel(const uint8_t* __restrict__ src, const int* __restrict__ tables, PreAAGeom g, PrePatchGeom geom, float3 mean,
+                       float3 stdv, OUT* __restrict__ out) {
+    extern __shared__ float aa_smem[];
+    float* lut = aa_smem;                                                   // [3][256]
+    float* band = aa_smem + 768;                                            // [3][band_rows][PRE_AA_TX]
+    const int x0 = (blockIdx.x % g.tiles_x) * PRE_AA_TX, y0 = (blockIdx.x / g.tiles_x) * g.tile_rows;
+    const int nx = min(PRE_AA_TX, g.out_w - x0), ny = min(g.tile_rows, g.out_h - y0);
+    const int* first_h = tables;
+    const int* first_v = first_h + g.out_w;
+    const float* w_h = reinterpret_cast<const float*>(first_v + g.out_h);
+    const float* w_v = w_h + (size_t)g.out_w * g.htaps;
+    const int r0 = first_v[y0], nr = first_v[y0 + ny - 1] + g.vtaps - r0;  // input rows of this tile (<= band_rows, windows monotonic)
+    const uint8_t* img = src + (size_t)blockIdx.y * g.in_h * g.in_w * 3;
+    pre_fill_lut(lut, mean, stdv);
+
+    // ---- horizontal pass: thread = one output column x one input row, three channels
+    for (int i = threadIdx.x; i < nr * PRE_AA_TX; i += PRE_THREADS) {
+        const int r = i / PRE_AA_TX, xl = i - r * PRE_AA_TX;
+        if (xl >= nx) continue;
+        const int x = x0 + xl;
+        const uint8_t* p = img + ((size_t)(r0 + r) * g.in_w + first_h[x]) * 3;
+        const float* w = w_h + (size_t)x * g.htaps;
+        float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+        for (int j = 0; j < g.htaps; ++j) {
+            const float wj = __ldg(w + j);
+            a0 = __fmaf_rn((float)p[3 * j], wj, a0);
+            a1 = __fmaf_rn((float)p[3 * j + 1], wj, a1);
+            a2 = __fmaf_rn((float)p[3 * j + 2], wj, a2);
+        }
+        band[(0 * g.band_rows + r) * PRE_AA_TX + xl] = a0;
+        band[(1 * g.band_rows + r) * PRE_AA_TX + xl] = a1;
+        band[(2 * g.band_rows + r) * PRE_AA_TX + xl] = a2;
+    }
+    __syncthreads();
+
+    // ---- vertical pass, round half to even, clamp, normalise, patch rows
+    const int f = g.frame0 + blockIdx.y;
+    const int t0 = f % geom.temporal, nt = f + 1 < g.total_frames ? 1 : geom.temporal - t0;
+    const int gwm = g.out_w / (geom.patch * geom.merge);
+    OUT* dst = out + (size_t)(f / geom.temporal) * (g.out_h / geom.patch) * (g.out_w / geom.patch) * (3 * geom.temporal * geom.patch * geom.patch);
+    for (int i = threadIdx.x; i < ny * PRE_AA_TX; i += PRE_THREADS) {
+        const int yl = i / PRE_AA_TX, xl = i - yl * PRE_AA_TX;
+        if (xl >= nx) continue;
+        const int y = y0 + yl;
+        const float* w = w_v + (size_t)y * g.vtaps;
+        const float* b = band + (first_v[y] - r0) * PRE_AA_TX + xl;
+        float a[3] = {0.f, 0.f, 0.f};
+        for (int j = 0; j < g.vtaps; ++j) {
+            const float wj = __ldg(w + j);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) a[c] = __fmaf_rn(b[(c * g.band_rows + j) * PRE_AA_TX], wj, a[c]);
+        }
+        float v[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) v[c] = lut[c * 256 + min(max(__float2int_rn(a[c]), 0), 255)];
+        pre_store_patch(dst, geom, gwm, y, x0 + xl, v, t0, nt);
+    }
+}
+
+// Host checks and launch geometry of video_resize_aa_kernel: every window inside its axis and the vertical windows monotonic; the
+// output rows per CTA (<= 32, a power of two) are the most whose band of input rows fits PRE_AA_MAX_SMEM.
+inline bool pre_plan_aa(int in_h, int in_w, int out_h, int out_w, const int32_t* first_h, int htaps, const int32_t* first_v, int vtaps,
+                        int patch, int merge, PreAAGeom& g, std::string& error) {
+    if (in_h <= 0 || in_w <= 0 || out_h <= 0 || out_w <= 0 || htaps <= 0 || vtaps <= 0 || htaps > in_w || vtaps > in_h) {
+        error = "bad sizes or tap counts";
+        return false;
+    }
+    if (out_h % (patch * merge) || out_w % (patch * merge)) { error = "the output size must be a multiple of patch * merge"; return false; }
+    for (int x = 0; x < out_w; ++x)
+        if (first_h[x] < 0 || first_h[x] > in_w - htaps) { error = "horizontal window outside the frame"; return false; }
+    for (int y = 0; y < out_h; ++y)
+        if (first_v[y] < 0 || first_v[y] > in_h - vtaps || (y && first_v[y] < first_v[y - 1])) {
+            error = "vertical windows outside the frame or not monotonic";
+            return false;
+        }
+    g = PreAAGeom{in_h, in_w, out_h, out_w, htaps, vtaps, 0, 0, (out_w + PRE_AA_TX - 1) / PRE_AA_TX, 0, 0};
+    for (int tile = 32; tile >= 1; tile >>= 1) {
+        int band = 0;
+        for (int y0 = 0; y0 < out_h; y0 += tile) {
+            const int y1 = (y0 + tile < out_h ? y0 + tile : out_h) - 1;
+            if (first_v[y1] + vtaps - first_v[y0] > band) band = first_v[y1] + vtaps - first_v[y0];
+        }
+        if (pre_aa_smem_bytes(band) <= (size_t)PRE_AA_MAX_SMEM) { g.tile_rows = tile; g.band_rows = band; return true; }
+    }
+    error = "downscale too steep for the device resize (vertical window exceeds shared memory)";
+    return false;
 }
 
 }  // namespace vqa

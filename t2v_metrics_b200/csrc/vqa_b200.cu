@@ -1215,6 +1215,82 @@ extern "C" int vqa_qwen_preprocess_video(const void* src, const int64_t* frame_o
                                         out_dtype, workspace, workspace_bytes, host_staging, reinterpret_cast<cudaStream_t>(stream));
 }
 
+static int qwen_video_aa_args(int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w, const int32_t* first_h, int32_t htaps,
+                              const int32_t* first_v, int32_t vtaps, int32_t patch, int32_t temporal_patch, int32_t merge, int32_t total_frames,
+                              PreAAGeom& g) {
+    if (!first_h || !first_v || patch <= 0 || merge <= 0 || temporal_patch <= 0 || total_frames <= 0)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "bad argument");
+    std::string error;
+    if (!pre_plan_aa(in_h, in_w, out_h, out_w, first_h, htaps, first_v, vtaps, patch, merge, g, error))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, error);
+    g.total_frames = total_frames;
+    return VQA_OK;
+}
+
+static size_t qwen_video_aa_table_bytes(const PreAAGeom& g) {
+    return ((size_t)g.out_w + g.out_h) * sizeof(int32_t) + ((size_t)g.out_w * g.htaps + (size_t)g.out_h * g.vtaps) * sizeof(float);
+}
+
+extern "C" int vqa_qwen_preprocess_video_aa_plan(int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w, const int32_t* first_h,
+                                                 int32_t htaps, const int32_t* first_v, int32_t vtaps, int32_t patch, int32_t temporal_patch,
+                                                 int32_t merge, int32_t total_frames, int64_t* total_patches, size_t* workspace_bytes) {
+    PreAAGeom g;
+    if (int rc = qwen_video_aa_args(in_h, in_w, out_h, out_w, first_h, htaps, first_v, vtaps, patch, temporal_patch, merge, total_frames, g))
+        return rc;
+    if (total_patches)
+        *total_patches = (int64_t)((total_frames + temporal_patch - 1) / temporal_patch) * (out_h / patch) * (out_w / patch);
+    if (workspace_bytes) *workspace_bytes = qwen_video_aa_table_bytes(g);
+    return VQA_OK;
+}
+
+extern "C" int vqa_qwen_preprocess_video_aa(const void* src, int32_t n_frames, int32_t frame0, int32_t total_frames, int32_t in_h, int32_t in_w,
+                                            int32_t out_h, int32_t out_w, const int32_t* first_h, const float* weights_h, int32_t htaps,
+                                            const int32_t* first_v, const float* weights_v, int32_t vtaps, int32_t patch, int32_t temporal_patch,
+                                            int32_t merge, const float* mean, const float* stdv, void* out, int32_t out_dtype, void* workspace,
+                                            size_t workspace_bytes, void* host_staging, void* stream) {
+    if (!src || !weights_h || !weights_v || !mean || !stdv || !out || !workspace) return fail(nullptr, VQA_ERR_INVALID_ARG, "null pointer");
+    PreAAGeom g;
+    if (int rc = qwen_video_aa_args(in_h, in_w, out_h, out_w, first_h, htaps, first_v, vtaps, patch, temporal_patch, merge, total_frames, g))
+        return rc;
+    if (n_frames <= 0 || n_frames > 65535 || frame0 < 0 || frame0 + n_frames > total_frames)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "frames [frame0, frame0 + n_frames) must lie in the video, at most 65535 per call");
+    if (out_dtype != VQA_DTYPE_F32 && out_dtype != VQA_DTYPE_BF16) return fail(nullptr, VQA_ERR_INVALID_ARG, "out_dtype must be f32 or bf16");
+    g.frame0 = frame0;
+    const size_t nb[4] = {(size_t)out_w * sizeof(int32_t), (size_t)out_h * sizeof(int32_t), (size_t)out_w * htaps * sizeof(float),
+                          (size_t)out_h * vtaps * sizeof(float)};
+    const void* parts[4] = {first_h, first_v, weights_h, weights_v};
+    const size_t bytes = qwen_video_aa_table_bytes(g);
+    if (workspace_bytes < bytes) return fail(nullptr, VQA_ERR_WORKSPACE, "pre-processing workspace too small");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    uint8_t* ws = static_cast<uint8_t*>(workspace);
+    cudaError_t e = cudaSuccess;
+    if (host_staging) {
+        // caller-owned (pinned) staging: one truly asynchronous copy; the caller keeps the buffer untouched until the stream passes it
+        uint8_t* hs = static_cast<uint8_t*>(host_staging);
+        for (size_t i = 0, o = 0; i < 4; o += nb[i], ++i) memcpy(hs + o, parts[i], nb[i]);
+        e = cudaMemcpyAsync(ws, hs, bytes, cudaMemcpyHostToDevice, st);
+    } else {
+        for (size_t i = 0, o = 0; i < 4 && e == cudaSuccess; o += nb[i], ++i) e = cudaMemcpyAsync(ws + o, parts[i], nb[i], cudaMemcpyHostToDevice, st);
+    }
+    if (e != cudaSuccess) return fail(nullptr, VQA_ERR_CUDA, std::string("pre-processing table upload: ") + cudaGetErrorString(e));
+    const float3 mu = make_float3(mean[0], mean[1], mean[2]), sd = make_float3(stdv[0], stdv[1], stdv[2]);
+    const PrePatchGeom geom{patch, merge, temporal_patch};
+    const dim3 grid(g.tiles_x * ((out_h + g.tile_rows - 1) / g.tile_rows), n_frames);
+    const size_t smem = pre_aa_smem_bytes(g.band_rows);
+    const uint8_t* s8 = static_cast<const uint8_t*>(src);
+    const int* tab = reinterpret_cast<const int*>(ws);
+    if (out_dtype == VQA_DTYPE_F32) {
+        e = cudaFuncSetAttribute(video_resize_aa_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, PRE_AA_MAX_SMEM);
+        if (e == cudaSuccess) video_resize_aa_kernel<float><<<grid, PRE_THREADS, smem, st>>>(s8, tab, g, geom, mu, sd, static_cast<float*>(out));
+    } else {
+        e = cudaFuncSetAttribute(video_resize_aa_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, PRE_AA_MAX_SMEM);
+        if (e == cudaSuccess) video_resize_aa_kernel<bf16><<<grid, PRE_THREADS, smem, st>>>(s8, tab, g, geom, mu, sd, static_cast<bf16*>(out));
+    }
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(nullptr, VQA_ERR_CUDA, std::string("pre-processing launch: ") + cudaGetErrorString(e));
+    return VQA_OK;
+}
+
 // Host-only: the fixed-point tap table of one resize axis, exactly as vqa_clip_preprocess builds it (for CPU tests of the host logic).
 // bounds: [count][2] (first source index, taps used), kk: [count][ksize] with ksize = return value (call with kk = NULL to size it).
 extern "C" int32_t vqa_resample_table(int32_t in_size, int32_t out_size, int32_t first, int32_t count, int32_t* bounds, int32_t* kk) {

@@ -8,6 +8,7 @@ current CUDA stream.
 from __future__ import annotations
 
 import collections
+import functools
 import ctypes as C
 from typing import Dict, Optional, Sequence
 
@@ -997,6 +998,87 @@ def qwen_preprocess_video_u8(items: Sequence[torch.Tensor], device, patch: int =
     ring.release(dev)
     _check(rc, None, "vqa_qwen_preprocess_video")
     return out, [tuple(int(grid[3 * i + k]) for k in range(3)) for i in range(n)]
+
+
+# Frames of a video file go to the device in slices of at most this many bytes (at least one frame), so that host and device staging
+# stay bounded for long or large clips.
+VIDEO_SLICE_BYTES = 32 << 20
+
+
+@functools.lru_cache(maxsize=64)
+def _aa_bicubic_taps(in_size: int, out_size: int):
+    """torch's fp32 weights of interpolate(mode="bicubic", antialias=True, align_corners=False) along one axis, in_size -> out_size, as
+    (first input of each output's window int32 [out], weights fp32 [out, taps], taps). They are read off torch itself: channel j of the
+    input holds an impulse at position j, so output i of channel j is weight (i, j) exactly, whatever order torch sums in (every other
+    term is 0). An axis whose size does not change is copied, as torch does (weight 1)."""
+    eye = torch.eye(in_size, dtype=torch.float32)[None, :, None, :]
+    w = torch.nn.functional.interpolate(eye, size=(1, out_size), mode="bicubic", antialias=True, align_corners=False)[0, :, 0, :].t()
+    nz = (w != 0).int()
+    lo, hi = nz.argmax(1), in_size - 1 - nz.flip(1).argmax(1)
+    # a window whose first tap has weight exactly 0 starts one later than its neighbour's: the suffix minimum keeps the starts
+    # non-decreasing (the kernel's bands need it) and only adds zero-weight taps
+    first = lo.flip(0).cummin(0).values.flip(0)
+    taps = int((hi - first).max()) + 1
+    first = torch.clamp(first, max=in_size - taps)
+    return first.to(torch.int32).contiguous(), torch.gather(w, 1, first[:, None] + torch.arange(taps)).contiguous(), taps
+
+
+def qwen_preprocess_video_file_u8(frames, size, device, n_frames: Optional[int] = None, patch: int = 14, temporal_patch: int = 2,
+                                  merge: int = 2, mean=CLIP_MEAN, std=CLIP_STD, out_dtype: torch.dtype = torch.float32):
+    """Frames sampled from one video file -> (pixel_patches [t*gh*gw, 3*temporal*patch^2] on the device, (t, gh, gw)), what qwen_vl_utils
+    fetch_video + Qwen2VLVideoProcessor(do_resize=False) make of them: torchvision's antialiased bicubic resize to size = (rh, rw) in
+    fp32 with torch's weights, round half to even, then the frame-stack patch rows of qwen_preprocess_video_u8. `frames` is uint8
+    [n, h, w, 3] RGB (host or device), or an iterable of such slices of one video with n_frames their total; a host tensor goes to the
+    device in slices of VIDEO_SLICE_BYTES. One kernel launch (vqa_qwen_preprocess_video_aa) per slice. The resized uint8 frames equal
+    models/vqascore_models/qwen_utils.qwen_video_file_to_patches's except where torch's fp32 value is a rounding tie that a different
+    summation order on the host's CPU puts on the other side (DESIGN §4)."""
+    lib = _lib.load()
+    dev = torch.device(device)
+    if isinstance(frames, torch.Tensor) or hasattr(frames, "__array__"):
+        frames = torch.as_tensor(frames)
+        n_frames = int(frames.shape[0])
+        per = max(1, VIDEO_SLICE_BYTES // max(1, frames[0].numel()))
+        frames = [frames[i:i + per] for i in range(0, n_frames, per)]
+    assert n_frames is not None and n_frames > 0, "n_frames must be given with an iterable of slices"
+    rh, rw = (int(s) for s in size)
+    i32p, f32p = C.POINTER(C.c_int32), C.POINTER(C.c_float)
+    ip = lambda t: C.cast(t.data_ptr(), i32p)
+    fp = lambda t: C.cast(t.data_ptr(), f32p)
+    ring = _staging(dev)
+    hw, out, done = None, None, 0
+    for sl in frames:
+        sl = torch.as_tensor(sl)
+        assert sl.dtype == torch.uint8 and sl.dim() == 4 and sl.shape[-1] == 3, "frames must be uint8 [n, h, w, 3]"
+        k = int(sl.shape[0])
+        if hw is None:
+            hw = (int(sl.shape[1]), int(sl.shape[2]))
+            (fh, wh, th), (fv, wv, tv) = _aa_bicubic_taps(hw[1], rw), _aa_bicubic_taps(hw[0], rh)
+            rows, need = C.c_int64(0), C.c_size_t(0)
+            _check(lib.vqa_qwen_preprocess_video_aa_plan(hw[0], hw[1], rh, rw, ip(fh), th, ip(fv), tv, patch, temporal_patch, merge, n_frames,
+                                                         C.byref(rows), C.byref(need)), None, "vqa_qwen_preprocess_video_aa_plan")
+            out = torch.empty(int(rows.value), 3 * temporal_patch * patch * patch, dtype=out_dtype, device=dev)
+            wsb = torch.empty(int(need.value), dtype=torch.uint8, device=dev)
+        assert tuple(sl.shape[1:3]) == hw, "all frames of a video must have one size"
+        assert done + k <= n_frames, "more frames than n_frames"
+        if sl.is_cuda:
+            src = sl.contiguous()
+        else:
+            stage = ring.acquire(sl.numel())
+            stage[:sl.numel()].copy_(sl.reshape(-1))
+            src = torch.empty(sl.numel(), dtype=torch.uint8, device=dev)
+            src.copy_(stage[:sl.numel()], non_blocking=True)
+            ring.release(dev)
+        stage_buf = ring.acquire(wsb.numel())
+        with torch.cuda.device(dev):
+            rc = lib.vqa_qwen_preprocess_video_aa(_ptr(src), k, done, n_frames, hw[0], hw[1], rh, rw, ip(fh), fp(wh), th, ip(fv), fp(wv), tv,
+                                                  patch, temporal_patch, merge, (C.c_float * 3)(*mean), (C.c_float * 3)(*std), _ptr(out),
+                                                  _lib.VQA_DTYPE_F32 if out_dtype == torch.float32 else _lib.VQA_DTYPE_BF16, _ptr(wsb),
+                                                  wsb.numel(), stage_buf.data_ptr(), _stream_ptr(dev))
+        ring.release(dev)
+        _check(rc, None, "vqa_qwen_preprocess_video_aa")
+        done += k
+    assert done == n_frames, f"{done} frames given, n_frames = {n_frames}"
+    return out, ((n_frames + temporal_patch - 1) // temporal_patch, rh // patch, rw // patch)
 
 
 # ================================================================================================ Qwen2.5-VL

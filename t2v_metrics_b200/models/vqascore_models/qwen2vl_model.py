@@ -1,4 +1,4 @@
-"""Qwen2.5-VL VQAScore plugin backed by the H100 engine (image inputs).
+"""Qwen2.5-VL VQAScore plugin backed by the H100 engine (image and video inputs).
 
 Same plugin contract as the reference's `Qwen2VLModel` (t2v_metrics/models/vqascore_models/qwen2vl_model.py:93-301): class
 attributes, `forward(images, texts, question_template, answer_template, temperature) -> CPU fp32 Tensor[n]` with
@@ -10,7 +10,9 @@ pairs run as batched rollouts on the GPU decode loop, with the answer probabilit
 Videos arrive as decoded frame stacks: a 4-D `.npy` [n, h, w, 3] is scored as a video, as the reference's decoder-free path does
 (qwen2vl_model.py:145-153, a list of frames as `{"type": "video"}`), with its frames pre-processed on the device in the same launch as the
 still images of the call, video tokens in the prompt and the processor's `second_per_grid_ts`. Stills and videos mix freely in one call.
-Video files (.mp4, .avi, .mov, .mkv: decoding and fps frame sampling) are outside this engine's scope and raise.
+Video files (.mp4, .avi, .mov, .mkv) are scored when the plugin has a decoder (`video_reader=`, opt-in), as the reference's file path does
+(qwen2vl_model.py:135-144): qwen_vl_utils' frame sampling at `fps` and pixel budget on the host, torchvision's antialiased bicubic resize
+of the sampled frames on the device. Without a decoder they raise, before anything is launched.
 """
 from __future__ import annotations
 
@@ -41,6 +43,15 @@ QWEN_VL_UTILS_MAX_PIXELS = 16384 * 28 * 28
 HF_FRAME_LIST_FPS = 24
 
 _VIDEO_FILES = (".mp4", ".avi", ".mov", ".mkv")
+
+# The reference's video element for a file (qwen2vl_model.py:135-144): {"type": "video", "video": path, "max_pixels": 360*420, "fps": fps},
+# with fps None -> the model table's 8.0, and fps "dynamic" -> no "fps" key, so qwen_vl_utils' FPS = 2.0 applies.
+VIDEO_FILE_MAX_PIXELS = 360 * 420
+VIDEO_FILE_DEFAULT_FPS = 8.0
+
+
+def _is_video_file(path: str) -> bool:
+    return path[-4:].lower() in _VIDEO_FILES
 
 
 def _is_frame_stack(path: str) -> bool:
@@ -105,9 +116,20 @@ class Qwen2VLModel(VQAScoreModel):
     def __init__(self, model_name="qwen2.5-vl-7b", device="cuda", cache_dir=HF_CACHE_DIR, tokenizer=None,
                  state_dict: Optional[Dict[str, torch.Tensor]] = None, config: Optional[Qwen25VLConfig] = None,
                  checkpoint: Optional[str] = None, repetition_penalty: Optional[float] = None,
-                 min_pixels: int = QWEN_VL_UTILS_MIN_PIXELS, max_pixels: int = QWEN_VL_UTILS_MAX_PIXELS, **kwargs):
+                 min_pixels: int = QWEN_VL_UTILS_MIN_PIXELS, max_pixels: int = QWEN_VL_UTILS_MAX_PIXELS, video_reader=None, **kwargs):
+        """`video_reader` decodes video files: "opencv" (qwen_utils.OpenCVVideoReader) or any object with
+        open(path) -> (num_frames, avg_fps, get(indices) -> uint8 [k, h, w, 3] RGB). None (the default): video files raise, and videos
+        are given as decoded frame stacks (4-D .npy). It is opt-in because two decoders need not return the same pixels for one file,
+        and every parity guarantee of this engine starts from identical decoded pixels: the reference decodes with decord, so a reader
+        wrapping decord reproduces its frames, and OpenCV's may differ."""
         assert model_name in QWEN2_VL_MODELS
         self.min_pixels, self.max_pixels = int(min_pixels), int(max_pixels)
+        if video_reader == "opencv":
+            from .qwen_utils import OpenCVVideoReader
+            video_reader = OpenCVVideoReader()
+        elif video_reader is not None and not callable(getattr(video_reader, "open", None)):
+            raise ValueError("video_reader must be None, 'opencv' or an object with open(path) -> (num_frames, avg_fps, get)")
+        self.video_reader = video_reader
         # The reference's scores come out of `generate(..., output_scores=True)`, i.e. AFTER the logits processors the checkpoint's
         # generation_config.json configures (SURVEY F8; Qwen2.5-VL-Instruct ships repetition_penalty 1.05). None = read it from the
         # generation_config.json next to `checkpoint` when there is one, else 1.0 (off).
@@ -137,12 +159,25 @@ class Qwen2VLModel(VQAScoreModel):
         self.engine.load_state_dict(sd)
         self._state_dict = None
 
-    def load_images(self, image: List[str]):
+    def load_images(self, image: List[str], fps=None):
         """-> (patches fp32 [sum P, 1176] on the device, [(t, gh, gw), ...]): t = 1 for a still image, ceil(n / 2) for a 4-D .npy stack
-        of n frames (a video)."""
-        if any(p[-4:].lower() in _VIDEO_FILES for p in image):
-            raise NotImplementedError("video files need decoding, which is outside the engine's scope: pass the decoded frames as a 4-D "
-                                      ".npy [n, h, w, 3]")
+        of n frames or for n frames sampled from a video file at `fps` (a video)."""
+        files = [p for p in image if _is_video_file(p)]
+        if files and getattr(self, "video_reader", None) is None:
+            raise NotImplementedError("video files need a decoder: construct the model with video_reader='opencv' (or a reader object), "
+                                      "or pass the decoded frames as a 4-D .npy [n, h, w, 3]")
+        if files:
+            rest = [p for p in image if not _is_video_file(p)]
+            loaded = dict(zip(files, (self._load_video_file(p, fps) for p in files)))
+            if rest:
+                patches, grids = self.load_images(rest)
+                o = 0
+                for p, g in zip(rest, grids):
+                    n = g[0] * g[1] * g[2]
+                    loaded[p] = (patches[o:o + n], g)
+                    o += n
+            parts = [loaded[p] for p in image]
+            return torch.cat([x for x, _ in parts]), [g for _, g in parts]
         # PIL decode on the host, everything else (smart_resize, PIL-exact bicubic, normalise, frame duplication or pairing, merge-order
         # patch rows) in ONE device kernel -- bit-identical to qwen_utils.qwen_image_to_patches / qwen_video_to_patches, the CPU paths
         # the reference runs per image / per video
@@ -170,14 +205,32 @@ class Qwen2VLModel(VQAScoreModel):
         return pre(raw, self.engine.device, self.cfg.patch_size, self.cfg.temporal_patch_size, self.cfg.spatial_merge_size,
                    min_pixels=self.min_pixels, max_pixels=self.max_pixels)
 
-    def _vision(self, images: List[str]):
+    def _load_video_file(self, path: str, fps):
+        """One video file -> (patches on the device, (t, gh, gw)): the reader's frames at qwen_vl_utils' sampled indices, sent to the
+        device in slices of engine.VIDEO_SLICE_BYTES and resized there (engine.qwen_preprocess_video_file_u8)."""
+        import numpy as np
+        from ...engine import VIDEO_SLICE_BYTES, qwen_preprocess_video_file_u8
+        from .qwen_utils import qwen_video_file_plan
+        fps = VIDEO_FILE_DEFAULT_FPS if fps is None else fps
+        total, avg_fps, get = self.video_reader.open(path)
+        first = np.asarray(get([0]))             # every sampling starts at frame 0, and its size is the video's
+        idx, _, size = qwen_video_file_plan(total, avg_fps, first.shape[1], first.shape[2], fps=None if fps == "dynamic" else float(fps),
+                                            max_pixels=VIDEO_FILE_MAX_PIXELS)
+        per = max(1, VIDEO_SLICE_BYTES // first[0].size)
+        slices = (torch.from_numpy(np.ascontiguousarray(get(idx[i:i + per]), dtype=np.uint8)) for i in range(0, len(idx), per))
+        return qwen_preprocess_video_file_u8(slices, size, self.engine.device, n_frames=len(idx), patch=self.cfg.patch_size,
+                                             temporal_patch=self.cfg.temporal_patch_size, merge=self.cfg.spatial_merge_size)
+
+    def _vision(self, images: List[str], fps=None):
         """Identical paths encoded once: -> (item of every pair, patches, grids, per-item prompt token id, per-item second_per_grid_ts
-        or None when there is no video)."""
+        or None when there is no video). A video file gets the 2/24 of a frame stack: the reference hands its frames to the processor as
+        a tensor without metadata, whose sampled_fps is 24 whatever `fps` sampled them (see HF_FRAME_LIST_FPS)."""
         uniq: Dict[str, int] = {}
         index = [uniq.setdefault(p, len(uniq)) for p in images]
         paths = list(uniq.keys())
-        patches, grids = self.load_images(paths)
-        video = [_is_frame_stack(p) for p in paths]
+        files = [_is_video_file(p) for p in paths]
+        patches, grids = self.load_images(paths, fps) if any(files) else self.load_images(paths)
+        video = [f or _is_frame_stack(p) for p, f in zip(paths, files)]
         tokens = [self.cfg.video_token_id if v else self.cfg.image_token_id for v in video]
         spg = [self.cfg.temporal_patch_size / HF_FRAME_LIST_FPS if v else 1.0 for v in video] if any(video) else None
         return index, patches, grids, tokens, spg
@@ -208,9 +261,10 @@ class Qwen2VLModel(VQAScoreModel):
         if max_new_tokens != 1:
             _require_rollout_engine(self)
             return self._trace_rollout(images, texts, question_template, answer_template, max_new_tokens, temperature, score_position, debug,
-                                       repetition_penalty)
+                                       repetition_penalty, fps)
         assert len(images) == len(texts), "Number of images/videos and texts must match"
-        probs, answer_ids, ids, top_p = self._score(images, texts, question_template, answer_template, temperature, repetition_penalty, 5)
+        probs, answer_ids, ids, top_p = self._score(images, texts, question_template, answer_template, temperature, repetition_penalty, 5,
+                                                    fps)
         dec = lambda t: self.tokenizer.decode([t]) if hasattr(self.tokenizer, "decode") else str(t)
         special = {getattr(self.tokenizer, n, None) for n in ("eos_token_id", "bos_token_id", "pad_token_id")} - {None}
         traces = []
@@ -240,7 +294,7 @@ class Qwen2VLModel(VQAScoreModel):
         return [int(e) for e in eos] if isinstance(eos, (list, tuple)) else [int(eos)]
 
     def _rollout(self, images: List[str], texts: List[str], question_template: str, answer_template: str, max_new_tokens: int,
-                 temperature: float, repetition_penalty: float, mode: str, top_k: int) -> List[dict]:
+                 temperature: float, repetition_penalty: float, mode: str, top_k: int, fps=None) -> List[dict]:
         """Scored greedy rollouts of max_new_tokens for every (image, text) pair: the scoring prompt, generate(do_sample=False) under the
         repetition penalty and the EOS ids of generation, and per step the log-probability of every answer token
         (engine.rollout_scores), then the reference's step selection (qwen_host.rollout_answer_score, `mode` "forward", "start" or "end").
@@ -252,7 +306,7 @@ class Qwen2VLModel(VQAScoreModel):
             raise ValueError("max_new_tokens must be at least 1")
         questions = [question_template.format(t) for t in texts]
         answers = [answer_template.format(t) for t in texts]
-        index, patches, grids, tokens, spg = self._vision(images)
+        index, patches, grids, tokens, spg = self._vision(images, fps)
         unit = self.cfg.spatial_merge_size ** 2
         cache = self._memo()
         prompts, answer_ids = [], []
@@ -280,11 +334,11 @@ class Qwen2VLModel(VQAScoreModel):
         return results
 
     def _trace_rollout(self, images, texts, question_template, answer_template, max_new_tokens, temperature, score_position, debug,
-                       repetition_penalty):
+                       repetition_penalty, fps=None):
         """forward_with_trace for max_new_tokens > 1 (reference qwen2vl_model.py:381-487): scored rollouts, answer tokens placed at the
         start or the end of the generation, and the reference's trace dictionary per sample."""
         pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
-        results = self._rollout(images, texts, question_template, answer_template, max_new_tokens, temperature, pen, score_position, 5)
+        results = self._rollout(images, texts, question_template, answer_template, max_new_tokens, temperature, pen, score_position, 5, fps)
         one = lambda t: self.tokenizer.decode([int(t)])
         traces = []
         for b, r in enumerate(results):
@@ -310,14 +364,15 @@ class Qwen2VLModel(VQAScoreModel):
         """Greedy text generation, the reference's Qwen2VLModel.generate (qwen2vl_model.py:495-563) with its default temperature 0: per
         sample, the chat prompt of the raw text and the image, generate(do_sample=False) under the checkpoint's repetition penalty, the
         prompt cut off, decoded with skip_special_tokens and stripped. Here the whole batch is one prefill and one decode loop on the
-        device (a call with a video: as few as fit VIDEO_WORKSPACE_BUDGET); identical paths are encoded once. `fps` does not change the
-        output for a .npy frame stack (see HF_FRAME_LIST_FPS). Sampling (temperature > 0 or do_sample=True, top-p) is not implemented."""
+        device (a call with a video: as few as fit VIDEO_WORKSPACE_BUDGET); identical paths are encoded once. `fps` samples the frames
+        of a video file and does not change the output for a .npy frame stack (see HF_FRAME_LIST_FPS). Sampling (temperature > 0 or
+        do_sample=True, top-p) is not implemented."""
         assert len(images) == len(texts), "Number of images/videos and texts must match"
         if do_sample is None:
             do_sample = temperature > 0
         if do_sample or temperature > 0:
             raise NotImplementedError("only greedy decoding is supported (temperature=0.0, do_sample=False); top-p sampling is not implemented")
-        index, patches, grids, tokens, spg = self._vision(images)
+        index, patches, grids, tokens, spg = self._vision(images, fps)
         unit = self.cfg.spatial_merge_size ** 2
         cache = self._memo()
         prompts = []
@@ -341,12 +396,12 @@ class Qwen2VLModel(VQAScoreModel):
         return _chunks(len(prompts), len(prompts), self.VIDEO_WORKSPACE_BUDGET, workspace_bytes, max(len(p) for p in prompts),
                        [t * h * w for t, h, w in grids])
 
-    def _score(self, images, texts, question_template, answer_template, temperature, repetition_penalty, top_k):
+    def _score(self, images, texts, question_template, answer_template, temperature, repetition_penalty, top_k, fps=None):
         """Single-prefill scores of the first answer token -> (probs fp32 CPU [n], answer ids, and with top_k > 0 the top-k ids / probs of
         the last position as lists, else None, None)."""
         questions = [question_template.format(t) for t in texts]
         answers = [answer_template.format(t) for t in texts]
-        index, patches, grids, tokens, spg = self._vision(images)
+        index, patches, grids, tokens, spg = self._vision(images, fps)
         unit = self.cfg.spatial_merge_size ** 2
         prompts, answer_ids = [], []
         cache = self._memo()
@@ -375,6 +430,7 @@ class Qwen2VLModel(VQAScoreModel):
                 debug: bool = False, repetition_penalty: Optional[float] = None) -> torch.Tensor:
         """Scores of (image or video, text) pairs. A 4-D .npy is a video; `fps` is accepted and does not change its score, as in the
         reference on transformers 5.5.0, whose processor takes a frame list's rate to be 24 fps whatever is passed (HF_FRAME_LIST_FPS).
+        A video file (with a `video_reader`) is a video whose frames are sampled at `fps` (None: 8.0; "dynamic": qwen_vl_utils' 2.0).
         A call with a video runs as few single-prefill engine calls as fit VIDEO_WORKSPACE_BUDGET; one with still images only, as one."""
         assert len(images) == len(texts), "Number of images/videos and texts must match"
         if max_new_tokens != 1:
@@ -383,5 +439,5 @@ class Qwen2VLModel(VQAScoreModel):
             _require_rollout_engine(self)
             pen = self.repetition_penalty if repetition_penalty is None else repetition_penalty
             return torch.tensor([r["score"] for r in self._rollout(images, texts, question_template, answer_template, max_new_tokens,
-                                                                    temperature, pen, "forward", 0)], dtype=torch.float32)
-        return self._score(images, texts, question_template, answer_template, temperature, repetition_penalty, 0)[0]
+                                                                    temperature, pen, "forward", 0, fps)], dtype=torch.float32)
+        return self._score(images, texts, question_template, answer_template, temperature, repetition_penalty, 0, fps)[0]

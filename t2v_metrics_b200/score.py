@@ -6,7 +6,8 @@ Differences, all above the drop-in boundary and result-preserving:
     image once. The reference loops `self.model.forward([image] * N, texts)` per image (score.py:104-106).
   * `batch_forward` scores a whole DataLoader batch per (visual, text) slot, as v3.0 did, instead of one pair at a time
     (v3.1 score.py:143-153).
-  * video inputs (the cv2 concat path, score.py:72-98) are CPU pre-processing outside this engine's scope and raise.
+  * video files reach a model that takes them directly (`video_mode == "direct"`, score.py:99-101) when the plugin has a decoder
+    (Qwen2.5-VL with `video_reader=`); otherwise, and for the cv2 concat path (score.py:72-98), video inputs raise.
 """
 from typing import List, Optional, TypedDict, Union
 
@@ -42,6 +43,10 @@ class Score(nn.Module):
     def list_all_models(self) -> List[str]:
         raise NotImplementedError("Subclasses must implement list_all_models")
 
+    def _takes_video_files(self) -> bool:
+        """The plugin decodes and scores video files itself: video_mode "direct" and a video reader."""
+        return getattr(self.model, "video_mode", None) == "direct" and getattr(self.model, "video_reader", None) is not None
+
     def forward(self, images: Optional[Union[str, List[str]]] = None, texts: Optional[Union[str, List[str]]] = None,
                 num_frames: Optional[int] = 8, **kwargs) -> torch.Tensor:
         """m images x n texts -> [m, n] tensor of scores on self.device."""
@@ -49,7 +54,7 @@ class Score(nn.Module):
             images = [images]
         if isinstance(texts, str):
             texts = [texts]
-        if any(isinstance(img, str) and img[-4:].lower() in VIDEO_EXTENSIONS for img in images):
+        if any(isinstance(img, str) and img[-4:].lower() in VIDEO_EXTENSIONS for img in images) and not self._takes_video_files():
             raise NotImplementedError("video inputs (frame extraction + concat, reference score.py:72-98) are outside the "
                                       "engine's hot-path scope; pass image files")
         m, n = len(images), len(texts)
@@ -80,19 +85,20 @@ class Score(nn.Module):
         """[num_samples, num_visuals, num_texts] scores for a dataset of {'images': [...], 'texts': [...]} items."""
         from torch.utils.data import DataLoader
         num_samples = len(dataset)
-        if "videos" in dataset[0]:
+        media = "videos" if "videos" in dataset[0] else "images"
+        if media == "videos" and not self._takes_video_files():
             raise NotImplementedError("video datasets are outside the engine's hot-path scope")
-        num_visuals = len(dataset[0]['images'])
+        num_visuals = len(dataset[0][media])
         num_texts = len(dataset[0]['texts'])
         scores = torch.zeros(num_samples, num_visuals, num_texts).to(self.device)
         dataloader = DataLoader(dataset, batch_size=batch_size, shuffle=False)
         counter = 0
         for batch_idx, batch in enumerate(dataloader):
-            cur = len(batch['images'][0])
-            assert len(batch['images']) == num_visuals and len(batch['texts']) == num_texts
+            cur = len(batch[media][0])
+            assert len(batch[media]) == num_visuals and len(batch['texts']) == num_texts
             for vis_idx in range(num_visuals):
                 for text_idx in range(num_texts):
                     scores[counter:counter + cur, vis_idx, text_idx] = self.model.forward(
-                        list(batch['images'][vis_idx]), list(batch['texts'][text_idx]), **kwargs).to(self.device)
+                        list(batch[media][vis_idx]), list(batch['texts'][text_idx]), **kwargs).to(self.device)
             counter += cur
         return scores
