@@ -311,6 +311,10 @@ int vqa_set_gemm_schedule(int32_t group_rows, int32_t chunk_rows);
  * (cudaOccupancyMaxActiveClusters); negative vqa_status on error. */
 int vqa_debug_max_active_clusters(int32_t cluster_size);
 
+/* 1 when this process launches the GEMM and attention kernels with programmatic dependent launch (VQA_PDL=1, read once per process),
+ * else 0. */
+int vqa_debug_pdl_enabled(void);
+
 const char* vqa_last_error(vqa_handle* h);
 void vqa_destroy(vqa_handle* h);
 
@@ -522,7 +526,9 @@ int vqa_op_gemm_bf16_f32acc(const void* A, int32_t lda, const void* W, int32_t l
  * and W as [w_rows, w_cols] (ldw); rows past those extents read as zero, so a batch's last A or W rows may run past them (the absorbed
  * cross-attention's score GEMM reads Sp - S rows past the encoder output in its last batch). Accepted when every batch's first row lies
  * inside its operand's rows ((nb - 1) * a_row_off < a_rows, (nb - 1) * w_row_off < w_rows) and its K columns inside its columns
- * ((nb - 1) * a_k_off + K <= a_cols, likewise W); lda, ldw, ldc, N, K, c_stride multiples of 8, a_cols <= lda, w_cols <= ldw, ldc >= N,
+ * ((nb - 1) * a_k_off + K <= a_cols, likewise W); K a multiple of 64, or a_cols == K or w_cols == K (the k blocks are 64 columns wide
+ * and are clipped only at the extents: with a K tail, the columns past K of the operand whose extent ends at K read as zero, and the other
+ * operand's columns there, inside its extent, must be finite); lda, ldw, ldc, N, K, c_stride multiples of 8, a_cols <= lda, w_cols <= ldw, ldc >= N,
  * offsets >= 0, A / W / C 16-byte aligned; else VQA_ERR_INVALID_ARG. variant as vqa_op_gemm_bf16. */
 int vqa_op_gemm_bf16_batched(const void* A, int32_t lda, const void* W, int32_t ldw, void* C, int32_t ldc, int32_t M, int32_t N, int32_t K,
                              int32_t nb, int32_t a_row_off, int32_t a_k_off, int32_t w_row_off, int32_t w_k_off, int64_t c_stride,

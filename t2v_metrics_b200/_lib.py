@@ -20,7 +20,7 @@ ABI_SYMBOLS = [
     "vqa_clip_preprocess_workspace_bytes", "vqa_clip_preprocess", "vqa_resample_table", "vqa_qwen_preprocess_plan",
     "vqa_qwen_preprocess", "vqa_clipt5_debug_layout", "vqa_qwen25vl_debug_layout", "vqa_set_gemm_schedule",
     "vqa_qwen25vl_topk", "vqa_op_gemm_bf16_normfuse",
-    "vqa_qwen25vl_packed_workspace_bytes", "vqa_qwen25vl_score_packed", "vqa_debug_max_active_clusters", "vqa_op_attention_d128_ex", "vqa_op_gemm_bf16_grouped", "vqa_op_gemm_bf16_splitk",
+    "vqa_qwen25vl_packed_workspace_bytes", "vqa_qwen25vl_score_packed", "vqa_debug_max_active_clusters", "vqa_debug_pdl_enabled", "vqa_op_attention_d128_ex", "vqa_op_gemm_bf16_grouped", "vqa_op_gemm_bf16_splitk",
     "vqa_qwen25vl_generate_workspace_bytes", "vqa_qwen25vl_generate_prefill", "vqa_qwen25vl_generate_step",
     "vqa_clipt5_generate_workspace_bytes", "vqa_clipt5_generate_prefill", "vqa_clipt5_generate_step",
     "vqa_qwen25vl_rollout_prefill", "vqa_qwen25vl_rollout_step", "vqa_op_answer_logprob",
@@ -232,6 +232,8 @@ def load() -> C.CDLL:
     lib.vqa_op_gemm_bf16_splitk.restype = C.c_int
     lib.vqa_debug_max_active_clusters.argtypes = [i32]
     lib.vqa_debug_max_active_clusters.restype = C.c_int
+    lib.vqa_debug_pdl_enabled.argtypes = []
+    lib.vqa_debug_pdl_enabled.restype = C.c_int
     lib.vqa_resample_table.argtypes = [i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32)]
     lib.vqa_resample_table.restype = i32
     _lib = lib

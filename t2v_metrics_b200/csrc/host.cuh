@@ -195,6 +195,12 @@ struct BatchSpec {
     long long a_rows, a_cols, w_rows, w_cols;   // full extents visible to TMA
 };
 
+// The kernel reads K in whole 64-column k blocks and clips them only at the operands' tensor-map extents (a_cols / w_cols, not K): with
+// K % 64 != 0 the last k block of every batch multiplies columns K .. roundup(K, 64) of its A and W rows. Those products vanish only when
+// one operand's extent ends at K, so that its tail reads TMA zero fill (that extent is then K wide, so the extents check has already
+// forced its batches to k offset 0).
+static bool batched_k_tail_ok(long long K, long long a_cols, long long w_cols) { return K % 64 == 0 || a_cols == K || w_cols == K; }
+
 // One GEMM: C[M, N] = epi(A[M, K] . W[N, K]^T) and its optional parts. The constructor sets the dense layout (lda = ldw = K, N weight
 // rows, ldc = N); the setters name what differs from it.
 struct Gemm {
@@ -268,6 +274,7 @@ static cudaError_t run_gemm(const Gemm& g, int num_sms, cudaStream_t st) {
     }
     if (g.batch.nb > 0) {
         const BatchSpec& bs = g.batch;
+        if (!batched_k_tail_ok(g.K, bs.a_cols, bs.w_cols)) return cudaErrorInvalidValue;
         L.w_rows = (int)bs.w_rows; L.a_rows = bs.a_rows; L.a_cols = bs.a_cols; L.w_cols = bs.w_cols;
         p.num_batches = bs.nb; p.a_row_off = bs.a_row_off; p.a_k_off = bs.a_k_off; p.w_row_off = bs.w_row_off;
         p.w_k_off = bs.w_k_off; p.c_batch_stride = bs.c_stride;

@@ -205,6 +205,9 @@ extern "C" int vqa_set_gemm_schedule(int32_t group_rows, int32_t chunk_rows) {
     return VQA_OK;
 }
 
+// 1 when this process launches the GEMM and attention kernels with programmatic dependent launch (VQA_PDL=1, read once), else 0.
+extern "C" int vqa_debug_pdl_enabled(void) { return pdl_enabled() ? 1 : 0; }
+
 // How many clusters of `cluster_size` CTAs of the 256-wide GEMM kernel (one CTA per SM: ~200 KB of shared memory) the current
 // device can hold at once (cudaOccupancyMaxActiveClusters). 132 SMs do not always divide into GPC-local clusters of 4 or 8: this is the
 // number a cluster-multicast variant of the GEMM has to be sized against. Returns the count, or a negative vqa_status.
@@ -825,6 +828,8 @@ extern "C" int vqa_op_gemm_bf16_batched(const void* A, int32_t lda, const void* 
     const long long last = nb - 1;
     if (last * a_row_off >= a_rows || last * w_row_off >= w_rows || last * a_k_off + K > a_cols || last * w_k_off + K > w_cols)
         return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: every batch's first A / W row and its K columns must lie inside the extents");
+    if (!batched_k_tail_ok(K, a_cols, w_cols))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: with K % 64 != 0, a_cols or w_cols must equal K");
     if (!gemm_variant_known(variant)) return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: unknown tile variant");
     Gemm g = abi_gemm(A, lda, W, ldw, (int)w_rows, C, ldc, M, N, K);
     g.batched(BatchSpec{nb, a_row_off, a_k_off, w_row_off, w_k_off, c_stride, a_rows, a_cols, w_rows, w_cols}, variant);

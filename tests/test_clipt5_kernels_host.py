@@ -97,6 +97,25 @@ def test_batched_gemm_argument_checks():
         assert call(**{k: None}) == INVALID, k
 
 
+@no_device
+def test_batched_gemm_k_tail_needs_one_operand_extent_at_k():
+    """The kernel reads K in 64-column k blocks clipped only at the extents: with K % 64 != 0 the tail block of every batch adds the
+    products of columns K .. roundup(K, 64), which vanish only when A's or W's extent ends at K (TMA zero fill). Refused otherwise, for
+    one batch, K-offset batches and row-offset batches alike; accepted with an extent at K (the `ctx = P x` launch has K = a_cols = Sp = 608)."""
+    lib = _lib.load()
+    call = lambda **kw: batched_call(lib, **kw)
+    q = dict(PRODUCTION["q~ = Wk^T q"], K=72, lda=72 * H, ldw=72 * H, a_off=(0, 72), w_off=(0, 72), a_ext=(MD, 72 * H), w_ext=(DM, 72 * H))
+    assert call(**q) == INVALID
+    assert call(**dict(q, w_off=(0, 0))) == INVALID and call(**dict(q, a_off=(0, 0))) == INVALID
+    assert call(**dict(q, nb=1)) == INVALID                                   # one batch: a 128-term dot product
+    assert call(**dict(q, nb=1, a_ext=(MD, 72))) == CUDA_ERR and call(**dict(q, nb=1, w_ext=(DM, 72))) == CUDA_ERR
+    assert call(**dict(q, a_off=(0, 0), a_ext=(MD, 72))) == CUDA_ERR       # W offset along K, A's tail zero-filled in every batch
+    assert call(**dict(q, K=128, a_off=(0, 128), w_off=(0, 128), lda=128 * H, ldw=128 * H, a_ext=(MD, 128 * H), w_ext=(DM, 128 * H))) == CUDA_ERR
+    assert call(K=DM - 8) == INVALID                                          # rows-offset scores launch: columns DM - 8 .. DM would be added
+    assert call(K=DM - 8, a_ext=(B * TH, DM - 8)) == CUDA_ERR and call(K=DM - 8, w_ext=(B * S, DM - 8)) == CUDA_ERR
+    assert call(**PRODUCTION["ctx = P x"]) == CUDA_ERR
+
+
 def cross_attn_workspace(B, T, S, H, Dm):
     """The documented mode-0 layout: xt | q~ | csc | ctx, each at the next multiple of 256 bytes."""
     r = lambda n: (n + 255) // 256 * 256
