@@ -4,6 +4,7 @@ Public surface mirrors the reference package (t2v_metrics/__init__.py:23-33): VQ
 get_score_model. The ffmpeg import gate of the reference is not reproduced: video decoding is outside this engine.
 """
 from .constants import HF_CACHE_DIR
+from .models.vqascore_models import accepted_vqascore_models
 from .vqascore import VQAScore, list_all_vqascore_models
 
 __all__ = ["VQAScore", "list_all_models", "get_score_model", "HF_CACHE_DIR"]
@@ -14,6 +15,6 @@ def list_all_models():
 
 
 def get_score_model(model='clip-flant5-xxl', device='cuda', cache_dir=HF_CACHE_DIR, **kwargs):
-    if model in list_all_vqascore_models():
+    if model in accepted_vqascore_models():
         return VQAScore(model, device=device, cache_dir=cache_dir, **kwargs)
     raise NotImplementedError()

@@ -2,6 +2,7 @@
 t2v_metrics/models/vqascore_models/mm_utils.py:182-241, reduced to what the kernels need)."""
 from __future__ import annotations
 
+import dataclasses
 from dataclasses import dataclass
 
 
@@ -75,6 +76,8 @@ class Qwen25VLConfig:
     mrope_section: tuple = (16, 24, 24)
     image_token_id: int = 151655
     video_token_id: int = 151656
+    # lm_head shares the embedding matrix (the checkpoint then stores no `lm_head.weight`)
+    tie_word_embeddings: bool = False
 
     @property
     def head_dim(self) -> int:
@@ -96,7 +99,63 @@ class Qwen25VLConfig:
     def qwen25_vl_7b() -> "Qwen25VLConfig":
         return Qwen25VLConfig()
 
+    @staticmethod
+    def qwen25_vl_3b() -> "Qwen25VLConfig":
+        """Qwen/Qwen2.5-VL-3B-Instruct's config.json: hidden_size 2048, num_hidden_layers 36, num_attention_heads 16,
+        num_key_value_heads 2, intermediate_size 11008, vocab_size 151936, tie_word_embeddings true; vision_config as the 7B's with
+        out_hidden_size 2048. A checkpoint directory's own config.json is compared against these values when it is loaded
+        (Qwen2VLModel.load_model), so a disagreement raises instead of binding wrong shapes."""
+        return Qwen25VLConfig(out_hidden=2048, hidden=2048, layers=36, heads=16, kv_heads=2, mlp=11008, vocab=151936,
+                              tie_word_embeddings=True)
 
+    @staticmethod
+    def from_hf_config(path_or_dict) -> "Qwen25VLConfig":
+        """The dims of a checkpoint's config.json (a path to the file or to its directory, or the parsed dict). Accepts both layouts
+        transformers reads: the published flat one (text fields at the top level, `rope_scaling`) and transformers 5.5.0's
+        `Qwen2_5_VLConfig.to_dict()` (text fields under `text_config`, `rope_parameters`); `vision_config` holds the tower in both.
+        Fields a file leaves out keep this class's defaults."""
+        import json
+        import os
+        d = path_or_dict
+        if not isinstance(d, dict):
+            path = os.path.join(d, "config.json") if os.path.isdir(d) else d
+            with open(path) as f:
+                d = json.load(f)
+        text = dict(d)
+        text.update(d.get("text_config") or {})
+        vis = d.get("vision_config") or {}
+        rope = text.get("rope_parameters") or text.get("rope_scaling") or {}
+        base = Qwen25VLConfig()
+        kw = dict(
+            vit_depth=vis.get("depth"), vit_hidden=vis.get("hidden_size"), vit_heads=vis.get("num_heads"), vit_mlp=vis.get("intermediate_size"),
+            patch_size=vis.get("patch_size"), temporal_patch_size=vis.get("temporal_patch_size"), spatial_merge_size=vis.get("spatial_merge_size"),
+            window_size=vis.get("window_size"), out_hidden=vis.get("out_hidden_size"), tokens_per_second=vis.get("tokens_per_second"),
+            hidden=text.get("hidden_size"), layers=text.get("num_hidden_layers"), heads=text.get("num_attention_heads"),
+            kv_heads=text.get("num_key_value_heads"), mlp=text.get("intermediate_size"), vocab=text.get("vocab_size"),
+            rms_eps=text.get("rms_norm_eps"), rope_theta=rope.get("rope_theta", text.get("rope_theta")),
+            image_token_id=d.get("image_token_id"), video_token_id=d.get("video_token_id"),
+            tie_word_embeddings=d.get("tie_word_embeddings", text.get("tie_word_embeddings")))
+        if vis.get("fullatt_block_indexes") is not None:
+            kw["fullatt_block_indexes"] = tuple(vis["fullatt_block_indexes"])
+        if rope.get("mrope_section") is not None:
+            kw["mrope_section"] = tuple(rope["mrope_section"])
+        kw = {k: v for k, v in kw.items() if v is not None}
+        for k in ("rms_eps", "rope_theta"):
+            if k in kw:
+                kw[k] = float(kw[k])
+        if "tie_word_embeddings" in kw:
+            kw["tie_word_embeddings"] = bool(kw["tie_word_embeddings"])
+        return dataclasses.replace(base, **kw)
+
+    def mismatches(self, other: "Qwen25VLConfig") -> dict:
+        """{field: (self's value, other's value)} over every field that decides a kernel shape, a weight binding or the arithmetic."""
+        return {f.name: (getattr(self, f.name), getattr(other, f.name)) for f in dataclasses.fields(self)
+                if getattr(self, f.name) != getattr(other, f.name)}
+
+
+# listed: the name appears in list_all_models(). That listing holds the sizes bench.py measures, so that every listed name is a bench.py
+# workload. The 3B is not a bench.py workload; VQAScore and get_score_model accept it by name.
 QWEN25VL_MODELS = {
-    "qwen2.5-vl-7b": dict(config=Qwen25VLConfig.qwen25_vl_7b, weights="Qwen/Qwen2.5-VL-7B-Instruct"),
+    "qwen2.5-vl-3b": dict(config=Qwen25VLConfig.qwen25_vl_3b, weights="Qwen/Qwen2.5-VL-3B-Instruct", listed=False),
+    "qwen2.5-vl-7b": dict(config=Qwen25VLConfig.qwen25_vl_7b, weights="Qwen/Qwen2.5-VL-7B-Instruct", listed=True),
 }

@@ -1088,7 +1088,8 @@ def convert_qwen_state_dict(sd: Dict[str, torch.Tensor], cfg, device) -> Dict[st
         scatters each 80-wide head into the 128-wide slots of the packed activation [L, 3*H*128] the attention kernel reads (pad columns
         zeroed once per forward), the attention kernel writes compact heads [L, H*hd];
       * vision gate|up rows concatenated with the MLP width zero-padded to a multiple of 128; down-projection columns padded;
-      * language-model q|k|v rows concatenated (+ biases), gate|up rows concatenated."""
+      * language-model q|k|v rows concatenated (+ biases), gate|up rows concatenated;
+      * with cfg.tie_word_embeddings, `llm.lm_head` is the same device tensor as `llm.embed`."""
     out: Dict[str, torch.Tensor] = {}
 
     def put(name, t):
@@ -1116,7 +1117,15 @@ def convert_qwen_state_dict(sd: Dict[str, torch.Tensor], cfg, device) -> Dict[st
     t = "model.language_model."
     put("llm.embed", sd[t + "embed_tokens.weight"])
     put("llm.norm", sd[t + "norm.weight"])
-    put("llm.lm_head", sd["lm_head.weight"])
+    if getattr(cfg, "tie_word_embeddings", False):
+        # one device tensor for both bindings; a tied checkpoint that also stores lm_head.weight loses it to the embedding, as HF's
+        # tie_weights() does
+        out["llm.lm_head"] = out["llm.embed"]
+    elif "lm_head.weight" in sd:
+        put("llm.lm_head", sd["lm_head.weight"])
+    else:
+        raise KeyError("the checkpoint has no lm_head.weight and its config does not tie the embeddings (tie_word_embeddings false): "
+                       "an untied Qwen2.5-VL checkpoint must carry its lm_head")
     for l in range(cfg.layers):
         p, q = t + f"layers.{l}.", f"llm.{l}."
         put(q + "ln1", sd[p + "input_layernorm.weight"]); put(q + "ln2", sd[p + "post_attention_layernorm.weight"])

@@ -25,7 +25,8 @@ from ...constants import HF_CACHE_DIR
 from .qwen_utils import qwen_image_to_patches, build_prompt_ids, default_question_template, default_answer_template
 from .vqa_model import VQAScoreModel
 
-QWEN2_VL_MODELS: Dict[str, dict] = {name: dict(model=dict(path=spec["weights"]), config=spec["config"]) for name, spec in _TABLE.items()}
+QWEN2_VL_MODELS: Dict[str, dict] = {name: dict(model=dict(path=spec["weights"]), config=spec["config"], listed=spec["listed"])
+                                    for name, spec in _TABLE.items()}
 
 
 # Pixel bounds of the resize the reference applies BEFORE the HF processor: `process_vision_info` (qwen_vl_utils.vision_process.fetch_image)
@@ -99,6 +100,21 @@ def _generation_config_penalty(checkpoint_path: str) -> float:
     return float(generation_config_value(checkpoint_path, "repetition_penalty", 1.0) or 1.0)
 
 
+def _checkpoint_config(checkpoint_path: str, expected: Qwen25VLConfig, model_name: str) -> Qwen25VLConfig:
+    """The architecture of the config.json in a checkpoint directory, which must agree with `expected` (the model table's entry or the
+    caller's `config=`) on every field: a checkpoint of another size, or a fine-tune that changed a dimension, raises here before any
+    weight is converted or bound. Without a config.json (a single weights file, or a directory without one) `expected` stands."""
+    import os
+    f = os.path.join(checkpoint_path, "config.json")
+    if not (os.path.isdir(checkpoint_path) and os.path.isfile(f)):
+        return expected
+    found = Qwen25VLConfig.from_hf_config(f)
+    diff = expected.mismatches(found)
+    if diff:
+        raise ValueError(f"{f} does not describe {model_name}: " + ", ".join(f"{k} = {b!r} (expected {a!r})" for k, (a, b) in diff.items()))
+    return found
+
+
 class Qwen2VLModel(VQAScoreModel):
     video_mode = "direct"
     allows_image = True
@@ -141,6 +157,8 @@ class Qwen2VLModel(VQAScoreModel):
         from ...engine import QwenVLEngine
         spec = QWEN2_VL_MODELS[self.model_name]
         self.cfg: Qwen25VLConfig = self._config_override or spec["config"]()
+        if self._state_dict is None:
+            self.cfg = _checkpoint_config(self._checkpoint or spec["model"]["path"], self.cfg, self.model_name)
         if self._tokenizer_override is not None:
             self.tokenizer = self._tokenizer_override
         else:

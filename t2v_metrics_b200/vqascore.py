@@ -18,4 +18,5 @@ class VQAScore(Score):
         return _registry.get_vqascore_model(model, device=device, cache_dir=cache_dir, **kwargs)
 
     def list_all_models(self) -> List[str]:
-        return _registry.list_all_vqascore_models()
+        """The names this scorer accepts: list_all_vqascore_models() and the sizes accepted by name only (qwen2.5-vl-3b)."""
+        return _registry.accepted_vqascore_models()

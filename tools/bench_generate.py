@@ -1,5 +1,5 @@
-"""Greedy generation on one H100: Qwen2.5-VL-7B width with synthetic weights drawn on the device, 448x448 images and 64 text tokens per
-prompt, B in {1, 8, 32}, 128 new tokens with no EOS ids so every run decodes the same number of steps. One JSON line per batch size:
+"""Greedy generation on one H100: Qwen2.5-VL width (--model, default qwen2.5-vl-7b) with synthetic weights drawn on the device, 448x448
+images and 64 text tokens per prompt, B in {1, 8, 32}, 128 new tokens with no EOS ids so every run decodes the same number of steps. One JSON line per batch size:
 prefill ms, median / spread of the decode step (CUDA events around each graph replay), generated tokens/s, launches per step, algorithmic
 bytes per step (every language-model weight read once + the K/V rows the step attends to) and the whole-step rate they give against the
 3.35 TB/s HBM3 data-sheet figure, per-category device time of one profiled step, and the GPU name and power limit read in the same run.
@@ -9,10 +9,9 @@ time, min_new_tokens = max_new_tokens, on the same GPU and weights (its rate doe
 
 The decode GEMMs split their K range (splitk_slices); run with VQA_GEMM_SPLITK=0 to time the step without the split.
 
-  python tools/bench_generate.py [--batches 1,8,32] [--new 128] [--no-hf] [--out results.jsonl]
+  python tools/bench_generate.py [--model qwen2.5-vl-3b] [--batches 1,8,32] [--new 128] [--no-hf] [--out results.jsonl]
 """
 import argparse
-import dataclasses
 import json
 import os
 import subprocess
@@ -25,6 +24,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch
 
 from oracle import qwen25vl_oracle as qo
+from qwen_bench_model import add_model_arg, engine, hf_model, model_config, synthetic_weights
 
 HBM_PEAK = 3.35e12
 
@@ -54,19 +54,16 @@ def main():
     ap.add_argument("--no-hf", action="store_true")
     ap.add_argument("--hf-samples", type=int, default=2)
     ap.add_argument("--out", default=None)
+    add_model_arg(ap)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_generate.py measures on a CUDA device; there is none")
-    from t2v_metrics_b200.config import Qwen25VLConfig
-    from t2v_metrics_b200.engine import QwenVLEngine
     dev = torch.device("cuda:0")
     gpu, power = gpu_identity()
-    cfg = qo.Qwen25VLConfig.qwen25_vl_7b()
+    cfg, ecfg = model_config(a.model)
     N = a.new
-    sd = qo.make_synthetic_state_dict(cfg, seed=0, gen_device=dev)
-    fields = {f.name for f in dataclasses.fields(Qwen25VLConfig)}
-    eng = QwenVLEngine(Qwen25VLConfig(**{k: v for k, v in dataclasses.asdict(cfg).items() if k in fields}), dev)
-    eng.load_state_dict(sd)
+    sd = synthetic_weights(cfg, ecfg, dev)
+    eng = engine(ecfg, sd, dev)
     W = weight_bytes(cfg)
     lines = []
     for B in [int(x) for x in a.batches.split(",")]:
@@ -105,7 +102,7 @@ def main():
         S_avg = sum(len(p) for p in prompts) / B
         kv = 2.0 * cfg.layers * B * cfg.kv_heads * cfg.head_dim * 2 * (S_avg + N / 2)      # K and V rows a step attends to, mean over the steps
         med = float(steps.median())
-        line = dict(workload="qwen2.5-vl-7b greedy generate", gpu=gpu, power_limit=power, batch=B, image=a.image, text_tokens=a.text,
+        line = dict(workload=f"{a.model} greedy generate", gpu=gpu, power_limit=power, batch=B, image=a.image, text_tokens=a.text,
                     prompt_tokens=S_avg, new_tokens=N, splitk=os.environ.get("VQA_GEMM_SPLITK", "1") != "0",
                     prefill_ms=round(min(pre), 3), step_ms_median=round(med, 4), step_ms_p10=round(float(steps.quantile(0.1)), 4),
                     step_ms_p90=round(float(steps.quantile(0.9)), 4), decode_tokens_per_s=round(B * (N - 1) / wall, 1),
@@ -119,8 +116,7 @@ def main():
     del eng
     torch.cuda.empty_cache()
     if not a.no_hf:
-        import hf_reference as hf
-        model = hf.build_hf_qwen(cfg, sd, dtype=torch.bfloat16, device=dev, attn="sdpa", assign=True)
+        model = hf_model(cfg, ecfg, sd, dev)
         inp = qo.make_synthetic_inputs(cfg, a.hf_samples, (a.image, a.image), a.text, seed=1)
         P = inp["grid_thw"][0][1] * inp["grid_thw"][0][2]
 

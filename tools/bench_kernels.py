@@ -7,6 +7,8 @@
                                                 # CUDA-event timing; --dump writes each shape's output (raw bytes) to DIR
   python tools/bench_kernels.py gemm-ncu        # same launches once each, in a fixed order, for `ncu --metrics dram__bytes_*`
   python tools/bench_kernels.py gemm-list       # prints that order (shape, group_rows, chunk_rows) as JSON
+  python tools/bench_kernels.py attn128 [--model qwen2.5-vl-3b]   # head_dim-128 attention at that model's heads (default the 7B)
+  SHAPES=qwen3b_qkv,qwen3b_o,qwen3b_gate_up,qwen3b_down python tools/bench_kernels.py gemm-time   # the 3B's prefill GEMMs
 """
 import json
 import os
@@ -81,8 +83,9 @@ def attn_one():
     torch.cuda.synchronize()
 
 
-def attn128():
-    """head_dim-128 attention at the Qwen2.5-VL-7B shapes: causal GQA prefill (B=32, S=320, 28/4 heads), vision windows (64 tokens) and whole frames."""
+def attn128(model="qwen2.5-vl-7b"):
+    """head_dim-128 attention at a Qwen2.5-VL size's shapes: causal GQA prefill (B=32, S=320; 7B 28/4 heads, 3B 16/2), vision windows (64
+    tokens) and whole frames."""
     import ctypes as C
     from t2v_metrics_b200 import _lib
     from t2v_metrics_b200.engine import _ptr, _stream_ptr, _check
@@ -95,7 +98,9 @@ def attn128():
         fn = lambda: _check(lib.vqa_op_attention_d128(_ptr(qkv), qkv.shape[1], qkv.shape[0], q0, k0, v0, _ptr(out), out_cols, n_seq, max_len, S, Hq,
                                                        group, _ptr(cu), None, float(scale), 1 if causal else 0, _stream_ptr(qkv.device)), None, "d128")
         return time_ms(fn), float(out.float().abs().sum())
-    B, S, Hq, Hkv = 32, 320, 28, 4
+    from t2v_metrics_b200.config import QWEN25VL_MODELS
+    cfg = QWEN25VL_MODELS[model]["config"]()
+    B, S, Hq, Hkv = 32, 320, cfg.heads, cfg.kv_heads
     qkv = (torch.randn(B * S, (Hq + 2 * Hkv) * 128, device="cuda") * 0.5).bfloat16()
     ms, cs = run(qkv, Hq * 128, B, S, S, Hq, Hq // Hkv, None, 128 ** -0.5, True, 0, Hq * 128, (Hq + Hkv) * 128)
     res["llm_causal"] = dict(ms=round(ms, 4), tflops=round(2.0 * B * Hq * S * S * 128 / ms / 1e9, 1), checksum=cs)
@@ -107,7 +112,7 @@ def attn128():
         cu = torch.arange(0, L + 1, wlen, dtype=torch.int32, device="cuda")
         ms, cs = run(vq, Hv * 128, L // wlen, wlen, 0, Hv, 1, cu, 80 ** -0.5, False, 0, Hv * 128, 2 * Hv * 128)
         res[name] = dict(ms=round(ms, 4), tflops_padded=round(4.0 * L * wlen * Hv * 128 / ms / 1e9, 1), checksum=cs)
-    print(json.dumps(dict(kernel="attn_wgmma_kernel d128", **res)))
+    print(json.dumps(dict(kernel="attn_wgmma_kernel d128", model=model, q_heads=Hq, kv_heads=Hkv, **res)))
 
 
 SHAPES = dict(   # name: (M, N, K, epilogue, residual, bias)   residual: None, "bf16" (in the output's place) or "f32" (fp32 stream, in place)
@@ -123,6 +128,11 @@ SHAPES = dict(   # name: (M, N, K, epilogue, residual, bias)   residual: None, "
     clip_out=(36928, 1024, 1024, "store", "f32", True),
     clip_fc1=(36928, 4096, 1024, "quick_gelu", None, True),
     clip_fc2=(36928, 1024, 4096, "store", "f32", True),
+    # Qwen2.5-VL-3B decoder layer at B=32 prompts of 320 tokens (448x448 image + 64 text ids)
+    qwen3b_qkv=(10240, 2560, 2048, "store", None, True),
+    qwen3b_o=(10240, 2048, 2048, "store", "bf16", False),
+    qwen3b_gate_up=(10240, 22016, 2048, "gated_silu", None, False),
+    qwen3b_down=(10240, 2048, 11008, "store", "bf16", False),
 )
 SCHEDULES = [(0, 0), (4096, -1), (1024, -1), (512, 2048), (512, 4096), (1024, 3072), (1024, 4096), (1024, 6144), (2048, 4096), (1024, 8192),
              (2048, 2048), (512, 6144)]
@@ -149,14 +159,14 @@ def gemm(mode, dump_dir=None):
         if os.environ.get("ZERO_OPERANDS"):
             a.zero_(); w.zero_()
         bias = (torch.randn(N, device="cuda") * 0.1).bfloat16() if has_bias else None
-        n_out = N // 2 if epi == "gated_gelu" else N
+        n_out = N // 2 if epi.startswith("gated") else N
         if res == "f32":
             c = torch.randn(M, n_out, device="cuda")
             fn = lambda: ops.gemm_f32acc(a, w, c, bias=bias)
         else:
             c = torch.empty(M, n_out, dtype=torch.bfloat16, device="cuda")
             r = torch.randn(M, n_out, device="cuda").bfloat16() if res == "bf16" else None
-            fn = lambda: ops.gemm(a, w, bias=bias, residual=r, epilogue=epi, out=c, gate_up_offset=N // 2 if epi == "gated_gelu" else 0)
+            fn = lambda: ops.gemm(a, w, bias=bias, residual=r, epilogue=epi, out=c, gate_up_offset=N // 2 if epi.startswith("gated") else 0)
         flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
         for (g, ch) in scheds:
             lib.vqa_set_gemm_schedule(g, ch)
@@ -188,7 +198,7 @@ if __name__ == "__main__":
     elif cmd == "attn-one":
         attn_one()
     elif cmd == "attn128":
-        attn128()
+        attn128(sys.argv[sys.argv.index("--model") + 1] if "--model" in sys.argv else "qwen2.5-vl-7b")
     elif cmd == "gemm-time":
         gemm("time", sys.argv[sys.argv.index("--dump") + 1] if "--dump" in sys.argv else None)
     elif cmd == "gemm-ncu":

@@ -1,4 +1,4 @@
-"""Scoring over a greedy rollout on one H100: Qwen2.5-VL-7B width with synthetic weights drawn on the device, 448x448 images and 64 text
+"""Scoring over a greedy rollout on one H100: Qwen2.5-VL width (--model, default qwen2.5-vl-7b) with synthetic weights drawn on the device, 448x448 images and 64 text
 tokens per prompt, B in {1, 8, 32}, k in {8, 64} new tokens with no EOS ids so every run decodes k steps. One JSON line per (B, k):
 the scored prefill, the median / p10 / p90 of the scored decode step (CUDA events around each graph replay), the plain generate step of
 the same shape measured the same way (the cost of the answer log-probability kernel is the difference), launches per step of both, and
@@ -9,10 +9,9 @@ and power limit read in the same run.
 The baseline is the reference's loop: HF Qwen2_5_VLForConditionalGeneration.generate(do_sample=False, output_scores=True) in bf16 with
 sdpa, one sample at a time, min_new_tokens = max_new_tokens, on the same GPU and weights (measured on --hf-samples samples per k).
 
-  python tools/bench_rollout_score.py [--batches 1,8,32] [--new 8,64] [--no-hf] [--out results.jsonl]
+  python tools/bench_rollout_score.py [--model qwen2.5-vl-3b] [--batches 1,8,32] [--new 8,64] [--no-hf] [--out results.jsonl]
 """
 import argparse
-import dataclasses
 import json
 import os
 import sys
@@ -25,6 +24,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import torch
 
 from oracle import qwen25vl_oracle as qo
+from qwen_bench_model import add_model_arg, engine, hf_model, model_config, synthetic_weights
 from bench_generate import gpu_identity
 
 ANSWER = [9454, 11, 432, 1558]          # a four-token answer
@@ -58,19 +58,16 @@ def main():
     ap.add_argument("--no-hf", action="store_true")
     ap.add_argument("--hf-samples", type=int, default=2)
     ap.add_argument("--out", default=None)
+    add_model_arg(ap)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_rollout_score.py measures on a CUDA device; there is none")
     from t2v_metrics_b200 import qwen_host
-    from t2v_metrics_b200.config import Qwen25VLConfig
-    from t2v_metrics_b200.engine import QwenVLEngine
     dev = torch.device("cuda:0")
     gpu, power = gpu_identity()
-    cfg = qo.Qwen25VLConfig.qwen25_vl_7b()
-    sd = qo.make_synthetic_state_dict(cfg, seed=0, gen_device=dev)
-    fields = {f.name for f in dataclasses.fields(Qwen25VLConfig)}
-    eng = QwenVLEngine(Qwen25VLConfig(**{k: v for k, v in dataclasses.asdict(cfg).items() if k in fields}), dev)
-    eng.load_state_dict(sd)
+    cfg, ecfg = model_config(a.model)
+    sd = synthetic_weights(cfg, ecfg, dev)
+    eng = engine(ecfg, sd, dev)
     news = [int(x) for x in a.new.split(",")]
     lines = []
     for B in [int(x) for x in a.batches.split(",")]:
@@ -114,7 +111,7 @@ def main():
             wall = (time.perf_counter() - t0) / runs
             assert all(len(t) == N for t in r["tokens"]) and len(scores) == B
             med, pmed = float(scored.median()), float(base.median())
-            line = dict(workload="qwen2.5-vl-7b scored greedy rollout", gpu=gpu, power_limit=power, batch=B, image=a.image, text_tokens=a.text,
+            line = dict(workload=f"{a.model} scored greedy rollout", gpu=gpu, power_limit=power, batch=B, image=a.image, text_tokens=a.text,
                         prompt_tokens=sum(len(p) for p in prompts) / B, new_tokens=N, answer_tokens=len(ANSWER), timed_steps=int(scored.numel()),
                         prefill_ms=round(min(pre), 3), step_ms_median=round(med, 4), step_ms_p10=round(float(scored.quantile(0.1)), 4),
                         step_ms_p90=round(float(scored.quantile(0.9)), 4), generate_step_ms_median=round(pmed, 4),
@@ -127,8 +124,7 @@ def main():
     del eng
     torch.cuda.empty_cache()
     if not a.no_hf:
-        import hf_reference as hf
-        model = hf.build_hf_qwen(cfg, sd, dtype=torch.bfloat16, device=dev, attn="sdpa", assign=True)
+        model = hf_model(cfg, ecfg, sd, dev)
         inp = qo.make_synthetic_inputs(cfg, a.hf_samples, (a.image, a.image), a.text, seed=1)
         P = inp["grid_thw"][0][1] * inp["grid_thw"][0][2]
 

@@ -1,15 +1,14 @@
 """Video-file scoring on one H100: a synthesized 640x360, 24 fps, 21 s clip (504 frames, the shape of the reference README's baby.mp4,
-MJPG in .avi, written to a temporary directory), Qwen2.5-VL-7B width with synthetic weights drawn on the device. For fps 8.0 (168 frames)
-and "dynamic" (qwen_vl_utils' 2.0: 42 frames), each resized to 280x504 under the 360*420 pixel budget, one JSON line per (fps, B):
+MJPG in .avi, written to a temporary directory), Qwen2.5-VL width (--model, default qwen2.5-vl-7b) with synthetic weights drawn on the
+device. For fps 8.0 (168 frames) and "dynamic" (qwen_vl_utils' 2.0: 42 frames), each resized to 280x504 under the 360*420 pixel budget, one JSON line per (fps, B):
   decode_ms      OpenCV decoding of the sampled frames (qwen_utils.OpenCVVideoReader: counting by decoding, then the frames), host clock
   preprocess_ms  engine.qwen_preprocess_video_file_u8 on the decoded frames (pinned staging, H2D, one kernel per slice), CUDA events
   score_ms       QwenVLEngine.score_prompts for B texts on the clip (one prefill of B prompts of the video tokens + 24 text ids)
 each the best of a few runs; the GPU name and power limit are read in the same run.
 
-  python tools/bench_video_file_score.py [--out results.jsonl]
+  python tools/bench_video_file_score.py [--model qwen2.5-vl-3b] [--out results.jsonl]
 """
 import argparse
-import dataclasses
 import json
 import os
 import sys
@@ -23,9 +22,9 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import numpy as np
 import torch
 
-from oracle import qwen25vl_oracle as qo
 from bench_generate import gpu_identity
 from bench_video_score import best_ms, prompts_for
+from qwen_bench_model import add_model_arg, engine, model_config, synthetic_weights
 
 
 def write_clip(path, frames=504, h=360, w=640, fps=24.0):
@@ -43,20 +42,18 @@ def write_clip(path, frames=504, h=360, w=640, fps=24.0):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
+    add_model_arg(ap)
     args = ap.parse_args()
-    from t2v_metrics_b200.config import Qwen25VLConfig
-    from t2v_metrics_b200.engine import QwenVLEngine, qwen_preprocess_video_file_u8
+    from t2v_metrics_b200.engine import qwen_preprocess_video_file_u8
     from t2v_metrics_b200.models.vqascore_models.qwen2vl_model import VIDEO_FILE_MAX_PIXELS
     from t2v_metrics_b200.models.vqascore_models.qwen_utils import OpenCVVideoReader, qwen_video_file_plan
     dev = torch.device("cuda:0")
-    cfg = qo.Qwen25VLConfig.qwen25_vl_7b()
-    sd = qo.make_synthetic_state_dict(cfg, seed=0, gen_device=dev)
-    fields = {f.name for f in dataclasses.fields(Qwen25VLConfig)}
-    eng = QwenVLEngine(Qwen25VLConfig(**{k: v for k, v in dataclasses.asdict(cfg).items() if k in fields}), dev)
-    eng.load_state_dict(sd)
+    cfg, ecfg = model_config(args.model)
+    sd = synthetic_weights(cfg, ecfg, dev)
+    eng = engine(ecfg, sd, dev)
     del sd
     name, power = gpu_identity()
-    ident = dict(gpu=name, power_limit=power)
+    ident = dict(model=args.model, gpu=name, power_limit=power)
     lines = []
     with tempfile.TemporaryDirectory() as d:
         path = os.path.join(d, "clip.avi")

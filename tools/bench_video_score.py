@@ -1,4 +1,4 @@
-"""Video scoring on one H100: Qwen2.5-VL-7B width with synthetic weights drawn on the device, decoded uint8 frame stacks on the host
+"""Video scoring on one H100: Qwen2.5-VL width (--model, default qwen2.5-vl-7b) with synthetic weights drawn on the device, decoded uint8 frame stacks on the host
 (8 frames of 448x448 = 1024 video tokens, 32 frames of 336x336 = 2304 video tokens), two videos per call with 1 or 8 texts each, scored
 with k = 1 (one prefill, QwenVLEngine.score_prompts) and k = 4 (a scored greedy rollout, QwenVLEngine.rollout_scores). One JSON line per
 (shape, texts, k): the device pre-processing of the call's stacks (qwen_preprocess_video_u8: pinned staging, H2D, one kernel), the
@@ -9,10 +9,9 @@ The baseline is the reference's loop on the same GPU and weights: per pair, the 
 (qwen_utils.qwen_video_to_patches, the restated qwen_vl_utils + processor path) and HF Qwen2_5_VLForConditionalGeneration in bf16 with
 sdpa: one forward for k = 1, generate(do_sample=False, output_scores=True, max_new_tokens=4) for k = 4.
 
-  python tools/bench_video_score.py [--no-hf] [--hf-samples 2] [--out results.jsonl]
+  python tools/bench_video_score.py [--model qwen2.5-vl-3b] [--no-hf] [--hf-samples 2] [--out results.jsonl]
 """
 import argparse
-import dataclasses
 import json
 import os
 import sys
@@ -26,6 +25,7 @@ import numpy as np
 import torch
 
 from oracle import qwen25vl_oracle as qo
+from qwen_bench_model import add_model_arg, engine, hf_model, model_config, synthetic_weights
 from bench_generate import gpu_identity
 
 SHAPES = [(8, 448), (32, 336)]          # (frames, side)
@@ -76,18 +76,16 @@ def main():
     ap.add_argument("--no-hf", action="store_true")
     ap.add_argument("--hf-samples", type=int, default=2)
     ap.add_argument("--out", default=None)
+    add_model_arg(ap)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_video_score.py measures on a CUDA device; there is none")
-    from t2v_metrics_b200.config import Qwen25VLConfig
-    from t2v_metrics_b200.engine import QwenVLEngine, qwen_preprocess_video_u8
+    from t2v_metrics_b200.engine import qwen_preprocess_video_u8
     dev = torch.device("cuda:0")
     gpu, power = gpu_identity()
-    cfg = qo.Qwen25VLConfig.qwen25_vl_7b()
-    sd = qo.make_synthetic_state_dict(cfg, seed=0, gen_device=dev)
-    fields = {f.name for f in dataclasses.fields(Qwen25VLConfig)}
-    eng = QwenVLEngine(Qwen25VLConfig(**{k: v for k, v in dataclasses.asdict(cfg).items() if k in fields}), dev)
-    eng.load_state_dict(sd)
+    cfg, ecfg = model_config(a.model)
+    sd = synthetic_weights(cfg, ecfg, dev)
+    eng = engine(ecfg, sd, dev)
     spg_of = lambda n: [cfg.temporal_patch_size / 24] * n
     lines = []
     for frames, side in SHAPES:
@@ -106,7 +104,7 @@ def main():
                                                       second_per_grid_ts=spg_of(VIDEOS))
                 call()
                 score_ms, _ = best_ms(call)
-                line = dict(workload="qwen2.5-vl-7b video scoring from host uint8 frame stacks", gpu=gpu, power_limit=power, frames=frames,
+                line = dict(workload=f"{a.model} video scoring from host uint8 frame stacks", gpu=gpu, power_limit=power, frames=frames,
                             side=side, videos=VIDEOS, texts_per_video=texts, pairs=len(prompts), video_tokens=grids[0][0] * grids[0][1] * grids[0][2] // 4,
                             prompt_tokens=len(prompts[0]), k=k, preprocess_ms=round(pre_ms, 3),
                             **{"prefill_ms" if k == 1 else "rollout_ms": round(score_ms, 3)},
@@ -116,9 +114,8 @@ def main():
     del eng
     torch.cuda.empty_cache()
     if not a.no_hf:
-        import hf_reference as hf
         from t2v_metrics_b200.models.vqascore_models.qwen_utils import qwen_video_to_patches
-        model = hf.build_hf_qwen(cfg, sd, dtype=torch.bfloat16, device=dev, attn="sdpa", assign=True)
+        model = hf_model(cfg, ecfg, sd, dev)
         for frames, side in SHAPES:
             vids = stacks(frames, side, a.hf_samples)
             for k in (1, 4):
