@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define VQA_B200_ABI_VERSION 1
+#define VQA_B200_ABI_VERSION 2
 
 typedef enum {
     VQA_OK = 0,
@@ -107,7 +107,7 @@ typedef struct {
 
 typedef struct vqa_handle vqa_handle;
 
-/* ABI / build info ("vqa_b200 abi=1 arch=sm_90a ..."). Never fails. */
+/* ABI / build info ("vqa_b200 abi=2 arch=sm_90a ..."). Never fails. */
 const char* vqa_version(void);
 
 /* Create an engine for a CLIP-FlanT5 model on CUDA device `device`. */
@@ -175,58 +175,73 @@ int vqa_create_qwen25vl(const vqa_qwen25vl_config* cfg, int device, vqa_handle**
 int vqa_qwen25vl_set_rope(vqa_handle* h, const float* text_inv_freq, const int32_t* text_axis, int32_t text_half,
                           const float* vis_inv_freq, const int32_t* vis_axis, int32_t vis_half);
 
-size_t vqa_qwen25vl_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches);
+/* The inputs of one prefill: `batch` prompts and the images / videos they show. All index arrays are DEVICE int32 and are produced by
+ * the host's mirror of the reference's index logic (rot_pos_emb :382-409, get_window_index :411-451, get_rope_index :1024-1133).
+ * Packed rows (a vqa_qwen25vl_packed is given) ignore seq_lens and seq_len: input_ids / feat_index [total_rows] and position_ids
+ * [3, total_rows] are then in packed row order.
+ * The library reads this struct, and every struct below, only during the call it is passed to and keeps no pointer to it; a CUDA graph
+ * captured from a call keeps the values the struct held at capture. */
+typedef struct {
+    const void* pixel_patches;     /* [n_patches, patch_dim], all images concatenated, processor (merge-block) order */
+    int32_t pixel_dtype;           /* F32 or BF16 */
+    int32_t n_patches;
+    const int32_t* vis_pos_hw;     /* [2, n_patches]  (h, w) index of every patch, already in WINDOW order */
+    const int32_t* window_index;   /* [n_patches / merge^2]  window order of the 2x2 patch groups */
+    const int32_t* reverse_index;  /* argsort(window_index) */
+    const int32_t* cu_window;      /* [n_windows + 1]  cumulative patch counts (window order) */
+    int32_t n_windows;
+    int32_t max_window_len;
+    const int32_t* cu_frames;      /* [n_frames + 1]  cumulative patch counts (window order) */
+    int32_t n_frames;
+    int32_t max_frame_len;
+    const int32_t* input_ids;      /* [batch, seq_len] right-padded */
+    const int32_t* seq_lens;       /* [batch] */
+    const int32_t* feat_index;     /* [batch, seq_len] row of the merged vision features for image-token positions, -1 elsewhere */
+    const int32_t* position_ids;   /* [3, batch*seq_len] (t, h, w) mRoPE positions */
+    int32_t batch;
+    int32_t seq_len;
+} vqa_qwen25vl_prompts;
 
-/* Score `batch` prompts in one prefill. All index arrays are DEVICE int32 and are produced by the host's mirror of the
- * reference's index logic (rot_pos_emb :382-409, get_window_index :411-451, get_rope_index :1024-1133):
- *   pixel_patches  [n_patches, patch_dim] (F32 or BF16), all images concatenated, processor (merge-block) order
- *   vis_pos_hw     [2, n_patches]  (h, w) index of every patch, already in WINDOW order
- *   window_index   [n_patches / merge^2]  window order of the 2x2 patch groups;  reverse_index = argsort(window_index)
- *   cu_window      [n_windows + 1], cu_frames [n_frames + 1]  cumulative patch counts (window order)
- *   input_ids      [batch, seq_len] right-padded; seq_lens [batch]
- *   feat_index     [batch, seq_len] row of the merged vision features for image-token positions, -1 elsewhere
- *   position_ids   [3, batch*seq_len] (t, h, w) mRoPE positions
- *   answer_ids     [batch] the answer's first token id
+/* KV-prefix sharing (SURVEY 8(f)1; reference score.py:104-106 repeats one image across N texts and qwen2vl_model.py:190 re-runs the whole
+ * prompt per text). The language-model tokens are given as PACKED rows: sequences stored back to back (cu_seqlens [n_seq + 1]); the
+ * [chat prefix + vision tokens] of an image is ONE sequence (kv_prefix = -1), each prompt's remaining tokens are a sequence of their own whose
+ * kv_prefix names the shared one: its rows attend to all prefix rows, then causally to themselves. Causality makes this exact (a prefix
+ * row never sees a suffix), and the prefix rows go through every layer once per image instead of once per prompt. */
+typedef struct {
+    int32_t total_rows;
+    const int32_t* cu_seqlens;     /* [n_seq + 1] */
+    const int32_t* kv_prefix;      /* [n_seq], -1 = none */
+    int32_t n_seq;
+    int32_t max_seq_len;           /* longest sequence */
+    const int32_t* pair_row;       /* [batch] packed row of each prompt's last token */
+    const int32_t* pair_seq;       /* [batch] the sequence holding it */
+    int32_t max_prompt_len;        /* longest prefix + suffix (repetition-penalty bitmap) */
+} vqa_qwen25vl_packed;
+
+/* Bytes of device workspace of one scoring call: n_prompts prompts in `rows` language-model rows (padded rows: batch * seq_len; packed
+ * rows: total_rows). */
+size_t vqa_qwen25vl_workspace_bytes(vqa_handle* h, int32_t n_prompts, int64_t rows, int32_t n_patches);
+
+/* Score prompts->batch prompts in one prefill, over padded rows (packed == NULL) or packed rows.
+ *   answer_ids     DEVICE [batch] the answer's first token id
  *   repetition_penalty  1.0 = off; otherwise HF's RepetitionPenaltyLogitsProcessor over each sample's prompt ids is applied to the
  *                  fp32 logits before the temperature (generation/utils.py:2762-2770; the checkpoint's generation_config.json
  *                  decides it in the reference, SURVEY F8)
- *   out_probs      [batch] softmax(processed last-position logits / temperature)[answer_id]; out_logprobs optional
+ *   out_probs      DEVICE [batch] softmax(processed last-position logits / temperature)[answer_id]; out_logprobs optional
  */
-int vqa_qwen25vl_score(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
-                       const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
-                       const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
-                       int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
-                       const int32_t* feat_index, const int32_t* position_ids, const int32_t* answer_ids, int32_t batch,
-                       int32_t seq_len, float temperature, float repetition_penalty, float* out_probs, float* out_logprobs,
-                       void* workspace, size_t workspace_bytes, void* stream);
+int vqa_qwen25vl_score(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_packed* packed, const int32_t* answer_ids,
+                       float temperature, float repetition_penalty, float* out_probs, float* out_logprobs, void* workspace,
+                       size_t workspace_bytes, void* stream);
 
 /* Trace output (reference forward_with_trace, qwen2vl_model.py:303-493, top-5 at :439-447): the k <= 8 most probable next tokens of every
- * prompt of the LAST scoring call on this handle (vqa_qwen25vl_score: total_rows = batch * seq_len; vqa_qwen25vl_score_packed: its
- * total_rows) with the same n_patches and the same workspace -- its final hidden states and, when repetition_penalty != 1, its prompt-token
+ * prompt of the LAST scoring call on this handle (vqa_qwen25vl_score: total_rows = batch * seq_len over padded rows, packed->total_rows
+ * over packed rows) with the same n_patches and the same workspace -- its final hidden states and, when repetition_penalty != 1, its prompt-token
  * bitmap are still there -- under the same processing as the score: bf16 logits -> fp32 -> repetition penalty -> 1/T -> softmax over the
  * whole vocabulary. out_ids / out_probs: DEVICE [batch, k], most probable first; out_ids[b][0] is the token generate(max_new_tokens=1,
  * do_sample=False) would emit. This call materialises [batch, vocab] bf16 logits of that one position in the workspace -- a debugging
  * aid; the scoring path never stores logits. */
 int vqa_qwen25vl_topk(vqa_handle* h, int32_t batch, int64_t total_rows, int32_t n_patches, int32_t k, float temperature,
                       float repetition_penalty, int32_t* out_ids, float* out_probs, void* workspace, size_t workspace_bytes, void* stream);
-
-/* KV-prefix sharing (SURVEY 8(f)1; reference score.py:104-106 repeats one image across N texts and qwen2vl_model.py:190 re-runs the whole
- * prompt per text). The language-model tokens are given as PACKED rows: sequences stored back to back (cu_seqlens [n_seq + 1]); the
- * [chat prefix + vision tokens] of an image is ONE sequence (kv_prefix = -1), each prompt's remaining tokens are a sequence of their own whose
- * kv_prefix names the shared one: its rows attend to all prefix rows, then causally to themselves. Causality makes this exact (a prefix
- * row never sees a suffix), and the prefix rows go through every layer once per image instead of once per prompt.
- *   input_ids / feat_index [total_rows], position_ids [3, total_rows]: as in vqa_qwen25vl_score, in packed row order
- *   pair_row [n_prompts]: packed row of each prompt's last token; pair_seq [n_prompts]: the sequence holding it
- *   max_seq_len: longest sequence; max_prompt_len: longest prefix + suffix (repetition-penalty bitmap) */
-size_t vqa_qwen25vl_packed_workspace_bytes(vqa_handle* h, int32_t n_prompts, int64_t total_rows, int32_t n_patches);
-int vqa_qwen25vl_score_packed(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches, const int32_t* vis_pos_hw,
-                              const int32_t* window_index, const int32_t* reverse_index, const int32_t* cu_window, int32_t n_windows,
-                              int32_t max_window_len, const int32_t* cu_frames, int32_t n_frames, int32_t max_frame_len,
-                              const int32_t* input_ids, const int32_t* feat_index, const int32_t* position_ids, int32_t total_rows,
-                              const int32_t* cu_seqlens, const int32_t* kv_prefix, int32_t n_seq, int32_t max_seq_len, const int32_t* pair_row,
-                              const int32_t* pair_seq, const int32_t* answer_ids, int32_t n_prompts, int32_t max_prompt_len, float temperature,
-                              float repetition_penalty, float* out_probs, float* out_logprobs, void* workspace, size_t workspace_bytes,
-                              void* stream);
 
 /* ---- Qwen2.5-VL greedy generation (reference Qwen2VLModel.generate, qwen2vl_model.py:495-563: generate(do_sample=False)) ----
  * One prefill, then one decode step per further token, all on the caller's stream. The prefill runs the vision tower and the padded-row
@@ -235,53 +250,48 @@ int vqa_qwen25vl_score_packed(vqa_handle* h, const void* pixel_patches, int32_t 
  * language model and selects the next one. Selection: bf16 lm_head logits -> fp32 -> HF's RepetitionPenaltyLogitsProcessor over the
  * prompt ids and the tokens generated so far (repetition_penalty 1.0 = off) -> arg-max, ties to the lowest id. A prompt finishes after
  * emitting one of eos_ids (which is kept in its output) or max_new_tokens tokens; later steps leave it unchanged.
- *   first_position [batch]  mRoPE position of the first generated token: the last prompt token's position + 1; token t sits at that + t
- *                           on all three axes (what transformers' generate() feeds)
- *   eos_ids [n_eos]         DEVICE; n_eos may be 0
- *   out_tokens [batch, max_new_tokens]  generated ids, -1 after a prompt's last one; out_lengths [batch] tokens generated so far;
- *   all_done [1]            1 once every prompt has finished
  * Every step-dependent value lives in device memory: the step takes the same arguments every time, so one CUDA graph of it can be
  * replayed for every token. The prefill and the steps must use the same workspace, sizes and pointers. batch <= 128. */
-size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, int32_t max_new_tokens);
-int vqa_qwen25vl_generate_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches, const int32_t* vis_pos_hw,
-                                  const int32_t* window_index, const int32_t* reverse_index, const int32_t* cu_window, int32_t n_windows,
-                                  int32_t max_window_len, const int32_t* cu_frames, int32_t n_frames, int32_t max_frame_len,
-                                  const int32_t* input_ids, const int32_t* seq_lens, const int32_t* feat_index, const int32_t* position_ids,
-                                  const int32_t* first_position, int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos,
-                                  int32_t max_new_tokens, float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
-                                  void* workspace, size_t workspace_bytes, void* stream);
-int vqa_qwen25vl_generate_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
-                               int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
-                               int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- Qwen2.5-VL scoring over a greedy rollout (reference Qwen2VLModel.forward / forward_with_trace with max_new_tokens > 1,
  * qwen2vl_model.py:169-493: generate(do_sample=False, output_scores=True), then softmax(scores[s] / T)[answer id] at chosen steps) ----
- * vqa_qwen25vl_generate_prefill / _step with one more kernel per token, between the lm_head and the selection: for every step s of every
+ * A generation with an answer score launches one more kernel per token, between the lm_head and the selection: for every step s of every
  * unfinished prompt b, the log-softmax of the step's processed scores (bf16 logits -> fp32 -> repetition penalty over the prompt and the
  * tokens generated before s -> / temperature), over the whole vocabulary, at each of the prompt's answer ids. The temperature only
- * affects these probabilities; the tokens are those of vqa_qwen25vl_generate_*, bit for bit. Same workspace
- * (vqa_qwen25vl_generate_workspace_bytes) and the same rules for it.
- *   answer_ids [batch, n_max]   DEVICE, prompt b's ids in its first answer_counts[b] entries (no cap on n_max)
- *   answer_counts [batch]       DEVICE
- *   out_logp [batch, max_new_tokens, n_max]          fp32, [b, s, j] = log p(s, answer_ids[b, j]); entries of steps a prompt did not
- *                                                    generate and of j >= answer_counts[b] are not written
- *   out_topk_ids / out_topk_probs [batch, max_new_tokens, top_k]  with 0 < top_k <= 8: the step's top_k ids (ties to the lower id) and
- *                                                    probabilities; may be NULL when top_k == 0
- * The outputs are caller-owned; a step takes the same arguments every time (one CUDA graph replays every token). */
-int vqa_qwen25vl_rollout_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches, const int32_t* vis_pos_hw,
-                                 const int32_t* window_index, const int32_t* reverse_index, const int32_t* cu_window, int32_t n_windows,
-                                 int32_t max_window_len, const int32_t* cu_frames, int32_t n_frames, int32_t max_frame_len,
-                                 const int32_t* input_ids, const int32_t* seq_lens, const int32_t* feat_index, const int32_t* position_ids,
-                                 const int32_t* first_position, int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos,
-                                 int32_t max_new_tokens, float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
-                                 const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, float temperature, int32_t top_k,
-                                 float* out_logp, int32_t* out_topk_ids, float* out_topk_probs, void* workspace, size_t workspace_bytes,
-                                 void* stream);
-int vqa_qwen25vl_rollout_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
-                              int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
-                              int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, const int32_t* answer_ids,
-                              const int32_t* answer_counts, int32_t n_max, float temperature, int32_t top_k, float* out_logp,
-                              int32_t* out_topk_ids, float* out_topk_probs, void* workspace, size_t workspace_bytes, void* stream);
+ * affects these probabilities; the tokens are those of the plain generation, bit for bit. Same workspace
+ * (vqa_qwen25vl_generate_workspace_bytes) and the same rules for it. The outputs are caller-owned. */
+typedef struct {
+    const int32_t* answer_ids;     /* DEVICE [batch, n_max], prompt b's ids in its first answer_counts[b] entries (no cap on n_max) */
+    const int32_t* answer_counts;  /* DEVICE [batch] */
+    int32_t n_max;
+    float temperature;
+    int32_t top_k;                 /* 0 <= top_k <= 8 */
+    float* out_logp;               /* [batch, max_new_tokens, n_max] fp32, [b, s, j] = log p(s, answer_ids[b, j]); entries of steps a
+                                      prompt did not generate and of j >= answer_counts[b] are not written */
+    int32_t* out_topk_ids;         /* [batch, max_new_tokens, top_k]: the step's top_k ids (ties to the lower id) and probabilities; */
+    float* out_topk_probs;         /* may be NULL when top_k == 0 */
+} vqa_qwen25vl_answer_score;
+
+/* The outputs and constants of a generation, the same for the prefill and every step. All pointers DEVICE. */
+typedef struct {
+    const int32_t* seq_lens;       /* [batch] prompt lengths: the prefill's prompts->seq_lens, the same pointer */
+    const int32_t* first_position; /* [batch] mRoPE position of the first generated token: the last prompt token's position + 1; token t
+                                      sits at that + t on all three axes (what transformers' generate() feeds) */
+    const int32_t* eos_ids;        /* [n_eos]; n_eos may be 0 */
+    int32_t n_eos;
+    int32_t max_new_tokens;
+    float repetition_penalty;
+    int32_t* out_tokens;           /* [batch, max_new_tokens] generated ids, -1 after a prompt's last one */
+    int32_t* out_lengths;          /* [batch] tokens generated so far */
+    int32_t* all_done;             /* [1] 1 once every prompt has finished */
+    const vqa_qwen25vl_answer_score* score;   /* HOST; NULL = plain greedy generation, else a scored rollout */
+} vqa_qwen25vl_generation;
+
+size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, int32_t max_new_tokens);
+int vqa_qwen25vl_generate_prefill(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+int vqa_qwen25vl_generate_step(vqa_handle* h, const vqa_qwen25vl_generation* gen, int32_t batch, int32_t seq_len, int32_t n_patches,
+                               void* workspace, size_t workspace_bytes, void* stream);
 
 /* Number of kernels the last vqa_clipt5_score call launched (for bench.py's gpu_launches). */
 int64_t vqa_last_launch_count(vqa_handle* h);
@@ -298,10 +308,10 @@ int vqa_profile_read(vqa_handle* h, float* ms, double* flops, double* bytes, int
  * that the reference exposes too (encoder_last_hidden_state, decoder_hidden_states[-1], ...). Valid after the stream has passed
  * the scoring call. CLIP-FlanT5 (n >= 6): {encoder output, decoder output (both after the final T5LayerNorm), projector output,
  * encoder / decoder residual streams, last vision-tower hidden state (fp32)}. Qwen2.5-VL (n >= 4): {last-position hidden state after the
- * final norm, merged vision features, residual stream, last-position residual}. */
+ * final norm, merged vision features, residual stream, last-position residual}; sizes as vqa_qwen25vl_workspace_bytes. */
 int vqa_clipt5_debug_layout(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, int32_t label_len, size_t* offsets,
                             int32_t n);
-int vqa_qwen25vl_debug_layout(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, size_t* offsets, int32_t n);
+int vqa_qwen25vl_debug_layout(vqa_handle* h, int32_t n_prompts, int64_t rows, int32_t n_patches, size_t* offsets, int32_t n);
 
 /* Process-wide override of the GEMM tile order (tuning): group_rows > 0 = A rows per M group, chunk_rows > 0 = W rows per
  * L2-resident chunk, chunk_rows < 0 = one chunk; 0 = automatic. */
@@ -424,8 +434,8 @@ int vqa_op_lmhead_logprob(const void* H, int32_t ldh, const void* W, int32_t ldw
                           float temperature, const uint32_t* pen_bitmap, float repetition_penalty, float* logprob, float* scratch,
                           size_t scratch_bytes, size_t* scratch_needed, void* stream);
 
-/* The per-step kernel of vqa_qwen25vl_rollout_* on caller-given bf16 logits [batch, V]: for every b with done[b] == 0, row lengths[b] of
- * out_logp [batch, max_new, n_max] (and of out_topk_ids / out_topk_probs [batch, max_new, top_k] when top_k > 0), under the penalty
+/* The per-step kernel of a scored rollout (vqa_qwen25vl_generation.score) on caller-given bf16 logits [batch, V]: for every b with
+ * done[b] == 0, row lengths[b] of out_logp [batch, max_new, n_max] (and of out_topk_ids / out_topk_probs [batch, max_new, top_k] when top_k > 0), under the penalty
  * bitmap pen_bitmap [batch, ceil(V / 32)] (NULL = none) and the temperature. All pointers DEVICE. */
 int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t V, const uint32_t* pen_bitmap, float repetition_penalty, float temperature,
                           const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, int32_t max_new, const int32_t* lengths,
@@ -623,7 +633,7 @@ int vqa_op_gather_rows(const void* src, void* dst, const int32_t* index, int32_t
 
 /* Embedding splice: row r = b * S + s of out [rows, D] (rows a multiple of S) is feats[feat_index[r]] when feat_index[r] >= 0, else
  * embed[ids[r]], for s < seq_lens[b]; zero past it (ids and feat_index are not read there). Padded rows: seq_lens [rows / S]; packed rows as
- * vqa_qwen25vl_score_packed: seq_lens = cu_seqlens + n_seq and S = rows. D a multiple of 8; embed / feats / out 16-byte aligned. */
+ * vqa_qwen25vl_score with a vqa_qwen25vl_packed: seq_lens = cu_seqlens + n_seq and S = rows. D a multiple of 8; embed / feats / out 16-byte aligned. */
 int vqa_op_qwen_embed(const int32_t* ids, const int32_t* feat_index, const int32_t* seq_lens, const void* embed, const void* feats, void* out,
                       int32_t rows, int32_t S, int32_t D, void* stream);
 

@@ -20,10 +20,10 @@ ABI_SYMBOLS = [
     "vqa_clip_preprocess_workspace_bytes", "vqa_clip_preprocess", "vqa_resample_table", "vqa_qwen_preprocess_plan",
     "vqa_qwen_preprocess", "vqa_clipt5_debug_layout", "vqa_qwen25vl_debug_layout", "vqa_set_gemm_schedule",
     "vqa_qwen25vl_topk", "vqa_op_gemm_bf16_normfuse",
-    "vqa_qwen25vl_packed_workspace_bytes", "vqa_qwen25vl_score_packed", "vqa_debug_max_active_clusters", "vqa_debug_pdl_enabled", "vqa_op_attention_d128_ex", "vqa_op_gemm_bf16_grouped", "vqa_op_gemm_bf16_splitk",
+    "vqa_debug_max_active_clusters", "vqa_debug_pdl_enabled", "vqa_op_attention_d128_ex", "vqa_op_gemm_bf16_grouped", "vqa_op_gemm_bf16_splitk",
     "vqa_qwen25vl_generate_workspace_bytes", "vqa_qwen25vl_generate_prefill", "vqa_qwen25vl_generate_step",
     "vqa_clipt5_generate_workspace_bytes", "vqa_clipt5_generate_prefill", "vqa_clipt5_generate_step",
-    "vqa_qwen25vl_rollout_prefill", "vqa_qwen25vl_rollout_step", "vqa_op_answer_logprob",
+    "vqa_op_answer_logprob",
     "vqa_op_kv_cache_write", "vqa_op_decode_attention_d128", "vqa_op_greedy_select", "vqa_t5_bucket_lut", "vqa_op_t5_decoder_self_attn",
     "vqa_op_t5_decode_self_attn", "vqa_op_gemm_bf16_f32acc", "vqa_op_gemm_bf16_batched", "vqa_op_t5_cross_attention", "vqa_op_layernorm_f32",
     "vqa_op_clip_embed_ln", "vqa_qwen_preprocess_video_plan", "vqa_qwen_preprocess_video",
@@ -53,6 +53,40 @@ class VqaQwen25VLConfig(C.Structure):
         ("fullatt_mask", C.c_uint64), ("hidden", C.c_int32), ("layers", C.c_int32), ("heads", C.c_int32),
         ("kv_heads", C.c_int32), ("mlp", C.c_int32), ("vocab", C.c_int32), ("rms_eps", C.c_float),
         ("emulate_bf16_rounding", C.c_int32),
+    ]
+
+
+# The Qwen2.5-VL call structs, field for field as include/vqa_b200.h declares them (tests/test_abi.py checks the layout). Pointer fields
+# hold device addresses (ints); VqaQwen25VLGeneration.score points to a VqaQwen25VLAnswerScore the caller keeps alive.
+class VqaQwen25VLPrompts(C.Structure):
+    _fields_ = [
+        ("pixel_patches", C.c_void_p), ("pixel_dtype", C.c_int32), ("n_patches", C.c_int32), ("vis_pos_hw", C.c_void_p),
+        ("window_index", C.c_void_p), ("reverse_index", C.c_void_p), ("cu_window", C.c_void_p), ("n_windows", C.c_int32),
+        ("max_window_len", C.c_int32), ("cu_frames", C.c_void_p), ("n_frames", C.c_int32), ("max_frame_len", C.c_int32),
+        ("input_ids", C.c_void_p), ("seq_lens", C.c_void_p), ("feat_index", C.c_void_p), ("position_ids", C.c_void_p),
+        ("batch", C.c_int32), ("seq_len", C.c_int32),
+    ]
+
+
+class VqaQwen25VLPacked(C.Structure):
+    _fields_ = [
+        ("total_rows", C.c_int32), ("cu_seqlens", C.c_void_p), ("kv_prefix", C.c_void_p), ("n_seq", C.c_int32), ("max_seq_len", C.c_int32),
+        ("pair_row", C.c_void_p), ("pair_seq", C.c_void_p), ("max_prompt_len", C.c_int32),
+    ]
+
+
+class VqaQwen25VLAnswerScore(C.Structure):
+    _fields_ = [
+        ("answer_ids", C.c_void_p), ("answer_counts", C.c_void_p), ("n_max", C.c_int32), ("temperature", C.c_float), ("top_k", C.c_int32),
+        ("out_logp", C.c_void_p), ("out_topk_ids", C.c_void_p), ("out_topk_probs", C.c_void_p),
+    ]
+
+
+class VqaQwen25VLGeneration(C.Structure):
+    _fields_ = [
+        ("seq_lens", C.c_void_p), ("first_position", C.c_void_p), ("eos_ids", C.c_void_p), ("n_eos", C.c_int32),
+        ("max_new_tokens", C.c_int32), ("repetition_penalty", C.c_float), ("out_tokens", C.c_void_p), ("out_lengths", C.c_void_p),
+        ("all_done", C.c_void_p), ("score", C.POINTER(VqaQwen25VLAnswerScore)),
     ]
 
 
@@ -117,30 +151,18 @@ def load() -> C.CDLL:
     lib.vqa_create_qwen25vl.restype = C.c_int
     lib.vqa_qwen25vl_set_rope.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(i32), i32, C.POINTER(C.c_float), C.POINTER(i32), i32]
     lib.vqa_qwen25vl_set_rope.restype = C.c_int
-    lib.vqa_qwen25vl_workspace_bytes.argtypes = [vp, i32, i32, i32]
+    lib.vqa_qwen25vl_workspace_bytes.argtypes = [vp, i32, i64, i32]
     lib.vqa_qwen25vl_workspace_bytes.restype = C.c_size_t
-    lib.vqa_qwen25vl_score.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, i32, i32, f32,
-                                       f32, vp, vp, vp, C.c_size_t, vp]
+    lib.vqa_qwen25vl_score.argtypes = [vp, C.POINTER(VqaQwen25VLPrompts), C.POINTER(VqaQwen25VLPacked), vp, f32, f32, vp, vp, vp, C.c_size_t, vp]
     lib.vqa_qwen25vl_score.restype = C.c_int
     lib.vqa_qwen25vl_topk.argtypes = [vp, i32, i64, i32, i32, f32, f32, vp, vp, vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_packed_workspace_bytes.argtypes = [vp, i32, i64, i32]
-    lib.vqa_qwen25vl_packed_workspace_bytes.restype = C.c_size_t
-    lib.vqa_qwen25vl_score_packed.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, i32, vp, vp, i32, i32, vp, vp,
-                                              vp, i32, i32, f32, f32, vp, vp, vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_score_packed.restype = C.c_int
     lib.vqa_qwen25vl_topk.restype = C.c_int
     lib.vqa_qwen25vl_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
     lib.vqa_qwen25vl_generate_workspace_bytes.restype = C.c_size_t
-    lib.vqa_qwen25vl_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp, i32,
-                                                  i32, f32, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.vqa_qwen25vl_generate_prefill.argtypes = [vp, C.POINTER(VqaQwen25VLPrompts), C.POINTER(VqaQwen25VLGeneration), vp, C.c_size_t, vp]
     lib.vqa_qwen25vl_generate_prefill.restype = C.c_int
-    lib.vqa_qwen25vl_generate_step.argtypes = [vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.vqa_qwen25vl_generate_step.argtypes = [vp, C.POINTER(VqaQwen25VLGeneration), i32, i32, i32, vp, C.c_size_t, vp]
     lib.vqa_qwen25vl_generate_step.restype = C.c_int
-    rollout = [vp, vp, i32, f32, i32, vp, vp, vp]          # answer ids, counts, n_max, temperature, top_k, logp, top-k ids, top-k probs
-    lib.vqa_qwen25vl_rollout_prefill.argtypes = list(lib.vqa_qwen25vl_generate_prefill.argtypes[:-3]) + rollout + [vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_rollout_prefill.restype = C.c_int
-    lib.vqa_qwen25vl_rollout_step.argtypes = list(lib.vqa_qwen25vl_generate_step.argtypes[:-3]) + rollout + [vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_rollout_step.restype = C.c_int
     lib.vqa_op_answer_logprob.argtypes = [vp, i32, i32, vp, f32, f32, vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, vp]
     lib.vqa_op_answer_logprob.restype = C.c_int
     lib.vqa_op_kv_cache_write.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, i32, vp]
@@ -220,7 +242,7 @@ def load() -> C.CDLL:
     lib.vqa_qwen_preprocess_video_aa.restype = C.c_int
     lib.vqa_clipt5_debug_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(C.c_size_t), i32]
     lib.vqa_clipt5_debug_layout.restype = C.c_int
-    lib.vqa_qwen25vl_debug_layout.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_size_t), i32]
+    lib.vqa_qwen25vl_debug_layout.argtypes = [vp, i32, i64, i32, C.POINTER(C.c_size_t), i32]
     lib.vqa_qwen25vl_debug_layout.restype = C.c_int
     lib.vqa_set_gemm_schedule.argtypes = [i32, i32]
     lib.vqa_set_gemm_schedule.restype = C.c_int

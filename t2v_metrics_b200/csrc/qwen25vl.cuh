@@ -72,19 +72,6 @@ static QwenWorkspace qwen_plan_rows(const vqa_qwen25vl_config& c, int B, size_t 
     return w;
 }
 
-static QwenWorkspace qwen_plan(const vqa_qwen25vl_config& c, int B, int S, int n_patches) { return qwen_plan_rows(c, B, (size_t)B * S, n_patches); }
-
-// Packed-rows layout of the language-model tokens (SURVEY 8(f)1, KV-prefix sharing): sequences are stored back to back (cu_seqlens);
-// a prompt's [system + vision] prefix is ONE sequence shared by every prompt over that image, each prompt's remaining tokens are their own
-// sequence whose kv_prefix points at it. Causal attention makes this exact: a prefix row never sees a suffix.
-struct QwenPacked {
-    int total_rows, n_seq, max_seq_len, max_prompt_len;
-    const int* cu_seqlens;   // [n_seq + 1]
-    const int* kv_prefix;    // [n_seq], -1 = none
-    const int* pair_row;     // [B] packed row of each prompt's last token
-    const int* pair_seq;     // [B] sequence holding that row
-};
-
 static int qwen_finalize(vqa_handle* h, QwenState& q) {
     const vqa_qwen25vl_config& c = q.cfg;
     bool ok = true;
@@ -124,15 +111,6 @@ static int qwen_finalize(vqa_handle* h, QwenState& q) {
     return VQA_OK;
 }
 
-// The vision and prompt inputs of one prefill (see vqa_qwen25vl_score)
-struct QwenPrompts {
-    const void* pixel_patches; int pixel_dtype, n_patches;
-    const int *vis_pos_hw, *window_index, *reverse_index, *cu_window; int n_windows, max_window_len;
-    const int* cu_frames; int n_frames, max_frame_len;
-    const int *input_ids, *seq_lens, *feat_index, *position_ids;
-    int B, S;
-};
-
 // K/V cache of a generate prefill: layer l's K and V at kc + l * layer_elems and vc + l * layer_elems, each [B, Hkv, cap, 128]
 struct QwenKVCache {
     bf16 *kc, *vc;
@@ -142,12 +120,12 @@ struct QwenKVCache {
 
 // Vision tower, embedding splice and every language-model layer of one prefill, into w.x. With `kv`, each layer's post-rope K/V rows are
 // also stored in the cache (one launch per layer after the rope).
-static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const QwenPrompts& in, const QwenPacked* pk,
+static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const vqa_qwen25vl_prompts& in, const vqa_qwen25vl_packed* pk,
                         const QwenKVCache* kv = nullptr) {
     const vqa_qwen25vl_config& c = q.cfg;
     cudaStream_t st = f.st;
     const void* pixel_patches = in.pixel_patches;
-    const int pixel_dtype = in.pixel_dtype, n_patches = in.n_patches, B = in.B, S = in.S;
+    const int pixel_dtype = in.pixel_dtype, n_patches = in.n_patches, B = in.batch, S = pk ? pk->total_rows : in.seq_len;
     const int *vis_pos_hw = in.vis_pos_hw, *window_index = in.window_index, *reverse_index = in.reverse_index, *cu_window = in.cu_window;
     const int n_windows = in.n_windows, max_window_len = in.max_window_len, n_frames = in.n_frames, max_frame_len = in.max_frame_len;
     const int *cu_frames = in.cu_frames, *input_ids = in.input_ids, *seq_lens = in.seq_lens, *feat_index = in.feat_index;
@@ -246,10 +224,10 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
 }
 
 // Last prompt position -> final norm (w.lastn); with a repetition penalty, also the bitmap of every prompt's ids (w.pen_bitmap).
-static int qwen_last_position(Forward& f, QwenState& q, const QwenWorkspace& w, const QwenPrompts& in, const QwenPacked* pk,
+static int qwen_last_position(Forward& f, QwenState& q, const QwenWorkspace& w, const vqa_qwen25vl_prompts& in, const vqa_qwen25vl_packed* pk,
                               float repetition_penalty) {
     const vqa_qwen25vl_config& c = q.cfg;
-    const int B = in.B, S = in.S, D = c.hidden;
+    const int B = in.batch, S = in.seq_len, D = c.hidden;
     const int *input_ids = in.input_ids, *seq_lens = in.seq_lens;
     auto P_ = [&](size_t off) { return f.at(off); };
     if (pk) TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_rows_by_index_kernel, B, 128, 0, P_(w.x), pk->pair_row, P_(w.last), D));
@@ -272,12 +250,12 @@ static int qwen_last_position(Forward& f, QwenState& q, const QwenWorkspace& w, 
     return VQA_OK;
 }
 
-static int qwen_score(vqa_handle* h, QwenState& q, const QwenPrompts& in, const int* answer_ids, float temperature, float repetition_penalty,
-                      float* out_probs, float* out_logprobs, void* workspace, size_t workspace_bytes, cudaStream_t st,
-                      const QwenPacked* pk = nullptr) {
+static int qwen_score(vqa_handle* h, QwenState& q, const vqa_qwen25vl_prompts& in, const vqa_qwen25vl_packed* pk, const int* answer_ids,
+                      float temperature, float repetition_penalty, float* out_probs, float* out_logprobs, void* workspace, size_t workspace_bytes,
+                      cudaStream_t st) {
     const vqa_qwen25vl_config& c = q.cfg;
-    const int B = in.B, D = c.hidden;
-    const QwenWorkspace w = pk ? qwen_plan_rows(c, B, (size_t)pk->total_rows, in.n_patches) : qwen_plan(c, B, in.S, in.n_patches);
+    const int B = in.batch, D = c.hidden;
+    const QwenWorkspace w = qwen_plan_rows(c, B, pk ? (size_t)pk->total_rows : (size_t)B * in.seq_len, in.n_patches);
     if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
     auto P_ = [&](size_t off) { return f.at(off); };
@@ -343,7 +321,7 @@ static bool decode_attn_group_supported(int G) { return G == 1 || G == 2 || G ==
 
 static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S, int n_patches, int max_new, int num_sms) {
     QwenGenWorkspace g;
-    g.w = qwen_plan(c, B, S, n_patches);
+    g.w = qwen_plan_rows(c, B, (size_t)B * S, n_patches);
     Plan pl;
     pl.off = g.w.total;
     g.cap = S + max_new;
@@ -364,60 +342,38 @@ static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S
     return g;
 }
 
-// Scoring hook of a rollout: the answer log-probabilities (and optionally the top-k) of every step, see answer_logprob_kernel
-struct QwenAnswerScore {
-    const int* answer_ids;       // [B, n_max]
-    const int* answer_counts;    // [B]
-    int n_max; float temperature; int top_k;
-    float* logp;                 // [B, max_new, n_max]
-    int* topk_ids;               // [B, max_new, top_k] (top_k > 0)
-    float* topk_probs;           // [B, max_new, top_k] (top_k > 0)
-};
-
-// Outputs and constants of a generation, the same for the prefill and every step
-struct QwenGenArgs {
-    const int* seq_lens;     // [B] prompt lengths
-    const int* first_pos;    // [B] mRoPE position of the first generated token (last prompt position + 1)
-    const int* eos_ids; int n_eos;
-    int max_new; float repetition_penalty;
-    int* tokens;             // [B, max_new], -1 after a sequence's last token
-    int* lengths;            // [B] tokens generated so far
-    int* all_done;           // 1 once every sequence has finished
-    const QwenAnswerScore* score = nullptr;      // rollout scoring: one more launch per token, before the selection
-};
-
 // lm_head on w.lastn into [B, vocab] bf16 logits, then (rollout scoring) the answer log-probabilities of this step, then the greedy token
 // of every unfinished sequence and its bookkeeping
-static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g, int B, const QwenGenArgs& a) {
+static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g, int B, const vqa_qwen25vl_generation& a) {
     const vqa_qwen25vl_config& c = q.cfg;
     const QwenWorkspace& w = g.w;
     bf16* logits = f.at(w.trace_logits);
     // The [B, vocab] bf16 logits are 0.3 MB per sequence against the 1.1 GB lm_head weight (7B) that the GEMM streams either way.
     TRY(f.gemm(Gemm(f.at(w.lastn), q.lm_head, logits, B, c.vocab, c.hidden), "lm_head"));
     const bool penalise = a.repetition_penalty != 1.0f;
-    if (const QwenAnswerScore* s = a.score)
+    if (const vqa_qwen25vl_answer_score* s = a.score)
         TRY(f.launch(CAT_OTHER, 0, "answer logprob", answer_logprob_kernel, B, ANSWER_THREADS, 0, (const bf16*)logits, c.vocab,
                      penalise ? (const uint32_t*)f.at<uint32_t>(w.pen_bitmap) : nullptr, (c.vocab + 31) / 32, a.repetition_penalty,
-                     1.0f / s->temperature, s->answer_ids, s->answer_counts, s->n_max, a.max_new, (const int*)a.lengths,
-                     (const int*)f.at<int>(g.done), s->top_k, s->logp, s->topk_ids, s->topk_probs));
+                     1.0f / s->temperature, s->answer_ids, s->answer_counts, s->n_max, a.max_new_tokens, (const int*)a.out_lengths,
+                     (const int*)f.at<int>(g.done), s->top_k, s->out_logp, s->out_topk_ids, s->out_topk_probs));
     return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, (const bf16*)logits, c.vocab,
                     penalise ? f.at<uint32_t>(w.pen_bitmap) : nullptr, (c.vocab + 31) / 32, a.repetition_penalty, a.eos_ids, a.n_eos,
-                    a.max_new, a.first_pos, B, a.tokens, a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done,
+                    a.max_new_tokens, a.first_position, B, a.out_tokens, a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done,
                     f.at<int>(g.next_ids), f.at<int>(g.pos3));
 }
 
 // The prefill of vqa_qwen25vl_score over the padded rows, with every layer's K/V stored in the cache, then the first token.
-static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const QwenPrompts& in, const QwenGenArgs& a, void* workspace,
+static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const vqa_qwen25vl_prompts& in, const vqa_qwen25vl_generation& a, void* workspace,
                                  size_t workspace_bytes, cudaStream_t st) {
-    const QwenGenWorkspace g = qwen_gen_plan(q.cfg, in.B, in.S, in.n_patches, a.max_new, h->num_sms);
+    const QwenGenWorkspace g = qwen_gen_plan(q.cfg, in.batch, in.seq_len, in.n_patches, a.max_new_tokens, h->num_sms);
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
-    TRY(f.launch(CAT_OTHER, 0, "generate init", generate_init_kernel, (in.B * a.max_new + 255) / 256, 256, 0, in.B, a.max_new, a.tokens,
-                 a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
+    TRY(f.launch(CAT_OTHER, 0, "generate init", generate_init_kernel, (in.batch * a.max_new_tokens + 255) / 256, 256, 0, in.batch, a.max_new_tokens,
+                 a.out_tokens, a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
     const QwenKVCache kv{f.at(g.kcache), f.at(g.vcache), g.layer_elems, g.cap};
     TRY(qwen_prefill(f, q, g.w, in, nullptr, &kv));
     TRY(qwen_last_position(f, q, g.w, in, nullptr, a.repetition_penalty));
-    return qwen_select_token(f, q, g, in.B, a);
+    return qwen_select_token(f, q, g, in.batch, a);
 }
 
 // decode_attn_partial_kernel for G q heads per KV head (the group sizes of the Qwen2.5-VL family: 7B 7, 3B 8, 32B 5, 72B 8)
@@ -440,10 +396,10 @@ static cudaError_t launch_decode_attn(int G, dim3 grid, cudaStream_t st, Args...
 // of the 128-wide N tiles that splitk_slices() counts, far fewer than 132 SMs, so their K range is split (2, 4 and 4 slices:
 // tools/bench_generate.py measures the step with and without). gate_up (N = 2 x 18944) and the lm_head (N = 152064) already make
 // 296 and 1188 tiles and have no split.
-static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_patches, const QwenGenArgs& a, void* workspace,
+static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_patches, const vqa_qwen25vl_generation& a, void* workspace,
                               size_t workspace_bytes, cudaStream_t st) {
     const vqa_qwen25vl_config& c = q.cfg;
-    const QwenGenWorkspace g = qwen_gen_plan(c, B, S, n_patches, a.max_new, h->num_sms);
+    const QwenGenWorkspace g = qwen_gen_plan(c, B, S, n_patches, a.max_new_tokens, h->num_sms);
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     const QwenWorkspace& w = g.w;
     Forward f(h, workspace, st);
@@ -470,11 +426,11 @@ static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_p
                      0, Hq + Hkv, 128, 128, F_(w.cos), F_(w.sin), (long long)B, c.emulate_bf16_rounding));
         bf16 *kc = f.at(g.kcache) + l * g.layer_elems, *vc = f.at(g.vcache) + l * g.layer_elems;
         TRY(f.launch(CAT_OTHER, 0, "kv cache append", kv_cache_write_kernel, (unsigned)((B * Hkv * 16 + 255) / 256), 256, 0, P_(w.qkv), qkv_cols,
-                     Hq * 128, (Hq + Hkv) * 128, Hkv, 1, (long long)B, a.seq_lens, (const int*)a.lengths, kc, vc, g.cap));
+                     Hq * 128, (Hq + Hkv) * 128, Hkv, 1, (long long)B, a.seq_lens, (const int*)a.out_lengths, kc, vc, g.cap));
         const double kv_bytes = 2.0 * B * Hkv * (double)g.cap * 128 * 2;      // upper bound: the full capacity
         TRY(f.op(CAT_ATTENTION, 4.0 * B * Hq * (double)g.cap * 128, kv_bytes, 2, "decode attention", [&] {
             const dim3 grid(g.splits, Hkv, B);
-            cudaError_t e = launch_decode_attn(G, grid, st, P_(w.qkv), qkv_cols, kc, vc, g.cap, a.seq_lens, a.lengths, Hkv, g.chunk, tscale,
+            cudaError_t e = launch_decode_attn(G, grid, st, P_(w.qkv), qkv_cols, kc, vc, g.cap, a.seq_lens, a.out_lengths, Hkv, g.chunk, tscale,
                                                F_(g.attn_o), F_(g.attn_ml));
             if (e != cudaSuccess) return e;
             decode_attn_merge_kernel<<<B * Hq, 128, 0, st>>>(F_(g.attn_o), F_(g.attn_ml), g.splits, P_(w.attn), Hq * 128, Hq);

@@ -6,7 +6,7 @@
 
 // ------------------------------------------------------------------------------------------------ C ABI: lifecycle
 extern "C" const char* vqa_version(void) {
-    return "vqa_b200 abi=1 arch=sm_90a kernels=wgmma-gemm,flash-d64,t5-norm,lmhead-lse";
+    return "vqa_b200 abi=2 arch=sm_90a kernels=wgmma-gemm,flash-d64,t5-norm,lmhead-lse";
 }
 
 // Host mirror of T5Attention._relative_position_bucket (modeling_t5.py:189-234), fp32 like torch.
@@ -186,10 +186,10 @@ extern "C" int vqa_clipt5_debug_layout(vqa_handle* h, int32_t batch, int32_t n_i
     return VQA_OK;
 }
 
-extern "C" int vqa_qwen25vl_debug_layout(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, size_t* offsets, int32_t n) {
-    if (!h || h->kind != 1 || !offsets || n < 4 || batch <= 0 || seq_len <= 0 || n_patches <= 0)
+extern "C" int vqa_qwen25vl_debug_layout(vqa_handle* h, int32_t n_prompts, int64_t rows, int32_t n_patches, size_t* offsets, int32_t n) {
+    if (!h || h->kind != 1 || !offsets || n < 4 || n_prompts <= 0 || rows <= 0 || n_patches <= 0)
         return fail(h, VQA_ERR_INVALID_ARG, "bad debug layout argument");
-    const QwenWorkspace w = qwen_plan(h->qwen->cfg, batch, seq_len, n_patches);
+    const QwenWorkspace w = qwen_plan_rows(h->qwen->cfg, n_prompts, (size_t)rows, n_patches);
     offsets[0] = w.lastn;       // last-position hidden state after the final RMSNorm [B, hidden] bf16
     offsets[1] = w.vfeat_orig;  // merged vision features in processor order         [n_patches / merge^2, out_hidden] bf16
     offsets[2] = w.x;           // language-model residual stream                     [B*S, hidden] bf16
@@ -316,40 +316,57 @@ extern "C" int vqa_qwen25vl_set_rope(vqa_handle* h, const float* text_inv_freq, 
     return VQA_OK;
 }
 
-extern "C" size_t vqa_qwen25vl_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches) {
-    if (!h || h->kind != 1 || batch <= 0 || seq_len <= 0 || n_patches <= 0) return 0;
-    return qwen_plan(h->qwen->cfg, batch, seq_len, n_patches).total;
-}
+// The ctypes mirrors in _lib.py are laid out by hand; tests/test_abi.py checks them against these numbers.
+static_assert(sizeof(vqa_qwen25vl_prompts) == 112 && offsetof(vqa_qwen25vl_prompts, seq_len) == 108, "vqa_qwen25vl_prompts layout");
+static_assert(sizeof(vqa_qwen25vl_packed) == 56 && offsetof(vqa_qwen25vl_packed, max_prompt_len) == 48, "vqa_qwen25vl_packed layout");
+static_assert(sizeof(vqa_qwen25vl_answer_score) == 56 && offsetof(vqa_qwen25vl_answer_score, out_topk_probs) == 48,
+              "vqa_qwen25vl_answer_score layout");
+static_assert(sizeof(vqa_qwen25vl_generation) == 72 && offsetof(vqa_qwen25vl_generation, score) == 64, "vqa_qwen25vl_generation layout");
 
-extern "C" int vqa_qwen25vl_score(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
-                                  const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
-                                  const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
-                                  int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
-                                  const int32_t* feat_index, const int32_t* position_ids, const int32_t* answer_ids, int32_t batch,
-                                  int32_t seq_len, float temperature, float repetition_penalty, float* out_probs, float* out_logprobs,
-                                  void* workspace,
-                                  size_t workspace_bytes, void* stream) {
+static int qwen_handle_check(vqa_handle* h) {
     if (!h || h->kind != 1) return fail(h, VQA_ERR_INVALID_ARG, "not a Qwen2.5-VL handle");
     if (!h->finalized) return fail(h, VQA_ERR_MISSING_WEIGHT, "vqa_finalize_weights has not succeeded");
-    if (!pixel_patches || !vis_pos_hw || !window_index || !reverse_index || !cu_window || !cu_frames || !input_ids || !seq_lens ||
-        !feat_index || !position_ids || !answer_ids || !out_probs || !workspace)
+    return VQA_OK;
+}
+
+// The inputs of a prefill; packed rows read neither seq_lens nor seq_len. After qwen_handle_check.
+static int qwen_prompts_check(vqa_handle* h, const vqa_qwen25vl_prompts* p, bool packed) {
+    if (!p || !p->pixel_patches || !p->vis_pos_hw || !p->window_index || !p->reverse_index || !p->cu_window || !p->cu_frames || !p->input_ids ||
+        (!packed && !p->seq_lens) || !p->feat_index || !p->position_ids)
         return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
     const int unit = h->qwen->cfg.spatial_merge * h->qwen->cfg.spatial_merge;
-    if (batch <= 0 || seq_len <= 0 || n_patches <= 0 || n_patches % unit || n_windows <= 0 || n_frames <= 0 || !(temperature > 0.f) ||
-        !(repetition_penalty > 0.f))
-        return fail(h, VQA_ERR_INVALID_ARG, "bad size / temperature / repetition penalty");
-    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
+    if (p->batch <= 0 || (!packed && p->seq_len <= 0) || p->n_patches <= 0 || p->n_patches % unit || p->n_windows <= 0 || p->n_frames <= 0)
+        return fail(h, VQA_ERR_INVALID_ARG, "bad prompt / vision sizes");
+    if (p->pixel_dtype != VQA_DTYPE_F32 && p->pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
+    return VQA_OK;
+}
+
+extern "C" size_t vqa_qwen25vl_workspace_bytes(vqa_handle* h, int32_t n_prompts, int64_t rows, int32_t n_patches) {
+    if (!h || h->kind != 1 || n_prompts <= 0 || rows <= 0 || n_patches <= 0) return 0;
+    return qwen_plan_rows(h->qwen->cfg, n_prompts, (size_t)rows, n_patches).total;
+}
+
+extern "C" int vqa_qwen25vl_score(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_packed* packed, const int32_t* answer_ids,
+                                  float temperature, float repetition_penalty, float* out_probs, float* out_logprobs, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+    if (int rc = qwen_handle_check(h)) return rc;
+    if (int rc = qwen_prompts_check(h, prompts, packed != nullptr)) return rc;
+    if (!answer_ids || !out_probs || !workspace) return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    if (!(temperature > 0.f) || !(repetition_penalty > 0.f)) return fail(h, VQA_ERR_INVALID_ARG, "bad temperature / repetition penalty");
+    if (packed) {
+        if (!packed->cu_seqlens || !packed->kv_prefix || !packed->pair_row || !packed->pair_seq)
+            return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+        if (packed->total_rows <= 0 || packed->n_seq <= 0 || packed->max_seq_len <= 0 || packed->max_prompt_len <= 0)
+            return fail(h, VQA_ERR_INVALID_ARG, "bad packed sizes");
+    }
     if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
-    const QwenPrompts in{pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows, max_window_len,
-                         cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index, position_ids, batch, seq_len};
-    return qwen_score(h, *h->qwen, in, answer_ids, temperature, repetition_penalty, out_probs, out_logprobs, workspace, workspace_bytes,
-                      reinterpret_cast<cudaStream_t>(stream));
+    return qwen_score(h, *h->qwen, *prompts, packed, answer_ids, temperature, repetition_penalty, out_probs, out_logprobs, workspace,
+                      workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vqa_qwen25vl_topk(vqa_handle* h, int32_t batch, int64_t total_rows, int32_t n_patches, int32_t k, float temperature,
                                  float repetition_penalty, int32_t* out_ids, float* out_probs, void* workspace, size_t workspace_bytes, void* stream) {
-    if (!h || h->kind != 1) return fail(h, VQA_ERR_INVALID_ARG, "not a Qwen2.5-VL handle");
-    if (!h->finalized) return fail(h, VQA_ERR_MISSING_WEIGHT, "vqa_finalize_weights has not succeeded");
+    if (int rc = qwen_handle_check(h)) return rc;
     if (!out_ids || !out_probs || !workspace || batch <= 0 || total_rows <= 0 || n_patches <= 0 || k <= 0 || k > TOPK_MAX || !(temperature > 0.f) ||
         !(repetition_penalty > 0.f))
         return fail(h, VQA_ERR_INVALID_ARG, "bad top-k argument (1 <= k <= 8)");
@@ -357,47 +374,23 @@ extern "C" int vqa_qwen25vl_topk(vqa_handle* h, int32_t batch, int64_t total_row
                      workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
-extern "C" size_t vqa_qwen25vl_packed_workspace_bytes(vqa_handle* h, int32_t n_prompts, int64_t total_rows, int32_t n_patches) {
-    if (!h || h->kind != 1 || n_prompts <= 0 || total_rows <= 0 || n_patches <= 0) return 0;
-    return qwen_plan_rows(h->qwen->cfg, n_prompts, (size_t)total_rows, n_patches).total;
-}
-
-extern "C" int vqa_qwen25vl_score_packed(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
-                                         const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
-                                         const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
-                                         int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* feat_index,
-                                         const int32_t* position_ids, int32_t total_rows, const int32_t* cu_seqlens, const int32_t* kv_prefix,
-                                         int32_t n_seq, int32_t max_seq_len, const int32_t* pair_row, const int32_t* pair_seq,
-                                         const int32_t* answer_ids, int32_t n_prompts, int32_t max_prompt_len, float temperature,
-                                         float repetition_penalty, float* out_probs, float* out_logprobs, void* workspace, size_t workspace_bytes,
-                                         void* stream) {
-    if (!h || h->kind != 1) return fail(h, VQA_ERR_INVALID_ARG, "not a Qwen2.5-VL handle");
-    if (!h->finalized) return fail(h, VQA_ERR_MISSING_WEIGHT, "vqa_finalize_weights has not succeeded");
-    if (!pixel_patches || !vis_pos_hw || !window_index || !reverse_index || !cu_window || !cu_frames || !input_ids || !feat_index || !position_ids ||
-        !cu_seqlens || !kv_prefix || !pair_row || !pair_seq || !answer_ids || !out_probs || !workspace)
-        return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
-    const int unit = h->qwen->cfg.spatial_merge * h->qwen->cfg.spatial_merge;
-    if (n_prompts <= 0 || total_rows <= 0 || n_seq <= 0 || max_seq_len <= 0 || max_prompt_len <= 0 || n_patches <= 0 || n_patches % unit ||
-        n_windows <= 0 || n_frames <= 0 || !(temperature > 0.f) || !(repetition_penalty > 0.f))
-        return fail(h, VQA_ERR_INVALID_ARG, "bad size / temperature / repetition penalty");
-    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VQA_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
-    QwenPacked pk;
-    pk.total_rows = total_rows; pk.n_seq = n_seq; pk.max_seq_len = max_seq_len; pk.max_prompt_len = max_prompt_len;
-    pk.cu_seqlens = cu_seqlens; pk.kv_prefix = kv_prefix; pk.pair_row = pair_row; pk.pair_seq = pair_seq;
-    const QwenPrompts in{pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows, max_window_len,
-                         cu_frames, n_frames, max_frame_len, input_ids, nullptr, feat_index, position_ids, n_prompts, total_rows};
-    return qwen_score(h, *h->qwen, in, answer_ids, temperature, repetition_penalty, out_probs, out_logprobs, workspace, workspace_bytes,
-                      reinterpret_cast<cudaStream_t>(stream), &pk);
-}
-
 // ------------------------------------------------------------------------------------------------ Qwen2.5-VL greedy generation
-static int qwen_gen_check(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, const QwenGenArgs& a, const void* workspace) {
-    if (!h || h->kind != 1) return fail(h, VQA_ERR_INVALID_ARG, "not a Qwen2.5-VL handle");
-    if (!h->finalized) return fail(h, VQA_ERR_MISSING_WEIGHT, "vqa_finalize_weights has not succeeded");
-    if (!a.seq_lens || !a.first_pos || (a.n_eos > 0 && !a.eos_ids) || !a.tokens || !a.lengths || !a.all_done || !workspace)
+static int qwen_rollout_check(vqa_handle* h, const vqa_qwen25vl_answer_score& s) {
+    if (!s.answer_ids || !s.answer_counts || !s.out_logp || (s.top_k > 0 && (!s.out_topk_ids || !s.out_topk_probs)))
         return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
-    if (batch <= 0 || batch > 128 || seq_len <= 0 || n_patches <= 0 || a.max_new <= 0 || a.n_eos < 0 || !(a.repetition_penalty > 0.f))
+    if (s.n_max <= 0 || !(s.temperature > 0.f) || s.top_k < 0 || s.top_k > ANSWER_TOPK_MAX)
+        return fail(h, VQA_ERR_INVALID_ARG, "bad answer size / temperature / top_k (n_max >= 1, temperature > 0, 0 <= top_k <= 8)");
+    return VQA_OK;
+}
+
+static int qwen_gen_check(vqa_handle* h, const vqa_qwen25vl_generation* a, int32_t batch, int32_t seq_len, int32_t n_patches, const void* workspace) {
+    if (!a) return fail(h, VQA_ERR_INVALID_ARG, "null generation");
+    if (a->score)
+        if (int rc = qwen_rollout_check(h, *a->score)) return rc;
+    if (int rc = qwen_handle_check(h)) return rc;
+    if (!a->seq_lens || !a->first_position || (a->n_eos > 0 && !a->eos_ids) || !a->out_tokens || !a->out_lengths || !a->all_done || !workspace)
+        return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    if (batch <= 0 || batch > 128 || seq_len <= 0 || n_patches <= 0 || a->max_new_tokens <= 0 || a->n_eos < 0 || !(a->repetition_penalty > 0.f))
         return fail(h, VQA_ERR_INVALID_ARG, "bad size / repetition penalty (1 <= batch <= 128, max_new_tokens >= 1)");
     if (!decode_attn_group_supported(h->qwen->cfg.heads / h->qwen->cfg.kv_heads))
         return fail(h, VQA_ERR_UNSUPPORTED, "decode attention supports 1, 2, 4, 5, 7 or 8 query heads per KV head");
@@ -410,86 +403,20 @@ extern "C" size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t b
     return qwen_gen_plan(h->qwen->cfg, batch, seq_len, n_patches, max_new_tokens, h->num_sms).total;
 }
 
-// vqa_qwen25vl_generate_prefill, and with `score` vqa_qwen25vl_rollout_prefill
-static int vqa_qwen25vl_generate_prefill_impl(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
-                                              const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
-                                              const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
-                                              int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
-                                              const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
-                                              int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
-                                              float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
-                                              const QwenAnswerScore* score, void* workspace, size_t workspace_bytes, void* stream) {
-    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done, score};
-    if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
-    if (!pixel_patches || !vis_pos_hw || !window_index || !reverse_index || !cu_window || !cu_frames || !input_ids || !feat_index || !position_ids)
-        return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
-    const int unit = h->qwen->cfg.spatial_merge * h->qwen->cfg.spatial_merge;
-    if (n_patches % unit || n_windows <= 0 || n_frames <= 0) return fail(h, VQA_ERR_INVALID_ARG, "bad vision sizes");
-    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
-    const QwenPrompts in{pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window, n_windows, max_window_len,
-                         cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index, position_ids, batch, seq_len};
-    return qwen_generate_prefill(h, *h->qwen, in, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
-}
-
-extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
-                                             const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
-                                             const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
-                                             int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
-                                             const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
-                                             int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
-                                             float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
                                              void* workspace, size_t workspace_bytes, void* stream) {
-    return vqa_qwen25vl_generate_prefill_impl(h, pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window,
-                                              n_windows, max_window_len, cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index,
-                                              position_ids, first_position, batch, seq_len, eos_ids, n_eos, max_new_tokens,
-                                              repetition_penalty, out_tokens, out_lengths, all_done, nullptr, workspace, workspace_bytes, stream);
+    if (!prompts) return fail(h, VQA_ERR_INVALID_ARG, "null prompts");
+    if (int rc = qwen_gen_check(h, gen, prompts->batch, prompts->seq_len, prompts->n_patches, workspace)) return rc;
+    if (int rc = qwen_prompts_check(h, prompts, false)) return rc;
+    // the steps read the prompt lengths from gen->seq_lens: the prefill must have used the same ones
+    if (gen->seq_lens != prompts->seq_lens) return fail(h, VQA_ERR_INVALID_ARG, "gen->seq_lens and prompts->seq_lens must be the same pointer");
+    return qwen_generate_prefill(h, *h->qwen, *prompts, *gen, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
-extern "C" int vqa_qwen25vl_generate_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
-                                          int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
-                                          int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes,
-                                          void* stream) {
-    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done};
-    if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
-    return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
-}
-
-static int qwen_rollout_check(vqa_handle* h, const QwenAnswerScore& s) {
-    if (!s.answer_ids || !s.answer_counts || !s.logp || (s.top_k > 0 && (!s.topk_ids || !s.topk_probs)))
-        return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
-    if (s.n_max <= 0 || !(s.temperature > 0.f) || s.top_k < 0 || s.top_k > ANSWER_TOPK_MAX)
-        return fail(h, VQA_ERR_INVALID_ARG, "bad answer size / temperature / top_k (n_max >= 1, temperature > 0, 0 <= top_k <= 8)");
-    return VQA_OK;
-}
-
-extern "C" int vqa_qwen25vl_rollout_prefill(vqa_handle* h, const void* pixel_patches, int32_t pixel_dtype, int32_t n_patches,
-                                            const int32_t* vis_pos_hw, const int32_t* window_index, const int32_t* reverse_index,
-                                            const int32_t* cu_window, int32_t n_windows, int32_t max_window_len, const int32_t* cu_frames,
-                                            int32_t n_frames, int32_t max_frame_len, const int32_t* input_ids, const int32_t* seq_lens,
-                                            const int32_t* feat_index, const int32_t* position_ids, const int32_t* first_position,
-                                            int32_t batch, int32_t seq_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
-                                            float repetition_penalty, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
-                                            const int32_t* answer_ids, const int32_t* answer_counts, int32_t n_max, float temperature,
-                                            int32_t top_k, float* out_logp, int32_t* out_topk_ids, float* out_topk_probs, void* workspace,
-                                            size_t workspace_bytes, void* stream) {
-    const QwenAnswerScore s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
-    if (int rc = qwen_rollout_check(h, s)) return rc;
-    return vqa_qwen25vl_generate_prefill_impl(h, pixel_patches, pixel_dtype, n_patches, vis_pos_hw, window_index, reverse_index, cu_window,
-                                              n_windows, max_window_len, cu_frames, n_frames, max_frame_len, input_ids, seq_lens, feat_index,
-                                              position_ids, first_position, batch, seq_len, eos_ids, n_eos, max_new_tokens,
-                                              repetition_penalty, out_tokens, out_lengths, all_done, &s, workspace, workspace_bytes, stream);
-}
-
-extern "C" int vqa_qwen25vl_rollout_step(vqa_handle* h, const int32_t* seq_lens, const int32_t* first_position, int32_t batch, int32_t seq_len,
-                                         int32_t n_patches, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, float repetition_penalty,
-                                         int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, const int32_t* answer_ids,
-                                         const int32_t* answer_counts, int32_t n_max, float temperature, int32_t top_k, float* out_logp,
-                                         int32_t* out_topk_ids, float* out_topk_probs, void* workspace, size_t workspace_bytes, void* stream) {
-    const QwenAnswerScore s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
-    if (int rc = qwen_rollout_check(h, s)) return rc;
-    const QwenGenArgs a{seq_lens, first_position, eos_ids, n_eos, max_new_tokens, repetition_penalty, out_tokens, out_lengths, all_done, &s};
-    if (int rc = qwen_gen_check(h, batch, seq_len, n_patches, a, workspace)) return rc;
-    return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+extern "C" int vqa_qwen25vl_generate_step(vqa_handle* h, const vqa_qwen25vl_generation* gen, int32_t batch, int32_t seq_len, int32_t n_patches,
+                                          void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = qwen_gen_check(h, gen, batch, seq_len, n_patches, workspace)) return rc;
+    return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, *gen, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ kernel-level ABI
@@ -622,7 +549,7 @@ extern "C" int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t 
                                      const int32_t* lengths, const int32_t* done, int32_t top_k, float* out_logp, int32_t* out_topk_ids,
                                      float* out_topk_probs, void* stream) {
     if (!logits || !lengths || !done || batch <= 0 || V <= 0 || max_new <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad answer logprob argument");
-    const QwenAnswerScore s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
+    const vqa_qwen25vl_answer_score s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
     if (int rc = qwen_rollout_check(nullptr, s)) return rc;
     answer_logprob_kernel<<<batch, ANSWER_THREADS, 0, (cudaStream_t)stream>>>(
         (const bf16*)logits, V, pen_bitmap, (V + 31) / 32, repetition_penalty, 1.0f / temperature, answer_ids, answer_counts, n_max, max_new,

@@ -358,32 +358,38 @@ class ClipT5Engine:
         MAX_GEN_GRAPHS most recently used shapes. The host reads the all-finished flag through pinned memory every `check_every` steps and
         never synchronises in between. Returns each prompt's generated ids, the EOS id included when one ended it."""
         st = self.generate_begin(pixel_values, input_ids, text_lens, max_new_tokens, eos_ids, image_index)
-        flag = self.__dict__.get("_gen_flag")
-        if flag is None:
-            flag = self._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)
-        ev = torch.cuda.Event()
-
-        def finished() -> bool:
-            flag.copy_(st["all_done"], non_blocking=True)
-            ev.record()
-            ev.synchronize()
-            return bool(flag[0])
-
-        for step in range(1, st["max_new"]):
-            if (step - 1) % check_every == 0 and finished():
-                break
-            if not use_graph:
-                self.generate_step(st)
-            elif st["graph"] is None:
-                self.generate_step(st)           # the first step runs directly (module loading, kernel attributes), then is captured
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    self.generate_step(st)
-                st["graph"] = graph
-            else:
-                st["graph"].replay()
+        _decode_loop(self, st, use_graph, check_every)
         tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
         return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]
+
+
+def _decode_loop(engine, st: dict, use_graph: bool, check_every: int):
+    """Decode steps (engine.generate_step) after generate_begin until every prompt has finished: a CUDA graph of the step captured once per
+    state, replayed. The host reads the all-finished flag through the engine's pinned buffer every `check_every` steps."""
+    flag = engine.__dict__.get("_gen_flag")
+    if flag is None:
+        flag = engine._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+    ev = torch.cuda.Event()
+
+    def finished() -> bool:
+        flag.copy_(st["all_done"], non_blocking=True)
+        ev.record()
+        ev.synchronize()
+        return bool(flag[0])
+
+    for step in range(1, st["max_new"]):
+        if (step - 1) % check_every == 0 and finished():
+            break
+        if not use_graph:
+            engine.generate_step(st)
+        elif st["graph"] is None:
+            engine.generate_step(st)             # the first step runs directly (module loading, kernel attributes), then is captured
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                engine.generate_step(st)
+            st["graph"] = graph
+        else:
+            st["graph"].replay()
 
 
 # ------------------------------------------------------------------------------------------------ single-kernel ops
@@ -1185,7 +1191,8 @@ class QwenVLEngine:
         self.bind_engine_tensors(convert_qwen_state_dict(sd, self.cfg, self.device))
 
     def vision_indices(self, grid_thw):
-        """Window order, rotary positions and cumulative lengths for a list of (t, h, w) grids; cached per grid tuple."""
+        """Window order, rotary positions and cumulative lengths for a list of (t, h, w) grids, keyed by their vqa_qwen25vl_prompts field
+        names; cached per grid tuple."""
         from . import qwen_host
         key = tuple(tuple(int(x) for x in g) for g in grid_thw)
         hit = self._vision_cache.get(key)
@@ -1201,12 +1208,34 @@ class QwenVLEngine:
         i32 = lambda t: t.to(torch.int32).contiguous().to(dev)
         out = dict(window_index=i32(widx), reverse_index=i32(torch.argsort(widx)), vis_pos_hw=i32(pos_win.t()),
                    cu_window=i32(cu_win), cu_frames=i32(cu_frames), n_windows=cu_win.numel() - 1, n_frames=cu_frames.numel() - 1,
-                   max_window=int((cu_win[1:] - cu_win[:-1]).max()), max_frame=int((cu_frames[1:] - cu_frames[:-1]).max()),
+                   max_window_len=int((cu_win[1:] - cu_win[:-1]).max()), max_frame_len=int((cu_frames[1:] - cu_frames[:-1]).max()),
                    n_patches=L)
         self._vision_cache[key] = out
         while len(self._vision_cache) > 64:          # a dataset with varied image sizes makes a new key per batch: keep the device memory bounded
             self._vision_cache.popitem(last=False)
         return out
+
+    def _prompts(self, pixel_patches, vi, input_ids, seq_lens, feat_index, position_ids, batch: int, seq_len: int = 0):
+        """The vqa_qwen25vl_prompts of one prefill (packed rows: no seq_lens, seq_len 0). It holds raw device addresses: the caller keeps
+        the tensors alive until the call that reads it has returned."""
+        pdt = _lib.VQA_DTYPE_F32 if pixel_patches.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
+        vision = {k: (_ptr(v) if torch.is_tensor(v) else v) for k, v in vi.items()}
+        return _lib.VqaQwen25VLPrompts(pixel_patches=_ptr(pixel_patches), pixel_dtype=pdt, input_ids=_ptr(input_ids), seq_lens=_ptr(seq_lens),
+                                       feat_index=_ptr(feat_index), position_ids=_ptr(position_ids), batch=batch, seq_len=seq_len, **vision)
+
+    def _score(self, prompts, packed, rows: int, answer_ids, temperature, repetition_penalty, out, logp):
+        """One vqa_qwen25vl_score call over `rows` language-model rows: padded rows (packed None) or packed rows."""
+        dev = self.device
+        need = int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, prompts.batch, rows, prompts.n_patches))
+        if self._workspace is None or self._workspace.numel() < need:
+            self._workspace = None
+            self._workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            rc = self.lib.vqa_qwen25vl_score(self._h, C.byref(prompts), None if packed is None else C.byref(packed), _ptr(answer_ids),
+                                             float(temperature), float(repetition_penalty), _ptr(out), _ptr(logp), _ptr(self._workspace),
+                                             self._workspace.numel(), _stream_ptr(dev))
+        _check(rc, self._h, "vqa_qwen25vl_score")
+        self._last_call = (prompts.batch, rows, prompts.n_patches)     # what topk_last() needs to find the final hidden states again
 
     def score_tensors(self, pixel_patches: torch.Tensor, grid_thw, input_ids: torch.Tensor, seq_lens: torch.Tensor,
                       feat_index: torch.Tensor, position_ids: torch.Tensor, answer_ids: torch.Tensor, temperature: float = 1.0,
@@ -1222,23 +1251,11 @@ class QwenVLEngine:
         for t in (input_ids, seq_lens, feat_index, position_ids, answer_ids):
             assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
         B, S = input_ids.shape
-        need = int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, B, S, vi["n_patches"]))
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = None
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=dev)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=dev)
         logp = torch.empty(B, dtype=torch.float32, device=dev) if return_logprobs else None
-        pdt = _lib.VQA_DTYPE_F32 if pixel_patches.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
-        with torch.cuda.device(dev):
-            rc = self.lib.vqa_qwen25vl_score(self._h, _ptr(pixel_patches), pdt, vi["n_patches"], _ptr(vi["vis_pos_hw"]),
-                                             _ptr(vi["window_index"]), _ptr(vi["reverse_index"]), _ptr(vi["cu_window"]), vi["n_windows"],
-                                             vi["max_window"], _ptr(vi["cu_frames"]), vi["n_frames"], vi["max_frame"], _ptr(input_ids),
-                                             _ptr(seq_lens), _ptr(feat_index), _ptr(position_ids), _ptr(answer_ids), B, S,
-                                             float(temperature), float(repetition_penalty), _ptr(out), _ptr(logp), _ptr(self._workspace),
-                                             self._workspace.numel(), _stream_ptr(dev))
-        _check(rc, self._h, "vqa_qwen25vl_score")
-        self._last_call = (B, B * S, vi["n_patches"])       # what topk_last() needs to find the final hidden states again
+        prompts = self._prompts(pixel_patches, vi, input_ids, seq_lens, feat_index, position_ids, B, S)
+        self._score(prompts, None, B * S, answer_ids, temperature, repetition_penalty, out, logp)
         return (out, logp) if return_logprobs else out
 
     def topk_last(self, k: int = 5, temperature: float = 1.0, repetition_penalty: float = 1.0):
@@ -1260,7 +1277,7 @@ class QwenVLEngine:
     def debug_tensors(self, batch: int, seq_len: int, n_patches: int) -> Dict[str, torch.Tensor]:
         """Views into the workspace of the LAST call with these sizes (synchronise first). Parity investigations only."""
         off = (C.c_size_t * 4)()
-        _check(self.lib.vqa_qwen25vl_debug_layout(self._h, batch, seq_len, n_patches, off, 4), self._h, "vqa_qwen25vl_debug_layout")
+        _check(self.lib.vqa_qwen25vl_debug_layout(self._h, batch, batch * seq_len, n_patches, off, 4), self._h, "vqa_qwen25vl_debug_layout")
         cfg, ws = self.cfg, self._workspace
         unit = cfg.spatial_merge_size ** 2
 
@@ -1276,23 +1293,13 @@ class QwenVLEngine:
         vi = self.vision_indices(grid_thw)
         assert pixel_patches.is_cuda and pixel_patches.is_contiguous() and pixel_patches.shape == (vi["n_patches"], self.cfg.patch_dim)
         B, R = int(answer_ids.numel()), int(packed["total_rows"])
-        need = int(self.lib.vqa_qwen25vl_packed_workspace_bytes(self._h, B, R, vi["n_patches"]))
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = None
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=dev)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=dev)
-        pdt = _lib.VQA_DTYPE_F32 if pixel_patches.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
-        with torch.cuda.device(dev):
-            rc = self.lib.vqa_qwen25vl_score_packed(
-                self._h, _ptr(pixel_patches), pdt, vi["n_patches"], _ptr(vi["vis_pos_hw"]), _ptr(vi["window_index"]), _ptr(vi["reverse_index"]),
-                _ptr(vi["cu_window"]), vi["n_windows"], vi["max_window"], _ptr(vi["cu_frames"]), vi["n_frames"], vi["max_frame"],
-                _ptr(packed["input_ids"]), _ptr(packed["feat_index"]), _ptr(packed["position_ids"]), R, _ptr(packed["cu_seqlens"]),
-                _ptr(packed["kv_prefix"]), int(packed["n_seq"]), int(packed["max_seq_len"]), _ptr(packed["pair_row"]), _ptr(packed["pair_seq"]),
-                _ptr(answer_ids), B, int(packed["max_prompt_len"]), float(temperature), float(repetition_penalty), _ptr(out), None,
-                _ptr(self._workspace), self._workspace.numel(), _stream_ptr(dev))
-        _check(rc, self._h, "vqa_qwen25vl_score_packed")
-        self._last_call = (B, R, vi["n_patches"])
+        prompts = self._prompts(pixel_patches, vi, packed["input_ids"], None, packed["feat_index"], packed["position_ids"], B)
+        pk = _lib.VqaQwen25VLPacked(total_rows=R, n_seq=int(packed["n_seq"]), max_seq_len=int(packed["max_seq_len"]),
+                                    max_prompt_len=int(packed["max_prompt_len"]),
+                                    **{k: _ptr(packed[k]) for k in ("cu_seqlens", "kv_prefix", "pair_row", "pair_seq")})
+        self._score(prompts, pk, R, answer_ids, temperature, repetition_penalty, out, None)
         return out
 
     def score_prompts(self, pixel_patches, grid_thw, prompts, answer_ids, image_of_sample=None, temperature: float = 1.0,
@@ -1329,7 +1336,7 @@ class QwenVLEngine:
 
     def score_workspace_bytes(self, batch: int, seq_len: int, n_patches: int) -> int:
         """Device bytes of one padded scoring prefill (vqa_qwen25vl_workspace_bytes), the most score_prompts needs; 0 for invalid sizes."""
-        return int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, batch, seq_len, n_patches))
+        return int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, batch, batch * seq_len, n_patches))
 
     def generate_workspace_bytes(self, batch: int, seq_len: int, n_patches: int, max_new_tokens: int) -> int:
         """Device bytes of one generation or scored rollout (vqa_qwen25vl_generate_workspace_bytes); 0 for invalid sizes."""
@@ -1340,7 +1347,7 @@ class QwenVLEngine:
         """The prefill of a greedy generation (vqa_qwen25vl_generate_prefill): vision tower, padded prompt prefill into the K/V cache, first
         token. Returns the generation state that generate_step() advances: device tensors `tokens` [B, max_new_tokens] (-1 after a prompt's
         last token), `lengths` [B] and `all_done` [1], all owned by the state of this call shape.
-        score = dict(answer_ids=[ids per prompt], temperature=T, top_k=k) makes it a scored rollout (vqa_qwen25vl_rollout_prefill): the
+        score = dict(answer_ids=[ids per prompt], temperature=T, top_k=k) makes it a scored rollout (an answer score in the generation): the
         state also holds `logp` [B, max_new_tokens, n_max] (NaN where nothing was written) and, with k > 0, `topk_ids` / `topk_probs`
         [B, max_new_tokens, k]."""
         from . import qwen_host
@@ -1375,14 +1382,22 @@ class QwenVLEngine:
         st = gens.get(key)
         if st is None:
             i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
-            st = gens[key] = dict(B=B, S=S, n_patches=vi["n_patches"], max_new=max_new, penalty=float(repetition_penalty), n_eos=len(eos),
-                                  seq_lens=i32(B), first=i32(B), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new), lengths=i32(B),
-                                  all_done=i32(1), graph=None, score=None)
+            st = gens[key] = dict(B=B, S=S, n_patches=vi["n_patches"], max_new=max_new, seq_lens=i32(B), first=i32(B), eos=i32(max(len(eos), 1)),
+                                  tokens=i32(B, max_new), lengths=i32(B), all_done=i32(1), graph=None, score=None)
+            # the vqa_qwen25vl_generation every call of this state passes, built once: its pointers are the state's own tensors
+            st["gen"] = _lib.VqaQwen25VLGeneration(
+                seq_lens=_ptr(st["seq_lens"]), first_position=_ptr(st["first"]), eos_ids=_ptr(st["eos"]), n_eos=len(eos), max_new_tokens=max_new,
+                repetition_penalty=float(repetition_penalty), out_tokens=_ptr(st["tokens"]), out_lengths=_ptr(st["lengths"]),
+                all_done=_ptr(st["all_done"]))
             if score is not None:
-                st["score"] = dict(n_max=n_max, temperature=temp, top_k=top_k, answer_ids=i32(B, n_max), counts=i32(B),
-                                   logp=torch.empty(B, max_new, n_max, dtype=torch.float32, device=dev),
-                                   topk_ids=i32(B, max_new, top_k) if top_k > 0 else None,
-                                   topk_probs=torch.empty(B, max_new, top_k, dtype=torch.float32, device=dev) if top_k > 0 else None)
+                sc = st["score"] = dict(n_max=n_max, temperature=temp, top_k=top_k, answer_ids=i32(B, n_max), counts=i32(B),
+                                        logp=torch.empty(B, max_new, n_max, dtype=torch.float32, device=dev),
+                                        topk_ids=i32(B, max_new, top_k) if top_k > 0 else None,
+                                        topk_probs=torch.empty(B, max_new, top_k, dtype=torch.float32, device=dev) if top_k > 0 else None)
+                sc["struct"] = _lib.VqaQwen25VLAnswerScore(answer_ids=_ptr(sc["answer_ids"]), answer_counts=_ptr(sc["counts"]), n_max=n_max,
+                                                           temperature=temp, top_k=top_k, out_logp=_ptr(sc["logp"]),
+                                                           out_topk_ids=_ptr(sc["topk_ids"]), out_topk_probs=_ptr(sc["topk_probs"]))
+                st["gen"].score = C.pointer(sc["struct"])
             while len(gens) > self.MAX_GEN_GRAPHS:
                 gens.pop(next(iter(gens)))
         st["seq_lens"].copy_(idx["seq_lens"], non_blocking=True)
@@ -1401,41 +1416,23 @@ class QwenVLEngine:
                 sc["topk_ids"].fill_(-1)
                 sc["topk_probs"].fill_(float("nan"))
         d = {k: v.to(dev) for k, v in idx.items()}
-        pdt = _lib.VQA_DTYPE_F32 if pixel_patches.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
 
         def prefill():
-            args = [self._h, _ptr(pixel_patches), pdt, vi["n_patches"], _ptr(vi["vis_pos_hw"]), _ptr(vi["window_index"]), _ptr(vi["reverse_index"]),
-                    _ptr(vi["cu_window"]), vi["n_windows"], vi["max_window"], _ptr(vi["cu_frames"]), vi["n_frames"], vi["max_frame"],
-                    _ptr(d["input_ids"]), _ptr(st["seq_lens"]), _ptr(d["feat_index"]), _ptr(d["position_ids"]), _ptr(st["first"]), B, S,
-                    _ptr(st["eos"]), len(eos), max_new, float(repetition_penalty), _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"])]
-            fn, name = self.lib.vqa_qwen25vl_generate_prefill, "vqa_qwen25vl_generate_prefill"
-            if sc is not None:
-                args += self._rollout_args(sc)
-                fn, name = self.lib.vqa_qwen25vl_rollout_prefill, "vqa_qwen25vl_rollout_prefill"
+            prompts = self._prompts(pixel_patches, vi, d["input_ids"], st["seq_lens"], d["feat_index"], d["position_ids"], B, S)
             with torch.cuda.device(dev):
-                rc = fn(*args, _ptr(self._gen_workspace), self._gen_workspace.numel(), _stream_ptr(dev))
-            _check(rc, self._h, name)
+                rc = self.lib.vqa_qwen25vl_generate_prefill(self._h, C.byref(prompts), C.byref(st["gen"]), _ptr(self._gen_workspace),
+                                                            self._gen_workspace.numel(), _stream_ptr(dev))
+            _check(rc, self._h, "vqa_qwen25vl_generate_prefill")
         st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
         prefill()
         return st
 
-    @staticmethod
-    def _rollout_args(sc: dict) -> list:
-        return [_ptr(sc["answer_ids"]), _ptr(sc["counts"]), sc["n_max"], sc["temperature"], sc["top_k"], _ptr(sc["logp"]),
-                _ptr(sc["topk_ids"]), _ptr(sc["topk_probs"])]
-
     def generate_step(self, st: dict):
-        """One decode step of the generation `st` (vqa_qwen25vl_generate_step, or vqa_qwen25vl_rollout_step for a scored rollout),
-        launched directly."""
-        args = [self._h, _ptr(st["seq_lens"]), _ptr(st["first"]), st["B"], st["S"], st["n_patches"], _ptr(st["eos"]), st["n_eos"],
-                st["max_new"], st["penalty"], _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"])]
-        fn, name = self.lib.vqa_qwen25vl_generate_step, "vqa_qwen25vl_generate_step"
-        if st["score"] is not None:
-            args += self._rollout_args(st["score"])
-            fn, name = self.lib.vqa_qwen25vl_rollout_step, "vqa_qwen25vl_rollout_step"
+        """One decode step of the generation `st` (vqa_qwen25vl_generate_step), launched directly."""
         with torch.cuda.device(self.device):
-            rc = fn(*args, _ptr(self._gen_workspace), self._gen_workspace.numel(), _stream_ptr(self.device))
-        _check(rc, self._h, name)
+            rc = self.lib.vqa_qwen25vl_generate_step(self._h, C.byref(st["gen"]), st["B"], st["S"], st["n_patches"], _ptr(self._gen_workspace),
+                                                     self._gen_workspace.numel(), _stream_ptr(self.device))
+        _check(rc, self._h, "vqa_qwen25vl_generate_step")
 
     def generate_prompts(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
                          repetition_penalty: float = 1.0, second_per_grid_ts=None, use_graph: bool = True, check_every: int = 16):
@@ -1445,7 +1442,7 @@ class QwenVLEngine:
         Returns each prompt's generated ids, the EOS id included when one ended it."""
         st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
                                  second_per_grid_ts)
-        self._decode_loop(st, use_graph, check_every)
+        _decode_loop(self, st, use_graph, check_every)
         tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
         return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]
 
@@ -1460,36 +1457,9 @@ class QwenVLEngine:
         answer), topk_ids / topk_probs [B, max_new_tokens, top_k] or None)."""
         st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
                                  second_per_grid_ts, score=dict(answer_ids=answer_ids, temperature=temperature, top_k=top_k))
-        self._decode_loop(st, use_graph, check_every)
+        _decode_loop(self, st, use_graph, check_every)
         sc = st["score"]
         tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
         cpu = lambda t: None if t is None else t.cpu()
         return dict(tokens=[tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])], lengths=lengths, logp=cpu(sc["logp"]),
                     topk_ids=cpu(sc["topk_ids"]), topk_probs=cpu(sc["topk_probs"]))
-
-    def _decode_loop(self, st: dict, use_graph: bool, check_every: int):
-        """Decode steps after generate_begin until every prompt has finished: a CUDA graph of the step captured once per state, replayed."""
-        flag = self.__dict__.get("_gen_flag")
-        if flag is None:
-            flag = self._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)
-        ev = torch.cuda.Event()
-
-        def finished() -> bool:
-            flag.copy_(st["all_done"], non_blocking=True)
-            ev.record()
-            ev.synchronize()
-            return bool(flag[0])
-
-        for step in range(1, st["max_new"]):
-            if (step - 1) % check_every == 0 and finished():
-                break
-            if not use_graph:
-                self.generate_step(st)
-            elif st["graph"] is None:
-                self.generate_step(st)           # the first step runs directly (module loading, kernel attributes), then is captured
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    self.generate_step(st)
-                st["graph"] = graph
-            else:
-                st["graph"].replay()

@@ -193,7 +193,7 @@ def build_packed_indices(input_ids: List[Sequence[int]], grids: Sequence[Sequenc
                          second_per_grid_ts: Optional[Sequence[float]] = None, align: int = 1):
     """KV-prefix sharing (SURVEY 8(f)1): prompts that start with the same tokens up to the end of their vision run -- the chat prefix and
     the image's pad tokens, i.e. every text scored against one image (reference score.py:104-106) -- share that prefix as ONE packed
-    sequence; each prompt keeps only its remaining tokens as its own sequence. Returns the int32 CPU arrays vqa_qwen25vl_score_packed takes
+    sequence; each prompt keeps only its remaining tokens as its own sequence. Returns the int32 CPU arrays vqa_qwen25vl_score takes over packed rows
     plus sizes: dict(input_ids [R], feat_index [R], position_ids [3, R], cu_seqlens [n_seq + 1], kv_prefix [n_seq], pair_row [B],
     pair_seq [B], total_rows, n_seq, max_seq_len, max_prompt_len, n_shared). A prompt whose prefix nobody else uses is stored whole
     (kv_prefix -1), so the packed form never has more rows than sum(len(prompt)).

@@ -23,6 +23,17 @@ def test_header_symbols_exported():
     assert sorted(_lib.ABI_SYMBOLS) == names
 
 
+def test_qwen_struct_layout_matches_header():
+    # field names in header order, and the sizes and last-field offsets vqa_b200.cu static_asserts, for the Qwen2.5-VL call structs
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "vqa_b200.h")).read(), flags=re.S)
+    for cls, name, size, offset in [(_lib.VqaQwen25VLPrompts, "vqa_qwen25vl_prompts", 112, 108), (_lib.VqaQwen25VLPacked, "vqa_qwen25vl_packed", 56, 48),
+                                    (_lib.VqaQwen25VLAnswerScore, "vqa_qwen25vl_answer_score", 56, 48),
+                                    (_lib.VqaQwen25VLGeneration, "vqa_qwen25vl_generation", 72, 64)]:
+        body = re.search(r"typedef struct \{([^}]*)\} " + name + ";", text).group(1)
+        assert [f[0] for f in cls._fields_] == re.findall(r"(\w+);", body), name
+        assert ctypes.sizeof(cls) == size and getattr(cls, cls._fields_[-1][0]).offset == offset, name
+
+
 def test_version_and_null_handling():
     lib = _lib.load()
     assert b"sm_90a" in lib.vqa_version()
