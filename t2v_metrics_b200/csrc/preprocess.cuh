@@ -8,8 +8,11 @@
 // coefficient tables are built on the host in double exactly as Pillow builds them (so the integers are identical), the two integer
 // passes run here, and the result is bit-identical to PIL for every pixel.
 //
-// One CTA = one image x one band of `tile_rows` output rows. The canvas rows the band needs are staged 8 at a time into shared memory
-// as three byte PLANES packed four pixels to a word (padding colour filled in, so the passes need no bounds checks). Each 22-bit tap is
+// One CTA = one image x one tile of `tile_rows` output rows by `tile_cols` output columns. An image whose filter windows fit the
+// shared-memory budget over its whole output width has one column tile; a wide canvas (frames concatenated side by side, then padded to
+// a square) is split into column tiles too, and each CTA stages only the canvas columns its own columns' windows touch. The canvas rows
+// the tile needs are staged up to 8 at a time into shared memory as three byte PLANES packed four pixels to a word (padding colour
+// filled in, so the passes need no bounds checks). Each 22-bit tap is
 // split on the host into three byte digits (k = d0 + 256 d1 + 65536 d2, d2 signed) and laid out in words aligned to the same groups of
 // four pixels, so one `dp4a` multiplies four pixels by four tap digits: 3 dp4a per 4 taps per channel, exact in int32
 // (acc0 + (acc1 << 8) + (acc2 << 16) is the same integer Pillow accumulates). The horizontal pass writes its uint8 result four ROWS
@@ -29,6 +32,7 @@ constexpr int PRE_THREADS = 256;
 constexpr int PRE_XL = 128;                         // x lanes; PRE_THREADS / PRE_XL row groups of 4 canvas rows each
 constexpr int PRE_RG = PRE_THREADS / PRE_XL;
 constexpr int PRE_MAX_SMEM = 200 * 1024;
+constexpr int PRE_MAX_CANVAS = 65500;               // largest padded CLIP canvas side (libjpeg's largest dimension)
 
 struct PreImage {            // one per image, lives in the workspace (device) and is built on the host
     long long src_off;       // byte offset of the HWC uint8 RGB image inside `src`
@@ -38,10 +42,10 @@ struct PreImage {            // one per image, lives in the workspace (device) a
     int htab, vtab;          // int offsets of the packed tap tables inside the workspace (layout: see pre_pack_table)
     int hnp, vnp;            // words of 4 taps per output pixel (horizontal / vertical)
     int tile_rows;           // output rows per CTA
+    int tile_cols, col_tiles;  // output columns per CTA (= out_w when one tile spans the width) and column tiles per row tile
     int band_groups;         // groups of 4 canvas rows the band buffer holds
     int out_h, out_w;        // output window (after the crop) of this image
     long long out_off;       // element offset of this image's output inside `out`
-    int x_lo4, span4;        // groups of 4 canvas columns [x_lo4, x_lo4 + span4) the horizontal tap words touch
     int chunk_groups;        // groups of 4 canvas rows staged per pass (1 or 2)
     int t0, nt;              // PRE_QWEN_PATCHES: temporal slots [t0, t0 + nt) of its patch rows this frame fills
 };
@@ -184,22 +188,26 @@ __device__ __forceinline__ void pre_store_patch(OUT* dst, PrePatchGeom geom, int
 // column (c * temporal + t) * ps*ps + py * ps + px, the frame written to temporal slots t in [t0, t0 + nt): every slot for a still
 // image, its own slot for a video frame (video_processing_qwen2_vl.py:255-272), and the remaining slots for the last frame of a stack.
 template <typename OUT, int LAYOUT>
-__global__ void __launch_bounds__(PRE_THREADS)
+__global__ void __launch_bounds__(PRE_THREADS, 3)
 image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restrict__ images, const int* __restrict__ tables,
                         uchar3 background, float3 mean, float3 stdv, PrePatchGeom geom, OUT* __restrict__ out) {
     pdl_launch_dependents();
     extern __shared__ uint32_t pre_smem[];
     const PreImage im = images[blockIdx.y];
-    const int y0 = blockIdx.x * im.tile_rows;
+    const int ty = blockIdx.x / im.col_tiles, tx = blockIdx.x - ty * im.col_tiles;
+    const int y0 = ty * im.tile_rows;
     if (y0 >= im.out_h) return;
-    const int out_w = im.out_w;
-    const int ny = min(im.tile_rows, im.out_h - y0);
+    const int out_w = im.out_w, tw = im.tile_cols, x0 = tx * tw;
+    const int ny = min(im.tile_rows, im.out_h - y0), nx = min(tw, out_w - x0);
     const int chunk_rows = im.chunk_groups * 4;
-    float* lut = reinterpret_cast<float*>(pre_smem);                          // [3][256] normalised value of every grey level
-    uint32_t* band = pre_smem + 768;                                           // [3][band_groups][out_w]: 4 canvas rows per word
-    uint32_t* stage = band + (size_t)3 * im.band_groups * out_w;               // [3][chunk_rows][span4]: 4 canvas columns per word
     const int* hstart = tables + im.htab;
     const uint32_t* hwords = reinterpret_cast<const uint32_t*>(hstart + 2 * out_w);
+    // groups of 4 canvas columns [x_lo4, x_lo4 + span4) the tap words of this tile's columns touch: the windows are monotonic in x
+    const int x_lo4 = hstart[x0];
+    const int span4 = hstart[x0 + nx - 1] + im.hnp - x_lo4;
+    float* lut = reinterpret_cast<float*>(pre_smem);                          // [3][256] normalised value of every grey level
+    uint32_t* band = pre_smem + 768;                                           // [3][band_groups][tile_cols]: 4 canvas rows per word
+    uint32_t* stage = band + (size_t)3 * im.band_groups * tw;                  // [3][chunk_rows][span4]: 4 canvas columns per word
     const int* vstart = tables + im.vtab;
     const int* vlast = vstart + im.out_h;
     const uint32_t* vwords = reinterpret_cast<const uint32_t*>(vstart + 2 * im.out_h);
@@ -219,8 +227,8 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
             const int sy = 4 * (g0 + cg) + rr - im.paste_y;
             const bool row_in = sy >= 0 && sy < im.h;
             const uint8_t* row = img + (size_t)(row_in ? sy : 0) * im.w * 3;
-            for (int gx = threadIdx.x; gx < im.span4; gx += PRE_THREADS) {
-                const int sx0 = 4 * (im.x_lo4 + gx) - im.paste_x;
+            for (int gx = threadIdx.x; gx < span4; gx += PRE_THREADS) {
+                const int sx0 = 4 * (x_lo4 + gx) - im.paste_x;
                 uint32_t pr, pg, pb;
                 if (row_in && sx0 >= 0 && sx0 + 3 < im.w) {
                     const uint8_t* p = row + (size_t)sx0 * 3;
@@ -247,16 +255,17 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
                         pb |= (in ? (uint32_t)p[2] : bgc[2]) << (8 * i);
                     }
                 }
-                stage[(size_t)(0 * chunk_rows + rr) * im.span4 + gx] = pr;
-                stage[(size_t)(1 * chunk_rows + rr) * im.span4 + gx] = pg;
-                stage[(size_t)(2 * chunk_rows + rr) * im.span4 + gx] = pb;
+                stage[(size_t)(0 * chunk_rows + rr) * span4 + gx] = pr;
+                stage[(size_t)(1 * chunk_rows + rr) * span4 + gx] = pg;
+                stage[(size_t)(2 * chunk_rows + rr) * span4 + gx] = pb;
             }
         }
         __syncthreads();
         // ---- horizontal pass (ImagingResampleHorizontal_8bpc): thread = one output column x one group of 4 canvas rows
         if (grp < ngc) {
-            for (int xx = lane_x; xx < out_w; xx += PRE_XL) {
-                const int s4 = hstart[xx] - im.x_lo4;
+            for (int xl = lane_x; xl < nx; xl += PRE_XL) {
+                const int xx = x0 + xl;
+                const int s4 = hstart[xx] - x_lo4;
                 const uint32_t* kw = hwords + (size_t)xx * im.hnp * 3;
                 unsigned a0[4][3], a1[4][3];
                 int a2[4][3];
@@ -270,7 +279,7 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
                     for (int q = 0; q < 4; ++q)
 #pragma unroll
                         for (int c = 0; c < 3; ++c) {
-                            const uint32_t px = stage[(size_t)(c * chunk_rows + grp * 4 + q) * im.span4 + s4 + pw];
+                            const uint32_t px = stage[(size_t)(c * chunk_rows + grp * 4 + q) * span4 + s4 + pw];
                             a0[q][c] = pre_dp4a_uu(px, d0, a0[q][c]);
                             a1[q][c] = pre_dp4a_uu(px, d1, a1[q][c]);
                             a2[q][c] = pre_dp4a_us(px, d2, a2[q][c]);
@@ -281,7 +290,7 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
                     uint32_t wv = 0;
 #pragma unroll
                     for (int q = 0; q < 4; ++q) wv |= pre_finish(a0[q][c], a1[q][c], a2[q][c]) << (8 * q);
-                    band[((size_t)c * im.band_groups + cg + grp) * out_w + xx] = wv;
+                    band[((size_t)c * im.band_groups + cg + grp) * tw + xl] = wv;
                 }
             }
         }
@@ -295,14 +304,15 @@ image_preprocess_kernel(const uint8_t* __restrict__ src, const PreImage* __restr
         const int y = y0 + yy;
         const int gs = vstart[y] - g0;
         const uint32_t* kw = vwords + (size_t)y * im.vnp * 3;
-        for (int xx = lane_x; xx < out_w; xx += PRE_XL) {
+        for (int xl = lane_x; xl < nx; xl += PRE_XL) {
+            const int xx = x0 + xl;
             unsigned a0[3] = {0, 0, 0}, a1[3] = {0, 0, 0};
             int a2[3] = {0, 0, 0};
             for (int pw = 0; pw < im.vnp; ++pw) {
                 const uint32_t d0 = __ldg(kw + pw * 3), d1 = __ldg(kw + pw * 3 + 1), d2 = __ldg(kw + pw * 3 + 2);
 #pragma unroll
                 for (int c = 0; c < 3; ++c) {
-                    const uint32_t px = band[((size_t)c * im.band_groups + gs + pw) * out_w + xx];
+                    const uint32_t px = band[((size_t)c * im.band_groups + gs + pw) * tw + xl];
                     a0[c] = pre_dp4a_uu(px, d0, a0[c]);
                     a1[c] = pre_dp4a_uu(px, d1, a1[c]);
                     a2[c] = pre_dp4a_us(px, d2, a2[c]);
@@ -336,18 +346,18 @@ struct PrePlan {
     size_t bytes() const { return images_bytes() + tables.size() * sizeof(int); }
 };
 
-struct PreTableKey { int ch, cw, nh, nw, top, left, oh, ow, htab, vtab, hnp, vnp, tile, band_groups, x_lo4, span4, chunk_groups; };
-inline size_t pre_smem_bytes(int band_groups, int out_w, int chunk_groups, int span4) {
-    return 768 * sizeof(float) + ((size_t)3 * band_groups * out_w + (size_t)3 * chunk_groups * 4 * span4) * sizeof(uint32_t);
+struct PreTableKey { int ch, cw, nh, nw, top, left, oh, ow, htab, vtab, hnp, vnp, tile, tile_cols, col_tiles, band_groups, span4, chunk_groups; };
+inline size_t pre_smem_bytes(int band_groups, int tile_cols, int chunk_groups, int span4) {
+    return 768 * sizeof(float) + ((size_t)3 * band_groups * tile_cols + (size_t)3 * chunk_groups * 4 * span4) * sizeof(uint32_t);
 }
 
-// Tables + band geometry for "resize the ch x cw canvas to nh x nw, keep the oh x ow window at (top, left)"; shared between images
+// Tables + tile geometry for "resize the ch x cw canvas to nh x nw, keep the oh x ow window at (top, left)"; shared between images
 // with the same geometry. Returns nullptr (plan.error set) when the filter windows cannot fit the shared-memory budget.
 inline const PreTableKey* pre_tables(PrePlan& plan, std::vector<PreTableKey>& cache, int ch, int cw, int nh, int nw, int top, int left,
                                      int oh, int ow) {
     for (const PreTableKey& k : cache)
         if (k.ch == ch && k.cw == cw && k.nh == nh && k.nw == nw && k.top == top && k.left == left && k.oh == oh && k.ow == ow) return &k;
-    PreTableKey k{ch, cw, nh, nw, top, left, oh, ow, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    PreTableKey k{ch, cw, nh, nw, top, left, oh, ow, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     std::vector<int> raw;
     int ks = pre_build_table(cw, nw, left, ow, raw);
     k.htab = (int)plan.tables.size();
@@ -358,33 +368,75 @@ inline const PreTableKey* pre_tables(PrePlan& plan, std::vector<PreTableKey>& ca
     k.vnp = pre_pack_table(raw.data(), raw.data() + (size_t)oh * 2, oh, ks, plan.tables);
     const int* hstart = plan.tables.data() + k.htab;
     const int* vstart = plan.tables.data() + k.vtab;
-    k.x_lo4 = hstart[0];                           // windows are monotonic: first word of the first output .. last word of the last
-    k.span4 = hstart[ow - 1] + k.hnp - k.x_lo4;
-    // output rows per CTA (<= 32) and groups of 4 canvas rows staged per pass (2 or 1): the largest that fit the shared-memory budget
-    int tile = 32, band = 0, chunk = PRE_RG;
-    for (; tile >= 1; tile >>= 1) {
-        band = 0;
+    // groups of 4 canvas rows the tallest band of `tile` output rows needs, and of 4 canvas columns the widest column tile of `tw` output
+    // columns stages (windows are monotonic: first word of the first output .. last word of the last)
+    auto band_of = [&](int tile) {
+        int band = 0;
         for (int y0 = 0; y0 < oh; y0 += tile) {
             const int y1 = (y0 + tile < oh ? y0 + tile : oh) - 1;
             const int groups = vstart[y1] + k.vnp - vstart[y0];
             if (groups > band) band = groups;
         }
-        for (chunk = PRE_RG; chunk > 1 && pre_smem_bytes(band, ow, chunk, k.span4) > (size_t)PRE_MAX_SMEM; chunk >>= 1) {}
-        if (pre_smem_bytes(band, ow, chunk, k.span4) <= (size_t)PRE_MAX_SMEM) break;
+        return band;
+    };
+    auto span_of = [&](int tw) {
+        int span = 0;
+        for (int x0 = 0; x0 < ow; x0 += tw) {
+            const int x1 = (x0 + tw < ow ? x0 + tw : ow) - 1;
+            if (hstart[x1] + k.hnp - hstart[x0] > span) span = hstart[x1] + k.hnp - hstart[x0];
+        }
+        return span;
+    };
+    // groups of 4 canvas rows staged per pass (2 or 1): the most that fit; 0 when nothing does
+    auto chunk_of = [&](int band, int tw, int span) {
+        for (int chunk = PRE_RG; chunk >= 1; chunk >>= 1)
+            if (pre_smem_bytes(band, tw, chunk, span) <= (size_t)PRE_MAX_SMEM) return chunk;
+        return 0;
+    };
+    // one column tile over the whole output width when it fits: the most output rows per CTA (<= 32)
+    const int span_all = span_of(ow);
+    for (int tile = 32; tile >= 1; tile >>= 1) {
+        const int band = band_of(tile), chunk = chunk_of(band, ow, span_all);
+        if (chunk) {
+            k.tile = tile; k.tile_cols = ow; k.col_tiles = 1; k.band_groups = band; k.span4 = span_all; k.chunk_groups = chunk;
+            cache.push_back(k);
+            return &cache.back();
+        }
     }
-    if (tile < 1) { plan.error = "image too large for the device resize (filter windows exceed shared memory)"; return nullptr; }
-    k.tile = tile; k.band_groups = band; k.chunk_groups = chunk;
+    // otherwise column tiles too: the (rows, columns) tile that fits with the least estimated work, counted in thread iterations of the
+    // staging loop (weighted by its three loads and three stores per word), the horizontal and vertical tap loops, plus a fixed cost per CTA
+    double best = 0.0;
+    for (int tile = 32; tile >= 1; tile >>= 1) {
+        const int band = band_of(tile), row_tiles = (oh + tile - 1) / tile;
+        for (int nct = 2, prev = 0; nct <= ow; ++nct) {
+            const int tw = (ow + nct - 1) / nct;
+            if (tw == prev) continue;
+            prev = tw;
+            const int span = span_of(tw), chunk = chunk_of(band, tw, span);
+            if (!chunk) continue;
+            const int cols = (ow + tw - 1) / tw, lanes = (tw + PRE_XL - 1) / PRE_XL;
+            const double stage = 4.0 * band * ((span + PRE_THREADS - 1) / PRE_THREADS);
+            const double horiz = (double)((band + chunk - 1) / chunk) * lanes * k.hnp * 12;
+            const double vert = (double)((tile + PRE_RG - 1) / PRE_RG) * lanes * k.vnp * 9;
+            const double cost = (double)row_tiles * cols * (6.0 * stage + horiz + vert + 256.0);
+            if (best == 0.0 || cost < best) {
+                best = cost;
+                k.tile = tile; k.tile_cols = tw; k.col_tiles = cols; k.band_groups = band; k.span4 = span; k.chunk_groups = chunk;
+            }
+        }
+    }
+    if (best == 0.0) { plan.error = "image too large for the device resize (filter windows exceed shared memory)"; return nullptr; }
     cache.push_back(k);
     return &cache.back();
 }
 
 inline void pre_finish_image(PrePlan& plan, PreImage& im, const PreTableKey& k) {
     im.htab = k.htab; im.vtab = k.vtab; im.hnp = k.hnp; im.vnp = k.vnp;
-    im.tile_rows = k.tile; im.band_groups = k.band_groups; im.out_h = k.oh; im.out_w = k.ow;
-    im.x_lo4 = k.x_lo4; im.span4 = k.span4; im.chunk_groups = k.chunk_groups;
-    const int tiles = (k.oh + k.tile - 1) / k.tile;
+    im.tile_rows = k.tile; im.tile_cols = k.tile_cols; im.col_tiles = k.col_tiles; im.band_groups = k.band_groups;
+    im.out_h = k.oh; im.out_w = k.ow; im.chunk_groups = k.chunk_groups;
+    const int tiles = (k.oh + k.tile - 1) / k.tile * k.col_tiles;
     if (tiles > plan.max_tiles) plan.max_tiles = tiles;
-    const size_t sm = pre_smem_bytes(k.band_groups, k.ow, k.chunk_groups, k.span4);
+    const size_t sm = pre_smem_bytes(k.band_groups, k.tile_cols, k.chunk_groups, k.span4);
     if (sm > plan.smem) plan.smem = sm;
 }
 
@@ -400,6 +452,7 @@ inline bool pre_plan(const int32_t* heights, const int32_t* widths, const int64_
         PreImage& im = plan.images[i];
         im.src_off = offsets[i]; im.h = h; im.w = w;
         const int side = h > w ? h : w;
+        if (pad && side > PRE_MAX_CANVAS) { plan.error = "image too large for the device resize (padded canvas side over 65500 px)"; return false; }
         im.canvas_h = pad ? side : h; im.canvas_w = pad ? side : w;
         im.paste_x = pad ? (side - w) / 2 : 0; im.paste_y = pad ? (side - h) / 2 : 0;
         const int ch = im.canvas_h, cw = im.canvas_w;

@@ -903,6 +903,30 @@ def clip_preprocess_u8(images: Sequence[torch.Tensor], out_size: int, device, pa
     return out
 
 
+# Decoded images of one CLIP call go to the device in slices of at most this many bytes of uint8 pixels (at least one image per slice):
+# the concatenated frames of a video are one wide image (a 1080p 8-frame canvas is 50 MB), so a call of many videos is uploaded and
+# resized piecewise into one output tensor instead of being staged whole in pinned memory.
+CLIP_SLICE_BYTES = 64 << 20
+
+
+def clip_preprocess_u8_sliced(images: Sequence[torch.Tensor], out_size: int, device, pad: bool = True,
+                              out_dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    """clip_preprocess_u8 over consecutive slices of `images` of at most CLIP_SLICE_BYTES each, one kernel launch per slice, written into
+    the rows of one [n, 3, S, S] tensor. A call whose images fit one slice is exactly one clip_preprocess_u8 call."""
+    n = len(images)
+    assert n > 0
+    out = torch.empty(n, 3, out_size, out_size, dtype=out_dtype, device=torch.device(device))
+    lo = 0
+    while lo < n:
+        hi, nbytes = lo + 1, int(images[lo].numel())
+        while hi < n and nbytes + int(images[hi].numel()) <= CLIP_SLICE_BYTES:
+            nbytes += int(images[hi].numel())
+            hi += 1
+        clip_preprocess_u8(images[lo:hi], out_size, device, pad=pad, out=out[lo:hi])
+        lo = hi
+    return out
+
+
 def qwen_preprocess_plan(sizes_hw: Sequence[Sequence[int]], patch: int = 14, merge: int = 2, min_pixels: int = 56 * 56,
                          max_pixels: int = 14 * 14 * 4 * 1280):
     """Host-only geometry of the Qwen pre-processing (smart_resize): -> ([(1, gh, gw), ...], total patch rows, workspace bytes)."""

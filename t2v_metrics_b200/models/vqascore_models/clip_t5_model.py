@@ -13,11 +13,12 @@ import torch
 
 from ...config import CLIPT5_MODELS as _MODEL_TABLE, ClipT5Config
 from ...constants import HF_CACHE_DIR, CONTEXT_LEN, SYSTEM_MSG, IGNORE_INDEX, DEFAULT_IMAGE_TOKEN, IMAGE_TOKEN_INDEX
-from .mm_utils import t5_tokenizer_image_token, clip_preprocess
+from .mm_utils import t5_tokenizer_image_token, clip_preprocess, video_canvas
 from .vqa_model import VQAScoreModel
 
 default_question_template = 'Does this figure show "{}"? Please answer yes or no.'  # V_3.0_README.md:211-215
 default_answer_template = "Yes"
+VIDEO_EXTENSIONS = ('.mp4', '.avi', '.mov', '.mkv')      # the suffixes the reference's score.py:72 treats as videos
 
 CLIP_T5_MODELS: Dict[str, dict] = {
     name: dict(tokenizer=dict(path=spec["tokenizer"], model_max_length=CONTEXT_LEN, padding_side="right"),
@@ -56,6 +57,9 @@ def prompt_token_ids(tokenizer, questions: List[str], context_len: int, vocab: i
 class CLIPT5Model(VQAScoreModel):
     """VQAScore with CLIP-FlanT5 on the H100 engine."""
     video_mode = "concat"
+    # video files may be passed to forward(): the plugin concatenates their frames into one canvas per video itself (Score.forward hands
+    # a "concat" plugin video files only when it sets this)
+    builds_video_canvases = True
     allows_image = True
 
     def __init__(self, model_name="clip-flant5-xxl", device="cuda", cache_dir=HF_CACHE_DIR, tokenizer=None,
@@ -107,14 +111,17 @@ class CLIPT5Model(VQAScoreModel):
         return normalise_clipt5_keys(load_state_dict(path), vision)
 
     # ---- pre-processing ------------------------------------------------------------------------------------------
-    def load_images(self, image: List[str]) -> torch.Tensor:
-        """image_loader (PIL decode, host) -> uint8 HWC -> ONE device kernel doing expand2square(mean colour) + PIL-exact bicubic
+    def load_images(self, image: List[str], num_frames: int = 8) -> torch.Tensor:
+        """image_loader (PIL decode, host) -> uint8 HWC -> a device kernel doing expand2square(mean colour) + PIL-exact bicubic
         resize + centre crop + /255 + normalise (engine.clip_preprocess_u8; bit-identical to the CPU path `clip_preprocess`, which
-        is what the reference runs per image on the host: mm_utils.py:128-139 + CLIPImageProcessor). fp32 [n,3,S,S] on the device."""
+        is what the reference runs per image on the host: mm_utils.py:128-139 + CLIPImageProcessor). fp32 [n,3,S,S] on the device.
+        A video file becomes the canvas of `num_frames` frames side by side that the reference scores for it (mm_utils.video_canvas).
+        One launch per slice of engine.CLIP_SLICE_BYTES of pixels (a call of still images of ordinary size is one launch)."""
         import numpy as np
-        from ...engine import clip_preprocess_u8
-        raw = [torch.from_numpy(np.ascontiguousarray(np.asarray(self.image_loader(p).convert("RGB"), dtype=np.uint8))) for p in image]
-        return clip_preprocess_u8(raw, self.cfg.image_size, self.engine.device, pad=self.image_aspect_ratio == "pad")
+        from ...engine import clip_preprocess_u8_sliced
+        raw = [torch.from_numpy(video_canvas(p, num_frames) if p[-4:].lower() in VIDEO_EXTENSIONS else
+                                np.ascontiguousarray(np.asarray(self.image_loader(p).convert("RGB"), dtype=np.uint8))) for p in image]
+        return clip_preprocess_u8_sliced(raw, self.cfg.image_size, self.engine.device, pad=self.image_aspect_ratio == "pad")
 
     def _prompt_ids(self, questions: List[str]) -> List[List[int]]:
         cache = self.__dict__.setdefault("_chunk_cache", {})
@@ -175,6 +182,8 @@ class CLIPT5Model(VQAScoreModel):
         cache (393 KB per sample per token at xxl width). The batch runs as one encoder pass and one decode loop on the device, in calls of
         at most GENERATE_MAX_PAIRS pairs. Sampling (temperature > 0 or do_sample=True) is not implemented."""
         assert len(images) == len(texts), "Number of images and texts must match"
+        if any(p[-4:].lower() in VIDEO_EXTENSIONS for p in images):
+            raise NotImplementedError("generate takes image files; video files are scored by forward only")
         if do_sample is None:
             do_sample = temperature > 0
         if do_sample or temperature > 0:
@@ -202,8 +211,12 @@ class CLIPT5Model(VQAScoreModel):
     # ---- scoring -------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, images: List[str], texts: List[str], question_template: str = default_question_template,
-                answer_template: str = default_answer_template) -> torch.Tensor:
+                answer_template: str = default_answer_template, num_frames: int = 8) -> torch.Tensor:
+        """One score per (images[i], texts[i]) pair. An image path ending in .mp4 / .avi / .mov / .mkv is a video: it is scored as the
+        horizontal concatenation of `num_frames` equally spaced frames, as the reference's Score.forward does for this model."""
         assert len(images) == len(texts), "Number of images and texts must match"
+        if num_frames < 1:
+            raise ValueError(f"num_frames must be >= 1, got {num_frames}")
         questions = [format_question(question_template.format(t), self.conversational_style) for t in texts]
         answers = [format_answer(answer_template.format(t), self.conversational_style) for t in texts]
         input_ids, lens, labels = self._tokenize(questions, answers)
@@ -212,7 +225,7 @@ class CLIPT5Model(VQAScoreModel):
         index = []
         for p in images:
             index.append(uniq.setdefault(p, len(uniq)))
-        pixels = self.load_images(list(uniq.keys()))
+        pixels = self.load_images(list(uniq.keys()), num_frames)
         dev = self.engine.device
         image_index = torch.tensor(index, dtype=torch.int32).to(dev, non_blocking=True)
         args = (pixels, input_ids.to(dev, non_blocking=True), lens.to(dev, non_blocking=True), labels.to(dev, non_blocking=True))

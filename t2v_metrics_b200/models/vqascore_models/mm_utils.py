@@ -1,4 +1,5 @@
 """Host-side pieces of the CLIP-FlanT5 path that survive in the reference's mm_utils.py, rebuilt for this engine."""
+import io
 from typing import Callable, List, Optional, Sequence
 
 import numpy as np
@@ -66,3 +67,63 @@ def clip_preprocess(pil_img: Image.Image, image_size: int, pad: bool = True) -> 
     arr = np.asarray(img, dtype=np.float32) / 255.0
     arr = (arr - np.asarray(CLIP_IMAGE_MEAN, dtype=np.float32)) / np.asarray(CLIP_IMAGE_STD, dtype=np.float32)
     return torch.from_numpy(arr).permute(2, 0, 1).contiguous()
+
+
+# ------------------------------------------------------------------------------------------------ videos for single-image models
+CONCAT_GAP = 10                 # black columns between two frames of the canvas (the reference's dist_images)
+JPEG_MAX_SIDE = 65500           # libjpeg's largest dimension: a wider canvas cannot be stored as the JPEG the reference reads back
+
+
+def _jpeg_round_trip(bgr: np.ndarray):
+    import cv2
+    ok, buf = cv2.imencode(".jpg", bgr)
+    if not ok:
+        raise ValueError(f"cannot encode a {bgr.shape[1]}x{bgr.shape[0]} image as JPEG")
+    return buf
+
+
+def video_frames_bgr(path: str, num_frames: int) -> List[np.ndarray]:
+    """`num_frames` frames of a video file as the reference's extract_frames + cv2.imread leave them (BGR uint8 [h, w, 3]), in temporal
+    order: the container's frame count, step = count // num_frames, a seek to frame i * step before each read (every read seeks to frame
+    0 when the clip has fewer frames than num_frames), a failed read skipped, and each frame through one JPEG encode / decode at OpenCV's
+    default quality -- in memory instead of through frame files."""
+    import cv2
+    if num_frames < 1:
+        raise ValueError(f"num_frames must be >= 1, got {num_frames}")
+    cap = cv2.VideoCapture(path)
+    try:
+        step = int(cap.get(cv2.CAP_PROP_FRAME_COUNT)) // num_frames
+        frames = []
+        for i in range(num_frames):
+            cap.set(cv2.CAP_PROP_POS_FRAMES, i * step)
+            ok, frame = cap.read()
+            if ok:
+                frames.append(cv2.imdecode(_jpeg_round_trip(frame), cv2.IMREAD_COLOR))
+    finally:
+        cap.release()
+    if not frames:
+        raise ValueError(f"no frame could be read from {path!r}")
+    return frames
+
+
+def concat_frames_rgb(frames_bgr: Sequence[np.ndarray], gap: int = CONCAT_GAP) -> np.ndarray:
+    """Frames side by side, top-aligned, `gap` black columns apart, on a canvas as tall as the tallest frame (the reference's
+    concatenate_images_horizontal), then through the JPEG the reference writes and PIL's decode of it -> RGB uint8 [h, W, 3]."""
+    width = sum(f.shape[1] for f in frames_bgr) + gap * (len(frames_bgr) - 1)
+    height = max(f.shape[0] for f in frames_bgr)
+    if width > JPEG_MAX_SIDE or height > JPEG_MAX_SIDE:
+        raise ValueError(f"the concatenated canvas is {width}x{height} px; JPEG allows at most {JPEG_MAX_SIDE} px a side")
+    canvas = np.zeros((height, width, 3), dtype=np.uint8)
+    x = 0
+    for f in frames_bgr:
+        canvas[:f.shape[0], x:x + f.shape[1]] = f
+        x += f.shape[1] + gap
+    buf = _jpeg_round_trip(canvas)
+    return np.array(Image.open(io.BytesIO(buf.tobytes())).convert("RGB"), dtype=np.uint8)
+
+
+def video_canvas(path: str, num_frames: int = 8) -> np.ndarray:
+    """What a single-image model of the reference scores for a video file: `num_frames` frames concatenated into one image, RGB uint8
+    [h, W, 3] (reference score.py:78-98 with mm_utils.extract_frames and concatenate_images_horizontal), bit for bit, with the frames in
+    temporal order."""
+    return concat_frames_rgb(video_frames_bgr(path, num_frames))

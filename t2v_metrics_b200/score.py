@@ -7,7 +7,9 @@ Differences, all above the drop-in boundary and result-preserving:
   * `batch_forward` scores a whole DataLoader batch per (visual, text) slot, as v3.0 did, instead of one pair at a time
     (v3.1 score.py:143-153).
   * video files reach a model that takes them directly (`video_mode == "direct"`, score.py:99-101) when the plugin has a decoder
-    (Qwen2.5-VL with `video_reader=`); otherwise, and for the cv2 concat path (score.py:72-98), video inputs raise.
+    (Qwen2.5-VL with `video_reader=`), and a `video_mode == "concat"` model (score.py:72-98) when the plugin builds the frame canvases
+    itself (`builds_video_canvases`, CLIP-FlanT5), with `num_frames`; otherwise video inputs raise. In a call that mixes videos and
+    image files the images stay images (the reference sends every input of such a call through frame extraction).
 """
 from typing import List, Optional, TypedDict, Union
 
@@ -17,6 +19,10 @@ import torch.nn as nn
 from .constants import HF_CACHE_DIR
 
 VIDEO_EXTENSIONS = {'.mp4', '.avi', '.mov', '.mkv'}
+
+
+def _is_video(path) -> bool:
+    return isinstance(path, str) and path[-4:].lower() in VIDEO_EXTENSIONS
 
 
 class ImageTextDict(TypedDict):
@@ -44,8 +50,18 @@ class Score(nn.Module):
         raise NotImplementedError("Subclasses must implement list_all_models")
 
     def _takes_video_files(self) -> bool:
-        """The plugin decodes and scores video files itself: video_mode "direct" and a video reader."""
-        return getattr(self.model, "video_mode", None) == "direct" and getattr(self.model, "video_reader", None) is not None
+        """The plugin decodes and scores video files itself: video_mode "direct" and a video reader, or video_mode "concat" and a plugin
+        that concatenates the frames into canvases itself."""
+        mode = getattr(self.model, "video_mode", None)
+        if mode == "concat":
+            return bool(getattr(self.model, "builds_video_canvases", False))
+        return mode == "direct" and getattr(self.model, "video_reader", None) is not None
+
+    def _video_kwargs(self, visuals, num_frames, kwargs) -> dict:
+        """kwargs of one plugin call: a "concat" plugin gets num_frames when the call holds a video file (image-only calls are unchanged)."""
+        if getattr(self.model, "video_mode", None) == "concat" and any(_is_video(v) for v in visuals):
+            return dict(kwargs, num_frames=num_frames)
+        return kwargs
 
     def forward(self, images: Optional[Union[str, List[str]]] = None, texts: Optional[Union[str, List[str]]] = None,
                 num_frames: Optional[int] = 8, **kwargs) -> torch.Tensor:
@@ -54,7 +70,7 @@ class Score(nn.Module):
             images = [images]
         if isinstance(texts, str):
             texts = [texts]
-        if any(isinstance(img, str) and img[-4:].lower() in VIDEO_EXTENSIONS for img in images) and not self._takes_video_files():
+        if any(_is_video(img) for img in images) and not self._takes_video_files():
             raise NotImplementedError("video inputs (frame extraction + concat, reference score.py:72-98) are outside the "
                                       "engine's hot-path scope; pass image files")
         m, n = len(images), len(texts)
@@ -69,7 +85,8 @@ class Score(nn.Module):
         pair_texts = [t for _ in range(end - start) for t in texts]
         out = [torch.zeros(0)]
         for s in range(0, len(pair_images), self.max_pairs):
-            out.append(self.model.forward(pair_images[s:s + self.max_pairs], pair_texts[s:s + self.max_pairs], **kwargs).float().cpu())
+            chunk = pair_images[s:s + self.max_pairs]
+            out.append(self.model.forward(chunk, pair_texts[s:s + self.max_pairs], **self._video_kwargs(chunk, num_frames, kwargs)).float().cpu())
         local = torch.cat(out)
         if world > 1:
             # equal-sized shards of `per` images (the last ranks may hold fewer or none: zero rows, trimmed after the gather)
@@ -82,7 +99,9 @@ class Score(nn.Module):
         return local.view(m, n).to(self.device)
 
     def batch_forward(self, dataset: List[ImageTextDict], batch_size: int = 16, num_frames: int = 4, **kwargs) -> torch.Tensor:
-        """[num_samples, num_visuals, num_texts] scores for a dataset of {'images': [...], 'texts': [...]} items."""
+        """[num_samples, num_visuals, num_texts] scores for a dataset of {'images': [...], 'texts': [...]} items. For {'videos': [...]}
+        items a "concat" plugin scores each video's canvas of `num_frames` frames (the reference passes num_frames=4 but through a keyword
+        its forward does not take, score.py:150)."""
         from torch.utils.data import DataLoader
         num_samples = len(dataset)
         media = "videos" if "videos" in dataset[0] else "images"
@@ -98,7 +117,8 @@ class Score(nn.Module):
             assert len(batch[media]) == num_visuals and len(batch['texts']) == num_texts
             for vis_idx in range(num_visuals):
                 for text_idx in range(num_texts):
+                    visuals = list(batch[media][vis_idx])
                     scores[counter:counter + cur, vis_idx, text_idx] = self.model.forward(
-                        list(batch[media][vis_idx]), list(batch['texts'][text_idx]), **kwargs).to(self.device)
+                        visuals, list(batch['texts'][text_idx]), **self._video_kwargs(visuals, num_frames, kwargs)).to(self.device)
             counter += cur
         return scores
