@@ -293,10 +293,11 @@ int vqa_qwen25vl_generate_prefill(vqa_handle* h, const vqa_qwen25vl_prompts* pro
 int vqa_qwen25vl_generate_step(vqa_handle* h, const vqa_qwen25vl_generation* gen, int32_t batch, int32_t seq_len, int32_t n_patches,
                                void* workspace, size_t workspace_bytes, void* stream);
 
-/* Number of kernels the last vqa_clipt5_score call launched (for bench.py's gpu_launches). */
+/* Number of kernels, memsets and copies the last forward call on this handle (vqa_clipt5_score, vqa_qwen25vl_score, vqa_qwen25vl_topk,
+ * a generate prefill or step) enqueued (for bench.py's gpu_launches). */
 int64_t vqa_last_launch_count(vqa_handle* h);
 
-/* Optional device-side timing of the forward: with profiling on, every launch of vqa_clipt5_score is bracketed by CUDA
+/* Optional device-side timing of the forward: with profiling on, every launch of a forward call (as above) is bracketed by CUDA
  * events on the caller's stream. After the caller synchronised the stream, vqa_profile_read returns, per category
  * {0 gemm, 1 attention, 2 norm, 3 other} (arrays of 4): device ms, algorithmic FLOPs (2MNK / 4*S*S*d), algorithmic bytes
  * (GEMM: A and W read once, C written once, residual read once) and scope counts of the LAST call. Used by bench.py for the
@@ -402,7 +403,9 @@ int vqa_qwen_preprocess_video_aa(const void* src, int32_t n_frames, int32_t fram
  * arguments). Either output pointer may be NULL. */
 int32_t vqa_resample_table(int32_t in_size, int32_t out_size, int32_t first, int32_t count, int32_t* bounds, int32_t* kk);
 
-/* ---- kernel-level entry points (used by tests/ and bench.py to exercise single kernels through the same ABI) ---- */
+/* ---- kernel-level entry points (used by tests/ and bench.py to exercise single kernels through the same ABI) ----
+ * Each one checks its arguments, then launches through the same stage function (grid, block, shared memory, arguments) as the forwards, so
+ * a test of an entry point covers the launch the forwards make. */
 
 /* C[M,N] = epilogue(A[M,K] . W[N,K]^T); all DEVICE bf16 row-major. epilogue: 0 store, 1 quick_gelu, 2 gelu(erf),
  * 3 gated gelu_new, 5 relu, 6 gated silu (C = bf16(bf16(silu(bf16(gate + b_gate))) * bf16(up + b_up)), the Qwen2.5-VL MLPs). The gated
@@ -492,11 +495,9 @@ int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, int32_t cap,
 int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32_t H, const int32_t* seq_lens,
                          const float* bias_table, float scale, int32_t bias_const_from, int32_t round_scores, void* stream);
 
-/* T5LayerNorm / nn.LayerNorm on [rows, D] bf16. beta == NULL selects T5 RMS norm: y = gamma * bf16(x * rsqrt(mean(x^2) + eps)), fp32
- * statistics; D a multiple of 8 up to 8192. LayerNorm: D in {256, 512, 768, 1024, 1280}. rows >= 1; x, gamma, beta and y 16-byte aligned;
- * else VQA_ERR_INVALID_ARG before anything launches. */
-int vqa_op_norm(const void* x, const void* gamma, const void* beta, void* y, int32_t rows, int32_t D, float eps,
-                void* stream);
+/* T5LayerNorm / Qwen RMSNorm on [rows, D] bf16: y = gamma * bf16(x * rsqrt(mean(x^2) + eps)), fp32 statistics. D a multiple of 8 up to
+ * 8192, rows >= 1; x, gamma and y 16-byte aligned; else VQA_ERR_INVALID_ARG before anything launches. */
+int vqa_op_norm(const void* x, const void* gamma, void* y, int32_t rows, int32_t D, float eps, void* stream);
 
 /* head_dim-128 attention on a packed buffer [rows, ld]: q heads at q_col0 + h*128, k/v heads at k_col0/v_col0 + (h/kv_group)*128,
  * out[row * ldo + h * 128 + d]. cu_seqlens [n_seq+1] (variable-length sequences) or NULL with fixed stride S and optional seq_lens [n_seq]:

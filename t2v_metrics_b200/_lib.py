@@ -143,7 +143,7 @@ def load() -> C.CDLL:
     lib.vqa_op_lmhead_logprob.restype = C.c_int
     lib.vqa_op_attention_d64.argtypes = [vp, vp, i32, i32, i32, vp, vp, f32, i32, i32, vp]
     lib.vqa_op_attention_d64.restype = C.c_int
-    lib.vqa_op_norm.argtypes = [vp, vp, vp, vp, i32, i32, f32, vp]
+    lib.vqa_op_norm.argtypes = [vp, vp, vp, i32, i32, f32, vp]
     lib.vqa_op_norm.restype = C.c_int
     lib.vqa_op_attention_d128.argtypes = [vp, i32, i64, i32, i32, i32, vp, i32, i32, i32, i32, i32, i32, vp, vp, f32, i32, vp]
     lib.vqa_op_attention_d128.restype = C.c_int

@@ -5,7 +5,7 @@
 #include "attention.cuh"
 #include "attention_sm90.cuh"
 #include "qwen_kernels.cuh"   // cast_f32_bf16_kernel, gather_rows_by_index_kernel
-#include "qwen_decode.cuh"    // generate_init_kernel, greedy_select_kernel
+#include "qwen_decode.cuh"    // generate_init, greedy_select
 #include "t5_decode.cuh"
 
 static int clipt5_finalize(vqa_handle* h) {
@@ -174,8 +174,9 @@ __global__ void __launch_bounds__(256) row_ssq_kernel(const bf16* __restrict__ x
 }
 
 // ------------------------------------------------------------------------------------------------ glue launches
-// The launches of the scoring path's glue kernels. The forwards below and the kernel-level entry points (vqa_b200.cu) both call these, so
-// the two cannot launch a kernel with different geometry.
+// Every kernel a forward shares with a kernel-level entry point (vqa_b200.cu) is launched by one stage function taking the forward's
+// Forward: here for CLIP-FlanT5, in qwen25vl.cuh for the Qwen glue, in qwen_decode.cuh for the decode loops and in host.cuh for the lm_head
+// tail. The forwards and the entry points both call these, so the two cannot launch a kernel with different geometry.
 
 // Pixels [n_images, 3, image_size, image_size] (fp32 or bf16) -> patch rows out [n_images * P, kpad] bf16.
 static int clipt5_patchify(Forward& f, const void* pixels, int pixel_dtype, bf16* out, int n_images, int image_size, int patch, int kpad) {
@@ -207,19 +208,48 @@ static int clipt5_decoder_embed(Forward& f, const int* labels, const bf16* share
     return f.launch(CAT_OTHER, 0, "decoder embed", decoder_embed_kernel, B * T, 128, 0, labels, shared, y, T, D, start_id, pad_id);
 }
 
-// The score's tail: the EPI_LSE lm_head GEMM g (M = B * T rows) with its (max, sum) partials and label logits, then lse_finalize_kernel into
-// scores [B] and, unless NULL, logprobs [B * T].
-static int clipt5_lmhead_score(Forward& f, Gemm g, const int* labels, float* lse_max, float* lse_sum, float* label_logit, float* scores,
-                               float* logprobs, int B, int T) {
-    const int ntiles = LMHEAD_PARTS * ((g.N + LMHEAD_BN - 1) / LMHEAD_BN);
-    TRY(f.gemm(g.lse(labels, lse_max, lse_sum, label_logit), "lm_head"));
-    return f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, (const float*)lse_max, (const float*)lse_sum,
-                    (const float*)label_logit, labels, scores, logprobs, B, T, ntiles);
-}
-
 // Sum of squares of the rows of x [rows, D] into slot 0 of ssq [rows, stride].
 static int clipt5_row_ssq(Forward& f, const bf16* x, float* ssq, int rows, int D, int stride) {
     return f.launch(CAT_NORM, 0, "row ssq", row_ssq_kernel, (rows + 7) / 8, 256, 0, x, ssq, rows, D, stride);
+}
+
+// The CLIP embeddings and pre_layrnorm: patch rows [n_images * P, D] -> fp32 y [n_images * (P + 1), D].
+static int clipt5_embed_ln(Forward& f, const bf16* patch, const bf16* cls, const bf16* pos, const bf16* gamma, const bf16* beta, float* y,
+                           int n_images, int P, int D, float eps) {
+    const int blocks = (n_images * (P + 1) + 7) / 8;
+    if (D == 1024)
+        return f.launch(CAT_NORM, 0, "clip_embed_ln", clip_embed_ln_kernel<1024>, blocks, 256, 0, patch, cls, pos, gamma, beta, y, n_images, P, eps);
+    if (D == 256)
+        return f.launch(CAT_NORM, 0, "clip_embed_ln", clip_embed_ln_kernel<256>, blocks, 256, 0, patch, cls, pos, gamma, beta, y, n_images, P, eps);
+    return fail(f.h, VQA_ERR_UNSUPPORTED, "vit_hidden must be 1024 or 256");
+}
+
+// Head-dim-64 attention of the vision tower and the T5 encoder: packed qkv [B * S, 3 * H * 64] -> out [B * S, H * 64] (launch_attn_tc).
+static int clipt5_attention_d64(Forward& f, const char* what, const bf16* qkv, bf16* out, int B, int S, int H, const int* seq_lens,
+                                const float* bias_table, float scale, int bias_const_from, bool round_scores) {
+    const int inner = H * 64;
+    return f.attention(4.0 * B * (double)H * S * S * 64, what, [&] {
+        return launch_attn_tc(qkv, 3 * inner, 0, inner, 2 * inner, out, inner, B, S, H, seq_lens, bias_table, scale, bias_const_from, round_scores,
+                              f.st);
+    });
+}
+
+// The scoring path's decoder self-attention over T target rows: packed qkv [B * T, 3 * H * 64] -> out [B * T, H * 64].
+static int clipt5_decoder_self_attention(Forward& f, const bf16* qkv, bf16* out, const bf16* rel_emb, const int* lut, int max_distance, int B,
+                                         int T, int H, int round_scores) {
+    return f.launch(CAT_ATTENTION, 4.0 * B * (double)H * T * T * 64, "decoder self attention", t5_decoder_self_attn_kernel, (B * H * T + 3) / 4,
+                    128, 4 * T * sizeof(float), qkv, out, rel_emb, lut, max_distance, B, T, H, round_scores);
+}
+
+// One cached decoder self-attention layer of a generation step: the step's K / V rows of qkv [B, 3 * H * 64] appended to kc / vc
+// [B, H, cap, 64] (t5_kv_cache_append_kernel), then each row attends to its cache (t5_decode_self_attn_kernel) into out [B, H * 64].
+constexpr int T5_DEC_ATTN_WARPS = 4;
+static int clipt5_cached_self_attention(Forward& f, const bf16* qkv, bf16* kc, bf16* vc, int cap, const int* lengths, bf16* out,
+                                        const bf16* rel_emb, const int* lut, int max_distance, int B, int H, int round_scores) {
+    TRY(f.launch(CAT_OTHER, 0, "kv cache append", t5_kv_cache_append_kernel, (B * H * 8 + 255) / 256, 256, 0, qkv, B, H, lengths, kc, vc, cap));
+    return f.launch(CAT_ATTENTION, 4.0 * B * (double)H * cap * 64, "decoder self attention (cached)", t5_decode_self_attn_kernel,
+                    (B * H + T5_DEC_ATTN_WARPS - 1) / T5_DEC_ATTN_WARPS, 32 * T5_DEC_ATTN_WARPS, T5_DEC_ATTN_WARPS * cap * sizeof(float), qkv,
+                    (const bf16*)kc, (const bf16*)vc, cap, lengths, out, rel_emb, lut, max_distance, B, H, round_scores);
 }
 
 // ------------------------------------------------------------------------------------------------ forward
@@ -243,7 +273,6 @@ struct ClipT5Prompts {
 static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Prompts& in) {
     vqa_handle* h = f.h;
     const vqa_clipt5_config& c = h->cfg;
-    cudaStream_t st = f.st;
     const void* pixels = in.pixels;
     const int pixel_dtype = in.pixel_dtype, n_images = in.n_images, B = in.B, L = in.L;
     const int *image_index = in.image_index, *input_ids = in.input_ids, *text_lens = in.text_lens;
@@ -268,22 +297,12 @@ static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Promp
     // ---------------- vision tower (CLIP ViT, layers 0 .. vit_layers_run-1; hidden_states[-2]) ----------------
     TRY(clipt5_patchify(f, pixels, pixel_dtype, P_(w.patches), n_images, c.image_size, c.patch_size, h->kpad));
     TRY(f.gemm(Gemm(P_(w.patches), h->patch_w, P_(w.patch_out), Mp, Dv, h->kpad)));
-    if (Dv == 1024)
-        TRY(f.launch(CAT_NORM, 0, "clip_embed_ln", clip_embed_ln_kernel<1024>, (Mv + 7) / 8, 256, 0, P_(w.patch_out), h->cls, h->pos,
-                     h->pre_ln_w, h->pre_ln_b, hv, n_images, P, c.vit_ln_eps));
-    else if (Dv == 256)
-        TRY(f.launch(CAT_NORM, 0, "clip_embed_ln", clip_embed_ln_kernel<256>, (Mv + 7) / 8, 256, 0, P_(w.patch_out), h->cls, h->pos,
-                     h->pre_ln_w, h->pre_ln_b, hv, n_images, P, c.vit_ln_eps));
-    else
-        return fail(h, VQA_ERR_UNSUPPORTED, "vit_hidden must be 1024 or 256");
+    TRY(clipt5_embed_ln(f, P_(w.patch_out), h->cls, h->pos, h->pre_ln_w, h->pre_ln_b, hv, n_images, P, Dv, c.vit_ln_eps));
     for (int l = 0; l < c.vit_layers_run; ++l) {
         const VitLayerW& Lw = h->vit[l];
         TRY(f.layernorm_f32(hv, Lw.ln1_w, Lw.ln1_b, P_(w.vn), Mv, Dv, c.vit_ln_eps));
         TRY(f.gemm(Gemm(P_(w.vn), Lw.qkv_w, P_(w.vqkv), Mv, 3 * Dv, Dv).with_bias(Lw.qkv_b)));
-        TRY(f.attention(4.0 * n_images * (double)Hv * (P + 1) * (P + 1) * 64, "vit attention", [&] {
-            return launch_attn_tc(P_(w.vqkv), 3 * Dv, 0, Dv, 2 * Dv, P_(w.vattn), Dv, n_images, P + 1, Hv, nullptr, nullptr, 0.125f, 0,
-                                  round_attn, st);
-        }));
+        TRY(clipt5_attention_d64(f, "vit attention", P_(w.vqkv), P_(w.vattn), n_images, P + 1, Hv, nullptr, nullptr, 0.125f, 0, round_attn));
         TRY(f.gemm(Gemm(P_(w.vattn), Lw.out_w, hv, Mv, Dv, Dv).with_bias(Lw.out_b).accumulate_f32(), "gemm (fp32 residual)"));
         TRY(f.layernorm_f32(hv, Lw.ln2_w, Lw.ln2_b, P_(w.vn), Mv, Dv, c.vit_ln_eps));
         TRY(f.gemm(Gemm(P_(w.vn), Lw.fc1_w, P_(w.vmlp), Mv, c.vit_mlp, Dv).with_bias(Lw.fc1_b).with_epilogue(EPI_QUICK_GELU)));
@@ -335,10 +354,8 @@ static int clipt5_encode(Forward& f, const ClipT5Workspace& w, const ClipT5Promp
             TRY(f.rmsnorm(P_(w.x), Lw.ln0, P_(w.xn), M, Dm, c.t5_ln_eps));
             TRY(f.gemm(Gemm(P_(w.xn), Lw.qkv, P_(w.qkv), M, 3 * inner, Dm)));
         }
-        TRY(f.attention(4.0 * B * (double)H * S * S * 64, "t5 encoder attention", [&] {
-            return launch_attn_tc(P_(w.qkv), 3 * inner, 0, inner, 2 * inner, P_(w.attn), inner, B, S, H, seq_lens, bias_table, 1.0f,
-                                  c.rel_max_distance, round_attn, st);
-        }));
+        TRY(clipt5_attention_d64(f, "t5 encoder attention", P_(w.qkv), P_(w.attn), B, S, H, seq_lens, bias_table, 1.0f, c.rel_max_distance,
+                                 round_attn));
         if (fuse_norms) {
             nf_prod.ssq_out = ssq_nxt;
             TRY(f.gemm(Gemm(P_(w.attn), Lw.o, P_(w.x), M, Dm, inner).with_residual(P_(w.x)).with_norm(nf_prod)));
@@ -441,8 +458,7 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
         // self-attention
         TRY(f.rmsnorm(P_(w.y), Lw.ln0, P_(w.yn), Md, Dm, c.t5_ln_eps));
         TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.qkv, P_(w.dqkv), Md, 3 * inner, Dm))));
-        TRY(f.launch(CAT_ATTENTION, 4.0 * B * (double)H * T * T * 64, "decoder self attention", t5_decoder_self_attn_kernel, (B * H * T + 3) / 4,
-                     128, 4 * T * sizeof(float), P_(w.dqkv), P_(w.dattn), h->dec_rel, h->lut_unidir, c.rel_max_distance, B, T, H, rnd));
+        TRY(clipt5_decoder_self_attention(f, P_(w.dqkv), P_(w.dattn), h->dec_rel, h->lut_unidir, c.rel_max_distance, B, T, H, rnd));
         TRY(f.gemm(dec(Gemm(P_(w.dattn), Lw.o, P_(w.y), Md, Dm, inner).with_residual(P_(w.y)))));
         TRY(f.rmsnorm(P_(w.y), Lw.ln1, P_(w.yn), Md, Dm, c.t5_ln_eps));
         TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.cq, P_(w.dq), Md, inner, Dm))));
@@ -460,8 +476,8 @@ static int clipt5_score(vqa_handle* h, const void* pixels, int pixel_dtype, int 
     TRY(f.rmsnorm(P_(w.y), h->dec_final_ln, P_(w.yn), Md, Dm, c.t5_ln_eps));
 
     // ---------------- lm_head x hidden, fused log-sum-exp + label gather; logits never reach HBM ----------------
-    return clipt5_lmhead_score(f, Gemm(P_(w.yn), h->lm_head, nullptr, Md, c.vocab, Dm), labels, f.at<float>(w.lse_max), f.at<float>(w.lse_sum),
-                               f.at<float>(w.label_logit), out_scores, out_logprobs, B, T);
+    return lmhead_score(f, Gemm(P_(w.yn), h->lm_head, nullptr, Md, c.vocab, Dm), labels, f.at<float>(w.lse_max), f.at<float>(w.lse_sum),
+                        f.at<float>(w.label_logit), out_scores, out_logprobs, B, T);
 }
 
 // ================================================================================================ greedy generation
@@ -502,8 +518,6 @@ struct ClipT5GenArgs {
     int* all_done;           // 1 once every sequence has finished
 };
 
-constexpr int T5_DEC_ATTN_WARPS = 4;
-
 // One decoder position per sequence: the start token (first) or the last selected token (next_ids), through every decoder layer with
 // its self-attention K/V appended to the cache, then the final norm, the lm_head into [B, vocab] bf16 logits, and the greedy token of
 // every unfinished sequence. Finished sequences recompute their frozen last position, which changes nothing they output.
@@ -525,12 +539,8 @@ static int clipt5_decode_step(Forward& f, const ClipT5GenWorkspace& g, int B, in
         bf16 *kc = f.at(g.kcache) + l * g.layer_elems, *vc = f.at(g.vcache) + l * g.layer_elems;
         TRY(f.rmsnorm(P_(w.y), Lw.ln0, P_(w.yn), B, Dm, c.t5_ln_eps));
         TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.qkv, P_(w.dqkv), B, 3 * inner, Dm))));
-        TRY(f.launch(CAT_OTHER, 0, "kv cache append", t5_kv_cache_append_kernel, (B * H * 8 + 255) / 256, 256, 0, (const bf16*)P_(w.dqkv), B, H,
-                     (const int*)a.lengths, kc, vc, g.cap));
-        TRY(f.launch(CAT_ATTENTION, 4.0 * B * (double)H * g.cap * 64, "decoder self attention (cached)", t5_decode_self_attn_kernel,
-                     (B * H + T5_DEC_ATTN_WARPS - 1) / T5_DEC_ATTN_WARPS, 32 * T5_DEC_ATTN_WARPS, T5_DEC_ATTN_WARPS * g.cap * sizeof(float),
-                     (const bf16*)P_(w.dqkv), (const bf16*)kc, (const bf16*)vc, g.cap, (const int*)a.lengths, P_(w.dattn), h->dec_rel,
-                     (const int*)h->lut_unidir, c.rel_max_distance, B, H, rnd));
+        TRY(clipt5_cached_self_attention(f, P_(w.dqkv), kc, vc, g.cap, a.lengths, P_(w.dattn), h->dec_rel, h->lut_unidir, c.rel_max_distance, B, H,
+                                         rnd));
         TRY(f.gemm(dec(Gemm(P_(w.dattn), Lw.o, P_(w.y), B, Dm, inner).with_residual(P_(w.y)))));
         TRY(f.rmsnorm(P_(w.y), Lw.ln1, P_(w.yn), B, Dm, c.t5_ln_eps));
         TRY(f.gemm(dec(Gemm(P_(w.yn), Lw.cq, P_(w.dq), B, inner, Dm))));
@@ -544,9 +554,8 @@ static int clipt5_decode_step(Forward& f, const ClipT5GenWorkspace& g, int B, in
     // The [B, vocab] bf16 logits are 64 KB per sequence against the 263 MB lm_head weight (xxl) that the GEMM streams either way.
     bf16* logits = f.at(g.logits);
     TRY(f.gemm(Gemm(P_(w.yn), h->lm_head, logits, B, c.vocab, Dm), "lm_head"));
-    return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, (const bf16*)logits, c.vocab, (uint32_t*)nullptr,
-                    0, 1.0f, a.eos_ids, a.n_eos, a.max_new, (const int*)nullptr, B, a.tokens, a.lengths, f.at<int>(g.done),
-                    f.at<int>(g.n_done), a.all_done, next_ids, (int*)nullptr);
+    return greedy_select(f, logits, B, c.vocab, nullptr, 1.0f, a.eos_ids, a.n_eos, a.max_new, nullptr, a.tokens, a.lengths, f.at<int>(g.done),
+                         f.at<int>(g.n_done), a.all_done, next_ids, nullptr);
 }
 
 // Encoder pass of vqa_clipt5_score, the generation state reset, then the first decoder position (the start token) and the first token.
@@ -556,8 +565,7 @@ static int clipt5_generate_prefill(vqa_handle* h, const ClipT5Prompts& in, const
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
     TRY(clipt5_encode(f, g.w, in));
-    TRY(f.launch(CAT_OTHER, 0, "generate init", generate_init_kernel, (in.B * a.max_new + 255) / 256, 256, 0, in.B, a.max_new, a.tokens,
-                 a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
+    TRY(generate_init(f, in.B, a.max_new, a.tokens, a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
     const int P = (h->cfg.image_size / h->cfg.patch_size) * (h->cfg.image_size / h->cfg.patch_size);
     return clipt5_decode_step(f, g, in.B, in.L - 1 + P, a, true);
 }

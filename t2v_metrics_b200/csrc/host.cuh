@@ -238,6 +238,13 @@ struct Gemm {
         epi = EPI_LSE; labels = labels_; lse_max = max; lse_sum = sum; label_logit = label;
         return *this;
     }
+    // the Qwen score's logit processing in the EPI_LSE epilogue: HF's repetition penalty on the ids set in bitmap [M, ceil(N / 32)] (none
+    // when rep_penalty is 1), then 1 / temperature
+    Gemm& processed(float temperature, const uint32_t* bitmap, float rep_penalty) {
+        lse_scale = 1.0f / temperature;
+        penalty_bitmap = rep_penalty != 1.0f ? bitmap : nullptr; penalty_words = (N + 31) / 32; penalty = rep_penalty;
+        return *this;
+    }
     // algorithmic work: A and W read once, C written once (+ residual read once); elem = bytes per C element, none for the lm_head
     double flops() const { return (batch.nb > 0 ? batch.nb : 1) * 2.0 * M * (double)N * K; }
     double bytes() const {
@@ -337,16 +344,6 @@ static cudaError_t run_layernorm_f32(const float* x, const bf16* g, const bf16* 
     else if (D == 256)  layernorm_kernel<256, float><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
     else if (D == 512)  layernorm_kernel<512, float><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
     else if (D == 768)  layernorm_kernel<768, float><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
-    else return cudaErrorInvalidValue;
-    return cudaGetLastError();
-}
-static cudaError_t run_layernorm(const bf16* x, const bf16* g, const bf16* b, bf16* y, int rows, int D, float eps, cudaStream_t st) {
-    const int blocks = (rows + 7) / 8;
-    if (D == 1024)      layernorm_kernel<1024><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
-    else if (D == 256)  layernorm_kernel<256><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
-    else if (D == 512)  layernorm_kernel<512><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
-    else if (D == 768)  layernorm_kernel<768><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
-    else if (D == 1280) layernorm_kernel<1280><<<blocks, 256, 0, st>>>(x, g, b, y, rows, eps);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
@@ -462,3 +459,13 @@ struct Forward {
     }
 };
 #define TRY(x) do { int _rc = (x); if (_rc) return _rc; } while (0)
+
+// The score's tail of both forwards: the EPI_LSE lm_head GEMM g (M = B * T rows) with its (max, sum) partials and label logits, then
+// lse_finalize_kernel into scores [B] and, unless NULL, logprobs [B * T].
+static int lmhead_score(Forward& f, Gemm g, const int* labels, float* lse_max, float* lse_sum, float* label_logit, float* scores,
+                        float* logprobs, int B, int T) {
+    const int ntiles = LMHEAD_PARTS * ((g.N + LMHEAD_BN - 1) / LMHEAD_BN);
+    TRY(f.gemm(g.lse(labels, lse_max, lse_sum, label_logit), "lm_head"));
+    return f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, (const float*)lse_max, (const float*)lse_sum,
+                    (const float*)label_logit, labels, scores, logprobs, B, T, ntiles);
+}

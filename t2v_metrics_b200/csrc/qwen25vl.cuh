@@ -111,6 +111,54 @@ static int qwen_finalize(vqa_handle* h, QwenState& q) {
     return VQA_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ glue launches (see clipt5.cuh)
+
+// cos / sin tables [rows, 2 * half] of the positions pos [n_axes, rows]; round_bf16: the text model's bf16 tables.
+static int qwen_rope_table(Forward& f, const char* what, const int* pos, int rows, const int* axis_of_dim, const float* inv_freq, int half,
+                           float* cos_t, float* sin_t, int round_bf16) {
+    return f.launch(CAT_OTHER, 0, what, rope_table_kernel, (unsigned)(((long long)rows * half + GLUE_THREADS - 1) / GLUE_THREADS), GLUE_THREADS,
+                    0, pos, rows, axis_of_dim, inv_freq, half, cos_t, sin_t, round_bf16);
+}
+
+// In-place rotary embedding of n_heads heads (head h at column col0 + h * head_stride) of x [rows, ld] with the tables of qwen_rope_table.
+static int qwen_rope(Forward& f, const char* what, bf16* x, int ld, int col0, int n_heads, int head_stride, int head_dim, const float* cos_t,
+                     const float* sin_t, long long rows, int bf16_products) {
+    return f.launch(CAT_OTHER, 0, what, rope_inplace_kernel, (unsigned)((rows * n_heads * (head_dim / 16) + GLUE_THREADS - 1) / GLUE_THREADS),
+                    GLUE_THREADS, 0, x, ld, col0, n_heads, head_stride, head_dim, cos_t, sin_t, rows, bf16_products);
+}
+
+// dst row r = src row index[r / group] * group + r % group, for r < rows.
+static int qwen_gather_rows(Forward& f, const char* what, const bf16* src, bf16* dst, const int* index, int rows, int group, int D) {
+    return f.launch(CAT_OTHER, 0, what, gather_rows_kernel, rows, ROW_COPY_THREADS, 0, src, dst, index, group, D);
+}
+
+// The language model's input out [rows, D]: row b * S + s < seq_lens[b] takes feats[feat_index] or embed[ids], the rest zero.
+static int qwen_embed(Forward& f, const int* ids, const int* feat_index, const int* seq_lens, const bf16* embed, const bf16* feats, bf16* out,
+                      int rows, int S, int D) {
+    return f.launch(CAT_OTHER, 0, "llm embed", qwen_embed_kernel, rows, ROW_COPY_THREADS, 0, ids, feat_index, seq_lens, embed, feats, out, S, D);
+}
+
+// The prompt ids OR-ed into the repetition-penalty bitmap [B, ceil(vocab / 32)]: padded rows ids [B, S] up to seq_lens[b] ...
+static int qwen_token_bitmap(Forward& f, const int* ids, const int* seq_lens, int B, int S, int vocab, uint32_t* bitmap) {
+    return f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_kernel, (unsigned)(((long long)B * S + GLUE_THREADS - 1) / GLUE_THREADS),
+                    GLUE_THREADS, 0, ids, seq_lens, B, S, vocab, bitmap, token_bitmap_words(vocab));
+}
+// ... or packed rows: pair b's prompt is its prefix sequence (kv_prefix[pair_seq[b]], if any) and its own sequence
+static int qwen_token_bitmap_packed(Forward& f, const int* ids, const int* cu_seqlens, const int* kv_prefix, const int* pair_seq, int max_prompt_len,
+                                    int B, int vocab, uint32_t* bitmap) {
+    return f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_packed_kernel, dim3((max_prompt_len + GLUE_THREADS - 1) / GLUE_THREADS, B),
+                    GLUE_THREADS, 0, ids, cu_seqlens, kv_prefix, pair_seq, vocab, bitmap, token_bitmap_words(vocab));
+}
+
+// The K most probable ids of every row of logits [B, ldl] (first V columns) under the score's processing: the repetition penalty on the
+// ids set in pen_bitmap (none when the penalty is 1), then 1 / temperature.
+static int qwen_topk_softmax(Forward& f, const bf16* logits, long long ldl, int B, int V, float temperature, const uint32_t* pen_bitmap,
+                             float penalty, int K, int* out_ids, float* out_probs) {
+    return f.launch(CAT_OTHER, 0, "top-k softmax", topk_softmax_kernel, B, GLUE_THREADS, 0, logits, ldl, V, 1.0f / temperature,
+                    penalty != 1.0f ? pen_bitmap : nullptr, token_bitmap_words(V), penalty, K, out_ids, out_probs);
+}
+
+// ------------------------------------------------------------------------------------------------ forward
 // K/V cache of a generate prefill: layer l's K and V at kc + l * layer_elems and vc + l * layer_elems, each [B, Hkv, cap, 128]
 struct QwenKVCache {
     bf16 *kc, *vc;
@@ -146,14 +194,13 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
         else
             TRY(f.copy(P_(w.patches), pixel_patches, n * 2, "pixel copy"));
         // rotary table of the (already window-ordered) patch positions: [h freqs | w freqs] duplicated (:404-409, :487)
-        TRY(f.launch(CAT_OTHER, 0, "vision rope table", rope_table_kernel, rope_table_blocks(L, hdv / 2), GLUE_THREADS, 0, vis_pos_hw, L, q.vis_axis,
-                     q.vis_inv_freq, hdv / 2, F_(w.vcos), F_(w.vsin), 0));
+        TRY(qwen_rope_table(f, "vision rope table", vis_pos_hw, L, q.vis_axis, q.vis_inv_freq, hdv / 2, F_(w.vcos), F_(w.vsin), 0));
     }
     // patch embedding (Conv3d == GEMM), then re-order 2x2 groups into window order (:470-472)
     TRY(f.gemm(Gemm(P_(w.patches), q.patch_w, P_(w.vxn), L, Dv, c.patch_dim)));
     {
         auto g = f.group(CAT_OTHER);
-        TRY(f.launch(CAT_OTHER, 0, "window reorder", gather_rows_kernel, L, ROW_COPY_THREADS, 0, P_(w.vxn), P_(w.vx), window_index, unit, Dv));
+        TRY(qwen_gather_rows(f, "window reorder", P_(w.vxn), P_(w.vx), window_index, L, unit, Dv));
         // the qkv GEMMs write head_dim of every 128-wide head slot; the attention kernel contracts q.k over all 128: zero the rest once
         if (hdv < 128) TRY(f.memset0(P_(w.vqkv), (size_t)L * 3 * Hv * 128 * 2, "vision qkv clear"));
     }
@@ -166,8 +213,7 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
         qkv.ldc = 3 * Hv * 128;
         if (hdv < 128) { qkv.c_group_in = hdv; qkv.c_group_out = 128; }
         TRY(f.gemm(qkv.with_bias(Lw.qkv_b), "vision qkv gemm"));
-        TRY(f.launch(CAT_OTHER, 0, "vision rope", rope_inplace_kernel, rope_inplace_blocks(L, 2 * Hv, hdv), GLUE_THREADS, 0, P_(w.vqkv), 3 * Hv * 128, 0, 2 * Hv,
-                     128, hdv, F_(w.vcos), F_(w.vsin), L, 0));
+        TRY(qwen_rope(f, "vision rope", P_(w.vqkv), 3 * Hv * 128, 0, 2 * Hv, 128, hdv, F_(w.vcos), F_(w.vsin), L, 0));
         const int nseq = full ? n_frames : n_windows, mlen = full ? max_frame_len : max_window_len;
         static const bool no_pairs = getenv("VQA_ATTN128_NO_PAIRS") != nullptr;     // A/B switch
         TRY(f.attention(4.0 * (double)L * mlen * Hv * hdv, "vision attention", [&] {
@@ -186,14 +232,11 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
     TRY(f.gemm(Gemm(P_(w.vfc1), q.fc2_w, P_(w.vfeat), L / unit, c.out_hidden, Dv * unit).with_bias(q.fc2_b)));
     {
         auto g = f.group(CAT_OTHER);
-        TRY(f.launch(CAT_OTHER, 0, "merger reorder", gather_rows_kernel, L / unit, ROW_COPY_THREADS, 0, P_(w.vfeat), P_(w.vfeat_orig), reverse_index, 1,
-                     c.out_hidden));
+        TRY(qwen_gather_rows(f, "merger reorder", P_(w.vfeat), P_(w.vfeat_orig), reverse_index, L / unit, 1, c.out_hidden));
         // ---------------- language model input ----------------
         // packed rows: one "sample" of M rows, all valid (its length is the last entry of cu_seqlens)
-        TRY(f.launch(CAT_OTHER, 0, "llm embed", qwen_embed_kernel, M, ROW_COPY_THREADS, 0, input_ids, feat_index, pk ? pk->cu_seqlens + pk->n_seq : seq_lens,
-                     q.embed, P_(w.vfeat_orig), P_(w.x), pk ? M : S, D));
-        TRY(f.launch(CAT_OTHER, 0, "llm rope table", rope_table_kernel, rope_table_blocks(M, 64), GLUE_THREADS, 0, position_ids, M, q.text_axis,
-                     q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1));
+        TRY(qwen_embed(f, input_ids, feat_index, pk ? pk->cu_seqlens + pk->n_seq : seq_lens, q.embed, P_(w.vfeat_orig), P_(w.x), M, pk ? M : S, D));
+        TRY(qwen_rope_table(f, "llm rope table", position_ids, M, q.text_axis, q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1));
     }
     const int Hq = c.heads, Hkv = c.kv_heads, qkv_cols = (Hq + 2 * Hkv) * 128;
     const float tscale = 1.0f / sqrtf(128.0f);
@@ -202,12 +245,10 @@ static int qwen_prefill(Forward& f, QwenState& q, const QwenWorkspace& w, const 
         TRY(f.rmsnorm(P_(w.x), Lw.ln1, P_(w.xn), M, D, c.rms_eps));
         TRY(f.gemm(Gemm(P_(w.xn), Lw.qkv_w, P_(w.qkv), M, qkv_cols, D).with_bias(Lw.qkv_b)));
         // q heads and k heads are contiguous in the packed buffer -> one launch rotates Hq + Hkv heads
-        TRY(f.launch(CAT_OTHER, 0, "llm rope", rope_inplace_kernel, rope_inplace_blocks(M, Hq + Hkv, 128), GLUE_THREADS, 0, P_(w.qkv), qkv_cols, 0, Hq + Hkv,
-                     128, 128, F_(w.cos), F_(w.sin), M, c.emulate_bf16_rounding));
+        TRY(qwen_rope(f, "llm rope", P_(w.qkv), qkv_cols, 0, Hq + Hkv, 128, 128, F_(w.cos), F_(w.sin), M, c.emulate_bf16_rounding));
         if (kv)
-            TRY(f.launch(CAT_OTHER, 0, "kv cache write", kv_cache_write_kernel, (unsigned)(((long long)M * Hkv * 16 + 255) / 256), 256, 0, P_(w.qkv),
-                         qkv_cols, Hq * 128, (Hq + Hkv) * 128, Hkv, S, (long long)M, seq_lens, nullptr, kv->kc + l * kv->layer_elems,
-                         kv->vc + l * kv->layer_elems, kv->cap));
+            TRY(kv_cache_write(f, P_(w.qkv), qkv_cols, Hq * 128, (Hq + Hkv) * 128, Hkv, S, M, seq_lens, nullptr, kv->kc + l * kv->layer_elems,
+                               kv->vc + l * kv->layer_elems, kv->cap));
         TRY(f.attention(2.0 * B * (double)Hq * S * S * 128, pk ? "llm attention (packed)" : "llm attention", [&] {
             if (pk)
                 return launch_attn_tc128(P_(w.qkv), qkv_cols, M, 0, Hq * 128, (Hq + Hkv) * 128, P_(w.attn), Hq * 128, pk->n_seq, pk->max_seq_len,
@@ -233,19 +274,16 @@ static int qwen_last_position(Forward& f, QwenState& q, const QwenWorkspace& w, 
     if (pk) TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_rows_by_index_kernel, B, 128, 0, P_(w.x), pk->pair_row, P_(w.last), D));
     else    TRY(f.launch(CAT_OTHER, 0, "last-row gather", gather_last_rows_kernel, B, 128, 0, P_(w.x), seq_lens, P_(w.last), S, D));
     TRY(f.rmsnorm(P_(w.last), q.final_norm, P_(w.lastn), B, D, c.rms_eps));
-    const int pen_words = token_bitmap_words(c.vocab);
     uint32_t* bitmap = f.at<uint32_t>(w.pen_bitmap);
     if (repetition_penalty != 1.0f) {
         // HF applies RepetitionPenaltyLogitsProcessor over the prompt ids before the scores are returned (generation/utils.py:2762-2770,
         // logits_process.py): one bit per (sample, vocabulary id) that occurs in the sample's prompt.
         auto g = f.group(CAT_OTHER);
-        TRY(f.memset0(bitmap, (size_t)B * pen_words * 4, "penalty bitmap clear"));
+        TRY(f.memset0(bitmap, (size_t)B * token_bitmap_words(c.vocab) * 4, "penalty bitmap clear"));
         if (pk)
-            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_packed_kernel, token_bitmap_packed_grid(pk->max_prompt_len, B), GLUE_THREADS, 0, input_ids,
-                         pk->cu_seqlens, pk->kv_prefix, pk->pair_seq, c.vocab, bitmap, pen_words));
+            TRY(qwen_token_bitmap_packed(f, input_ids, pk->cu_seqlens, pk->kv_prefix, pk->pair_seq, pk->max_prompt_len, B, c.vocab, bitmap));
         else
-            TRY(f.launch(CAT_OTHER, 0, "penalty bitmap", token_bitmap_kernel, token_bitmap_blocks(B, S), GLUE_THREADS, 0, input_ids, seq_lens, B, S, c.vocab,
-                         bitmap, pen_words));
+            TRY(qwen_token_bitmap(f, input_ids, seq_lens, B, S, c.vocab, bitmap));
     }
     return VQA_OK;
 }
@@ -254,28 +292,19 @@ static int qwen_score(vqa_handle* h, QwenState& q, const vqa_qwen25vl_prompts& i
                       float temperature, float repetition_penalty, float* out_probs, float* out_logprobs, void* workspace, size_t workspace_bytes,
                       cudaStream_t st) {
     const vqa_qwen25vl_config& c = q.cfg;
-    const int B = in.batch, D = c.hidden;
+    const int B = in.batch;
     const QwenWorkspace w = qwen_plan_rows(c, B, pk ? (size_t)pk->total_rows : (size_t)B * in.seq_len, in.n_patches);
     if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
-    auto P_ = [&](size_t off) { return f.at(off); };
     auto F_ = [&](size_t off) { return f.at<float>(off); };
     TRY(qwen_prefill(f, q, w, in, pk));
     TRY(qwen_last_position(f, q, w, in, pk, repetition_penalty));
     // ---------------- lm_head with fused log-softmax gather ----------------
-    const int ntiles = LMHEAD_PARTS * ((c.vocab + LMHEAD_BN - 1) / LMHEAD_BN);
-    const int pen_words = (c.vocab + 31) / 32;
-    const bool penalise = repetition_penalty != 1.0f;
-    const uint32_t* bitmap = f.at<uint32_t>(w.pen_bitmap);
-    Gemm lm(P_(w.lastn), q.lm_head, nullptr, B, c.vocab, D);
-    lm.lse(answer_ids, F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit));
-    lm.lse_scale = 1.0f / temperature;
-    lm.penalty_bitmap = penalise ? bitmap : nullptr; lm.penalty_words = pen_words; lm.penalty = repetition_penalty;
-    TRY(f.gemm(lm, "lm_head"));
     // T = 1 target per row: score = exp(logprob) = softmax(logits / T)[answer] (qwen2vl_model.py:160-167)
-    TRY(f.launch(CAT_OTHER, 0, "lse finalize", lse_finalize_kernel, (B + 3) / 4, 128, 0, F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit),
-                 answer_ids, out_probs, out_logprobs ? out_logprobs : F_(w.logprob), B, 1, ntiles));
-    return VQA_OK;
+    const Gemm lm = Gemm(f.at(w.lastn), q.lm_head, nullptr, B, c.vocab, c.hidden).processed(temperature, f.at<uint32_t>(w.pen_bitmap),
+                                                                                          repetition_penalty);
+    return lmhead_score(f, lm, answer_ids, F_(w.lse_max), F_(w.lse_sum), F_(w.label_logit), out_probs, out_logprobs ? out_logprobs : F_(w.logprob),
+                        B, 1);
 }
 
 // forward_with_trace support: top-k of the last-position distribution of the LAST scoring call (its final hidden states -- and, when a
@@ -286,17 +315,11 @@ static int qwen_topk(vqa_handle* h, QwenState& q, int B, size_t rows, int n_patc
     const vqa_qwen25vl_config& c = q.cfg;
     const QwenWorkspace w = qwen_plan_rows(c, B, rows, n_patches);
     if (workspace_bytes < w.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
-    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    bf16* lastn = reinterpret_cast<bf16*>(ws + w.lastn);
-    bf16* logits = reinterpret_cast<bf16*>(ws + w.trace_logits);
-    const int pen_words = (c.vocab + 31) / 32;
-    const bool penalise = repetition_penalty != 1.0f;
-    const uint32_t* bitmap = reinterpret_cast<const uint32_t*>(ws + w.pen_bitmap);      // built by the scoring call with the same penalty
-    cudaError_t e = run_gemm(Gemm(lastn, q.lm_head, logits, B, c.vocab, c.hidden), h->num_sms, st);
-    if (e == cudaSuccess)
-        topk_softmax_kernel<<<B, GLUE_THREADS, 0, st>>>(logits, (long long)c.vocab, c.vocab, 1.0f / temperature, penalise ? bitmap : nullptr, pen_words,
-                                               repetition_penalty, K, out_ids, out_probs);
-    return cuda_status(h, e, "top-k");
+    Forward f(h, workspace, st);
+    bf16* logits = f.at(w.trace_logits);
+    TRY(f.gemm(Gemm(f.at(w.lastn), q.lm_head, logits, B, c.vocab, c.hidden), "lm_head"));
+    // the bitmap was built by the scoring call with the same penalty
+    return qwen_topk_softmax(f, logits, c.vocab, B, c.vocab, temperature, f.at<uint32_t>(w.pen_bitmap), repetition_penalty, K, out_ids, out_probs);
 }
 
 // ================================================================================================ greedy generation
@@ -306,18 +329,9 @@ static int qwen_topk(vqa_handle* h, QwenState& q, int B, size_t rows, int n_patc
 struct QwenGenWorkspace {
     QwenWorkspace w;
     size_t kcache, vcache, attn_o, attn_ml, splitk, next_ids, pos3, done, n_done, total;
-    int cap, splits, chunk;
+    int cap, splits;
     size_t layer_elems;
 };
-
-// Key splits of decode_attn_partial_kernel over a cache of `cap` slots: enough for two CTAs per SM (at B = 1 the 4 KV heads alone would
-// occupy 4 of 132 SMs), at least 16 keys each. Fixed by the capacity, not the live lengths, so a step's launch shapes never change.
-static int decode_attn_splits(int B, int kv_heads, int cap, int num_sms) {
-    return std::max(1, std::min((2 * num_sms + B * kv_heads - 1) / (B * kv_heads), (cap + 15) / 16));
-}
-
-// the group sizes (q heads per KV head) launch_decode_attn instantiates
-static bool decode_attn_group_supported(int G) { return G == 1 || G == 2 || G == 4 || G == 5 || G == 7 || G == 8; }
 
 static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S, int n_patches, int max_new, int num_sms) {
     QwenGenWorkspace g;
@@ -326,7 +340,6 @@ static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S
     pl.off = g.w.total;
     g.cap = S + max_new;
     g.splits = decode_attn_splits(B, c.kv_heads, g.cap, num_sms);
-    g.chunk = (g.cap + g.splits - 1) / g.splits;
     g.layer_elems = (size_t)B * c.kv_heads * g.cap * 128;
     g.kcache = pl.take((size_t)c.layers * g.layer_elems * 2);
     g.vcache = pl.take((size_t)c.layers * g.layer_elems * 2);
@@ -350,16 +363,11 @@ static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g
     bf16* logits = f.at(w.trace_logits);
     // The [B, vocab] bf16 logits are 0.3 MB per sequence against the 1.1 GB lm_head weight (7B) that the GEMM streams either way.
     TRY(f.gemm(Gemm(f.at(w.lastn), q.lm_head, logits, B, c.vocab, c.hidden), "lm_head"));
-    const bool penalise = a.repetition_penalty != 1.0f;
+    uint32_t* bitmap = a.repetition_penalty != 1.0f ? f.at<uint32_t>(w.pen_bitmap) : nullptr;
     if (const vqa_qwen25vl_answer_score* s = a.score)
-        TRY(f.launch(CAT_OTHER, 0, "answer logprob", answer_logprob_kernel, B, ANSWER_THREADS, 0, (const bf16*)logits, c.vocab,
-                     penalise ? (const uint32_t*)f.at<uint32_t>(w.pen_bitmap) : nullptr, (c.vocab + 31) / 32, a.repetition_penalty,
-                     1.0f / s->temperature, s->answer_ids, s->answer_counts, s->n_max, a.max_new_tokens, (const int*)a.out_lengths,
-                     (const int*)f.at<int>(g.done), s->top_k, s->out_logp, s->out_topk_ids, s->out_topk_probs));
-    return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, (const bf16*)logits, c.vocab,
-                    penalise ? f.at<uint32_t>(w.pen_bitmap) : nullptr, (c.vocab + 31) / 32, a.repetition_penalty, a.eos_ids, a.n_eos,
-                    a.max_new_tokens, a.first_position, B, a.out_tokens, a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done,
-                    f.at<int>(g.next_ids), f.at<int>(g.pos3));
+        TRY(answer_logprob(f, logits, B, c.vocab, bitmap, a.repetition_penalty, *s, a.max_new_tokens, a.out_lengths, f.at<int>(g.done)));
+    return greedy_select(f, logits, B, c.vocab, bitmap, a.repetition_penalty, a.eos_ids, a.n_eos, a.max_new_tokens, a.first_position, a.out_tokens,
+                         a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done, f.at<int>(g.next_ids), f.at<int>(g.pos3));
 }
 
 // The prefill of vqa_qwen25vl_score over the padded rows, with every layer's K/V stored in the cache, then the first token.
@@ -368,27 +376,11 @@ static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const vqa_qwen25vl
     const QwenGenWorkspace g = qwen_gen_plan(q.cfg, in.batch, in.seq_len, in.n_patches, a.max_new_tokens, h->num_sms);
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
-    TRY(f.launch(CAT_OTHER, 0, "generate init", generate_init_kernel, (in.batch * a.max_new_tokens + 255) / 256, 256, 0, in.batch, a.max_new_tokens,
-                 a.out_tokens, a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
+    TRY(generate_init(f, in.batch, a.max_new_tokens, a.out_tokens, a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
     const QwenKVCache kv{f.at(g.kcache), f.at(g.vcache), g.layer_elems, g.cap};
     TRY(qwen_prefill(f, q, g.w, in, nullptr, &kv));
     TRY(qwen_last_position(f, q, g.w, in, nullptr, a.repetition_penalty));
     return qwen_select_token(f, q, g, in.batch, a);
-}
-
-// decode_attn_partial_kernel for G q heads per KV head (the group sizes of the Qwen2.5-VL family: 7B 7, 3B 8, 32B 5, 72B 8)
-template <typename... Args>
-static cudaError_t launch_decode_attn(int G, dim3 grid, cudaStream_t st, Args... args) {
-    switch (G) {
-        case 1: decode_attn_partial_kernel<1><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
-        case 2: decode_attn_partial_kernel<2><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
-        case 4: decode_attn_partial_kernel<4><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
-        case 5: decode_attn_partial_kernel<5><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
-        case 7: decode_attn_partial_kernel<7><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
-        case 8: decode_attn_partial_kernel<8><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
 }
 
 // One decode step: every sequence feeds its last token (finished ones recompute their frozen last step, which writes nothing new).
@@ -405,7 +397,7 @@ static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_p
     Forward f(h, workspace, st);
     auto P_ = [&](size_t off) { return f.at(off); };
     auto F_ = [&](size_t off) { return f.at<float>(off); };
-    const int D = c.hidden, Hq = c.heads, Hkv = c.kv_heads, G = Hq / Hkv, qkv_cols = (Hq + 2 * Hkv) * 128;
+    const int D = c.hidden, Hq = c.heads, Hkv = c.kv_heads, qkv_cols = (Hq + 2 * Hkv) * 128;
     float* skw = F_(g.splitk);
     auto skinny = [&](Gemm gm) {
         const int s = splitk_slices(gm.M, gm.N, gm.K, f.nsm);
@@ -414,28 +406,18 @@ static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_p
     {
         auto grp = f.group(CAT_OTHER);
         TRY(f.launch(CAT_OTHER, 0, "decode embed", gather_rows_by_index_kernel, B, 128, 0, q.embed, f.at<int>(g.next_ids), P_(w.x), D));
-        TRY(f.launch(CAT_OTHER, 0, "decode rope table", rope_table_kernel, (B * 64 + 255) / 256, 256, 0, f.at<int>(g.pos3), B, q.text_axis,
-                     q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1));
+        TRY(qwen_rope_table(f, "decode rope table", f.at<int>(g.pos3), B, q.text_axis, q.text_inv_freq, 64, F_(w.cos), F_(w.sin), 1));
     }
     const float tscale = 1.0f / sqrtf(128.0f);
     for (int l = 0; l < c.layers; ++l) {
         const QwenLlmLayerW& Lw = q.llm[l];
         TRY(f.rmsnorm(P_(w.x), Lw.ln1, P_(w.xn), B, D, c.rms_eps));
         TRY(f.gemm(skinny(Gemm(P_(w.xn), Lw.qkv_w, P_(w.qkv), B, qkv_cols, D).with_bias(Lw.qkv_b)), "decode qkv gemm"));
-        TRY(f.launch(CAT_OTHER, 0, "decode rope", rope_inplace_kernel, (unsigned)((B * (Hq + Hkv) * 8 + 255) / 256), 256, 0, P_(w.qkv), qkv_cols,
-                     0, Hq + Hkv, 128, 128, F_(w.cos), F_(w.sin), (long long)B, c.emulate_bf16_rounding));
+        TRY(qwen_rope(f, "decode rope", P_(w.qkv), qkv_cols, 0, Hq + Hkv, 128, 128, F_(w.cos), F_(w.sin), B, c.emulate_bf16_rounding));
         bf16 *kc = f.at(g.kcache) + l * g.layer_elems, *vc = f.at(g.vcache) + l * g.layer_elems;
-        TRY(f.launch(CAT_OTHER, 0, "kv cache append", kv_cache_write_kernel, (unsigned)((B * Hkv * 16 + 255) / 256), 256, 0, P_(w.qkv), qkv_cols,
-                     Hq * 128, (Hq + Hkv) * 128, Hkv, 1, (long long)B, a.seq_lens, (const int*)a.out_lengths, kc, vc, g.cap));
-        const double kv_bytes = 2.0 * B * Hkv * (double)g.cap * 128 * 2;      // upper bound: the full capacity
-        TRY(f.op(CAT_ATTENTION, 4.0 * B * Hq * (double)g.cap * 128, kv_bytes, 2, "decode attention", [&] {
-            const dim3 grid(g.splits, Hkv, B);
-            cudaError_t e = launch_decode_attn(G, grid, st, P_(w.qkv), qkv_cols, kc, vc, g.cap, a.seq_lens, a.out_lengths, Hkv, g.chunk, tscale,
-                                               F_(g.attn_o), F_(g.attn_ml));
-            if (e != cudaSuccess) return e;
-            decode_attn_merge_kernel<<<B * Hq, 128, 0, st>>>(F_(g.attn_o), F_(g.attn_ml), g.splits, P_(w.attn), Hq * 128, Hq);
-            return cudaGetLastError();
-        }));
+        TRY(kv_cache_write(f, P_(w.qkv), qkv_cols, Hq * 128, (Hq + Hkv) * 128, Hkv, 1, B, a.seq_lens, a.out_lengths, kc, vc, g.cap));
+        TRY(decode_attention(f, P_(w.qkv), qkv_cols, kc, vc, g.cap, a.seq_lens, a.out_lengths, B, Hq, Hkv, tscale, g.splits, F_(g.attn_o),
+                             F_(g.attn_ml), P_(w.attn), Hq * 128));
         TRY(f.gemm(skinny(Gemm(P_(w.attn), Lw.o_w, P_(w.x), B, D, Hq * 128).with_residual(P_(w.x))), "decode o gemm"));
         TRY(f.rmsnorm(P_(w.x), Lw.ln2, P_(w.xn), B, D, c.rms_eps));
         TRY(f.gemm(Gemm(P_(w.xn), Lw.gu_w, P_(w.ff), B, 2 * c.mlp, D).with_epilogue(EPI_GATED_SILU, c.mlp), "decode gate_up gemm"));

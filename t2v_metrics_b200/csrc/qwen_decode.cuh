@@ -1,9 +1,8 @@
-// Kernels of the Qwen2.5-VL greedy decode loop: the K/V cache write, flash-decoding attention over the cache, and greedy token selection
-// with the per-step bookkeeping. Every step-dependent value (generated lengths, finished flags, next input ids and positions) lives in
-// device memory, so the launches of one decode step take the same arguments at every step and replay from one CUDA graph.
+// Kernels of the Qwen2.5-VL greedy decode loop and their launches: the K/V cache write, flash-decoding attention over the cache, and greedy
+// token selection with the per-step bookkeeping. Every step-dependent value (generated lengths, finished flags, next input ids and
+// positions) lives in device memory, so the launches of one decode step take the same arguments at every step and replay from one CUDA graph.
 #pragma once
-#include "ptx.cuh"
-#include "elementwise.cuh"
+#include "host.cuh"
 
 namespace vqa {
 
@@ -297,3 +296,72 @@ __global__ void __launch_bounds__(ANSWER_THREADS) answer_logprob_kernel(
 }
 
 }  // namespace vqa
+
+// ------------------------------------------------------------------------------------------------ decode-loop launches (see clipt5.cuh)
+
+// Generation state at the start of a prefill for B sequences of up to max_new tokens.
+static int generate_init(Forward& f, int B, int max_new, int* tokens, int* lengths, int* done, int* n_done, int* all_done) {
+    return f.launch(CAT_OTHER, 0, "generate init", generate_init_kernel, (B * max_new + 255) / 256, 256, 0, B, max_new, tokens, lengths, done,
+                    n_done, all_done);
+}
+
+// The K and V heads of the packed rows qkv [rows = B * S, ld] into the cache (prefill: gen_len NULL; decode: S == 1).
+static int kv_cache_write(Forward& f, const bf16* qkv, int ld, int k_col0, int v_col0, int Hkv, int S, long long rows, const int* seq_lens,
+                          const int* gen_len, bf16* kc, bf16* vc, int cap) {
+    return f.launch(CAT_OTHER, 0, "kv cache write", kv_cache_write_kernel, (unsigned)((rows * Hkv * 16 + 255) / 256), 256, 0, qkv, ld, k_col0,
+                    v_col0, Hkv, S, rows, seq_lens, gen_len, kc, vc, cap);
+}
+
+// Key splits of decode_attn_partial_kernel over a cache of `cap` slots: enough for two CTAs per SM (at B = 1 the 4 KV heads alone would
+// occupy 4 of 132 SMs), at least 16 keys each. Fixed by the capacity, not the live lengths, so a step's launch shapes never change.
+static int decode_attn_splits(int B, int kv_heads, int cap, int num_sms) {
+    return std::max(1, std::min((2 * num_sms + B * kv_heads - 1) / (B * kv_heads), (cap + 15) / 16));
+}
+
+// the group sizes (q heads per KV head) launch_decode_attn instantiates
+static bool decode_attn_group_supported(int G) { return G == 1 || G == 2 || G == 4 || G == 5 || G == 7 || G == 8; }
+
+// decode_attn_partial_kernel for G q heads per KV head (the group sizes of the Qwen2.5-VL family: 7B 7, 3B 8, 32B 5, 72B 8)
+template <typename... Args>
+static cudaError_t launch_decode_attn(int G, dim3 grid, cudaStream_t st, Args... args) {
+    switch (G) {
+        case 1: decode_attn_partial_kernel<1><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 2: decode_attn_partial_kernel<2><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 4: decode_attn_partial_kernel<4><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 5: decode_attn_partial_kernel<5><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 7: decode_attn_partial_kernel<7><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        case 8: decode_attn_partial_kernel<8><<<grid, 32 * DEC_ATTN_WARPS, 0, st>>>(args...); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+
+// Flash-decoding attention of the query rows q [B, ldq] over the cache: `splits` key ranges of ceil(cap / splits) slots into the fp32 partials
+// part_o [B * Hq * splits, 128] and part_ml [B * Hq * splits, 2], then their merge into out [B, ldo].
+static int decode_attention(Forward& f, const bf16* q, int ldq, const bf16* kc, const bf16* vc, int cap, const int* seq_lens, const int* gen_len,
+                            int B, int Hq, int Hkv, float scale, int splits, float* part_o, float* part_ml, bf16* out, int ldo) {
+    const double kv_bytes = 2.0 * B * Hkv * (double)cap * 128 * 2;      // upper bound: the full capacity
+    return f.op(CAT_ATTENTION, 4.0 * B * Hq * (double)cap * 128, kv_bytes, 2, "decode attention", [&] {
+        cudaError_t e = launch_decode_attn(Hq / Hkv, dim3(splits, Hkv, B), f.st, q, ldq, kc, vc, cap, seq_lens, gen_len, Hkv,
+                                           (cap + splits - 1) / splits, scale, part_o, part_ml);
+        if (e != cudaSuccess) return e;
+        decode_attn_merge_kernel<<<B * Hq, 128, 0, f.st>>>(part_o, part_ml, splits, out, ldo, Hq);
+        return cudaGetLastError();
+    });
+}
+
+// The answer log-probabilities of one step of a scored rollout from the step's bf16 logits [B, V] (penalty bitmap NULL = none).
+static int answer_logprob(Forward& f, const bf16* logits, int B, int V, const uint32_t* pen_bitmap, float penalty, const vqa_qwen25vl_answer_score& s,
+                          int max_new, const int* lengths, const int* done) {
+    return f.launch(CAT_OTHER, 0, "answer logprob", answer_logprob_kernel, B, ANSWER_THREADS, 0, logits, V, pen_bitmap, (V + 31) / 32, penalty,
+                    1.0f / s.temperature, s.answer_ids, s.answer_counts, s.n_max, max_new, lengths, done, s.top_k, s.out_logp, s.out_topk_ids,
+                    s.out_topk_probs);
+}
+
+// The greedy token of every unfinished sequence and its bookkeeping (penalty bitmap NULL = none; first_pos / pos3 NULL = no positions).
+static int greedy_select(Forward& f, const bf16* logits, int B, int V, uint32_t* pen_bitmap, float penalty, const int* eos_ids, int n_eos,
+                         int max_new, const int* first_pos, int* tokens, int* lengths, int* done, int* n_done, int* all_done, int* next_ids,
+                         int* pos3) {
+    return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, logits, V, pen_bitmap, (V + 31) / 32, penalty,
+                    eos_ids, n_eos, max_new, first_pos, B, tokens, lengths, done, n_done, all_done, next_ids, pos3);
+}

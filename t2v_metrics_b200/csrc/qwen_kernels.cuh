@@ -8,15 +8,9 @@
 
 namespace vqa {
 
-// Launch geometry of the glue kernels below, shared by the scoring path (qwen25vl.cuh) and their kernel-level entry points (vqa_b200.cu).
+// Block sizes of the glue kernels below (their launches: qwen25vl.cuh).
 constexpr int GLUE_THREADS = 256;        // rope, bitmaps, top-k
 constexpr int ROW_COPY_THREADS = 128;    // one block per row: gathers, embedding splice
-inline unsigned rope_table_blocks(int rows, int half) { return (unsigned)(((long long)rows * half + GLUE_THREADS - 1) / GLUE_THREADS); }
-inline unsigned rope_inplace_blocks(long long rows, int n_heads, int head_dim) {
-    return (unsigned)((rows * n_heads * (head_dim / 16) + GLUE_THREADS - 1) / GLUE_THREADS);
-}
-inline unsigned token_bitmap_blocks(int B, int S) { return (unsigned)(((long long)B * S + GLUE_THREADS - 1) / GLUE_THREADS); }
-inline dim3 token_bitmap_packed_grid(int max_prompt_len, int B) { return dim3((max_prompt_len + GLUE_THREADS - 1) / GLUE_THREADS, B); }
 inline int token_bitmap_words(int vocab) { return (vocab + 31) / 32; }
 
 // cos/sin table for rotary embeddings: for i < half: angle = pos[axis_of_dim[i]][row] * inv_freq[i];

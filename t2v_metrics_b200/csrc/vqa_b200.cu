@@ -431,6 +431,17 @@ static int device_sms() {
     return sms;
 }
 
+// Every entry point below checks its arguments, then runs the stage function a forward runs (or f.gemm / f.attention / f.rmsnorm) through
+// a Forward on the caller's stream and, when given, the caller's workspace. Its handle only counts the launches and keeps the error text.
+template <typename Body>
+static int glue_launch(void* stream, Body&& body, void* workspace = nullptr) {
+    vqa_handle launcher;
+    launcher.num_sms = device_sms();
+    Forward f(&launcher, workspace, (cudaStream_t)stream);
+    const int rc = body(f);
+    return rc == VQA_OK ? VQA_OK : fail(nullptr, rc, launcher.err);
+}
+
 // a GEMM with the ABI's explicit layout
 static Gemm abi_gemm(const void* A, int lda, const void* W, int ldw, int w_rows, void* C, int ldc, int M, int N, int K) {
     Gemm g((const bf16*)A, (const bf16*)W, C, M, N, K);
@@ -457,7 +468,7 @@ extern "C" int vqa_op_gemm_bf16(const void* A, int32_t lda, const void* W, int32
     if (int rc = check_gated(epilogue, N, w_rows, gate_up_offset)) return rc;
     Gemm g = abi_gemm(A, lda, W, ldw, w_rows, C, ldc, M, N, K);
     g.bias = (const bf16*)bias; g.residual = residual; g.ldr = ldr; g.epi = epilogue; g.gate_up_offset = gate_up_offset; g.variant = variant;
-    return cuda_status(nullptr, run_gemm(g, device_sms(), (cudaStream_t)stream), "gemm launch");
+    return glue_launch(stream, [&](Forward& f) { return f.gemm(g); });
 }
 
 // vqa_op_gemm_bf16 (plain store epilogue) whose output columns are written in groups: logical column c lands at (c / group_in) * group_out + c % group_in
@@ -468,7 +479,7 @@ extern "C" int vqa_op_gemm_bf16_grouped(const void* A, int32_t lda, const void* 
     if (lda % 8 || ldw % 8 || ldc % 8 || N % 8 || K % 8) return fail(nullptr, VQA_ERR_INVALID_ARG, "gemm: ld/N/K must be multiples of 8");
     Gemm g = abi_gemm(A, lda, W, ldw, w_rows, C, ldc, M, N, K);
     g.bias = (const bf16*)bias; g.c_group_in = group_in; g.c_group_out = group_out; g.variant = variant;
-    return cuda_status(nullptr, run_gemm(g, device_sms(), (cudaStream_t)stream), "gemm launch");
+    return glue_launch(stream, [&](Forward& f) { return f.gemm(g); });
 }
 
 // Skinny GEMM (M <= 128) with the K range cut into slices that run as one launch, partial tiles in `workspace` (fp32, splits * M * N floats; the
@@ -484,7 +495,7 @@ extern "C" int vqa_op_gemm_bf16_splitk(const void* A, int32_t lda, const void* W
     if (!workspace || workspace_bytes < (size_t)splits * M * N * 4) return fail(nullptr, VQA_ERR_WORKSPACE, "split-K workspace too small");
     Gemm g = abi_gemm(A, lda, W, ldw, w_rows, C, ldc, M, N, K);
     g.bias = (const bf16*)bias; g.residual = residual; g.ldr = ldr;
-    return cuda_status(nullptr, run_gemm(g.split_k(splits, (float*)workspace), device_sms(), (cudaStream_t)stream), "gemm launch");
+    return glue_launch(stream, [&](Forward& f) { return f.gemm(g.split_k(splits, (float*)workspace)); });
 }
 
 // vqa_op_gemm_bf16 with the fused-RMSNorm hooks (GemmParams::ssq_*): ssq_in [M, stride] partial sums of squares of the rows of A (the
@@ -505,7 +516,7 @@ extern "C" int vqa_op_gemm_bf16_normfuse(const void* A, int32_t lda, const void*
     Gemm g = abi_gemm(A, lda, W, ldw, w_rows, C, ldc, M, N, K);
     g.residual = residual; g.ldr = ldr; g.epi = epilogue; g.gate_up_offset = gate_up_offset; g.variant = variant;
     g.nf.ssq_in = ssq_in; g.nf.ssq_out = ssq_out; g.nf.stride = stride; g.nf.inv_dim = 1.0f / (float)norm_dim; g.nf.eps = eps;
-    return cuda_status(nullptr, run_gemm(g, device_sms(), (cudaStream_t)stream), "gemm launch");
+    return glue_launch(stream, [&](Forward& f) { return f.gemm(g); });
 }
 
 // Scratch of vqa_op_lmhead_logprob, in floats: lse_max | lse_sum ([M, LMHEAD_PARTS * n tiles] each) | label_logit [M] | scores [M].
@@ -528,20 +539,12 @@ extern "C" int vqa_op_lmhead_logprob(const void* Hs, int32_t ldh, const void* W,
     if (scratch_needed) *scratch_needed = need * sizeof(float);
     if (!scratch || !aligned(scratch, 4) || scratch_bytes < need * sizeof(float))
         return fail(nullptr, VQA_ERR_WORKSPACE, "lmhead logprob: scratch smaller than lmhead_scratch_floats(M, N) floats");
-    const int ntiles = LMHEAD_PARTS * ((N + LMHEAD_BN - 1) / LMHEAD_BN);
-    float* lse_max = scratch;
-    float* lse_sum = lse_max + (size_t)M * ntiles;
-    float* label_logit = lse_sum + (size_t)M * ntiles;
-    float* scores = label_logit + M;            // one target per row: exp(logprob), not returned
-    cudaStream_t st = (cudaStream_t)stream;
-    // the launch of qwen_score's lm_head
-    Gemm g = abi_gemm(Hs, ldh, W, ldw, N, nullptr, 0, M, N, K);
-    g.lse(labels, lse_max, lse_sum, label_logit);
-    g.lse_scale = 1.0f / temperature;
-    g.penalty_bitmap = repetition_penalty != 1.0f ? pen_bitmap : nullptr; g.penalty_words = token_bitmap_words(N); g.penalty = repetition_penalty;
-    if (int rc = cuda_status(nullptr, run_gemm(g, device_sms(), st), "lmhead launch")) return rc;
-    lse_finalize_kernel<<<(M + 3) / 4, 128, 0, st>>>(lse_max, lse_sum, label_logit, labels, scores, logprob, M, 1, ntiles);
-    return cuda_status(nullptr, cudaGetLastError(), "lse finalize");
+    const size_t parts = (size_t)M * LMHEAD_PARTS * ((N + LMHEAD_BN - 1) / LMHEAD_BN);
+    // one target per row; the scores exp(logprob) land in the scratch's last M floats and are not returned
+    return glue_launch(stream, [&](Forward& f) {
+        return lmhead_score(f, abi_gemm(Hs, ldh, W, ldw, N, nullptr, 0, M, N, K).processed(temperature, pen_bitmap, repetition_penalty), labels,
+                            scratch, scratch + parts, scratch + 2 * parts, scratch + 2 * parts + M, logprob, M, 1);
+    });
 }
 
 extern "C" int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t V, const uint32_t* pen_bitmap, float repetition_penalty,
@@ -551,13 +554,11 @@ extern "C" int vqa_op_answer_logprob(const void* logits, int32_t batch, int32_t 
     if (!logits || !lengths || !done || batch <= 0 || V <= 0 || max_new <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad answer logprob argument");
     const vqa_qwen25vl_answer_score s{answer_ids, answer_counts, n_max, temperature, top_k, out_logp, out_topk_ids, out_topk_probs};
     if (int rc = qwen_rollout_check(nullptr, s)) return rc;
-    answer_logprob_kernel<<<batch, ANSWER_THREADS, 0, (cudaStream_t)stream>>>(
-        (const bf16*)logits, V, pen_bitmap, (V + 31) / 32, repetition_penalty, 1.0f / temperature, answer_ids, answer_counts, n_max, max_new,
-        lengths, done, top_k, out_logp, out_topk_ids, out_topk_probs);
-    return cuda_status(nullptr, cudaGetLastError(), "answer logprob launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return answer_logprob(f, (const bf16*)logits, batch, V, pen_bitmap, repetition_penalty, s, max_new, lengths, done);
+    });
 }
 
-// kv_cache_write_kernel: the 16-byte chunks of the K and V heads of every row go to their cache slot.
 extern "C" int vqa_op_kv_cache_write(const void* qkv, int32_t ld, int32_t k_col0, int32_t v_col0, int32_t kv_heads, int32_t B, int32_t S,
                                      const int32_t* seq_lens, const int32_t* gen_len, void* kc, void* vc, int32_t cap, void* stream) {
     if (!qkv || !seq_lens || !kc || !vc) return fail(nullptr, VQA_ERR_INVALID_ARG, "kv cache write: null pointer");
@@ -566,13 +567,11 @@ extern "C" int vqa_op_kv_cache_write(const void* qkv, int32_t ld, int32_t k_col0
         return fail(nullptr, VQA_ERR_INVALID_ARG, "kv cache write: bad size (S <= cap, S == 1 in decode mode, heads inside ld)");
     if (ld % 8 || k_col0 % 8 || v_col0 % 8 || !aligned(qkv, 16) || !aligned(kc, 16) || !aligned(vc, 16))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "kv cache write: ld, column offsets and pointers must be 16-byte aligned");
-    const long long rows = (long long)B * S;
-    kv_cache_write_kernel<<<(unsigned)((rows * kv_heads * 16 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        (const bf16*)qkv, ld, k_col0, v_col0, kv_heads, S, rows, seq_lens, gen_len, (bf16*)kc, (bf16*)vc, cap);
-    return cuda_status(nullptr, cudaGetLastError(), "kv cache write launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return kv_cache_write(f, (const bf16*)qkv, ld, k_col0, v_col0, kv_heads, S, (long long)B * S, seq_lens, gen_len, (bf16*)kc, (bf16*)vc, cap);
+    });
 }
 
-// decode_attn_partial_kernel over `splits` key ranges of the cache, then decode_attn_merge_kernel; the fp32 partials live in `workspace`.
 extern "C" int vqa_op_decode_attention_d128(const void* q, int32_t ldq, const void* kc, const void* vc, int32_t cap, const int32_t* seq_lens,
                                             const int32_t* gen_len, int32_t B, int32_t q_heads, int32_t kv_heads, float scale, int32_t splits,
                                             void* workspace, size_t workspace_bytes, int32_t* splits_out, void* out, int32_t ldo, void* stream) {
@@ -592,19 +591,12 @@ extern "C" int vqa_op_decode_attention_d128(const void* q, int32_t ldq, const vo
     if (!workspace || !aligned(workspace, 4) || workspace_bytes < rows * 130 * 4)
         return fail(nullptr, VQA_ERR_WORKSPACE, "decode attention: workspace smaller than B * q_heads * splits * 130 floats");
     float* part_o = static_cast<float*>(workspace);
-    float* part_ml = part_o + rows * 128;
-    const int chunk = (cap + splits - 1) / splits;
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = launch_decode_attn(G, dim3(splits, kv_heads, B), st, (const bf16*)q, ldq, (const bf16*)kc, (const bf16*)vc, cap, seq_lens,
-                                       gen_len, kv_heads, chunk, scale, part_o, part_ml);
-    if (e == cudaSuccess) {
-        decode_attn_merge_kernel<<<B * q_heads, 128, 0, st>>>(part_o, part_ml, splits, (bf16*)out, ldo, q_heads);
-        e = cudaGetLastError();
-    }
-    return cuda_status(nullptr, e, "decode attention launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return decode_attention(f, (const bf16*)q, ldq, (const bf16*)kc, (const bf16*)vc, cap, seq_lens, gen_len, B, q_heads, kv_heads, scale, splits,
+                                part_o, part_o + rows * 128, (bf16*)out, ldo);
+    });
 }
 
-// greedy_select_kernel on caller-owned generation state.
 extern "C" int vqa_op_greedy_select(const void* logits, int32_t B, int32_t V, uint32_t* pen_bitmap, float repetition_penalty, const int32_t* eos_ids,
                                     int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
                                     int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, void* stream) {
@@ -612,10 +604,10 @@ extern "C" int vqa_op_greedy_select(const void* logits, int32_t B, int32_t V, ui
         return fail(nullptr, VQA_ERR_INVALID_ARG, "greedy select: null pointer (first_pos and pos3 are given together or not at all)");
     if (B <= 0 || V <= 0 || max_new <= 0 || n_eos < 0 || !(repetition_penalty > 0.f))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "greedy select: bad size / repetition penalty");
-    greedy_select_kernel<<<B, SELECT_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, V, pen_bitmap, (V + 31) / 32, repetition_penalty,
-                                                                         eos_ids, n_eos, max_new, first_pos, B, tokens, lengths, done, n_done,
-                                                                         all_done, next_ids, pos3);
-    return cuda_status(nullptr, cudaGetLastError(), "greedy select launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return greedy_select(f, (const bf16*)logits, B, V, pen_bitmap, repetition_penalty, eos_ids, n_eos, max_new, first_pos, tokens, lengths, done,
+                             n_done, all_done, next_ids, pos3);
+    });
 }
 
 static int check_t5_self_attn(const void* qkv, const void* out, const void* rel_emb, const int32_t* bucket_lut, int max_distance, int B, int H) {
@@ -625,17 +617,15 @@ static int check_t5_self_attn(const void* qkv, const void* out, const void* rel_
     return VQA_OK;
 }
 
-// t5_decoder_self_attn_kernel (the scoring path's decoder self-attention over T target rows), launched as vqa_clipt5_score does.
 extern "C" int vqa_op_t5_decoder_self_attn(const void* qkv, void* out, const void* rel_emb, const int32_t* bucket_lut, int32_t max_distance, int32_t B,
                                            int32_t T, int32_t H, int32_t round_scores, void* stream) {
     if (int rc = check_t5_self_attn(qkv, out, rel_emb, bucket_lut, max_distance, B, H)) return rc;
     if (T <= 0 || T > 256) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 decoder self attention: 1 <= T <= 256");
-    t5_decoder_self_attn_kernel<<<(B * H * T + 3) / 4, 128, 4 * T * sizeof(float), (cudaStream_t)stream>>>(
-        (const bf16*)qkv, (bf16*)out, (const bf16*)rel_emb, bucket_lut, max_distance, B, T, H, round_scores);
-    return cuda_status(nullptr, cudaGetLastError(), "t5 decoder self attention launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_decoder_self_attention(f, (const bf16*)qkv, (bf16*)out, (const bf16*)rel_emb, bucket_lut, max_distance, B, T, H, round_scores);
+    });
 }
 
-// One cached decoder self-attention layer of a generation step: t5_kv_cache_append_kernel, then t5_decode_self_attn_kernel.
 extern "C" int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, int32_t cap, const int32_t* lengths, void* out, const void* rel_emb,
                                           const int32_t* bucket_lut, int32_t max_distance, int32_t B, int32_t H, int32_t round_scores, void* stream) {
     if (int rc = check_t5_self_attn(qkv, out, rel_emb, bucket_lut, max_distance, B, H)) return rc;
@@ -643,25 +633,19 @@ extern "C" int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, i
     if (cap <= 0 || cap > 2048) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 decode self attention: 1 <= cap <= 2048");
     if (!aligned(qkv, 16) || !aligned(kc, 16) || !aligned(vc, 16))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 decode self attention: qkv and caches must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    t5_kv_cache_append_kernel<<<(B * H * 8 + 255) / 256, 256, 0, st>>>((const bf16*)qkv, B, H, lengths, (bf16*)kc, (bf16*)vc, cap);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) {
-        t5_decode_self_attn_kernel<<<(B * H + T5_DEC_ATTN_WARPS - 1) / T5_DEC_ATTN_WARPS, 32 * T5_DEC_ATTN_WARPS,
-                                     T5_DEC_ATTN_WARPS * cap * sizeof(float), st>>>((const bf16*)qkv, (const bf16*)kc, (const bf16*)vc, cap, lengths,
-                                                                                    (bf16*)out, (const bf16*)rel_emb, bucket_lut, max_distance, B,
-                                                                                    H, round_scores);
-        e = cudaGetLastError();
-    }
-    return cuda_status(nullptr, e, "t5 decode self attention launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_cached_self_attention(f, (const bf16*)qkv, (bf16*)kc, (bf16*)vc, cap, lengths, (bf16*)out, (const bf16*)rel_emb, bucket_lut,
+                                            max_distance, B, H, round_scores);
+    });
 }
 
 extern "C" int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32_t H, const int32_t* seq_lens,
                                     const float* bias_table, float scale, int32_t bias_const_from, int32_t round_scores, void* stream) {
     if (!qkv || !out || B <= 0 || S <= 0 || H <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad attention argument");
-    cudaError_t e = launch_attn_tc((const bf16*)qkv, 3 * H * 64, 0, H * 64, 2 * H * 64, (bf16*)out, H * 64, B, S, H, seq_lens, bias_table,
-                                   scale, bias_const_from, round_scores != 0, (cudaStream_t)stream);
-    return cuda_status(nullptr, e, "attention launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_attention_d64(f, "attention", (const bf16*)qkv, (bf16*)out, B, S, H, seq_lens, bias_table, scale, bias_const_from,
+                                    round_scores != 0);
+    });
 }
 
 // What attn_wgmma_kernel trusts of its arguments: every q / k / v head inside the row of `ld` columns, 16-byte aligned TMA columns and
@@ -691,9 +675,12 @@ extern "C" int vqa_op_attention_d128(const void* qkv, int32_t ld, int64_t rows, 
     // which covers max_len rows per sequence, must reach them
     if (!cu_seqlens && (S < 1 || (long long)n_seq * S > rows || max_len < S))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: fixed stride needs S >= 1, n_seq * S <= rows and max_len >= S");
-    cudaError_t e = launch_attn_tc128((const bf16*)qkv, ld, rows, q_col0, k_col0, v_col0, (bf16*)out, ldo, n_seq, max_len, S, q_heads, kv_group,
-                                      cu_seqlens, seq_lens, scale, causal != 0, (cudaStream_t)stream);
-    return cuda_status(nullptr, e, "attention d128 launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return f.attention(0, "attention d128", [&] {
+            return launch_attn_tc128((const bf16*)qkv, ld, rows, q_col0, k_col0, v_col0, (bf16*)out, ldo, n_seq, max_len, S, q_heads, kv_group,
+                                     cu_seqlens, seq_lens, scale, causal != 0, f.st);
+        });
+    });
 }
 
 // The same kernel with its variable-length extras: a shared key/value prefix per sequence, two short sequences per 128-row tile, compact output heads.
@@ -706,22 +693,20 @@ extern "C" int vqa_op_attention_d128_ex(const void* qkv, int32_t ld, int64_t row
         return rc;
     if (pair_sequences && (max_len > 64 || causal || kv_prefix))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d128: pair_sequences takes sequences of <= 64 rows, non-causal, without kv_prefix");
-    cudaError_t e = launch_attn_tc128((const bf16*)qkv, ld, rows, q_col0, k_col0, v_col0, (bf16*)out, ldo, n_seq, max_len, 0, q_heads, kv_group,
-                                      cu_seqlens, nullptr, scale, causal != 0, (cudaStream_t)stream, kv_prefix, pair_sequences != 0, o_head_stride, d_out);
-    return cuda_status(nullptr, e, "attention d128 launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return f.attention(0, "attention d128", [&] {
+            return launch_attn_tc128((const bf16*)qkv, ld, rows, q_col0, k_col0, v_col0, (bf16*)out, ldo, n_seq, max_len, 0, q_heads, kv_group,
+                                     cu_seqlens, nullptr, scale, causal != 0, f.st, kv_prefix, pair_sequences != 0, o_head_stride, d_out);
+        });
+    });
 }
 
-extern "C" int vqa_op_norm(const void* x, const void* gamma, const void* beta, void* y, int32_t rows, int32_t D, float eps,
-                           void* stream) {
+extern "C" int vqa_op_norm(const void* x, const void* gamma, void* y, int32_t rows, int32_t D, float eps, void* stream) {
     if (!x || !gamma || !y) return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: null pointer");
     if (rows <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: rows must be >= 1");
-    if (beta ? !(D == 256 || D == 512 || D == 768 || D == 1024 || D == 1280) : (D <= 0 || D % 8 || D > 8192))
-        return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: LayerNorm takes D = 256, 512, 768, 1024 or 1280; RMSNorm a multiple of 8 up to 8192");
-    if (!aligned(x, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 16))
-        return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: x / gamma / beta / y must be 16-byte aligned");
-    cudaError_t e = beta ? run_layernorm((const bf16*)x, (const bf16*)gamma, (const bf16*)beta, (bf16*)y, rows, D, eps, (cudaStream_t)stream)
-                         : run_rmsnorm((const bf16*)x, (const bf16*)gamma, (bf16*)y, rows, D, eps, (cudaStream_t)stream);
-    return cuda_status(nullptr, e, "norm launch");
+    if (D <= 0 || D % 8 || D > 8192) return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: D must be a multiple of 8 up to 8192");
+    if (!aligned(x, 16) || !aligned(gamma, 16) || !aligned(y, 16)) return fail(nullptr, VQA_ERR_INVALID_ARG, "norm: x / gamma / y must be 16-byte aligned");
+    return glue_launch(stream, [&](Forward& f) { return f.rmsnorm((const bf16*)x, (const bf16*)gamma, (bf16*)y, rows, D, eps); });
 }
 
 // ------------------------------------------------------------------------------------------------ kernel-level ABI: the CLIP-FlanT5 scoring path
@@ -738,7 +723,7 @@ extern "C" int vqa_op_gemm_bf16_f32acc(const void* A, int32_t lda, const void* W
     if (!gemm_variant_known(variant)) return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32-accumulate gemm: unknown tile variant");
     Gemm g = abi_gemm(A, lda, W, ldw, w_rows, C, ldc, M, N, K);
     g.bias = (const bf16*)bias; g.variant = variant;
-    return cuda_status(nullptr, run_gemm(g.accumulate_f32(), device_sms(), (cudaStream_t)stream), "gemm launch");
+    return glue_launch(stream, [&](Forward& f) { return f.gemm(g.accumulate_f32()); });
 }
 
 // `nb` GEMMs of one shape in one launch (BatchSpec), plain store epilogue. See include/vqa_b200.h for the acceptance rule.
@@ -760,7 +745,7 @@ extern "C" int vqa_op_gemm_bf16_batched(const void* A, int32_t lda, const void* 
     if (!gemm_variant_known(variant)) return fail(nullptr, VQA_ERR_INVALID_ARG, "batched gemm: unknown tile variant");
     Gemm g = abi_gemm(A, lda, W, ldw, (int)w_rows, C, ldc, M, N, K);
     g.batched(BatchSpec{nb, a_row_off, a_k_off, w_row_off, w_k_off, c_stride, a_rows, a_cols, w_rows, w_cols}, variant);
-    return cuda_status(nullptr, run_gemm(g, device_sms(), (cudaStream_t)stream), "gemm launch");
+    return glue_launch(stream, [&](Forward& f) { return f.gemm(g); });
 }
 
 // One decoder layer's cross-attention as vqa_clipt5_score runs it: mode 0 the absorbed sequence (the encoder transpose, then
@@ -783,21 +768,15 @@ extern "C" int vqa_op_t5_cross_attention(const void* q, const void* x, const int
     if (workspace_needed) *workspace_needed = pl.off;
     if (!workspace || workspace_bytes < pl.off) return fail(nullptr, VQA_ERR_WORKSPACE, "t5 cross attention: workspace too small");
     if (!aligned(workspace, 256)) return fail(nullptr, VQA_ERR_INVALID_ARG, "t5 cross attention: workspace must be 256-byte aligned");
-    vqa_handle launcher;        // a Forward needs a handle; this one only collects the launch count and the error text
-    launcher.num_sms = device_sms();
-    Forward f(&launcher, workspace, (cudaStream_t)stream);
-    int rc;
-    if (mode == 0) {
-        rc = clipt5_transpose_encoder(f, (const bf16*)x, f.at(xb.xt), B, S, d_model);
-        if (rc == VQA_OK)
-            rc = clipt5_absorbed_cross_attention(f, AbsorbedCrossAttn{(const bf16*)q, (const bf16*)x, f.at(xb.xt), seq_lens, (const bf16*)wkT,
-                                                                      (const bf16*)wkv + (size_t)inner * d_model, f.at(xb.qt), f.at(xb.csc),
-                                                                      f.at(xb.ctx), (bf16*)out, B, T, S, H, d_model});
-    } else {
-        rc = clipt5_reference_cross_attention(f, (const bf16*)q, (const bf16*)x, (const bf16*)wkv, f.at(kv), (bf16*)out, seq_lens, B, T, S, H,
-                                              d_model, round_scores);
-    }
-    return rc == VQA_OK ? VQA_OK : fail(nullptr, rc, launcher.err);
+    return glue_launch(stream, [&](Forward& f) {
+        if (mode == 1)
+            return clipt5_reference_cross_attention(f, (const bf16*)q, (const bf16*)x, (const bf16*)wkv, f.at(kv), (bf16*)out, seq_lens, B, T, S, H,
+                                                    d_model, round_scores);
+        TRY(clipt5_transpose_encoder(f, (const bf16*)x, f.at(xb.xt), B, S, d_model));
+        return clipt5_absorbed_cross_attention(f, AbsorbedCrossAttn{(const bf16*)q, (const bf16*)x, f.at(xb.xt), seq_lens, (const bf16*)wkT,
+                                                                    (const bf16*)wkv + (size_t)inner * d_model, f.at(xb.qt), f.at(xb.csc),
+                                                                    f.at(xb.ctx), (bf16*)out, B, T, S, H, d_model});
+    }, workspace);
 }
 
 // LayerNorm of the CLIP tower's fp32 residual stream: x fp32 [rows, D] -> y bf16 [rows, D].
@@ -806,37 +785,19 @@ extern "C" int vqa_op_layernorm_f32(const float* x, const void* gamma, const voi
     if (D != 256 && D != 512 && D != 768 && D != 1024) return fail(nullptr, VQA_ERR_UNSUPPORTED, "fp32 layernorm: D must be 256, 512, 768 or 1024");
     if (!aligned(x, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 16))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "fp32 layernorm: pointers must be 16-byte aligned");
-    return cuda_status(nullptr, run_layernorm_f32(x, (const bf16*)gamma, (const bf16*)beta, (bf16*)y, rows, D, eps, (cudaStream_t)stream),
-                       "layernorm launch");
+    return glue_launch(stream, [&](Forward& f) { return f.layernorm_f32(x, (const bf16*)gamma, (const bf16*)beta, (bf16*)y, rows, D, eps); });
 }
 
-// The CLIP embeddings and pre_layrnorm as vqa_clipt5_score launches them: patch rows [n_images * P, D] -> fp32 y [n_images * (P + 1), D].
 extern "C" int vqa_op_clip_embed_ln(const void* patch, const void* cls, const void* pos, const void* gamma, const void* beta, float* y,
                                     int32_t n_images, int32_t P, int32_t D, float eps, void* stream) {
     if (!patch || !cls || !pos || !gamma || !beta || !y || n_images <= 0 || P <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "clip embed: bad argument");
     if (D != 256 && D != 1024) return fail(nullptr, VQA_ERR_UNSUPPORTED, "clip embed: D must be 256 or 1024");
     if (!aligned(patch, 16) || !aligned(cls, 16) || !aligned(pos, 16) || !aligned(gamma, 16) || !aligned(beta, 16) || !aligned(y, 16))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "clip embed: pointers must be 16-byte aligned");
-    const int rows = n_images * (P + 1);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (D == 1024)
-        clip_embed_ln_kernel<1024><<<(rows + 7) / 8, 256, 0, st>>>((const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma,
-                                                                   (const bf16*)beta, y, n_images, P, eps);
-    else
-        clip_embed_ln_kernel<256><<<(rows + 7) / 8, 256, 0, st>>>((const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma,
-                                                                  (const bf16*)beta, y, n_images, P, eps);
-    return cuda_status(nullptr, cudaGetLastError(), "clip embed launch");
-}
-
-// The glue launches of clipt5.cuh on the caller's stream, through a handle of their own that only counts the launches and keeps the error
-// text.
-template <typename Body>
-static int glue_launch(void* stream, Body&& body) {
-    vqa_handle launcher;
-    launcher.num_sms = device_sms();
-    Forward f(&launcher, nullptr, (cudaStream_t)stream);
-    const int rc = body(f);
-    return rc == VQA_OK ? VQA_OK : fail(nullptr, rc, launcher.err);
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_embed_ln(f, (const bf16*)patch, (const bf16*)cls, (const bf16*)pos, (const bf16*)gamma, (const bf16*)beta, y, n_images, P, D,
+                               eps);
+    });
 }
 
 extern "C" int vqa_op_patchify(const void* pixels, int32_t pixel_dtype, int32_t n_images, int32_t image_size, int32_t patch, int32_t kpad, void* out,
@@ -905,8 +866,8 @@ extern "C" int vqa_op_lmhead_score(const void* Hs, int32_t ldh, const void* W, i
         return fail(nullptr, VQA_ERR_WORKSPACE, "lmhead score: scratch smaller than lmhead_scratch_floats(B * T, N) floats");
     const size_t parts = (size_t)M * LMHEAD_PARTS * ((N + LMHEAD_BN - 1) / LMHEAD_BN);
     return glue_launch(stream, [&](Forward& f) {
-        return clipt5_lmhead_score(f, abi_gemm(Hs, ldh, W, ldw, N, nullptr, 0, M, N, K), labels, scratch, scratch + parts, scratch + 2 * parts, scores,
-                                   logprobs, B, T);
+        return lmhead_score(f, abi_gemm(Hs, ldh, W, ldw, N, nullptr, 0, M, N, K), labels, scratch, scratch + parts, scratch + 2 * parts, scores,
+                            logprobs, B, T);
     });
 }
 
@@ -918,7 +879,6 @@ extern "C" int vqa_op_row_ssq(const void* x, float* ssq, int32_t rows, int32_t D
 }
 
 // ------------------------------------------------------------------------------------------------ kernel-level ABI: the Qwen2.5-VL scoring path
-// Each entry launches one glue kernel of qwen_prefill / qwen_last_position / qwen_topk with their geometry (qwen_kernels.cuh).
 
 // rope_table_kernel into the caller's tables, then rope_inplace_kernel on n_heads heads of x; text_mode: bf16 table and bf16 products.
 extern "C" int vqa_op_qwen_rope(const int32_t* positions, int32_t rows, const int32_t* axis_of_dim, const float* inv_freq, int32_t half, float* cos_t,
@@ -931,29 +891,21 @@ extern "C" int vqa_op_qwen_rope(const int32_t* positions, int32_t rows, const in
         return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen rope: ld, col0, head_stride multiples of 8, heads inside ld");
     if (!aligned(x, 16) || !aligned(cos_t, 16) || !aligned(sin_t, 16))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen rope: x and the tables must be 16-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
     const int round = text_mode != 0 ? 1 : 0;
-    rope_table_kernel<<<rope_table_blocks(rows, half), GLUE_THREADS, 0, st>>>(positions, rows, axis_of_dim, inv_freq, half, cos_t, sin_t, round);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) {
-        rope_inplace_kernel<<<rope_inplace_blocks(rows, n_heads, head_dim), GLUE_THREADS, 0, st>>>((bf16*)x, ld, col0, n_heads, head_stride, head_dim,
-                                                                                                  cos_t, sin_t, rows, round);
-        e = cudaGetLastError();
-    }
-    return cuda_status(nullptr, e, "qwen rope launch");
+    return glue_launch(stream, [&](Forward& f) {
+        TRY(qwen_rope_table(f, "rope table", positions, rows, axis_of_dim, inv_freq, half, cos_t, sin_t, round));
+        return qwen_rope(f, "rope", (bf16*)x, ld, col0, n_heads, head_stride, head_dim, cos_t, sin_t, rows, round);
+    });
 }
 
-// gather_rows_kernel: dst row r = src row index[r / group] * group + r % group, for r < rows.
 extern "C" int vqa_op_gather_rows(const void* src, void* dst, const int32_t* index, int32_t rows, int32_t group, int32_t D, void* stream) {
     if (!src || !dst || !index) return fail(nullptr, VQA_ERR_INVALID_ARG, "gather rows: null pointer");
     if (rows <= 0 || group <= 0 || rows % group || D <= 0 || D % 8)
         return fail(nullptr, VQA_ERR_INVALID_ARG, "gather rows: bad size (rows a multiple of group, D a multiple of 8)");
     if (!aligned(src, 16) || !aligned(dst, 16)) return fail(nullptr, VQA_ERR_INVALID_ARG, "gather rows: src / dst must be 16-byte aligned");
-    gather_rows_kernel<<<rows, ROW_COPY_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)src, (bf16*)dst, index, group, D);
-    return cuda_status(nullptr, cudaGetLastError(), "gather rows launch");
+    return glue_launch(stream, [&](Forward& f) { return qwen_gather_rows(f, "gather rows", (const bf16*)src, (bf16*)dst, index, rows, group, D); });
 }
 
-// qwen_embed_kernel over `rows` = n * S output rows: row b * S + s < seq_lens[b] takes feats[feat_index] or embed[ids], the rest zero.
 extern "C" int vqa_op_qwen_embed(const int32_t* ids, const int32_t* feat_index, const int32_t* seq_lens, const void* embed, const void* feats, void* out,
                                  int32_t rows, int32_t S, int32_t D, void* stream) {
     if (!ids || !feat_index || !seq_lens || !embed || !feats || !out) return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen embed: null pointer");
@@ -961,32 +913,29 @@ extern "C" int vqa_op_qwen_embed(const int32_t* ids, const int32_t* feat_index, 
         return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen embed: bad size (rows a multiple of S, D a multiple of 8)");
     if (!aligned(embed, 16) || !aligned(feats, 16) || !aligned(out, 16))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "qwen embed: embed / feats / out must be 16-byte aligned");
-    qwen_embed_kernel<<<rows, ROW_COPY_THREADS, 0, (cudaStream_t)stream>>>(ids, feat_index, seq_lens, (const bf16*)embed, (const bf16*)feats,
-                                                                           (bf16*)out, S, D);
-    return cuda_status(nullptr, cudaGetLastError(), "qwen embed launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return qwen_embed(f, ids, feat_index, seq_lens, (const bf16*)embed, (const bf16*)feats, (bf16*)out, rows, S, D);
+    });
 }
 
-// The repetition-penalty bitmap: token_bitmap_kernel (cu_seqlens NULL) or token_bitmap_packed_kernel, OR-ed into the caller's bitmap.
+// The repetition-penalty bitmap of padded (cu_seqlens NULL) or packed rows, OR-ed into the caller's bitmap.
 extern "C" int vqa_op_token_bitmap(const int32_t* ids, const int32_t* seq_lens, int32_t B, int32_t S, const int32_t* cu_seqlens, const int32_t* kv_prefix,
                                    const int32_t* pair_seq, int32_t max_prompt_len, int32_t vocab, uint32_t* bitmap, void* stream) {
     if (!ids || !bitmap) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: null pointer");
     if (B <= 0 || vocab <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: bad size");
     if (!aligned(bitmap, 4)) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: bitmap must be 4-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int words = token_bitmap_words(vocab);
     if (cu_seqlens) {
         if (!pair_seq || max_prompt_len <= 0)
             return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: packed rows need pair_seq and max_prompt_len >= 1");
-        token_bitmap_packed_kernel<<<token_bitmap_packed_grid(max_prompt_len, B), GLUE_THREADS, 0, st>>>(ids, cu_seqlens, kv_prefix, pair_seq, vocab,
-                                                                                                       bitmap, words);
-    } else {
-        if (!seq_lens || S <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: padded rows need seq_lens and S >= 1");
-        token_bitmap_kernel<<<token_bitmap_blocks(B, S), GLUE_THREADS, 0, st>>>(ids, seq_lens, B, S, vocab, bitmap, words);
+        return glue_launch(stream, [&](Forward& f) {
+            return qwen_token_bitmap_packed(f, ids, cu_seqlens, kv_prefix, pair_seq, max_prompt_len, B, vocab, bitmap);
+        });
     }
-    return cuda_status(nullptr, cudaGetLastError(), "token bitmap launch");
+    if (!seq_lens || S <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "token bitmap: padded rows need seq_lens and S >= 1");
+    return glue_launch(stream, [&](Forward& f) { return qwen_token_bitmap(f, ids, seq_lens, B, S, vocab, bitmap); });
 }
 
-// topk_softmax_kernel (the trace output of qwen_topk) on caller logits [B, ldl].
+// The trace output of vqa_qwen25vl_topk on caller logits [B, ldl].
 extern "C" int vqa_op_topk_softmax(const void* logits, int64_t ldl, int32_t B, int32_t V, float temperature, const uint32_t* pen_bitmap,
                                    float repetition_penalty, int32_t K, int32_t* out_ids, float* out_probs, void* stream) {
     if (!logits || !out_ids || !out_probs) return fail(nullptr, VQA_ERR_INVALID_ARG, "top-k softmax: null pointer");
@@ -994,11 +943,9 @@ extern "C" int vqa_op_topk_softmax(const void* logits, int64_t ldl, int32_t B, i
     if (!(temperature > 0.f) || !(repetition_penalty > 0.f))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "top-k softmax: temperature and repetition penalty must be > 0");
     if (!aligned(logits, 2) || !aligned(pen_bitmap, 4)) return fail(nullptr, VQA_ERR_INVALID_ARG, "top-k softmax: misaligned logits / bitmap");
-    const bool penalise = repetition_penalty != 1.0f;
-    topk_softmax_kernel<<<B, GLUE_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, (long long)ldl, V, 1.0f / temperature,
-                                                                      penalise ? pen_bitmap : nullptr, token_bitmap_words(V), repetition_penalty, K,
-                                                                      out_ids, out_probs);
-    return cuda_status(nullptr, cudaGetLastError(), "top-k softmax launch");
+    return glue_launch(stream, [&](Forward& f) {
+        return qwen_topk_softmax(f, (const bf16*)logits, ldl, B, V, temperature, pen_bitmap, repetition_penalty, K, out_ids, out_probs);
+    });
 }
 
 // ---------------------------------------------------------------------------------------------- image pre-processing (SURVEY 8(f)2)

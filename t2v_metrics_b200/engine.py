@@ -575,11 +575,11 @@ class ops:
         return out
 
     @staticmethod
-    def norm(x: torch.Tensor, gamma: torch.Tensor, beta=None, eps=1e-6, out=None):
+    def norm(x: torch.Tensor, gamma: torch.Tensor, eps=1e-6, out=None):
+        """T5LayerNorm / Qwen RMSNorm of the rows of x [rows, D] bf16: gamma * bf16(x * rsqrt(mean(x^2) + eps))."""
         lib = _lib.load()
         y = torch.empty_like(x) if out is None else out
-        rc = lib.vqa_op_norm(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(y), x.shape[0], x.shape[1], float(eps),
-                             _stream_ptr(x.device))
+        rc = lib.vqa_op_norm(_ptr(x), _ptr(gamma), _ptr(y), x.shape[0], x.shape[1], float(eps), _stream_ptr(x.device))
         _check(rc, None, "vqa_op_norm")
         return y
 

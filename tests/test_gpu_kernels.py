@@ -291,20 +291,14 @@ def test_gemm_fused_rmsnorm_hooks(ops, M, D, N):
     assert float((h.float() - ref_h).abs().mean()) <= 1e-2 * float(ref_h.abs().mean()) + 2e-3
 
 
-def test_norms(ops):
+def test_rmsnorm(ops):
     torch.manual_seed(6)
     for D in (4096, 3584, 2048, 1280, 256, 128, 5120):   # warp-per-row (D % 256 == 0, <= 4096) and the generic block-per-row path
         x = torch.randn(333, D, device="cuda").bfloat16()
         g = (1 + 0.1 * torch.randn(D, device="cuda")).bfloat16()
         var = x.float().pow(2).mean(-1, keepdim=True)
         ref = (g.float() * (x.float() * torch.rsqrt(var + 1e-6)).bfloat16().float()).bfloat16()
-        assert float((ops.norm(x, g, None, 1e-6).float() - ref.float()).abs().max()) <= 0.016
-    for D in (1024, 256):
-        x = torch.randn(333, D, device="cuda").bfloat16()
-        g = (1 + 0.1 * torch.randn(D, device="cuda")).bfloat16()
-        b = (0.1 * torch.randn(D, device="cuda")).bfloat16()
-        ref = torch.nn.functional.layer_norm(x.float(), (D,), g.float(), b.float(), 1e-5).bfloat16()
-        assert float((ops.norm(x, g, b, 1e-5).float() - ref.float()).abs().max()) <= 0.016
+        assert float((ops.norm(x, g, 1e-6).float() - ref.float()).abs().max()) <= 0.016
 
 
 def test_lmhead_logprob_never_materialises_logits(ops):

@@ -79,7 +79,7 @@ def test_qwen_engine_matches_oracle(dev, hw, n_images):
 @pytest.mark.parametrize("packed,pen", [(False, 1.0), (True, 1.0), (False, 1.3), (True, 1.3)])
 def test_qwen_launch_count_equals_captured_graph_nodes(dev, packed, pen):
     """last_launch_count() is what one forward enqueues (the nodes of a CUDA graph that captures it), padded and packed, with and
-    without the repetition-penalty bitmap."""
+    without the repetition-penalty bitmap, and then what the top-k of that call enqueues (lm_head and top-k softmax)."""
     from t2v_metrics_b200 import qwen_host
     from test_gpu_clipt5 import captured_node_count
     cfg = qo.Qwen25VLConfig.tiny(**TINY)
@@ -98,6 +98,7 @@ def test_qwen_launch_count_equals_captured_graph_nodes(dev, packed, pen):
     else:
         fn = lambda: eng.score_tensors(pix, grids, d["input_ids"], d["seq_lens"], d["feat_index"], d["position_ids"], ans, repetition_penalty=pen)
     assert captured_node_count(fn) == eng.last_launch_count()
+    assert captured_node_count(lambda: eng.topk_last(5, repetition_penalty=pen)) == eng.last_launch_count() == 2
 
 @pytest.mark.parametrize("frames,hw", [(2, (56, 84)), (4, (84, 56))])
 def test_qwen_engine_video_grid(dev, frames, hw):
