@@ -326,6 +326,20 @@ int vqa_debug_max_active_clusters(int32_t cluster_size);
  * else 0. */
 int vqa_debug_pdl_enabled(void);
 
+/* Process-wide override of the image pre-processing tile plan (vqa_clip_preprocess, vqa_qwen_preprocess, vqa_qwen_preprocess_video; tests
+ * and tuning): every image gets tile_rows (1..32) output rows and min(tile_cols, out_w) output columns per CTA, i.e. ceil(out_w / tile_cols)
+ * column tiles, and stages chunk_groups (1 or 2) groups of 4 canvas rows per pass. A plan call for an image whose forced plan does not fit
+ * the kernel's shared memory fails with an error naming this override. All zero = the automatic plan (the default). */
+int vqa_debug_set_preprocess_tiles(int32_t tile_rows, int32_t tile_cols, int32_t chunk_groups);
+
+/* Host-only: the tile plan of each item of a pre-processing call, as the planner (with any override above) makes it. layout 0 = CLIP
+ * (heights, widths, n_items, out_size, pad_to_square as vqa_clip_preprocess_workspace_bytes), 1 = Qwen patch rows (n_frames, heights,
+ * widths, is_video, n_items, patch, temporal_patch, merge, min_pixels, max_pixels as vqa_qwen_preprocess_video_plan; n_frames and
+ * is_video NULL = still images). geometry HOST [n_items][5] = (tile_rows, tile_cols, col_tiles, chunk_groups, band_groups). */
+int vqa_debug_preprocess_geometry(int32_t layout, const int32_t* n_frames, const int32_t* heights, const int32_t* widths,
+                                  const int32_t* is_video, int32_t n_items, int32_t out_size, int32_t pad_to_square, int32_t patch,
+                                  int32_t temporal_patch, int32_t merge, int64_t min_pixels, int64_t max_pixels, int32_t* geometry);
+
 const char* vqa_last_error(vqa_handle* h);
 void vqa_destroy(vqa_handle* h);
 

@@ -29,7 +29,7 @@ ABI_SYMBOLS = [
     "vqa_op_clip_embed_ln", "vqa_qwen_preprocess_video_plan", "vqa_qwen_preprocess_video",
     "vqa_op_qwen_rope", "vqa_op_gather_rows", "vqa_op_qwen_embed", "vqa_op_token_bitmap", "vqa_op_topk_softmax",
     "vqa_op_patchify", "vqa_op_splice_embed", "vqa_op_decoder_embed", "vqa_op_t5_bias_table", "vqa_op_lmhead_score", "vqa_op_row_ssq",
-    "vqa_qwen_preprocess_video_aa_plan", "vqa_qwen_preprocess_video_aa",
+    "vqa_qwen_preprocess_video_aa_plan", "vqa_qwen_preprocess_video_aa", "vqa_debug_set_preprocess_tiles", "vqa_debug_preprocess_geometry",
 ]
 
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
@@ -256,6 +256,11 @@ def load() -> C.CDLL:
     lib.vqa_debug_max_active_clusters.restype = C.c_int
     lib.vqa_debug_pdl_enabled.argtypes = []
     lib.vqa_debug_pdl_enabled.restype = C.c_int
+    lib.vqa_debug_set_preprocess_tiles.argtypes = [i32, i32, i32]
+    lib.vqa_debug_set_preprocess_tiles.restype = C.c_int
+    lib.vqa_debug_preprocess_geometry.argtypes = [i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, i32, i32,
+                                                  i32, i64, i64, C.POINTER(i32)]
+    lib.vqa_debug_preprocess_geometry.restype = C.c_int
     lib.vqa_resample_table.argtypes = [i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32)]
     lib.vqa_resample_table.restype = i32
     _lib = lib

@@ -351,6 +351,11 @@ inline size_t pre_smem_bytes(int band_groups, int tile_cols, int chunk_groups, i
     return 768 * sizeof(float) + ((size_t)3 * band_groups * tile_cols + (size_t)3 * chunk_groups * 4 * span4) * sizeof(uint32_t);
 }
 
+// Process-wide forced tile plan (vqa_debug_set_preprocess_tiles; tests and tuning): every image gets tile_rows output rows and
+// min(tile_cols, out_w) output columns per CTA and stages chunk_groups groups of 4 canvas rows per pass. All zero = the planner's choice.
+struct PreTileOverride { int tile_rows, tile_cols, chunk_groups; };
+inline PreTileOverride g_pre_tile_override{0, 0, 0};
+
 // Tables + tile geometry for "resize the ch x cw canvas to nh x nw, keep the oh x ow window at (top, left)"; shared between images
 // with the same geometry. Returns nullptr (plan.error set) when the filter windows cannot fit the shared-memory budget.
 inline const PreTableKey* pre_tables(PrePlan& plan, std::vector<PreTableKey>& cache, int ch, int cw, int nh, int nw, int top, int left,
@@ -393,6 +398,20 @@ inline const PreTableKey* pre_tables(PrePlan& plan, std::vector<PreTableKey>& ca
             if (pre_smem_bytes(band, tw, chunk, span) <= (size_t)PRE_MAX_SMEM) return chunk;
         return 0;
     };
+    const PreTileOverride force = g_pre_tile_override;
+    if (force.tile_rows) {
+        const int tw = force.tile_cols < ow ? force.tile_cols : ow, band = band_of(force.tile_rows), span = span_of(tw);
+        const size_t bytes = pre_smem_bytes(band, tw, force.chunk_groups, span);
+        if (bytes > (size_t)PRE_MAX_SMEM) {
+            plan.error = "the forced tile plan of vqa_debug_set_preprocess_tiles needs " + std::to_string(bytes) +
+                         " bytes of shared memory for this image, over the " + std::to_string(PRE_MAX_SMEM) + "-byte budget";
+            return nullptr;
+        }
+        k.tile = force.tile_rows; k.tile_cols = tw; k.col_tiles = (ow + tw - 1) / tw; k.band_groups = band; k.span4 = span;
+        k.chunk_groups = force.chunk_groups;
+        cache.push_back(k);
+        return &cache.back();
+    }
     // one column tile over the whole output width when it fits: the most output rows per CTA (<= 32)
     const int span_all = span_of(ow);
     for (int tile = 32; tile >= 1; tile >>= 1) {

@@ -1094,6 +1094,53 @@ extern "C" int vqa_qwen_preprocess_video(const void* src, const int64_t* frame_o
                                         out_dtype, workspace, workspace_bytes, host_staging, reinterpret_cast<cudaStream_t>(stream));
 }
 
+// Process-wide forced tile plan of image_preprocess_kernel (tests / tuning): tile_rows output rows, min(tile_cols, out_w) output columns
+// and chunk_groups groups of 4 canvas rows per pass for every image; all zero = the planner's choice (pre_tables).
+extern "C" int vqa_debug_set_preprocess_tiles(int32_t tile_rows, int32_t tile_cols, int32_t chunk_groups) {
+    const bool automatic = tile_rows == 0 && tile_cols == 0 && chunk_groups == 0;
+    if (!automatic && (tile_rows < 1 || tile_rows > 32 || tile_cols < 1 || chunk_groups < 1 || chunk_groups > PRE_RG))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "preprocess tiles: tile_rows in [1, 32], tile_cols >= 1 and chunk_groups 1 or 2, or all zero");
+    g_pre_tile_override = PreTileOverride{tile_rows, tile_cols, chunk_groups};
+    return VQA_OK;
+}
+
+// Host-only: the launch geometry the planner gives each item of a vqa_clip_preprocess (layout 0: heights / widths / n_items / out_size /
+// pad_to_square) or vqa_qwen_preprocess(_video) call (layout 1: n_frames / is_video NULL = still images). geometry [n_items][5] =
+// (tile_rows, tile_cols, col_tiles, chunk_groups, band_groups); the frames of a stack share their item's geometry.
+extern "C" int vqa_debug_preprocess_geometry(int32_t layout, const int32_t* n_frames, const int32_t* heights, const int32_t* widths,
+                                             const int32_t* is_video, int32_t n_items, int32_t out_size, int32_t pad_to_square, int32_t patch,
+                                             int32_t temporal_patch, int32_t merge, int64_t min_pixels, int64_t max_pixels, int32_t* geometry) {
+    if (!heights || !widths || !geometry || n_items <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad argument");
+    PrePlan plan;
+    std::vector<int> first(n_items);                       // index in plan.images of each item's first frame
+    if (layout == PRE_CHW) {
+        if (out_size <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad size");
+        std::vector<int64_t> off(n_items, 0);
+        if (!pre_plan(heights, widths, off.data(), n_items, out_size, pad_to_square != 0, plan)) return fail(nullptr, VQA_ERR_INVALID_ARG, plan.error);
+        for (int i = 0; i < n_items; ++i) first[i] = i;
+    } else if (layout == PRE_QWEN_PATCHES) {
+        const std::vector<int32_t> one(n_items, 1), still(n_items, 0);
+        if (!n_frames) n_frames = one.data();
+        if (!is_video) is_video = still.data();
+        int64_t frames = 0;
+        if (int rc = qwen_video_args(n_frames, heights, widths, is_video, n_items, patch, temporal_patch, merge, min_pixels, max_pixels, &frames))
+            return rc;
+        std::vector<int64_t> off(frames, 0);
+        if (!pre_plan_qwen_video(n_frames, heights, widths, is_video, off.data(), n_items, patch, merge, temporal_patch, min_pixels, max_pixels,
+                                 plan, nullptr, nullptr))
+            return fail(nullptr, VQA_ERR_INVALID_ARG, plan.error);
+        for (int i = 0, f = 0; i < n_items; f += n_frames[i++]) first[i] = f;
+    } else {
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "layout must be 0 (CLIP, channel planes) or 1 (Qwen patch rows)");
+    }
+    for (int i = 0; i < n_items; ++i) {
+        const PreImage& im = plan.images[first[i]];
+        const int32_t g[5] = {im.tile_rows, im.tile_cols, im.col_tiles, im.chunk_groups, im.band_groups};
+        for (int j = 0; j < 5; ++j) geometry[5 * i + j] = g[j];
+    }
+    return VQA_OK;
+}
+
 static int qwen_video_aa_args(int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w, const int32_t* first_h, int32_t htaps,
                               const int32_t* first_v, int32_t vtaps, int32_t patch, int32_t temporal_patch, int32_t merge, int32_t total_frames,
                               PreAAGeom& g) {

@@ -13,7 +13,8 @@ import torch
 from PIL import Image
 
 from oracle import clipt5_oracle as orc
-from t2v_metrics_b200.models.vqascore_models.mm_utils import CLIP_IMAGE_MEAN, CLIP_IMAGE_STD, clip_preprocess
+from preprocess_ref import canvas, pil_reference
+from t2v_metrics_b200.models.vqascore_models.mm_utils import clip_preprocess
 
 pytestmark = pytest.mark.gpu
 
@@ -25,36 +26,6 @@ def dev():
     if not torch.cuda.is_available():
         pytest.skip("needs a GPU")
     return torch.device("cuda", 0)
-
-
-def canvas(w, h, seed):
-    """Frames-like content: a smooth gradient with noise and saturated blocks (exercises the clip8 over/undershoot). A tall image is
-    built from 97 distinct rows so that pil_reference stays cheap for it."""
-    rng = np.random.default_rng(seed)
-    y, x = np.mgrid[0:(97 if h > w else h), 0:w]
-    a = np.stack([(x * 7 + y) % 256, (y * 3 + x // 5) % 256, ((x // 37 + y // 23) % 2) * 255], -1).astype(np.int32)
-    a = np.clip(a + rng.integers(-20, 21, a.shape), 0, 255).astype(np.uint8)
-    return a[(np.arange(h) * 31) % 97] if h > w else a
-
-
-def pil_reference(a, size=336):
-    """mm_utils.clip_preprocess (pad on) without materialising the padded square: Pillow resizes the canvas horizontally into a uint8
-    image and then vertically (Resample.c), and skips an axis whose size does not change, so resizing each distinct canvas row on its
-    own (width only) and then the stacked rows (height only) runs Pillow's own two passes on the same pixels."""
-    h, w = a.shape[:2]
-    side = max(h, w)
-    bg = tuple(int(v * 255) for v in CLIP_IMAGE_MEAN)
-    py, px = (side - h) // 2, (side - w) // 2
-    uniq, inv = np.unique(a.reshape(h, -1), axis=0, return_inverse=True)
-    rows = np.empty((len(uniq) + 1, side, 3), np.uint8)
-    rows[:] = bg
-    rows[:-1, px:px + w] = uniq.reshape(-1, w, 3)
-    hz = np.asarray(Image.fromarray(rows).resize((size, len(rows)), Image.BICUBIC))
-    inter = np.repeat(hz[-1:], side, 0)
-    inter[py:py + h] = hz[inv.reshape(-1)]
-    out = np.asarray(Image.fromarray(inter).resize((size, size), Image.BICUBIC), dtype=np.float32) / 255.0
-    out = (out - np.asarray(CLIP_IMAGE_MEAN, dtype=np.float32)) / np.asarray(CLIP_IMAGE_STD, dtype=np.float32)
-    return torch.from_numpy(out).permute(2, 0, 1).contiguous()
 
 
 def test_two_pass_restatement_equals_the_pil_path():

@@ -8,6 +8,7 @@ import pytest
 import torch
 from PIL import Image
 
+import preprocess_ref as pr
 from oracle import clipt5_oracle as orc
 from t2v_metrics_b200 import _lib
 
@@ -110,3 +111,112 @@ def test_qwen_plan_matches_python_smart_resize():
     assert total == sum(h // 14 * (w // 14) for h, w in ref) and wsb > 0
     with pytest.raises(RuntimeError, match="aspect ratio"):
         qwen_preprocess_plan([(10, 2500)])
+
+
+# ---------------------------------------------------------------------------------------------- tile plans of image_preprocess_kernel
+@pytest.fixture
+def automatic_plans():
+    """Leaves the process-wide tile-plan override at automatic whatever the test did."""
+    yield _lib.load()
+    assert _lib.load().vqa_debug_set_preprocess_tiles(0, 0, 0) == 0
+
+
+@pytest.mark.parametrize("layout", ["clip", "qwen"])
+def test_production_geometries_reach_every_plan_branch(layout):
+    """The automatic plans of the GPU production list (tests/test_gpu_preprocess_tiles.py) include, in each output layout, column tiles,
+    one 4-row group staged per pass, and at most 4 output rows per CTA over a single column tile -- so that list keeps running those
+    kernel paths bit-exactly against Pillow if the planner's cost model changes."""
+    if layout == "clip":
+        plans = [pr.geometry(0, [(h, w)], size, pad)[0] for h, w, size, pad in pr.CLIP_PRODUCTION]
+    else:
+        plans = [pr.geometry(1, [(h, w)], pixels=px, frames=[f])[0] for h, w, f, px in pr.QWEN_PRODUCTION]
+    assert any(g[2] > 1 for g in plans), plans
+    assert any(g[3] == 1 for g in plans), plans
+    assert any(g[0] <= 4 and g[2] == 1 for g in plans), plans
+
+
+def random_items(n, seed):
+    """n seeded (layout, axes, geometry call) triples over the CLIP (pad on / off, S 224 / 336) and Qwen (plugin bounds and
+    max_pixels 1003520) planners, sizes log-uniform from 1 to 40000 px a side."""
+    rng = np.random.default_rng(seed)
+    items = []
+    while len(items) < n:
+        h, w = (int(v) for v in np.exp(rng.uniform(0, np.log(40000), 2)))
+        if rng.random() < 0.5:
+            size, pad = int(rng.choice([224, 336])), bool(rng.random() < 0.5)
+            if pad and max(h, w) > 65500:
+                continue
+            items.append(("clip", pr.clip_axes(h, w, size, pad), lambda h=h, w=w, s=size, p=pad: pr.geometry(0, [(h, w)], s, p)[0]))
+        else:
+            if max(h, w) / min(h, w) > 200:
+                continue
+            px = pr.PLUGIN_PIXELS if rng.random() < 0.5 else (pr.PLUGIN_PIXELS[0], 1003520)
+            items.append(("qwen", pr.qwen_axes(h, w, *px), lambda h=h, w=w, px=px: pr.geometry(1, [(h, w)], pixels=px)[0]))
+    return items
+
+
+def test_automatic_plans_fit_and_cover_their_windows():
+    """For seeded random geometries, the automatic plan fits the shared-memory budget (restated from the tap tables), its column tiles
+    cover the output width with no empty tile, and its band holds the 4-row groups of every row tile's vertical windows."""
+    for layout, axes, plan in random_items(300, 0):
+        tr, tc, ct, cg, band = plan()
+        ow = len(axes[0][0])
+        need, need_band = pr.plan_needs(axes, tr, tc, cg)
+        assert 1 <= tr <= 32 and cg in (1, 2), (layout, tr, cg)
+        assert tc * ct >= ow and (ct - 1) * tc < ow and (ct > 1 or tc == ow), (layout, ow, tc, ct)
+        assert band >= need_band, (layout, band, need_band)
+        assert need <= pr.PRE_MAX_SMEM, (layout, need)
+
+
+def test_forced_plans_are_used_or_refused(automatic_plans):
+    """A forced tile plan is used exactly when it fits shared memory and is refused with an error naming the override otherwise; bad
+    override values are rejected and leave the override as it was; zeros restore every automatic plan."""
+    lib = automatic_plans
+    rng = np.random.default_rng(1)
+    items = random_items(120, 2)
+    auto = [plan() for _, _, plan in items]
+    used = refused = 0
+    for layout, axes, plan in items:
+        tr, tc, cg = int(rng.choice([1, 2, 4, 8, 16, 32])), int(rng.integers(1, 2000)), int(rng.integers(1, 3))
+        assert lib.vqa_debug_set_preprocess_tiles(tr, tc, cg) == 0
+        ow = len(axes[0][0])
+        try:
+            g = plan()
+        except RuntimeError as e:
+            assert "vqa_debug_set_preprocess_tiles" in str(e)
+            assert pr.plan_needs(axes, tr, tc, cg)[0] > pr.PRE_MAX_SMEM, (layout, tr, tc, cg)
+            refused += 1
+            continue
+        assert pr.plan_needs(axes, tr, tc, cg)[0] <= pr.PRE_MAX_SMEM
+        assert g[:4] == (tr, min(tc, ow), -(-ow // min(tc, ow)), cg) and g[4] == pr.plan_needs(axes, tr, tc, cg)[1]
+        used += 1
+    assert used >= 40 and refused >= 10, (used, refused)
+    # a 4000 x 6000 photo at the Qwen plugin's bounds needs column tiles: one 32-row tile over all 4368 columns does not fit
+    assert lib.vqa_debug_set_preprocess_tiles(32, 1 << 16, 2) == 0
+    with pytest.raises(RuntimeError, match="vqa_debug_set_preprocess_tiles"):
+        pr.geometry(1, [(4000, 6000)])
+    # out-of-range values are rejected and keep the override in force
+    assert lib.vqa_debug_set_preprocess_tiles(4, 100, 1) == 0
+    for bad in [(0, 100, 1), (4, 0, 1), (4, 100, 0), (33, 100, 1), (4, 100, 3), (-1, 100, 1), (4, -5, 1)]:
+        assert lib.vqa_debug_set_preprocess_tiles(*bad) != 0, bad
+    assert pr.geometry(0, [(512, 512)])[0][:4] == (4, 100, 4, 1)
+    assert lib.vqa_debug_set_preprocess_tiles(0, 0, 0) == 0
+    assert [plan() for _, _, plan in items] == auto
+
+
+def test_qwen_restatement_equals_the_plugin_path():
+    """tests/preprocess_ref.qwen_reference (Pillow's uint8 resize, a 768-entry normalisation table, patch rows by reshape) equals the
+    plugin's CPU path at its pixel bounds: noise that smart_resize leaves at its size (84 x 140), so that every level of every channel
+    goes through the table, a resized photo, and a 3-frame stack."""
+    from t2v_metrics_b200.models.vqascore_models.qwen_utils import qwen_image_to_patches, qwen_video_to_patches
+    mn, mx = pr.PLUGIN_PIXELS
+    noise = np.random.default_rng(3).integers(0, 256, (84, 140, 3), dtype=np.uint8)
+    assert all(len(np.unique(noise[..., c])) == 256 for c in range(3))
+    for a in (noise, pr.photo(333, 517, 4)):
+        got, grid = pr.qwen_reference(a, mn, mx)
+        ref, gref = qwen_image_to_patches(Image.fromarray(a), min_pixels=mn, max_pixels=mx)
+        assert grid == gref and torch.equal(got, ref)
+    stack = np.stack([pr.photo(61, 95, k) for k in range(3)])
+    got, grid = pr.qwen_reference(stack, mn, mx)
+    ref, gref = qwen_video_to_patches(stack, min_pixels=mn, max_pixels=mx)
+    assert grid == gref and torch.equal(got, ref)
