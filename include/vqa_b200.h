@@ -505,7 +505,9 @@ int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, int32_t cap,
  * bias_const_from > 0: the caller guarantees bias_table[h][.] is constant for |key - query| >= bias_const_from on each side (T5's
  * relative_attention_max_distance, modeling_t5.py:189-234), which lets far key tiles fold the bias into one FFMA; 0: no assumption.
  * round_scores != 0: reproduce the bf16 tensors the reference's eager attention forms before its fp32 softmax (q.k^T as bf16, then the
- * bf16 `scores += position_bias`, modeling_t5.py:308-331); 0: scores and bias stay fp32. */
+ * bf16 `scores += position_bias`, modeling_t5.py:308-331); 0: scores and bias stay fp32.
+ * B, S, H >= 1 with 3 * H * 64, B * S and H * B * ceil(S / 128) inside int32; qkv / out 16-byte aligned, bias_table / seq_lens 4-byte
+ * aligned; with a bias table S <= 16496 (its row must fit in shared memory); else VQA_ERR_INVALID_ARG before anything launches. */
 int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32_t H, const int32_t* seq_lens,
                          const float* bias_table, float scale, int32_t bias_const_from, int32_t round_scores, void* stream);
 

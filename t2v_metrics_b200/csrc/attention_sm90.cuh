@@ -330,8 +330,16 @@ constexpr int A64_TILE = 128 * 64 * 2;   // Q, K or V tile: 128 rows x 64 bf16, 
 // padding included, lies within [-127, 2S + 125] of index key - query + S - 1, so a score reads its bias without clamping the index.
 constexpr int A64_BIAS_PAD = 128;
 
-inline size_t attn64_smem_bytes(int stages, int bias_entries) {
+constexpr size_t A64_SMEM_MAX = 227 * 1024;   // dynamic shared memory of one CTA on sm_90
+
+constexpr size_t attn64_smem_bytes(int stages, int bias_entries) {
     return 1024 + (2 + 2 * (size_t)stages) * A64_TILE + 128 + (size_t)bias_entries * 4;
+}
+
+// The longest S whose padded bias row (2S - 1 + 2 A64_BIAS_PAD floats) fits next to a K/V ring of `stages` stages. A bias table longer than
+// the 2-stage limit does not fit at all.
+constexpr int attn64_max_bias_len(int stages) {
+    return (int)(((A64_SMEM_MAX - attn64_smem_bytes(stages, 0)) / 4 + 1 - 2 * A64_BIAS_PAD) / 2);
 }
 
 // S = Q K^T for a 128-key tile
@@ -669,19 +677,21 @@ inline cudaError_t launch_attn_tc(const __nv_bfloat16* qkv, int ld, int q_col0, 
     if (!tmap_bf16_2d_cached(&tm, qkv, (uint64_t)B * S, (uint64_t)ld, (uint64_t)ld, 128)) return cudaErrorInvalidValue;
     Attn64Params p = {};
     p.o = o; p.ldo = ldo; p.seq_lens = seq_lens;
-    p.B = B; p.S = S; p.H = H; p.n_qt = (S + 127) / 128;
+    p.B = B; p.S = S; p.H = H; p.n_qt = (int)((S + 127LL) / 128);
     p.q_col0 = q_col0; p.k_col0 = k_col0; p.v_col0 = v_col0;
     p.scale_log2e = scale * 1.4426950408889634f;
     p.bias_table = bias_table;
     p.bias_const_from = bias_const_from > 0 ? bias_const_from : 0;
     const long long n_items = (long long)H * B * p.n_qt;
     if (n_items > INT32_MAX) return cudaErrorInvalidValue;
-    // the deepest K/V ring that fits next to the bias row (sequences longer than ~12K rows with a bias table do not fit at all)
+    // the deepest K/V ring that fits next to the bias row: 4 stages up to S = attn64_max_bias_len(4), then 3, then 2 up to
+    // attn64_max_bias_len(2); longer sequences with a bias table do not fit at all
+    if (bias_table && S > attn64_max_bias_len(2)) return cudaErrorInvalidValue;
     const int bias_entries = bias_table ? 2 * S - 1 + 2 * A64_BIAS_PAD : 0;
     p.stages = A64_MAX_STAGES;
-    while (p.stages > 2 && attn64_smem_bytes(p.stages, bias_entries) > 227 * 1024) --p.stages;
+    while (bias_table && p.stages > 2 && S > attn64_max_bias_len(p.stages)) --p.stages;
     const size_t smem = attn64_smem_bytes(p.stages, bias_entries);
-    if (smem > 227 * 1024) return cudaErrorInvalidValue;
+    if (smem > A64_SMEM_MAX) return cudaErrorInvalidValue;
     const int sms = sm_count();
     if (sms <= 0) return cudaErrorInvalidDevice;
     const dim3 grid((unsigned)std::min<long long>(n_items, sms));

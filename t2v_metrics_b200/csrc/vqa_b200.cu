@@ -639,9 +639,24 @@ extern "C" int vqa_op_t5_decode_self_attn(const void* qkv, void* kc, void* vc, i
     });
 }
 
+// What attn64_ws_kernel trusts of its arguments: int32 row / column / work-item arithmetic, 16-byte aligned TMA rows and output rows, 4-byte
+// aligned lengths and bias entries, and a padded bias row that fits in shared memory next to the 2-stage K/V ring.
+static int check_attn_d64(const void* qkv, const void* out, int B, int S, int H, const int32_t* seq_lens, const float* bias_table) {
+    if (!qkv || !out) return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d64: null pointer");
+    if (B < 1 || S < 1 || H < 1) return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d64: B, S and H must be >= 1");
+    if (3LL * H * 64 > INT32_MAX || (long long)B * S > INT32_MAX || (long long)H * B * ((S + 127LL) / 128) > INT32_MAX)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d64: 3 * H * 64, B * S and H * B * ceil(S / 128) must fit in int32");
+    if (!aligned(qkv, 16) || !aligned(out, 16) || !aligned(bias_table, 4) || !aligned(seq_lens, 4))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "attention d64: qkv / out 16-byte aligned, bias_table / seq_lens 4-byte aligned");
+    if (bias_table && S > attn64_max_bias_len(2))
+        return fail(nullptr, VQA_ERR_INVALID_ARG,
+                    "attention d64: with a bias table S must be <= " + std::to_string(attn64_max_bias_len(2)) + " (its row must fit in shared memory)");
+    return VQA_OK;
+}
+
 extern "C" int vqa_op_attention_d64(const void* qkv, void* out, int32_t B, int32_t S, int32_t H, const int32_t* seq_lens,
                                     const float* bias_table, float scale, int32_t bias_const_from, int32_t round_scores, void* stream) {
-    if (!qkv || !out || B <= 0 || S <= 0 || H <= 0) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad attention argument");
+    if (int rc = check_attn_d64(qkv, out, B, S, H, seq_lens, bias_table)) return rc;
     return glue_launch(stream, [&](Forward& f) {
         return clipt5_attention_d64(f, "attention", (const bf16*)qkv, (bf16*)out, B, S, H, seq_lens, bias_table, scale, bias_const_from,
                                     round_scores != 0);

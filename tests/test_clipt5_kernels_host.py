@@ -150,6 +150,42 @@ def test_cross_attention_argument_checks():
 
 
 @no_device
+def test_attention_d64_argument_checks():
+    """Every call the head-dim-64 kernel cannot serve is refused before the tensor-map build: misaligned TMA rows or output rows (the kernel's
+    4-byte stores to a misaligned `out` would fault), misaligned lengths or bias entries, int32 overflow of the row, column or work-item
+    arithmetic, and a bias row longer than shared memory holds next to the 2-stage K/V ring (S = 16,496 is the longest that fits)."""
+    lib = _lib.load()
+    I32_MAX = 2 ** 31 - 1
+
+    def call(qkv=P, out=P, B=2, S=672, H=64, lens=P, table=P, const_from=128, round_scores=1):
+        return lib.vqa_op_attention_d64(qkv, out, B, S, H, lens, table, 1.0, const_from, round_scores, None)
+
+    assert call() == CUDA_ERR and call(round_scores=0, const_from=0) == CUDA_ERR
+    assert call(lens=None) == CUDA_ERR and call(table=None) == CUDA_ERR and call(lens=None, table=None) == CUDA_ERR
+    # alignment: qkv / out rows are TMA rows and 16-byte output rows, seq_lens / bias_table are read as 4-byte words
+    assert call(qkv=at(8)) == INVALID and call(out=at(2)) == INVALID and call(out=at(8)) == INVALID
+    assert call(qkv=at(16)) == CUDA_ERR and call(out=at(16)) == CUDA_ERR
+    assert call(table=at(2)) == INVALID and call(lens=at(2)) == INVALID
+    assert call(table=at(4)) == CUDA_ERR and call(lens=at(4)) == CUDA_ERR
+    # the bias row: 4 stages up to S = 8,304, 3 up to 12,400, 2 up to 16,496, refused past that; without a table S is not limited by it
+    for S in (8304, 8305, 12400, 12401, 16496):
+        assert call(B=1, H=2, S=S) == CUDA_ERR, S
+    assert call(B=1, H=2, S=16497) == INVALID and call(B=1, H=2, S=16497, const_from=0) == INVALID
+    assert call(B=1, H=2, S=16497, table=None) == CUDA_ERR and call(B=1, H=2, S=1 << 20, table=None) == CUDA_ERR
+    # int32 arithmetic: the qkv row of 3 * H * 64 columns, B * S rows, H * B * ceil(S / 128) work items
+    h_max = I32_MAX // (3 * 64)
+    assert call(B=1, S=1, H=h_max, table=None) == CUDA_ERR and call(B=1, S=1, H=h_max + 1, table=None) == INVALID
+    assert call(B=1 << 16, S=(1 << 15) - 1, H=1, table=None) == CUDA_ERR and call(B=1 << 16, S=1 << 15, H=1, table=None) == INVALID
+    assert call(B=(1 << 24) - 1, S=128, H=128, table=None) == CUDA_ERR and call(B=(1 << 24) - 1, S=128, H=129, table=None) == INVALID
+    assert call(B=(1 << 24) - 1, S=1, H=128, table=None) == CUDA_ERR and call(B=(1 << 24) - 1, S=1, H=129, table=None) == INVALID
+    assert call(B=1, S=I32_MAX, H=1, table=None) == CUDA_ERR       # ceil(S / 128) without overflowing S + 127
+    # null pointers and sizes below 1
+    assert call(qkv=None) == INVALID and call(out=None) == INVALID
+    for kw in ("B", "S", "H"):
+        assert call(**{kw: 0}) == INVALID and call(**{kw: -1}) == INVALID, kw
+
+
+@no_device
 def test_layernorm_f32_argument_checks():
     lib = _lib.load()
 

@@ -139,124 +139,6 @@ def test_gemm_linearity_full_size(ops):
     assert abs(float(c.float().sum()) - float(ref.float().sum())) <= 1e-3 * float(ref.float().abs().sum()) ** 0.5 + 50
 
 
-@pytest.mark.parametrize("B,S,H,use_bias,ragged,scale", [(2, 100, 4, True, True, 1.0), (3, 577, 16, False, False, 0.125),
-                                                         (2, 672, 8, True, True, 1.0), (1, 64, 1, True, False, 1.0),
-                                                         (2, 65, 2, False, True, 0.125),
-                                                         (5, 300, 64, True, True, 1.0)])   # B*H >= 296: one CTA per (sample, head), all query tiles
-def test_attention_matches_torch(ops, B, S, H, use_bias, ragged, scale):
-    torch.manual_seed(5)
-    qkv = (torch.randn(B * S, 3 * H * 64, device="cuda") * 0.5).bfloat16()
-    lens = torch.randint(max(1, S // 2), S + 1, (B,), device="cuda", dtype=torch.int32) if ragged else None
-    table = (torch.randn(H, 2 * S - 1, device="cuda") * 0.5).bfloat16().float().contiguous() if use_bias else None
-    out = ops.attention(qkv, B, S, H, seq_lens=lens, bias_table=table, scale=scale)
-    q, k, v = qkv.float().view(B, S, 3, H, 64).permute(2, 0, 3, 1, 4)
-    sc = torch.matmul(q, k.transpose(-1, -2)) * scale
-    if use_bias:
-        idx = (torch.arange(S, device="cuda")[None, :] - torch.arange(S, device="cuda")[:, None]) + S - 1
-        sc = sc + table[:, idx][None]
-    L = lens if lens is not None else torch.full((B,), S, device="cuda", dtype=torch.int32)
-    kmask = torch.arange(S, device="cuda")[None, :] < L[:, None]
-    sc = sc.masked_fill(~kmask[:, None, None, :], float("-inf"))
-    ref = torch.matmul(torch.softmax(sc, -1), v).permute(0, 2, 1, 3).reshape(B * S, H * 64)
-    qmask = kmask.reshape(B * S)
-    assert float((out[qmask].float() - ref[qmask]).abs().max()) < 0.02
-    assert float(out[~qmask].float().abs().max()) == 0.0 if (~qmask).any() else True
-
-
-@pytest.mark.parametrize("use_bias", [True, False])
-def test_attention_edge_lengths_and_growing_maxima(ops, use_bias):
-    """Every boundary of the split-row softmax stage in one launch: lengths around the 32-key chunk, 64-key half and 128-key tile edges
-    (a half with no chunk to read, the chunk that straddles the length, query quadrants that are all padding, a single valid key), and
-    scores whose row maximum grows by far more than the lazy-rescale threshold (2^8) from one key tile to the next, so the deferred
-    rescale of O and l runs in every tile."""
-    torch.manual_seed(21)
-    lens_list = [1, 2, 31, 32, 33, 63, 64, 65, 96, 97, 127, 128, 129, 160, 161, 255, 256, 257, 290, 300]
-    B, S, H = len(lens_list), 300, 2
-    x = torch.randn(B, S, 3, H, 64, device="cuda") * 0.5
-    ramp = 1.0 + 0.9 * (torch.arange(S, device="cuda") // 64).float()           # later keys are longer vectors: maxima keep growing
-    x[:, :, 1] *= ramp[None, :, None, None]
-    x[:, :, 0] *= 2.0
-    qkv = x.reshape(B * S, 3 * H * 64).bfloat16()
-    lens = torch.tensor(lens_list, device="cuda", dtype=torch.int32)
-    table = (torch.randn(H, 2 * S - 1, device="cuda") * 0.5).bfloat16().float().contiguous() if use_bias else None
-    out = ops.attention(qkv, B, S, H, seq_lens=lens, bias_table=table, scale=1.0)
-    q, k, v = qkv.float().view(B, S, 3, H, 64).permute(2, 0, 3, 1, 4)
-    sc = torch.matmul(q, k.transpose(-1, -2))
-    if use_bias:
-        idx = (torch.arange(S, device="cuda")[None, :] - torch.arange(S, device="cuda")[:, None]) + S - 1
-        sc = sc + table[:, idx][None]
-    kmask = torch.arange(S, device="cuda")[None, :] < lens[:, None]
-    sc = sc.masked_fill(~kmask[:, None, None, :], float("-inf"))
-    assert float((sc.amax(-1)[:, :, :, None] - sc[..., :128].amax(-1)[:, :, :, None]).max()) > 16.0      # the fixture does exercise the rescale
-    ref = torch.matmul(torch.softmax(sc, -1), v).permute(0, 2, 1, 3).reshape(B * S, H * 64)
-    qmask = kmask.reshape(B * S)
-    err = (out[qmask].float() - ref[qmask]).abs()
-    assert float(err.max()) < 0.03, float(err.max())
-    assert float(out[~qmask].float().abs().max()) == 0.0
-
-
-@pytest.mark.parametrize("S,dist,ragged", [(672, 128, False), (672, 128, True), (400, 40, True), (300, 299, False)])
-def test_attention_saturating_t5_bias(ops, S, dist, ragged):
-    """T5 buckets saturate at relative_attention_max_distance: the bias is one value per head and side for |key - query| >= dist
-    (large magnitudes, many key tiles). The kernel against the torch reference."""
-    torch.manual_seed(11)
-    B, H = 2, 3
-    qkv = (torch.randn(B * S, 3 * H * 64, device="cuda") * 0.5).bfloat16()
-    lens = torch.randint(S // 2, S + 1, (B,), device="cuda", dtype=torch.int32) if ragged else None
-    rel = torch.arange(-(S - 1), S, device="cuda").clamp(-dist, dist) + dist                    # saturating buckets
-    table = (torch.randn(H, 2 * dist + 1, device="cuda") * 2.0).bfloat16().float()[:, rel].contiguous()
-    out = ops.attention(qkv, B, S, H, seq_lens=lens, bias_table=table, scale=1.0, bias_const_from=dist)
-    generic = ops.attention(qkv, B, S, H, seq_lens=lens, bias_table=table, scale=1.0)          # no constancy promise: every tile reads the table
-    q, k, v = qkv.float().view(B, S, 3, H, 64).permute(2, 0, 3, 1, 4)
-    idx = (torch.arange(S, device="cuda")[None, :] - torch.arange(S, device="cuda")[:, None]) + S - 1
-    sc = torch.matmul(q, k.transpose(-1, -2)) + table[:, idx][None]
-    L = lens if lens is not None else torch.full((B,), S, device="cuda", dtype=torch.int32)
-    kmask = torch.arange(S, device="cuda")[None, :] < L[:, None]
-    sc = sc.masked_fill(~kmask[:, None, None, :], float("-inf"))
-    ref = torch.matmul(torch.softmax(sc, -1), v).permute(0, 2, 1, 3).reshape(B * S, H * 64)
-    qmask = kmask.reshape(B * S)
-    assert float((out[qmask].float() - ref[qmask]).abs().max()) < 0.02
-    assert float((generic[qmask].float() - ref[qmask]).abs().max()) < 0.02
-
-
-@pytest.mark.parametrize("S,use_bias,scale", [(672, True, 1.0), (577, False, 0.125), (200, True, 1.0)])
-def test_attention_reference_rounding_points(ops, S, use_bias, scale):
-    """round_scores=True forms the bf16 tensors of the reference's eager attention before the fp32 softmax (modeling_t5.py:308-331:
-    `scores = matmul(q, k^T)` is bf16, `scores += position_bias` is a bf16 add; modeling_clip.py:271: bf16 matmul * 2^-3). Large
-    scores (|s| ~ 20) so that the rounding is visible: the kernel must follow the rounded reference more closely than the fp32-score one."""
-    torch.manual_seed(3)
-    B, H = 2, 4
-    qkv = (torch.randn(B * S, 3 * H * 64, device="cuda") * 1.5).bfloat16()
-    table = None
-    if use_bias:
-        rel = torch.arange(-(S - 1), S, device="cuda").clamp(-128, 128) + 128
-        table = (torch.randn(H, 257, device="cuda") * 2.0).bfloat16().float()[:, rel].contiguous()
-    got = ops.attention(qkv, B, S, H, bias_table=table, scale=scale, bias_const_from=128 if use_bias else 0, round_scores=True).float()
-    plain = ops.attention(qkv, B, S, H, bias_table=table, scale=scale, bias_const_from=128 if use_bias else 0, round_scores=False).float()
-    q, k, v = qkv.float().view(B, S, 3, H, 64).permute(2, 0, 3, 1, 4)
-    raw = torch.matmul(q, k.transpose(-1, -2))
-    idx = (torch.arange(S, device="cuda")[None, :] - torch.arange(S, device="cuda")[:, None]) + S - 1
-    # bf16 matmul output, computed like the reference does (bf16 operands, fp32 accumulation, one rounding). Rounding the fp32 product
-    # of float copies instead moves a few scores that sit on a bf16 rounding boundary by one ulp (0.125 at |s| ~ 20) -- the summation
-    # order decides those, and one such flip changes a near-tied row's output by ~0.3.
-    qb, kb = qkv.view(B, S, 3, H, 64).permute(2, 0, 3, 1, 4)[:2]
-    sc = torch.matmul(qb, kb.transpose(-1, -2))
-    if use_bias:
-        sc = (sc + table[:, idx][None].bfloat16())                        # bf16 + bf16 -> bf16
-    sc = (sc * scale).float()                                             # * 2^-3 is exact in bf16
-    p = torch.softmax(sc, -1).bfloat16().float()
-    ref_rounded = torch.matmul(p, v).permute(0, 2, 1, 3).reshape(B * S, H * 64)
-    exact = raw * scale + (table[:, idx][None] if use_bias else 0.0)
-    ref_exact = torch.matmul(torch.softmax(exact, -1), v).permute(0, 2, 1, 3).reshape(B * S, H * 64)
-    e_round = float((got - ref_rounded).abs().mean())
-    e_cross = float((got - ref_exact).abs().mean())
-    e_plain = float((plain - ref_exact).abs().mean())
-    print(f"\n[S={S} bias={use_bias}] round_scores kernel vs rounded reference {e_round:.2e}, vs exact-score reference {e_cross:.2e}; "
-          f"fp32-score kernel vs exact reference {e_plain:.2e}")
-    assert e_round < 0.6 * e_cross          # it follows the reference's rounding, not the exact scores
-    assert float((got - ref_rounded).abs().max()) < 0.05 and float((plain - ref_exact).abs().max()) < 0.05
-
-
 @pytest.mark.parametrize("M,D,N", [(700, 4096, 4096), (300, 256, 256), (130, 2048, 512)])
 def test_gemm_fused_rmsnorm_hooks(ops, M, D, N):
     """north_star: 'RMSNorm ... fused into the adjacent matmul epilogue'. Producer: a residual GEMM leaves per-row partial sums of squares of

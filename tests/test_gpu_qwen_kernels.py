@@ -11,6 +11,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from attention_ref import assert_attn, assert_discriminates, attn_ref, bf16_ulp
 from t2v_metrics_b200 import qwen_host
 
 SENTINEL = -1280.0          # exact in bf16 and fp32
@@ -44,46 +45,7 @@ def assert_guards(big, rows, cols, pad_rows=8, what=""):
     assert bool((big[keep] == SENTINEL).all()), f"{what}: a guard element was written"
 
 
-def bf16_ulp(x):
-    """Spacing of bf16 at |x| (8 significant bits)."""
-    a = x.abs().double().clamp_min(2.0 ** -126)
-    return torch.exp2(torch.floor(torch.log2(a)) - 7)
-
-
 # ================================================================================================ A. head-dim-128 attention
-def attn_ref(q, k, v, scale, causal, q_off=0):
-    """fp64 attention of q [H, n, d] over k, v [H, m, d]; query i sits at key position i + q_off (causal: sees keys j <= i + q_off).
-    Returns (exact, the same with P = exp(s - rowmax) rounded to bf16 before P.V and l summed unrounded): the kernel's one deliberate rounding."""
-    q, k, v = q.double(), k.double(), v.double()
-    s = torch.matmul(q, k.transpose(1, 2)) * scale
-    if causal:
-        i = torch.arange(q.shape[1], device=q.device)[:, None] + q_off
-        j = torch.arange(k.shape[1], device=q.device)[None, :]
-        s = s.masked_fill(j > i, float("-inf"))
-    e = torch.exp(s - s.amax(-1, keepdim=True))
-    l = e.sum(-1, keepdim=True)
-    return torch.matmul(e, v) / l, torch.matmul(e.to(torch.bfloat16).double(), v) / l
-
-
-def attn_bound(ref, ref_p):
-    """Per element: one bf16 ulp of the output plus 2x the largest error of the P-rounding restatement in that head (the kernel rounds P at
-    its own exponent reference, so its rounding errors are another draw of the same size, not the same errors)."""
-    return bf16_ulp(ref) + 2.0 * (ref_p - ref).abs().amax((-2, -1), keepdim=True)
-
-
-def assert_attn(got, ref, ref_p, what):
-    assert bool(torch.isfinite(got).all()), f"{what}: non-finite output"
-    tol = attn_bound(ref, ref_p)
-    excess = (got.double() - ref).abs() - tol
-    assert float(excess.max()) <= 0.0, f"{what}: {int((excess > 0).sum())} elements past the bound, worst by {float(excess.max()):.3g}"
-    return tol
-
-
-def assert_discriminates(wrong, ref, tol, what, factor=4.0):
-    """A plausible kernel mistake, applied to the reference, must move some element by `factor` x the tolerance."""
-    assert bool(((wrong - ref).abs() > factor * tol).any()), f"fixture cannot see {what}"
-
-
 def qkv_layout(Hq, Hkv):
     """qwen_prefill's packed qkv row: q heads, then k heads, then v heads; 64 unread NaN columns after them."""
     return dict(ld=(Hq + 2 * Hkv) * 128 + 64, q0=0, k0=Hq * 128, v0=(Hq + Hkv) * 128)
