@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define VQA_B200_ABI_VERSION 2
+#define VQA_B200_ABI_VERSION 3
 
 typedef enum {
     VQA_OK = 0,
@@ -107,7 +107,7 @@ typedef struct {
 
 typedef struct vqa_handle vqa_handle;
 
-/* ABI / build info ("vqa_b200 abi=2 arch=sm_90a ..."). Never fails. */
+/* ABI / build info ("vqa_b200 abi=3 arch=sm_90a ..."). Never fails. */
 const char* vqa_version(void);
 
 /* Create an engine for a CLIP-FlanT5 model on CUDA device `device`. */
@@ -326,9 +326,9 @@ int vqa_debug_max_active_clusters(int32_t cluster_size);
  * else 0. */
 int vqa_debug_pdl_enabled(void);
 
-/* Process-wide override of the image pre-processing tile plan (vqa_clip_preprocess, vqa_qwen_preprocess, vqa_qwen_preprocess_video; tests
- * and tuning): every image gets tile_rows (1..32) output rows and min(tile_cols, out_w) output columns per CTA, i.e. ceil(out_w / tile_cols)
- * column tiles, and stages chunk_groups (1 or 2) groups of 4 canvas rows per pass. A plan call for an image whose forced plan does not fit
+/* Process-wide override of the image pre-processing tile plan (vqa_clip_preprocess, vqa_qwen_preprocess_video; tests and tuning): every
+ * image gets tile_rows (1..32) output rows and min(tile_cols, out_w) output columns per CTA, i.e. ceil(out_w / tile_cols) column tiles,
+ * and stages chunk_groups (1 or 2) groups of 4 canvas rows per pass. A plan call for an image whose forced plan does not fit
  * the kernel's shared memory fails with an error naming this override. All zero = the automatic plan (the default). */
 int vqa_debug_set_preprocess_tiles(int32_t tile_rows, int32_t tile_cols, int32_t chunk_groups);
 
@@ -361,21 +361,12 @@ int vqa_clip_preprocess(const void* src, const int64_t* offsets, const int32_t* 
                         int32_t out_size, int32_t pad_to_square, const uint8_t* background, const float* mean, const float* stdv,
                         void* out, int32_t out_dtype, void* workspace, size_t workspace_bytes, void* host_staging, void* stream);
 
-/* Qwen2.5-VL still-image pre-processing on the device: smart_resize (qwen_vl_utils / image_processing_qwen2_vl.py:62-87) + PIL-exact
- * bicubic resize + /255 + normalise + frame duplication + 14x14 patch rows in 2x2 merge-block order
- * (image_processing_qwen2_vl.py:191-220). vqa_qwen_preprocess_plan is host-only: grid_hw [n][2] = (h, w) patch grid of each image,
- * total_patches = rows of `out`, workspace_bytes = device scratch needed. out: DEVICE [total_patches, 3*temporal_patch*patch^2]. */
-int vqa_qwen_preprocess_plan(const int32_t* heights, const int32_t* widths, int32_t n_images, int32_t patch, int32_t merge,
-                             int64_t min_pixels, int64_t max_pixels, int32_t* grid_hw, int64_t* total_patches, size_t* workspace_bytes);
-int vqa_qwen_preprocess(const void* src, const int64_t* offsets, const int32_t* heights, const int32_t* widths, int32_t n_images,
-                        int32_t patch, int32_t temporal_patch, int32_t merge, int64_t min_pixels, int64_t max_pixels, const float* mean,
-                        const float* stdv, void* out, int32_t out_dtype, void* workspace, size_t workspace_bytes, void* host_staging,
-                        void* stream);
-
-/* Qwen2.5-VL still images and decoded video frame stacks in one launch: each frame goes through the still-image path above
- * (qwen_vl_utils fetch_video on a list of frames runs fetch_image on each), then Qwen2VLVideoProcessor._preprocess with
- * do_resize=False (video_processing_qwen2_vl.py:228-275): frames 2k and 2k+1 fill temporal slots 0 and 1 of temporal group k's patch
- * rows, and an odd last frame fills both (the processor's padding with copies of the last frame; no second read of the source).
+/* Qwen2.5-VL still images and decoded video frame stacks in one launch. Every frame gets the still-image pre-processing: smart_resize
+ * (qwen_vl_utils / image_processing_qwen2_vl.py:62-87) + PIL-exact bicubic resize + /255 + normalise + 14x14 patch rows in 2x2 merge-block
+ * order (image_processing_qwen2_vl.py:191-220); qwen_vl_utils fetch_video on a list of frames runs fetch_image on each. A stack then
+ * goes through Qwen2VLVideoProcessor._preprocess with do_resize=False (video_processing_qwen2_vl.py:228-275): frames 2k and 2k+1 fill
+ * temporal slots 0 and 1 of temporal group k's patch rows, and an odd last frame fills both (the processor's padding with copies of the
+ * last frame; no second read of the source).
  *   n_frames / heights / widths / is_video   HOST arrays [n_items]; all frames of an item share its size. is_video[i] == 0: a still
  *              image (n_frames[i] must be 1), its frame written to every temporal slot, grid (1, gh, gw); else a video of
  *              ceil(n_frames / temporal_patch) temporal groups. A 1-frame video has the pixels of a still but is a video grid.

@@ -12,27 +12,8 @@ from pathlib import Path
 _HERE = Path(__file__).resolve().parent
 LIB_PATH = _HERE / "libvqa_b200.so"
 
-ABI_SYMBOLS = [
-    "vqa_version", "vqa_create_clipt5", "vqa_bind_weights", "vqa_finalize_weights", "vqa_clipt5_workspace_bytes",
-    "vqa_clipt5_score", "vqa_set_profile", "vqa_profile_read", "vqa_last_launch_count", "vqa_last_error", "vqa_destroy", "vqa_op_gemm_bf16",
-    "vqa_op_lmhead_logprob", "vqa_op_attention_d64", "vqa_op_norm", "vqa_op_attention_d128",
-    "vqa_create_qwen25vl", "vqa_qwen25vl_set_rope", "vqa_qwen25vl_workspace_bytes", "vqa_qwen25vl_score",
-    "vqa_clip_preprocess_workspace_bytes", "vqa_clip_preprocess", "vqa_resample_table", "vqa_qwen_preprocess_plan",
-    "vqa_qwen_preprocess", "vqa_clipt5_debug_layout", "vqa_qwen25vl_debug_layout", "vqa_set_gemm_schedule",
-    "vqa_qwen25vl_topk", "vqa_op_gemm_bf16_normfuse",
-    "vqa_debug_max_active_clusters", "vqa_debug_pdl_enabled", "vqa_op_attention_d128_ex", "vqa_op_gemm_bf16_grouped", "vqa_op_gemm_bf16_splitk",
-    "vqa_qwen25vl_generate_workspace_bytes", "vqa_qwen25vl_generate_prefill", "vqa_qwen25vl_generate_step",
-    "vqa_clipt5_generate_workspace_bytes", "vqa_clipt5_generate_prefill", "vqa_clipt5_generate_step",
-    "vqa_op_answer_logprob",
-    "vqa_op_kv_cache_write", "vqa_op_decode_attention_d128", "vqa_op_greedy_select", "vqa_t5_bucket_lut", "vqa_op_t5_decoder_self_attn",
-    "vqa_op_t5_decode_self_attn", "vqa_op_gemm_bf16_f32acc", "vqa_op_gemm_bf16_batched", "vqa_op_t5_cross_attention", "vqa_op_layernorm_f32",
-    "vqa_op_clip_embed_ln", "vqa_qwen_preprocess_video_plan", "vqa_qwen_preprocess_video",
-    "vqa_op_qwen_rope", "vqa_op_gather_rows", "vqa_op_qwen_embed", "vqa_op_token_bitmap", "vqa_op_topk_softmax",
-    "vqa_op_patchify", "vqa_op_splice_embed", "vqa_op_decoder_embed", "vqa_op_t5_bias_table", "vqa_op_lmhead_score", "vqa_op_row_ssq",
-    "vqa_qwen_preprocess_video_aa_plan", "vqa_qwen_preprocess_video_aa", "vqa_debug_set_preprocess_tiles", "vqa_debug_preprocess_geometry",
-]
-
 VQA_DTYPE_BF16, VQA_DTYPE_F32, VQA_DTYPE_I32 = 0, 1, 2
+VQA_OK, VQA_ERR_INVALID_ARG, VQA_ERR_MISSING_WEIGHT, VQA_ERR_CUDA, VQA_ERR_WORKSPACE, VQA_ERR_UNSUPPORTED = 0, -1, -2, -3, -4, -5   # vqa_status
 
 
 class VqaClipT5Config(C.Structure):
@@ -95,11 +76,94 @@ class VqaTensor(C.Structure):
                 ("dtype", C.c_int32)]
 
 
+# Every function include/vqa_b200.h declares: name -> (restype, argtypes). tests/test_abi.py checks each entry against the header.
+_vp, _i32, _i64, _f32, _sz, _P = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t, C.POINTER
+PROTOTYPES = {
+    "vqa_version": (C.c_char_p, []),
+    "vqa_create_clipt5": (_i32, [_P(VqaClipT5Config), _i32, _P(_vp)]),
+    "vqa_bind_weights": (_i32, [_vp, _P(VqaTensor), _i32]),
+    "vqa_finalize_weights": (_i32, [_vp]),
+    "vqa_clipt5_workspace_bytes": (_sz, [_vp, _i32, _i32, _i32, _i32]),
+    "vqa_clipt5_score": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _vp]),
+    "vqa_clipt5_generate_workspace_bytes": (_sz, [_vp, _i32, _i32, _i32, _i32]),
+    "vqa_clipt5_generate_prefill": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "vqa_clipt5_generate_step": (_i32, [_vp, _i32, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "vqa_create_qwen25vl": (_i32, [_P(VqaQwen25VLConfig), _i32, _P(_vp)]),
+    "vqa_qwen25vl_set_rope": (_i32, [_vp, _P(_f32), _P(_i32), _i32, _P(_f32), _P(_i32), _i32]),
+    "vqa_qwen25vl_workspace_bytes": (_sz, [_vp, _i32, _i64, _i32]),
+    "vqa_qwen25vl_score": (_i32, [_vp, _P(VqaQwen25VLPrompts), _P(VqaQwen25VLPacked), _vp, _f32, _f32, _vp, _vp, _vp, _sz, _vp]),
+    "vqa_qwen25vl_topk": (_i32, [_vp, _i32, _i64, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _sz, _vp]),
+    "vqa_qwen25vl_generate_workspace_bytes": (_sz, [_vp, _i32, _i32, _i32, _i32]),
+    "vqa_qwen25vl_generate_prefill": (_i32, [_vp, _P(VqaQwen25VLPrompts), _P(VqaQwen25VLGeneration), _vp, _sz, _vp]),
+    "vqa_qwen25vl_generate_step": (_i32, [_vp, _P(VqaQwen25VLGeneration), _i32, _i32, _i32, _vp, _sz, _vp]),
+    "vqa_last_launch_count": (_i64, [_vp]),
+    "vqa_set_profile": (_i32, [_vp, _i32]),
+    "vqa_profile_read": (_i32, [_vp, _P(_f32), _P(C.c_double), _P(C.c_double), _P(_i64)]),
+    "vqa_clipt5_debug_layout": (_i32, [_vp, _i32, _i32, _i32, _i32, _P(_sz), _i32]),
+    "vqa_qwen25vl_debug_layout": (_i32, [_vp, _i32, _i64, _i32, _P(_sz), _i32]),
+    "vqa_set_gemm_schedule": (_i32, [_i32, _i32]),
+    "vqa_debug_max_active_clusters": (_i32, [_i32]),
+    "vqa_debug_pdl_enabled": (_i32, []),
+    "vqa_debug_set_preprocess_tiles": (_i32, [_i32, _i32, _i32]),
+    "vqa_debug_preprocess_geometry": (_i32, [_i32, _P(_i32), _P(_i32), _P(_i32), _P(_i32), _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64,
+                                             _P(_i32)]),
+    "vqa_last_error": (C.c_char_p, [_vp]),
+    "vqa_destroy": (None, [_vp]),
+    "vqa_clip_preprocess_workspace_bytes": (_sz, [_P(_i32), _P(_i32), _i32, _i32, _i32]),
+    "vqa_clip_preprocess": (_i32, [_vp, _P(_i64), _P(_i32), _P(_i32), _i32, _i32, _i32, _P(C.c_uint8), _P(_f32), _P(_f32), _vp, _i32, _vp, _sz,
+                                   _vp, _vp]),
+    "vqa_qwen_preprocess_video_plan": (_i32, [_P(_i32), _P(_i32), _P(_i32), _P(_i32), _i32, _i32, _i32, _i32, _i64, _i64, _P(_i32), _P(_i64),
+                                              _P(_sz)]),
+    "vqa_qwen_preprocess_video": (_i32, [_vp, _P(_i64), _P(_i32), _P(_i32), _P(_i32), _P(_i32), _i32, _i32, _i32, _i32, _i64, _i64, _P(_f32),
+                                         _P(_f32), _vp, _i32, _vp, _sz, _vp, _vp]),
+    "vqa_qwen_preprocess_video_aa_plan": (_i32, [_i32, _i32, _i32, _i32, _P(_i32), _i32, _P(_i32), _i32, _i32, _i32, _i32, _i32, _P(_i64),
+                                                 _P(_sz)]),
+    "vqa_qwen_preprocess_video_aa": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _P(_i32), _P(_f32), _i32, _P(_i32), _P(_f32), _i32,
+                                            _i32, _i32, _i32, _P(_f32), _P(_f32), _vp, _i32, _vp, _sz, _vp, _vp]),
+    "vqa_resample_table": (_i32, [_i32, _i32, _i32, _i32, _P(_i32), _P(_i32)]),
+    "vqa_op_gemm_bf16": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "vqa_op_gemm_bf16_normfuse": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _i32, _i32,
+                                         _f32, _P(_i32), _vp]),
+    "vqa_op_lmhead_logprob": (_i32, [_vp, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _f32, _vp, _f32, _vp, _vp, _sz, _P(_sz), _vp]),
+    "vqa_op_answer_logprob": (_i32, [_vp, _i32, _i32, _vp, _f32, _f32, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "vqa_op_kv_cache_write": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "vqa_op_decode_attention_d128": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _vp, _sz, _P(_i32), _vp, _i32,
+                                            _vp]),
+    "vqa_op_greedy_select": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vqa_t5_bucket_lut": (_i32, [_i32, _i32, _i32, _P(_i32)]),
+    "vqa_op_t5_decoder_self_attn": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "vqa_op_t5_decode_self_attn": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "vqa_op_attention_d64": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _f32, _i32, _i32, _vp]),
+    "vqa_op_norm": (_i32, [_vp, _vp, _vp, _i32, _i32, _f32, _vp]),
+    "vqa_op_attention_d128": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _i32, _vp]),
+    "vqa_op_attention_d128_ex": (_i32, [_vp, _i32, _i64, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _f32, _i32, _i32, _i32,
+                                        _i32, _vp]),
+    "vqa_op_gemm_bf16_splitk": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _sz, _P(_i32), _vp]),
+    "vqa_op_gemm_bf16_grouped": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _vp]),
+    "vqa_op_gemm_bf16_f32acc": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _i32, _vp]),
+    "vqa_op_gemm_bf16_batched": (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64,
+                                        _i64, _i32, _vp]),
+    "vqa_op_t5_cross_attention": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _P(_sz), _vp]),
+    "vqa_op_layernorm_f32": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp]),
+    "vqa_op_clip_embed_ln": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp]),
+    "vqa_op_patchify": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "vqa_op_splice_embed": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "vqa_op_decoder_embed": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "vqa_op_t5_bias_table": (_i32, [_vp, _vp, _i32, _vp, _i32, _i32, _vp]),
+    "vqa_op_lmhead_score": (_i32, [_vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _P(_sz), _vp]),
+    "vqa_op_row_ssq": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp]),
+    "vqa_op_qwen_rope": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "vqa_op_gather_rows": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "vqa_op_qwen_embed": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "vqa_op_token_bitmap": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp]),
+    "vqa_op_topk_softmax": (_i32, [_vp, _i64, _i32, _i32, _f32, _vp, _f32, _i32, _vp, _vp, _vp]),
+}
+
 _lib = None
 
 
 def load() -> C.CDLL:
-    """dlopen libvqa_b200.so and declare prototypes. Raises if the library is absent (no CPU fallback exists)."""
+    """dlopen libvqa_b200.so and declare PROTOTYPES. Raises if the library is absent (no CPU fallback exists)."""
     global _lib
     if _lib is not None:
         return _lib
@@ -109,160 +173,11 @@ def load() -> C.CDLL:
             f"{path} not found: build it first (python -c 'import __graft_entry__ as g; g.build()'). "
             "t2v_metrics_b200 has no CPU or PyTorch fallback for the scoring path.")
     lib = C.CDLL(str(path))
-    for sym in ABI_SYMBOLS:
-        if not hasattr(lib, sym):
-            raise ImportError(f"{path} does not export {sym}")
-    vp, i32, f32, i64 = C.c_void_p, C.c_int32, C.c_float, C.c_int64
-    lib.vqa_version.restype = C.c_char_p
-    lib.vqa_create_clipt5.argtypes = [C.POINTER(VqaClipT5Config), C.c_int, C.POINTER(vp)]
-    lib.vqa_create_clipt5.restype = C.c_int
-    lib.vqa_bind_weights.argtypes = [vp, C.POINTER(VqaTensor), i32]
-    lib.vqa_bind_weights.restype = C.c_int
-    lib.vqa_finalize_weights.argtypes = [vp]
-    lib.vqa_finalize_weights.restype = C.c_int
-    lib.vqa_clipt5_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
-    lib.vqa_clipt5_workspace_bytes.restype = C.c_size_t
-    lib.vqa_clipt5_score.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, C.c_size_t, vp]
-    lib.vqa_clipt5_score.restype = C.c_int
-    lib.vqa_set_profile.argtypes = [vp, i32]
-    lib.vqa_set_profile.restype = C.c_int
-    lib.vqa_profile_read.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
-    lib.vqa_profile_read.restype = C.c_int
-    lib.vqa_last_launch_count.argtypes = [vp]
-    lib.vqa_last_launch_count.restype = i64
-    lib.vqa_last_error.argtypes = [vp]
-    lib.vqa_last_error.restype = C.c_char_p
-    lib.vqa_destroy.argtypes = [vp]
-    lib.vqa_destroy.restype = None
-    lib.vqa_op_gemm_bf16.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, vp, vp, i32, i32, i32, i32, vp]
-    lib.vqa_op_gemm_bf16.restype = C.c_int
-    lib.vqa_op_gemm_bf16_normfuse.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, vp, i32, i32, i32, vp, vp, i32, i32, f32,
-                                              C.POINTER(i32), vp]
-    lib.vqa_op_gemm_bf16_normfuse.restype = C.c_int
-    lib.vqa_op_lmhead_logprob.argtypes = [vp, i32, vp, i32, i32, i32, i32, vp, f32, vp, f32, vp, vp, C.c_size_t, C.POINTER(C.c_size_t), vp]
-    lib.vqa_op_lmhead_logprob.restype = C.c_int
-    lib.vqa_op_attention_d64.argtypes = [vp, vp, i32, i32, i32, vp, vp, f32, i32, i32, vp]
-    lib.vqa_op_attention_d64.restype = C.c_int
-    lib.vqa_op_norm.argtypes = [vp, vp, vp, i32, i32, f32, vp]
-    lib.vqa_op_norm.restype = C.c_int
-    lib.vqa_op_attention_d128.argtypes = [vp, i32, i64, i32, i32, i32, vp, i32, i32, i32, i32, i32, i32, vp, vp, f32, i32, vp]
-    lib.vqa_op_attention_d128.restype = C.c_int
-    lib.vqa_create_qwen25vl.argtypes = [C.POINTER(VqaQwen25VLConfig), C.c_int, C.POINTER(vp)]
-    lib.vqa_create_qwen25vl.restype = C.c_int
-    lib.vqa_qwen25vl_set_rope.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(i32), i32, C.POINTER(C.c_float), C.POINTER(i32), i32]
-    lib.vqa_qwen25vl_set_rope.restype = C.c_int
-    lib.vqa_qwen25vl_workspace_bytes.argtypes = [vp, i32, i64, i32]
-    lib.vqa_qwen25vl_workspace_bytes.restype = C.c_size_t
-    lib.vqa_qwen25vl_score.argtypes = [vp, C.POINTER(VqaQwen25VLPrompts), C.POINTER(VqaQwen25VLPacked), vp, f32, f32, vp, vp, vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_score.restype = C.c_int
-    lib.vqa_qwen25vl_topk.argtypes = [vp, i32, i64, i32, i32, f32, f32, vp, vp, vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_topk.restype = C.c_int
-    lib.vqa_qwen25vl_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
-    lib.vqa_qwen25vl_generate_workspace_bytes.restype = C.c_size_t
-    lib.vqa_qwen25vl_generate_prefill.argtypes = [vp, C.POINTER(VqaQwen25VLPrompts), C.POINTER(VqaQwen25VLGeneration), vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_generate_prefill.restype = C.c_int
-    lib.vqa_qwen25vl_generate_step.argtypes = [vp, C.POINTER(VqaQwen25VLGeneration), i32, i32, i32, vp, C.c_size_t, vp]
-    lib.vqa_qwen25vl_generate_step.restype = C.c_int
-    lib.vqa_op_answer_logprob.argtypes = [vp, i32, i32, vp, f32, f32, vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, vp]
-    lib.vqa_op_answer_logprob.restype = C.c_int
-    lib.vqa_op_kv_cache_write.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, i32, vp]
-    lib.vqa_op_kv_cache_write.restype = C.c_int
-    lib.vqa_op_decode_attention_d128.argtypes = [vp, i32, vp, vp, i32, vp, vp, i32, i32, i32, f32, i32, vp, C.c_size_t, C.POINTER(i32), vp,
-                                                 i32, vp]
-    lib.vqa_op_decode_attention_d128.restype = C.c_int
-    lib.vqa_op_greedy_select.argtypes = [vp, i32, i32, vp, f32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.vqa_op_greedy_select.restype = C.c_int
-    lib.vqa_t5_bucket_lut.argtypes = [i32, i32, i32, C.POINTER(i32)]
-    lib.vqa_t5_bucket_lut.restype = C.c_int
-    lib.vqa_op_t5_decoder_self_attn.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]
-    lib.vqa_op_t5_decoder_self_attn.restype = C.c_int
-    lib.vqa_op_t5_decode_self_attn.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
-    lib.vqa_op_t5_decode_self_attn.restype = C.c_int
-    lib.vqa_op_gemm_bf16_f32acc.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, vp, i32, vp]
-    lib.vqa_op_gemm_bf16_f32acc.restype = C.c_int
-    lib.vqa_op_gemm_bf16_batched.argtypes = [vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i64, i64, i64, i64, i64, i32, vp]
-    lib.vqa_op_gemm_bf16_batched.restype = C.c_int
-    lib.vqa_op_t5_cross_attention.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, C.c_size_t, C.POINTER(C.c_size_t), vp]
-    lib.vqa_op_t5_cross_attention.restype = C.c_int
-    lib.vqa_op_layernorm_f32.argtypes = [vp, vp, vp, vp, i32, i32, f32, vp]
-    lib.vqa_op_layernorm_f32.restype = C.c_int
-    lib.vqa_op_clip_embed_ln.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp]
-    lib.vqa_op_clip_embed_ln.restype = C.c_int
-    lib.vqa_op_qwen_rope.argtypes = [vp, i32, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
-    lib.vqa_op_qwen_rope.restype = C.c_int
-    lib.vqa_op_gather_rows.argtypes = [vp, vp, vp, i32, i32, i32, vp]
-    lib.vqa_op_gather_rows.restype = C.c_int
-    lib.vqa_op_qwen_embed.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]
-    lib.vqa_op_qwen_embed.restype = C.c_int
-    lib.vqa_op_token_bitmap.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, vp]
-    lib.vqa_op_token_bitmap.restype = C.c_int
-    lib.vqa_op_topk_softmax.argtypes = [vp, i64, i32, i32, f32, vp, f32, i32, vp, vp, vp]
-    lib.vqa_op_topk_softmax.restype = C.c_int
-    lib.vqa_op_patchify.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp]
-    lib.vqa_op_patchify.restype = C.c_int
-    lib.vqa_op_splice_embed.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, i32, i32, i32, i32, i32, vp]
-    lib.vqa_op_splice_embed.restype = C.c_int
-    lib.vqa_op_decoder_embed.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, vp]
-    lib.vqa_op_decoder_embed.restype = C.c_int
-    lib.vqa_op_t5_bias_table.argtypes = [vp, vp, i32, vp, i32, i32, vp]
-    lib.vqa_op_t5_bias_table.restype = C.c_int
-    lib.vqa_op_lmhead_score.argtypes = [vp, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, C.c_size_t, C.POINTER(C.c_size_t), vp]
-    lib.vqa_op_lmhead_score.restype = C.c_int
-    lib.vqa_op_row_ssq.argtypes = [vp, vp, i32, i32, i32, vp]
-    lib.vqa_op_row_ssq.restype = C.c_int
-    lib.vqa_clipt5_generate_workspace_bytes.argtypes = [vp, i32, i32, i32, i32]
-    lib.vqa_clipt5_generate_workspace_bytes.restype = C.c_size_t
-    lib.vqa_clipt5_generate_prefill.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]
-    lib.vqa_clipt5_generate_prefill.restype = C.c_int
-    lib.vqa_clipt5_generate_step.argtypes = [vp, i32, i32, i32, vp, i32, i32, vp, vp, vp, vp, C.c_size_t, vp]
-    lib.vqa_clipt5_generate_step.restype = C.c_int
-    lib.vqa_clip_preprocess_workspace_bytes.argtypes = [C.POINTER(i32), C.POINTER(i32), i32, i32, i32]
-    lib.vqa_clip_preprocess_workspace_bytes.restype = C.c_size_t
-    lib.vqa_clip_preprocess.argtypes = [vp, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, C.POINTER(C.c_uint8),
-                                        C.POINTER(C.c_float), C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
-    lib.vqa_clip_preprocess.restype = C.c_int
-    lib.vqa_qwen_preprocess_plan.argtypes = [C.POINTER(i32), C.POINTER(i32), i32, i32, i32, i64, i64, C.POINTER(i32), C.POINTER(i64),
-                                             C.POINTER(C.c_size_t)]
-    lib.vqa_qwen_preprocess_plan.restype = C.c_int
-    lib.vqa_qwen_preprocess.argtypes = [vp, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, i32, i64, i64,
-                                        C.POINTER(C.c_float), C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
-    lib.vqa_qwen_preprocess.restype = C.c_int
-    lib.vqa_qwen_preprocess_video_plan.argtypes = [C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, i32, i64, i64,
-                                                   C.POINTER(i32), C.POINTER(i64), C.POINTER(C.c_size_t)]
-    lib.vqa_qwen_preprocess_video_plan.restype = C.c_int
-    lib.vqa_qwen_preprocess_video.argtypes = [vp, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, i32,
-                                              i32, i64, i64, C.POINTER(C.c_float), C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
-    lib.vqa_qwen_preprocess_video.restype = C.c_int
-    lib.vqa_qwen_preprocess_video_aa_plan.argtypes = [i32, i32, i32, i32, C.POINTER(i32), i32, C.POINTER(i32), i32, i32, i32, i32, i32,
-                                                      C.POINTER(i64), C.POINTER(C.c_size_t)]
-    lib.vqa_qwen_preprocess_video_aa_plan.restype = C.c_int
-    lib.vqa_qwen_preprocess_video_aa.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, C.POINTER(i32), C.POINTER(C.c_float), i32,
-                                                 C.POINTER(i32), C.POINTER(C.c_float), i32, i32, i32, i32, C.POINTER(C.c_float),
-                                                 C.POINTER(C.c_float), vp, i32, vp, C.c_size_t, vp, vp]
-    lib.vqa_qwen_preprocess_video_aa.restype = C.c_int
-    lib.vqa_clipt5_debug_layout.argtypes = [vp, i32, i32, i32, i32, C.POINTER(C.c_size_t), i32]
-    lib.vqa_clipt5_debug_layout.restype = C.c_int
-    lib.vqa_qwen25vl_debug_layout.argtypes = [vp, i32, i64, i32, C.POINTER(C.c_size_t), i32]
-    lib.vqa_qwen25vl_debug_layout.restype = C.c_int
-    lib.vqa_set_gemm_schedule.argtypes = [i32, i32]
-    lib.vqa_set_gemm_schedule.restype = C.c_int
-    lib.vqa_op_attention_d128_ex.argtypes = [vp, i32, i64, i32, i32, i32, vp, i32, i32, i32, i32, i32, vp, vp, f32, i32, i32, i32, i32, vp]
-    lib.vqa_op_attention_d128_ex.restype = C.c_int
-    lib.vqa_op_gemm_bf16_grouped.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, vp, i32, i32, i32, vp]
-    lib.vqa_op_gemm_bf16_grouped.restype = C.c_int
-    lib.vqa_op_gemm_bf16_splitk.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, i32, i32, vp, vp, i32, i32, vp, C.c_size_t, C.POINTER(i32), vp]
-    lib.vqa_op_gemm_bf16_splitk.restype = C.c_int
-    lib.vqa_debug_max_active_clusters.argtypes = [i32]
-    lib.vqa_debug_max_active_clusters.restype = C.c_int
-    lib.vqa_debug_pdl_enabled.argtypes = []
-    lib.vqa_debug_pdl_enabled.restype = C.c_int
-    lib.vqa_debug_set_preprocess_tiles.argtypes = [i32, i32, i32]
-    lib.vqa_debug_set_preprocess_tiles.restype = C.c_int
-    lib.vqa_debug_preprocess_geometry.argtypes = [i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), i32, i32, i32, i32, i32,
-                                                  i32, i64, i64, C.POINTER(i32)]
-    lib.vqa_debug_preprocess_geometry.restype = C.c_int
-    lib.vqa_resample_table.argtypes = [i32, i32, i32, i32, C.POINTER(i32), C.POINTER(i32)]
-    lib.vqa_resample_table.restype = i32
+    for name, (restype, argtypes) in PROTOTYPES.items():
+        if not hasattr(lib, name):
+            raise ImportError(f"{path} does not export {name}")
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 

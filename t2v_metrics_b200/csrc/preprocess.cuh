@@ -552,19 +552,6 @@ inline bool pre_plan_qwen_video(const int32_t* n_frames, const int32_t* heights,
     return true;
 }
 
-// Qwen still images only: image i's rows start at sum_{j<i} gh_j * gw_j. grid_hw[i] = (gh, gw) in patches.
-inline bool pre_plan_qwen(const int32_t* heights, const int32_t* widths, const int64_t* offsets, int n, int patch, int merge, int temporal,
-                          long long min_pixels, long long max_pixels, PrePlan& plan, int32_t* grid_hw, long long* total_rows) {
-    const std::vector<int32_t> one(n, 1), still(n, 0);
-    std::vector<int32_t> thw(3 * (size_t)n);
-    if (!pre_plan_qwen_video(one.data(), heights, widths, still.data(), offsets, n, patch, merge, temporal, min_pixels, max_pixels, plan,
-                             thw.data(), total_rows))
-        return false;
-    if (grid_hw)
-        for (int i = 0; i < n; ++i) { grid_hw[2 * i] = thw[3 * i + 1]; grid_hw[2 * i + 1] = thw[3 * i + 2]; }
-    return true;
-}
-
 // ---------------------------------------------------------------------------------------------- torch's antialiased bicubic resize
 // A video FILE reaches the Qwen processor through qwen_vl_utils fetch_video, which resizes the sampled frames as one tensor with
 // torchvision resize(BICUBIC, antialias=True): uint8 -> fp32, torch's _upsample_bicubic2d_aa, clamp to [0, 255], round half to even, uint8.

@@ -6,7 +6,7 @@
 
 // ------------------------------------------------------------------------------------------------ C ABI: lifecycle
 extern "C" const char* vqa_version(void) {
-    return "vqa_b200 abi=2 arch=sm_90a kernels=wgmma-gemm,flash-d64,t5-norm,lmhead-lse";
+    return "vqa_b200 abi=3 arch=sm_90a kernels=wgmma-gemm,flash-d64,t5-norm,lmhead-lse";
 }
 
 // Host mirror of T5Attention._relative_position_bucket (modeling_t5.py:189-234), fp32 like torch.
@@ -1031,37 +1031,6 @@ extern "C" int vqa_clip_preprocess(const void* src, const int64_t* offsets, cons
                                host_staging, reinterpret_cast<cudaStream_t>(stream));
 }
 
-extern "C" int vqa_qwen_preprocess_plan(const int32_t* heights, const int32_t* widths, int32_t n_images, int32_t patch, int32_t merge,
-                                        int64_t min_pixels, int64_t max_pixels, int32_t* grid_hw, int64_t* total_patches,
-                                        size_t* workspace_bytes) {
-    if (!heights || !widths || n_images <= 0 || patch <= 0 || merge <= 0 || min_pixels <= 0 || max_pixels < min_pixels)
-        return fail(nullptr, VQA_ERR_INVALID_ARG, "bad argument");
-    PrePlan plan;
-    std::vector<int64_t> off(n_images, 0);
-    long long rows = 0;
-    if (!pre_plan_qwen(heights, widths, off.data(), n_images, patch, merge, 1, min_pixels, max_pixels, plan, grid_hw, &rows))
-        return fail(nullptr, VQA_ERR_INVALID_ARG, plan.error);
-    if (total_patches) *total_patches = rows;
-    if (workspace_bytes) *workspace_bytes = plan.bytes();
-    return VQA_OK;
-}
-
-extern "C" int vqa_qwen_preprocess(const void* src, const int64_t* offsets, const int32_t* heights, const int32_t* widths, int32_t n_images,
-                                   int32_t patch, int32_t temporal_patch, int32_t merge, int64_t min_pixels, int64_t max_pixels,
-                                   const float* mean, const float* stdv, void* out, int32_t out_dtype, void* workspace,
-                                   size_t workspace_bytes, void* host_staging, void* stream) {
-    if (!src || !offsets || !heights || !widths || !mean || !stdv || !out || !workspace) return fail(nullptr, VQA_ERR_INVALID_ARG, "null pointer");
-    if (n_images <= 0 || patch <= 0 || merge <= 0 || temporal_patch <= 0 || min_pixels <= 0 || max_pixels < min_pixels)
-        return fail(nullptr, VQA_ERR_INVALID_ARG, "bad argument");
-    if (out_dtype != VQA_DTYPE_F32 && out_dtype != VQA_DTYPE_BF16) return fail(nullptr, VQA_ERR_INVALID_ARG, "out_dtype must be f32 or bf16");
-    PrePlan plan;
-    if (!pre_plan_qwen(heights, widths, offsets, n_images, patch, merge, temporal_patch, min_pixels, max_pixels, plan, nullptr, nullptr))
-        return fail(nullptr, VQA_ERR_INVALID_ARG, plan.error);
-    const uint8_t no_bg[3] = {0, 0, 0};
-    return pre_launch<PRE_QWEN_PATCHES>(plan, src, n_images, no_bg, mean, stdv, PrePatchGeom{patch, merge, temporal_patch}, out, out_dtype,
-                                        workspace, workspace_bytes, host_staging, reinterpret_cast<cudaStream_t>(stream));
-}
-
 static int qwen_video_args(const int32_t* n_frames, const int32_t* heights, const int32_t* widths, const int32_t* is_video, int32_t n_items,
                            int32_t patch, int32_t temporal_patch, int32_t merge, int64_t min_pixels, int64_t max_pixels, int64_t* frames) {
     if (!n_frames || !heights || !widths || !is_video || n_items <= 0 || patch <= 0 || merge <= 0 || temporal_patch <= 0 || min_pixels <= 0 ||
@@ -1120,7 +1089,7 @@ extern "C" int vqa_debug_set_preprocess_tiles(int32_t tile_rows, int32_t tile_co
 }
 
 // Host-only: the launch geometry the planner gives each item of a vqa_clip_preprocess (layout 0: heights / widths / n_items / out_size /
-// pad_to_square) or vqa_qwen_preprocess(_video) call (layout 1: n_frames / is_video NULL = still images). geometry [n_items][5] =
+// pad_to_square) or vqa_qwen_preprocess_video call (layout 1: n_frames / is_video NULL = still images). geometry [n_items][5] =
 // (tile_rows, tile_cols, col_tiles, chunk_groups, band_groups); the frames of a stack share their item's geometry.
 extern "C" int vqa_debug_preprocess_geometry(int32_t layout, const int32_t* n_frames, const int32_t* heights, const int32_t* widths,
                                              const int32_t* is_video, int32_t n_items, int32_t out_size, int32_t pad_to_square, int32_t patch,

@@ -30,9 +30,30 @@ def _stream_ptr(device) -> C.c_void_p:
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def _dtype_code(dtype: torch.dtype) -> int:
+    """The vqa_dtype of an fp32 or bf16 tensor."""
+    return _lib.VQA_DTYPE_F32 if dtype == torch.float32 else _lib.VQA_DTYPE_BF16
+
+
 def _check(rc: int, handle=None, what: str = ""):
     if rc != 0:
         raise RuntimeError(f"libvqa_b200 {what} failed (status {rc}): {_lib.last_error(handle)}")
+
+
+def _call(name: str, *args):
+    """Call `name` in libvqa_b200.so; a non-zero status raises RuntimeError naming it."""
+    _check(getattr(_lib.load(), name)(*args), None, name)
+
+
+def _size_query(name: str, ctype, head: tuple, tail: tuple) -> int:
+    """Call `name` without scratch (NULL, 0 bytes between `head` and `tail`). It stops at its scratch check with VQA_ERR_WORKSPACE and
+    reports through the pointer after the scratch arguments the size (or split count) it needs, which this returns. Any other status is
+    an argument error and raises."""
+    value = ctype(0)
+    rc = getattr(_lib.load(), name)(*head, None, 0, C.byref(value), *tail)
+    if rc != _lib.VQA_ERR_WORKSPACE:
+        raise RuntimeError(f"libvqa_b200 {name} without scratch returned status {rc}, not VQA_ERR_WORKSPACE: {_lib.last_error(None)}")
+    return int(value.value)
 
 
 def fold_norm_gain(weight: torch.Tensor, gamma: torch.Tensor) -> torch.Tensor:
@@ -110,37 +131,29 @@ def convert_state_dict(sd: Dict[str, torch.Tensor], cfg: ClipT5Config, device, f
     return out
 
 
-class ClipT5Engine:
-    """One engine = one model replica on one GPU (one process per GPU; SURVEY section 8e)."""
+class _Engine:
+    """What both engines share: one library handle on one device, weight binding, profiling, the scoring workspace, and greedy
+    generation (its own workspace, one state per call shape, the decode loop)."""
 
-    def __init__(self, cfg: ClipT5Config, device="cuda:0", emulate_bf16_rounding: bool = True,
-                 cross_attention_mode: str = "absorbed", round_attention_scores: bool = False, fuse_norms: bool = False):
-        """round_attention_scores: form the bf16 score tensors of the reference's eager attention before the softmax (off: fp32 scores --
-        closer to the exact result, and measured no closer to the bf16 reference, DESIGN.md section 4). fuse_norms: fold the encoder's
-        T5LayerNorms into the GEMMs around them (no normalised copy of the residual stream; a different, equally valid rounding point)."""
+    MAX_GEN_GRAPHS = 8
+
+    def __init__(self, cfg, device, create: str, config):
+        """create: the vqa_create_* entry point that makes the handle from the config struct `config`."""
         if not torch.cuda.is_available():
-            raise RuntimeError("ClipT5Engine needs a CUDA device (sm_90a); there is no CPU path")
+            raise RuntimeError(f"{type(self).__name__} needs a CUDA device (sm_90a); there is no CPU path")
         self.lib = _lib.load()
         self.cfg = cfg
         self.device = torch.device(device)
         idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        c = _lib.VqaClipT5Config(
-            image_size=cfg.image_size, patch_size=cfg.patch_size, vit_hidden=cfg.vit_hidden, vit_heads=cfg.vit_heads,
-            vit_mlp=cfg.vit_mlp, vit_layers_run=cfg.vit_layers - 1, vit_ln_eps=cfg.vit_ln_eps, d_model=cfg.d_model,
-            n_heads=cfg.n_heads, d_ff=cfg.d_ff, enc_layers=cfg.enc_layers, dec_layers=cfg.dec_layers, vocab=cfg.vocab,
-            rel_buckets=cfg.rel_buckets, rel_max_distance=cfg.rel_max_distance, t5_ln_eps=cfg.t5_ln_eps,
-            image_token_id=IMAGE_TOKEN_INDEX, pad_token_id=cfg.pad_token_id, decoder_start_id=cfg.decoder_start_id,
-            emulate_bf16_rounding=(1 if emulate_bf16_rounding else 0) | (2 if round_attention_scores else 0) | (4 if fuse_norms else 0),
-            cross_attention_mode={"absorbed": 0, "reference": 1}[cross_attention_mode])
-        self.fuse_norms = bool(fuse_norms)
-        if cfg.d_kv != 64:
-            raise ValueError("the engine's attention kernels are specialised for d_kv == 64")
         self._h = C.c_void_p()
         with torch.cuda.device(idx):
-            _check(self.lib.vqa_create_clipt5(C.byref(c), idx, C.byref(self._h)), None, "vqa_create_clipt5")
+            _check(getattr(self.lib, create)(C.byref(config), idx, C.byref(self._h)), None, create)
         self._weights: Dict[str, torch.Tensor] = {}
         self._workspace: Optional[torch.Tensor] = None
-        self._graphs: Dict[tuple, tuple] = {}      # CUDA graphs of whole forwards, keyed by the call's shapes (score_tensors_graphed)
+        self._graphs: Dict[tuple, tuple] = {}      # CUDA graphs of whole scoring forwards, keyed by the call's shapes
+        self._gen_workspace: Optional[torch.Tensor] = None
+        self._gen_states: "collections.OrderedDict[tuple, dict]" = collections.OrderedDict()   # per generation call shape, LRU order
+        self._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)                   # the decode loop's all-finished read-back
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -148,14 +161,24 @@ class ClipT5Engine:
             self.lib.vqa_destroy(h)
             self._h = C.c_void_p()
 
+    def _run(self, name: str, *args):
+        """Call the handle entry point `name` (the handle is its first argument) with the engine's device current -- the library launches
+        on the current device, and a process may drive several GPUs -- and raise on a non-zero status."""
+        with torch.cuda.device(self.device):
+            rc = getattr(self.lib, name)(self._h, *args)
+        _check(rc, self._h, name)
+
+    def _grow(self, attr: str, need: int, dependents: dict) -> torch.Tensor:
+        """The workspace self.<attr>, reallocated when it holds fewer than `need` bytes. The captured graphs or generation states in
+        `dependents` point into the old one and are dropped with it."""
+        if getattr(self, attr) is None or getattr(self, attr).numel() < need:
+            dependents.clear()
+            setattr(self, attr, None)        # free the old workspace before allocating the larger one
+            setattr(self, attr, torch.empty(need, dtype=torch.uint8, device=self.device))
+        return getattr(self, attr)
+
     # ---- weights
     def bind_engine_tensors(self, tensors: Dict[str, torch.Tensor]):
-        if getattr(self, "fuse_norms", False) and "t5.enc.0.qkv" in tensors and "t5.enc.0.qkv_g" not in tensors:
-            tensors = dict(tensors)       # engine-layout weights without the folded copies (synthetic / shared dicts): derive them
-            for l in range(self.cfg.enc_layers):
-                q = f"t5.enc.{l}."
-                tensors[q + "qkv_g"] = fold_norm_gain(tensors[q + "qkv"], tensors[q + "ln0"])
-                tensors[q + "wi_g"] = fold_norm_gain(tensors[q + "wi"], tensors[q + "ln1"])
         arr = (_lib.VqaTensor * len(tensors))()
         keep = []
         for i, (name, t) in enumerate(tensors.items()):
@@ -168,14 +191,114 @@ class ClipT5Engine:
                 arr[i].shape[d] = t.shape[d] if d < t.dim() else 1
             arr[i].ndim = t.dim()
             arr[i].dtype = _lib.VQA_DTYPE_BF16
-        _check(self.lib.vqa_bind_weights(self._h, arr, len(tensors)), self._h, "vqa_bind_weights")
+        self._run("vqa_bind_weights", arr, len(tensors))
         self._weights.update(tensors)  # keep the borrowed memory alive
-        _check(self.lib.vqa_finalize_weights(self._h), self._h, "vqa_finalize_weights")
+        self._run("vqa_finalize_weights")
+
+    # ---- launch count and profiling
+    def last_launch_count(self) -> int:
+        return int(self.lib.vqa_last_launch_count(self._h))
+
+    def set_profile(self, enable: bool):
+        self._run("vqa_set_profile", 1 if enable else 0)
+
+    def read_profile(self):
+        """After torch.cuda.synchronize(): {category: (device_ms, algorithmic_flops, scopes, algorithmic_bytes)} of the last call."""
+        ms = (C.c_float * 4)()
+        fl = (C.c_double * 4)()
+        by = (C.c_double * 4)()
+        sc = (C.c_int64 * 4)()
+        self._run("vqa_profile_read", ms, fl, by, sc)
+        names = ("gemm", "attention", "norm", "other")
+        return {n: (float(ms[i]), float(fl[i]), int(sc[i]), float(by[i])) for i, n in enumerate(names)}
+
+    # ---- greedy generation
+    def _gen_state(self, key: tuple, need: int, make) -> dict:
+        """The generation state of call shape `key`, made by make() on first use, with the generation workspace grown to `need` bytes.
+        The MAX_GEN_GRAPHS most recently used states (each with its captured step graph) are kept."""
+        self._grow("_gen_workspace", need, self._gen_states)
+        st = self._gen_states.get(key)
+        if st is None:
+            st = self._gen_states[key] = make()
+            while len(self._gen_states) > self.MAX_GEN_GRAPHS:
+                self._gen_states.popitem(last=False)         # least recently used shape first
+        self._gen_states.move_to_end(key)
+        return st
+
+    def _decode_loop(self, st: dict, use_graph: bool, check_every: int):
+        """Decode steps (generate_step) after generate_begin until every prompt has finished: a CUDA graph of the step captured once per
+        state, replayed. The host reads the all-finished flag through pinned memory every `check_every` steps. Returns (each prompt's
+        generated ids, lengths [B] on the host)."""
+        flag = self._gen_flag
+        ev = torch.cuda.Event()
+
+        def finished() -> bool:
+            flag.copy_(st["all_done"], non_blocking=True)
+            ev.record()
+            ev.synchronize()
+            return bool(flag[0])
+
+        for step in range(1, st["max_new"]):
+            if (step - 1) % check_every == 0 and finished():
+                break
+            if not use_graph:
+                self.generate_step(st)
+            elif st["graph"] is None:
+                self.generate_step(st)             # the first step runs directly (module loading, kernel attributes), then is captured
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    self.generate_step(st)
+                st["graph"] = graph
+            else:
+                st["graph"].replay()
+        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
+        return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])], lengths
+
+
+class ClipT5Engine(_Engine):
+    """One engine = one model replica on one GPU (one process per GPU; SURVEY section 8e)."""
+
+    def __init__(self, cfg: ClipT5Config, device="cuda:0", emulate_bf16_rounding: bool = True,
+                 cross_attention_mode: str = "absorbed", round_attention_scores: bool = False, fuse_norms: bool = False):
+        """round_attention_scores: form the bf16 score tensors of the reference's eager attention before the softmax (off: fp32 scores --
+        closer to the exact result, and measured no closer to the bf16 reference, DESIGN.md section 4). fuse_norms: fold the encoder's
+        T5LayerNorms into the GEMMs around them (no normalised copy of the residual stream; a different, equally valid rounding point)."""
+        c = _lib.VqaClipT5Config(
+            image_size=cfg.image_size, patch_size=cfg.patch_size, vit_hidden=cfg.vit_hidden, vit_heads=cfg.vit_heads,
+            vit_mlp=cfg.vit_mlp, vit_layers_run=cfg.vit_layers - 1, vit_ln_eps=cfg.vit_ln_eps, d_model=cfg.d_model,
+            n_heads=cfg.n_heads, d_ff=cfg.d_ff, enc_layers=cfg.enc_layers, dec_layers=cfg.dec_layers, vocab=cfg.vocab,
+            rel_buckets=cfg.rel_buckets, rel_max_distance=cfg.rel_max_distance, t5_ln_eps=cfg.t5_ln_eps,
+            image_token_id=IMAGE_TOKEN_INDEX, pad_token_id=cfg.pad_token_id, decoder_start_id=cfg.decoder_start_id,
+            emulate_bf16_rounding=(1 if emulate_bf16_rounding else 0) | (2 if round_attention_scores else 0) | (4 if fuse_norms else 0),
+            cross_attention_mode={"absorbed": 0, "reference": 1}[cross_attention_mode])
+        self.fuse_norms = bool(fuse_norms)
+        if cfg.d_kv != 64:
+            raise ValueError("the engine's attention kernels are specialised for d_kv == 64")
+        super().__init__(cfg, device, "vqa_create_clipt5", c)
+
+    # ---- weights
+    def bind_engine_tensors(self, tensors: Dict[str, torch.Tensor]):
+        if self.fuse_norms and "t5.enc.0.qkv" in tensors and "t5.enc.0.qkv_g" not in tensors:
+            tensors = dict(tensors)       # engine-layout weights without the folded copies (synthetic / shared dicts): derive them
+            for l in range(self.cfg.enc_layers):
+                q = f"t5.enc.{l}."
+                tensors[q + "qkv_g"] = fold_norm_gain(tensors[q + "qkv"], tensors[q + "ln0"])
+                tensors[q + "wi_g"] = fold_norm_gain(tensors[q + "wi"], tensors[q + "ln1"])
+        super().bind_engine_tensors(tensors)
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor]):
         self.bind_engine_tensors(convert_state_dict(sd, self.cfg, self.device, fuse_norms=self.fuse_norms))
 
     # ---- forward
+    @staticmethod
+    def _check_inputs(pixel_values: torch.Tensor, image_index: Optional[torch.Tensor], input_ids: torch.Tensor, *int32_tensors):
+        assert pixel_values.is_cuda and pixel_values.dim() == 4 and pixel_values.is_contiguous()
+        assert pixel_values.dtype in (torch.float32, torch.bfloat16)
+        for t in (input_ids, *int32_tensors):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+        if image_index is not None:
+            assert image_index.is_cuda and image_index.dtype == torch.int32 and image_index.shape == (input_ids.shape[0],)
+
     def workspace_bytes(self, batch: int, n_images: int, text_len: int, label_len: int) -> int:
         return int(self.lib.vqa_clipt5_workspace_bytes(self._h, batch, n_images, text_len, label_len))
 
@@ -186,29 +309,16 @@ class ClipT5Engine:
         labels [B,T] int32 (-100 = ignore); image_index [B] int32 or None. Returns scores [B] fp32 on the device
         (enqueued on the current stream; no synchronisation)."""
         dev = self.device
-        assert pixel_values.is_cuda and pixel_values.dim() == 4 and pixel_values.is_contiguous()
-        assert pixel_values.dtype in (torch.float32, torch.bfloat16)
-        for t in (input_ids, text_lens, labels):
-            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+        self._check_inputs(pixel_values, image_index, input_ids, text_lens, labels)
         B, L = input_ids.shape
         T = labels.shape[1]
         NI = pixel_values.shape[0]
-        if image_index is not None:
-            assert image_index.is_cuda and image_index.dtype == torch.int32 and image_index.shape == (B,)
-        need = self.workspace_bytes(B, NI, L, T)
-        if self._workspace is None or self._workspace.numel() < need:
-            self._graphs.clear()              # captured graphs point into the old workspace
-            self._workspace = None
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+        ws = self._grow("_workspace", self.workspace_bytes(B, NI, L, T), self._graphs)
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=dev)
         logp = torch.zeros(B, T, dtype=torch.float32, device=dev) if return_logprobs else None   # ignored (-100) positions stay 0
-        pdt = _lib.VQA_DTYPE_F32 if pixel_values.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
-        with torch.cuda.device(dev):      # the library launches on the CURRENT device: make it the engine's (a process may drive several GPUs)
-            rc = self.lib.vqa_clipt5_score(self._h, _ptr(pixel_values), pdt, NI, _ptr(image_index), _ptr(input_ids),
-                                           _ptr(text_lens), _ptr(labels), B, L, T, _ptr(out), _ptr(logp),
-                                           _ptr(self._workspace), self._workspace.numel(), _stream_ptr(dev))
-        _check(rc, self._h, "vqa_clipt5_score")
+        self._run("vqa_clipt5_score", _ptr(pixel_values), _dtype_code(pixel_values.dtype), NI, _ptr(image_index), _ptr(input_ids),
+                  _ptr(text_lens), _ptr(labels), B, L, T, _ptr(out), _ptr(logp), _ptr(ws), ws.numel(), _stream_ptr(dev))
         return (out, logp) if return_logprobs else out
 
     MAX_GRAPHS = 16
@@ -257,14 +367,11 @@ class ClipT5Engine:
         d = [t.to(dev, non_blocking=True) if t is not None else None for t in (input_ids, text_lens, labels, image_index)]
         return self.score_tensors(pixels, d[0], d[1], d[2], image_index=d[3]).cpu()
 
-    def last_launch_count(self) -> int:
-        return int(self.lib.vqa_last_launch_count(self._h))
-
     def debug_tensors(self, batch: int, n_images: int, text_len: int, label_len: int) -> Dict[str, torch.Tensor]:
         """Views into the workspace of the LAST call with these sizes (synchronise first): encoder / decoder outputs after their
         final norms, projector output, residual streams. Parity investigations only."""
         off = (C.c_size_t * 6)()
-        _check(self.lib.vqa_clipt5_debug_layout(self._h, batch, n_images, text_len, label_len, off, 6), self._h, "vqa_clipt5_debug_layout")
+        self._run("vqa_clipt5_debug_layout", batch, n_images, text_len, label_len, off, 6)
         cfg = self.cfg
         S = text_len - 1 + cfg.num_patches
         ws = self._workspace
@@ -277,22 +384,7 @@ class ClipT5Engine:
                     vit_hidden=ws[off[5]:off[5] + n_images * (cfg.num_patches + 1) * cfg.vit_hidden * 4].view(torch.float32)
                     .view(n_images, cfg.num_patches + 1, cfg.vit_hidden))
 
-    def set_profile(self, enable: bool):
-        _check(self.lib.vqa_set_profile(self._h, 1 if enable else 0), self._h, "vqa_set_profile")
-
-    def read_profile(self):
-        """After torch.cuda.synchronize(): {category: (device_ms, algorithmic_flops, scopes, algorithmic_bytes)} of the last call."""
-        ms = (C.c_float * 4)()
-        fl = (C.c_double * 4)()
-        by = (C.c_double * 4)()
-        sc = (C.c_int64 * 4)()
-        _check(self.lib.vqa_profile_read(self._h, ms, fl, by, sc), self._h, "vqa_profile_read")
-        names = ("gemm", "attention", "norm", "other")
-        return {n: (float(ms[i]), float(fl[i]), int(sc[i]), float(by[i])) for i, n in enumerate(names)}
-
     # ------------------------------------------------------------------------------------------ greedy generation
-    MAX_GEN_GRAPHS = 8
-
     def generate_begin(self, pixel_values: torch.Tensor, input_ids: torch.Tensor, text_lens: torch.Tensor, max_new_tokens: int,
                        eos_ids: Sequence[int], image_index: Optional[torch.Tensor] = None) -> dict:
         """The prefill of a greedy generation (vqa_clipt5_generate_prefill): the encoder pass of score_tensors over the same inputs (no
@@ -300,56 +392,36 @@ class ClipT5Engine:
         tensors `tokens` [B, max_new_tokens] (-1 after a prompt's last token), `lengths` [B] and `all_done` [1], all owned by the state of
         this call shape. The generation workspace is separate from the scoring one, so scoring graphs are never invalidated by it."""
         dev = self.device
-        assert pixel_values.is_cuda and pixel_values.dim() == 4 and pixel_values.is_contiguous()
-        assert pixel_values.dtype in (torch.float32, torch.bfloat16)
-        for t in (input_ids, text_lens):
-            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+        self._check_inputs(pixel_values, image_index, input_ids, text_lens)
         B, L = input_ids.shape
         NI = pixel_values.shape[0]
-        if image_index is not None:
-            assert image_index.is_cuda and image_index.dtype == torch.int32 and image_index.shape == (B,)
         max_new = int(max_new_tokens)
         eos = [int(e) for e in eos_ids]
         need = int(self.lib.vqa_clipt5_generate_workspace_bytes(self._h, B, NI, L, max_new))
         if need == 0:
             raise ValueError(f"bad generation size: batch {B}, images {NI}, prompt length {L}, max_new_tokens {max_new}")
-        gens = self.__dict__.setdefault("_gen_states", collections.OrderedDict())
-        ws = getattr(self, "_gen_workspace", None)
-        if ws is None or ws.numel() < need:
-            gens.clear()                         # captured step graphs point into the old workspace
-            self._gen_workspace = None
-            self._gen_workspace = torch.empty(need, dtype=torch.uint8, device=dev)
-        key = (B, NI, L, max_new, len(eos))
-        st = gens.get(key)
-        if st is None:
-            i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
-            st = gens[key] = dict(B=B, NI=NI, L=L, max_new=max_new, n_eos=len(eos), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new),
-                                  lengths=i32(B), all_done=i32(1), graph=None)
-            while len(gens) > self.MAX_GEN_GRAPHS:
-                gens.popitem(last=False)         # least recently used shape first
-        gens.move_to_end(key)
+        i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
+        st = self._gen_state((B, NI, L, max_new, len(eos)), need, lambda: dict(
+            B=B, NI=NI, L=L, max_new=max_new, n_eos=len(eos), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new), lengths=i32(B),
+            all_done=i32(1), graph=None))
         if eos:
             st["eos"].copy_(torch.as_tensor(eos, dtype=torch.int32), non_blocking=True)
-        pdt = _lib.VQA_DTYPE_F32 if pixel_values.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
+        pdt = _dtype_code(pixel_values.dtype)
 
         def prefill():
-            with torch.cuda.device(dev):
-                rc = self.lib.vqa_clipt5_generate_prefill(self._h, _ptr(pixel_values), pdt, NI, _ptr(image_index), _ptr(input_ids),
-                                                          _ptr(text_lens), B, L, _ptr(st["eos"]), len(eos), max_new, _ptr(st["tokens"]),
-                                                          _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(self._gen_workspace),
-                                                          self._gen_workspace.numel(), _stream_ptr(dev))
-            _check(rc, self._h, "vqa_clipt5_generate_prefill")
+            ws = self._gen_workspace
+            self._run("vqa_clipt5_generate_prefill", _ptr(pixel_values), pdt, NI, _ptr(image_index), _ptr(input_ids), _ptr(text_lens), B, L,
+                      _ptr(st["eos"]), len(eos), max_new, _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(ws),
+                      ws.numel(), _stream_ptr(dev))
         st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
         prefill()
         return st
 
     def generate_step(self, st: dict):
         """One decode step of the generation `st` (vqa_clipt5_generate_step), launched directly."""
-        with torch.cuda.device(self.device):
-            rc = self.lib.vqa_clipt5_generate_step(self._h, st["B"], st["NI"], st["L"], _ptr(st["eos"]), st["n_eos"], st["max_new"],
-                                                   _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(self._gen_workspace),
-                                                   self._gen_workspace.numel(), _stream_ptr(self.device))
-        _check(rc, self._h, "vqa_clipt5_generate_step")
+        ws = self._gen_workspace
+        self._run("vqa_clipt5_generate_step", st["B"], st["NI"], st["L"], _ptr(st["eos"]), st["n_eos"], st["max_new"], _ptr(st["tokens"]),
+                  _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(ws), ws.numel(), _stream_ptr(self.device))
 
     def generate_tensors(self, pixel_values: torch.Tensor, input_ids: torch.Tensor, text_lens: torch.Tensor, max_new_tokens: int,
                          eos_ids: Sequence[int], image_index: Optional[torch.Tensor] = None, use_graph: bool = True, check_every: int = 16):
@@ -358,38 +430,7 @@ class ClipT5Engine:
         MAX_GEN_GRAPHS most recently used shapes. The host reads the all-finished flag through pinned memory every `check_every` steps and
         never synchronises in between. Returns each prompt's generated ids, the EOS id included when one ended it."""
         st = self.generate_begin(pixel_values, input_ids, text_lens, max_new_tokens, eos_ids, image_index)
-        _decode_loop(self, st, use_graph, check_every)
-        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
-        return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]
-
-
-def _decode_loop(engine, st: dict, use_graph: bool, check_every: int):
-    """Decode steps (engine.generate_step) after generate_begin until every prompt has finished: a CUDA graph of the step captured once per
-    state, replayed. The host reads the all-finished flag through the engine's pinned buffer every `check_every` steps."""
-    flag = engine.__dict__.get("_gen_flag")
-    if flag is None:
-        flag = engine._gen_flag = torch.zeros(1, dtype=torch.int32, pin_memory=True)
-    ev = torch.cuda.Event()
-
-    def finished() -> bool:
-        flag.copy_(st["all_done"], non_blocking=True)
-        ev.record()
-        ev.synchronize()
-        return bool(flag[0])
-
-    for step in range(1, st["max_new"]):
-        if (step - 1) % check_every == 0 and finished():
-            break
-        if not use_graph:
-            engine.generate_step(st)
-        elif st["graph"] is None:
-            engine.generate_step(st)             # the first step runs directly (module loading, kernel attributes), then is captured
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                engine.generate_step(st)
-            st["graph"] = graph
-        else:
-            st["graph"].replay()
+        return self._decode_loop(st, use_graph, check_every)[0]
 
 
 # ------------------------------------------------------------------------------------------------ single-kernel ops
@@ -402,7 +443,6 @@ class ops:
     @staticmethod
     def gemm(a: torch.Tensor, w: torch.Tensor, bias=None, residual=None, epilogue="store", variant=0, out=None,
              gate_up_offset=0):
-        lib = _lib.load()
         M, K = a.shape
         n_rows = w.shape[0]
         epi = ops.EPI[epilogue]
@@ -410,10 +450,9 @@ class ops:
         n_out = n_rows // 2 if gated else n_rows
         if out is None:
             out = torch.empty(M, n_out, dtype=torch.bfloat16, device=a.device)
-        rc = lib.vqa_op_gemm_bf16(_ptr(a), a.stride(0), _ptr(w), w.stride(0), n_rows, _ptr(out), out.stride(0), M, n_rows,
-                                  K, _ptr(bias), _ptr(residual), residual.stride(0) if residual is not None else 0, epi,
-                                  gate_up_offset if gated else 0, variant, _stream_ptr(a.device))
-        _check(rc, None, "vqa_op_gemm_bf16")
+        _call("vqa_op_gemm_bf16", _ptr(a), a.stride(0), _ptr(w), w.stride(0), n_rows, _ptr(out), out.stride(0), M, n_rows, K, _ptr(bias),
+              _ptr(residual), residual.stride(0) if residual is not None else 0, epi, gate_up_offset if gated else 0, variant,
+              _stream_ptr(a.device))
         return out
 
     @staticmethod
@@ -421,7 +460,6 @@ class ops:
                       norm_dim: int = 0, eps: float = 1e-6, out=None):
         """GEMM with the fused-RMSNorm hooks (see include/vqa_b200.h). ssq_in / ssq_out: fp32 [M, stride] cuda, stride % 4 == 0.
         Returns (C, number of ssq_out slots written)."""
-        lib = _lib.load()
         M, K = a.shape
         n_rows = w.shape[0]
         epi = ops.EPI[epilogue]
@@ -431,11 +469,9 @@ class ops:
             out = torch.empty(M, n_out, dtype=torch.bfloat16, device=a.device)
         buf = ssq_in if ssq_in is not None else ssq_out
         parts = C.c_int32(0)
-        rc = lib.vqa_op_gemm_bf16_normfuse(_ptr(a), a.stride(0), _ptr(w), w.stride(0), n_rows, _ptr(out), out.stride(0), M, n_rows, K,
-                                           _ptr(residual), residual.stride(0) if residual is not None else 0, epi,
-                                           gate_up_offset if gated else 0, _ptr(ssq_in), _ptr(ssq_out), buf.shape[1], norm_dim or K, float(eps),
-                                           C.byref(parts), _stream_ptr(a.device))
-        _check(rc, None, "vqa_op_gemm_bf16_normfuse")
+        _call("vqa_op_gemm_bf16_normfuse", _ptr(a), a.stride(0), _ptr(w), w.stride(0), n_rows, _ptr(out), out.stride(0), M, n_rows, K,
+              _ptr(residual), residual.stride(0) if residual is not None else 0, epi, gate_up_offset if gated else 0, _ptr(ssq_in),
+              _ptr(ssq_out), buf.shape[1], norm_dim or K, float(eps), C.byref(parts), _stream_ptr(a.device))
         return out, int(parts.value)
 
     @staticmethod
@@ -443,19 +479,15 @@ class ops:
                        repetition_penalty: float = 1.0):
         """The Qwen2.5-VL score's lm_head: log softmax(penalised bf16 logits / temperature)[labels] of h [M, K] against w [N, K], without
         materialising the logits. pen_bitmap int32 [M, ceil(N / 32)] or None. Returns fp32 [M]."""
-        lib = _lib.load()
         M, K = h.shape
         N = w.shape[0]
         out = torch.empty(M, dtype=torch.float32, device=h.device)
-        need = C.c_size_t(0)
+        st = _stream_ptr(h.device)
         args = (_ptr(h), h.stride(0), _ptr(w), w.stride(0), M, N, K, _ptr(labels), float(temperature), _ptr(pen_bitmap), float(repetition_penalty),
                 _ptr(out))
-        rc = lib.vqa_op_lmhead_logprob(*args, None, 0, C.byref(need), _stream_ptr(h.device))
-        if rc != -4:        # a call without scratch stops at the scratch check and returns the size
-            _check(rc or -1, None, "vqa_op_lmhead_logprob")
-        scratch = torch.empty((need.value + 3) // 4, dtype=torch.float32, device=h.device)
-        rc = lib.vqa_op_lmhead_logprob(*args, _ptr(scratch), scratch.numel() * 4, None, _stream_ptr(h.device))
-        _check(rc, None, "vqa_op_lmhead_logprob")
+        need = _size_query("vqa_op_lmhead_logprob", C.c_size_t, args, (st,))
+        scratch = torch.empty((need + 3) // 4, dtype=torch.float32, device=h.device)
+        _call("vqa_op_lmhead_logprob", *args, _ptr(scratch), scratch.numel() * 4, None, st)
         return out
 
     @staticmethod
@@ -463,11 +495,9 @@ class ops:
                   bias_const_from: int = 0, round_scores: bool = False):
         """bias_const_from > 0 promises that bias_table[h] is constant for |key - query| >= bias_const_from on either side (T5:
         relative_attention_max_distance); 0 makes no assumption. round_scores: form the reference's bf16 score tensors before the softmax."""
-        lib = _lib.load()
         out = torch.empty(B * S, H * 64, dtype=torch.bfloat16, device=qkv.device)
-        rc = lib.vqa_op_attention_d64(_ptr(qkv), _ptr(out), B, S, H, _ptr(seq_lens), _ptr(bias_table), float(scale),
-                                      int(bias_const_from), 1 if round_scores else 0, _stream_ptr(qkv.device))
-        _check(rc, None, "vqa_op_attention_d64")
+        _call("vqa_op_attention_d64", _ptr(qkv), _ptr(out), B, S, H, _ptr(seq_lens), _ptr(bias_table), float(scale), int(bias_const_from),
+              1 if round_scores else 0, _stream_ptr(qkv.device))
         return out
 
     @staticmethod
@@ -477,7 +507,6 @@ class ops:
         """The per-step kernel of a scored rollout on given bf16 logits [B, V] (int32 answer_ids [B, n_max], answer_counts / lengths /
         done [B]; penalty_bitmap int32 [B, ceil(V / 32)] or None). Writes row lengths[b] of out_logp [B, max_new, n_max] and, with
         top_k > 0, of out_topk_ids / out_topk_probs [B, max_new, top_k]; returns the three outputs (allocated NaN / -1 when not given)."""
-        lib = _lib.load()
         B, V = logits.shape
         n_max = answer_ids.shape[1]
         dev = logits.device
@@ -486,10 +515,9 @@ class ops:
         if top_k > 0 and out_topk_ids is None:
             out_topk_ids = torch.full((B, max_new, top_k), -1, dtype=torch.int32, device=dev)
             out_topk_probs = torch.full((B, max_new, top_k), float("nan"), dtype=torch.float32, device=dev)
-        rc = lib.vqa_op_answer_logprob(_ptr(logits), B, V, _ptr(penalty_bitmap), float(repetition_penalty), float(temperature), _ptr(answer_ids),
-                                       _ptr(answer_counts), n_max, max_new, _ptr(lengths), _ptr(done), top_k, _ptr(out_logp), _ptr(out_topk_ids),
-                                       _ptr(out_topk_probs), _stream_ptr(dev))
-        _check(rc, None, "vqa_op_answer_logprob")
+        _call("vqa_op_answer_logprob", _ptr(logits), B, V, _ptr(penalty_bitmap), float(repetition_penalty), float(temperature), _ptr(answer_ids),
+              _ptr(answer_counts), n_max, max_new, _ptr(lengths), _ptr(done), top_k, _ptr(out_logp), _ptr(out_topk_ids), _ptr(out_topk_probs),
+              _stream_ptr(dev))
         return out_logp, out_topk_ids, out_topk_probs
 
     @staticmethod
@@ -497,11 +525,9 @@ class ops:
                        vc: torch.Tensor, gen_len=None):
         """The Qwen2.5-VL K/V cache write on packed rows qkv [B * S, ld] into kc / vc [B, kv_heads, cap, 128] (in place). gen_len None:
         prefill, row s < seq_lens[b] to slot s; gen_len int32 [B] (S == 1): decode, to slot seq_lens[b] + gen_len[b] - 1."""
-        lib = _lib.load()
         B, cap = kc.shape[0], kc.shape[2]
-        rc = lib.vqa_op_kv_cache_write(_ptr(qkv), qkv.stride(0), k_col0, v_col0, kv_heads, B, S, _ptr(seq_lens), _ptr(gen_len), _ptr(kc), _ptr(vc),
-                                       cap, _stream_ptr(qkv.device))
-        _check(rc, None, "vqa_op_kv_cache_write")
+        _call("vqa_op_kv_cache_write", _ptr(qkv), qkv.stride(0), k_col0, v_col0, kv_heads, B, S, _ptr(seq_lens), _ptr(gen_len), _ptr(kc),
+              _ptr(vc), cap, _stream_ptr(qkv.device))
 
     @staticmethod
     def decode_attention(q: torch.Tensor, kc: torch.Tensor, vc: torch.Tensor, seq_lens: torch.Tensor, gen_len: torch.Tensor, q_heads: int,
@@ -509,21 +535,16 @@ class ops:
         """Flash-decoding attention of query rows q [B, >= q_heads * 128] (row stride q.stride(0)) over kc / vc [B, kv_heads, cap, 128],
         sequence b over slots [0, seq_lens[b] + gen_len[b]). splits == 0: the generation's rule. Returns (out [B, q_heads * 128] or the given
         out, splits used)."""
-        lib = _lib.load()
         B, kv_heads, cap = kc.shape[0], kc.shape[1], kc.shape[2]
         if out is None:
             out = torch.empty(B, q_heads * 128, dtype=torch.bfloat16, device=q.device)
-        used = C.c_int32(0)
-        args = (_ptr(q), q.stride(0), _ptr(kc), _ptr(vc), cap, _ptr(seq_lens), _ptr(gen_len), B, q_heads, kv_heads, float(scale), splits)
-        if splits == 0:      # a call without workspace stops at the workspace check and returns the rule's split count
-            rc = lib.vqa_op_decode_attention_d128(*args, None, 0, C.byref(used), _ptr(out), out.stride(0), _stream_ptr(q.device))
-            if rc != -4:     # VQA_ERR_WORKSPACE is the expected answer; anything else is an argument error
-                _check(rc or -1, None, "vqa_op_decode_attention_d128")
-            splits = used.value
+        st = _stream_ptr(q.device)
+        args = (_ptr(q), q.stride(0), _ptr(kc), _ptr(vc), cap, _ptr(seq_lens), _ptr(gen_len), B, q_heads, kv_heads, float(scale))
+        if splits == 0:      # the rule's split count
+            splits = _size_query("vqa_op_decode_attention_d128", C.c_int32, (*args, 0), (_ptr(out), out.stride(0), st))
         ws = torch.empty(max(1, B * q_heads * splits * 130), dtype=torch.float32, device=q.device)
-        rc = lib.vqa_op_decode_attention_d128(*args[:-1], splits, _ptr(ws), ws.numel() * 4, C.byref(used), _ptr(out), out.stride(0),
-                                              _stream_ptr(q.device))
-        _check(rc, None, "vqa_op_decode_attention_d128")
+        used = C.c_int32(0)
+        _call("vqa_op_decode_attention_d128", *args, splits, _ptr(ws), ws.numel() * 4, C.byref(used), _ptr(out), out.stride(0), st)
         return out, int(used.value)
 
     @staticmethod
@@ -532,32 +553,26 @@ class ops:
                       first_pos=None, pos3=None):
         """One greedy selection step on bf16 logits [B, V] and the caller's int32 state (in place): tokens [B, max_new], lengths / done /
         next_ids [B], n_done / all_done [1], pen_bitmap [B, ceil(V / 32)] or None, first_pos [B] and pos3 [3, B] or both None."""
-        lib = _lib.load()
         B, V = logits.shape
         n_eos = eos_ids.numel() if eos_ids is not None else 0
-        rc = lib.vqa_op_greedy_select(_ptr(logits), B, V, _ptr(pen_bitmap), float(repetition_penalty), _ptr(eos_ids), n_eos, tokens.shape[1],
-                                      _ptr(first_pos), _ptr(tokens), _ptr(lengths), _ptr(done), _ptr(n_done), _ptr(all_done), _ptr(next_ids),
-                                      _ptr(pos3), _stream_ptr(logits.device))
-        _check(rc, None, "vqa_op_greedy_select")
+        _call("vqa_op_greedy_select", _ptr(logits), B, V, _ptr(pen_bitmap), float(repetition_penalty), _ptr(eos_ids), n_eos, tokens.shape[1],
+              _ptr(first_pos), _ptr(tokens), _ptr(lengths), _ptr(done), _ptr(n_done), _ptr(all_done), _ptr(next_ids), _ptr(pos3),
+              _stream_ptr(logits.device))
 
     @staticmethod
     def t5_bucket_lut(bidirectional: bool, num_buckets: int, max_distance: int) -> torch.Tensor:
         """The engine's relative-position bucket table (host): int32 [2 * max_distance + 1], entry rel + max_distance."""
-        lib = _lib.load()
         out = torch.empty(2 * max_distance + 1, dtype=torch.int32)
-        rc = lib.vqa_t5_bucket_lut(1 if bidirectional else 0, num_buckets, max_distance, C.cast(out.data_ptr(), C.POINTER(C.c_int32)))
-        _check(rc, None, "vqa_t5_bucket_lut")
+        _call("vqa_t5_bucket_lut", 1 if bidirectional else 0, num_buckets, max_distance, C.cast(out.data_ptr(), C.POINTER(C.c_int32)))
         return out
 
     @staticmethod
     def t5_decoder_self_attn(qkv: torch.Tensor, B: int, T: int, H: int, rel_emb: torch.Tensor, bucket_lut: torch.Tensor, max_distance: int,
                              round_scores: bool = False):
         """The scoring path's T5 decoder self-attention: qkv [B * T, 3 * H * 64] -> [B * T, H * 64]; bucket_lut on the device."""
-        lib = _lib.load()
         out = torch.empty(B * T, H * 64, dtype=torch.bfloat16, device=qkv.device)
-        rc = lib.vqa_op_t5_decoder_self_attn(_ptr(qkv), _ptr(out), _ptr(rel_emb), _ptr(bucket_lut), max_distance, B, T, H, 1 if round_scores else 0,
-                                             _stream_ptr(qkv.device))
-        _check(rc, None, "vqa_op_t5_decoder_self_attn")
+        _call("vqa_op_t5_decoder_self_attn", _ptr(qkv), _ptr(out), _ptr(rel_emb), _ptr(bucket_lut), max_distance, B, T, H,
+              1 if round_scores else 0, _stream_ptr(qkv.device))
         return out
 
     @staticmethod
@@ -565,34 +580,27 @@ class ops:
                             bucket_lut: torch.Tensor, max_distance: int, round_scores: bool = False, out=None):
         """One cached T5 decoder self-attention layer of a generation step: the row qkv [B, 3 * H * 64] of sequence b is appended to
         kc / vc [B, H, cap, 64] at min(lengths[b], cap - 1) (in place) and attends to the slots up to it. Returns out [B, H * 64]."""
-        lib = _lib.load()
         B, H, cap = kc.shape[0], kc.shape[1], kc.shape[2]
         if out is None:
             out = torch.empty(B, H * 64, dtype=torch.bfloat16, device=qkv.device)
-        rc = lib.vqa_op_t5_decode_self_attn(_ptr(qkv), _ptr(kc), _ptr(vc), cap, _ptr(lengths), _ptr(out), _ptr(rel_emb), _ptr(bucket_lut),
-                                            max_distance, B, H, 1 if round_scores else 0, _stream_ptr(qkv.device))
-        _check(rc, None, "vqa_op_t5_decode_self_attn")
+        _call("vqa_op_t5_decode_self_attn", _ptr(qkv), _ptr(kc), _ptr(vc), cap, _ptr(lengths), _ptr(out), _ptr(rel_emb), _ptr(bucket_lut),
+              max_distance, B, H, 1 if round_scores else 0, _stream_ptr(qkv.device))
         return out
 
     @staticmethod
     def norm(x: torch.Tensor, gamma: torch.Tensor, eps=1e-6, out=None):
         """T5LayerNorm / Qwen RMSNorm of the rows of x [rows, D] bf16: gamma * bf16(x * rsqrt(mean(x^2) + eps))."""
-        lib = _lib.load()
         y = torch.empty_like(x) if out is None else out
-        rc = lib.vqa_op_norm(_ptr(x), _ptr(gamma), _ptr(y), x.shape[0], x.shape[1], float(eps), _stream_ptr(x.device))
-        _check(rc, None, "vqa_op_norm")
+        _call("vqa_op_norm", _ptr(x), _ptr(gamma), _ptr(y), x.shape[0], x.shape[1], float(eps), _stream_ptr(x.device))
         return y
 
     @staticmethod
     def patchify(pixels: torch.Tensor, patch: int, kpad: int, out=None):
         """The patch gather of the CLIP tower: pixels [n, 3, S, S] fp32 / bf16 -> bf16 [n * (S / patch)^2, kpad]."""
-        lib = _lib.load()
         n, S = pixels.shape[0], pixels.shape[2]
         if out is None:
             out = torch.empty(n * (S // patch) ** 2, kpad, dtype=torch.bfloat16, device=pixels.device)
-        dt = _lib.VQA_DTYPE_F32 if pixels.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
-        rc = lib.vqa_op_patchify(_ptr(pixels), dt, n, S, patch, kpad, _ptr(out), _stream_ptr(pixels.device))
-        _check(rc, None, "vqa_op_patchify")
+        _call("vqa_op_patchify", _ptr(pixels), _dtype_code(pixels.dtype), n, S, patch, kpad, _ptr(out), _stream_ptr(pixels.device))
         return out
 
     @staticmethod
@@ -601,78 +609,64 @@ class ops:
         """The multimodal splice: ids int32 [B, L], text_lens int32 [B], image_index int32 [B] or None, shared [vocab, D], feats [rows, >= D]
         (row stride feats.stride(0)), image i's P feature rows from row i * rows_per_image + row_offset. Returns (out [B, L - 1 + P, D],
         seq_lens int32 [B])."""
-        lib = _lib.load()
         B, L = ids.shape
         D = shared.shape[1]
         if out is None:
             out = torch.empty(B, L - 1 + P, D, dtype=torch.bfloat16, device=ids.device)
         if seq_lens is None:
             seq_lens = torch.empty(B, dtype=torch.int32, device=ids.device)
-        rc = lib.vqa_op_splice_embed(_ptr(ids), _ptr(text_lens), _ptr(image_index), _ptr(shared), _ptr(feats), feats.stride(0), row_offset,
-                                     rows_per_image, _ptr(out), _ptr(seq_lens), B, L, P, D, image_token, _stream_ptr(ids.device))
-        _check(rc, None, "vqa_op_splice_embed")
+        _call("vqa_op_splice_embed", _ptr(ids), _ptr(text_lens), _ptr(image_index), _ptr(shared), _ptr(feats), feats.stride(0), row_offset,
+              rows_per_image, _ptr(out), _ptr(seq_lens), B, L, P, D, image_token, _stream_ptr(ids.device))
         return out, seq_lens
 
     @staticmethod
     def decoder_embed(labels, shared: torch.Tensor, B: int, T: int, start_id: int = 0, pad_id: int = 0, out=None):
         """Decoder input embeddings of shift_right(labels int32 [B, T]) (labels None: T = 1, the start token). Returns [B * T, D]."""
-        lib = _lib.load()
         D = shared.shape[1]
         if out is None:
             out = torch.empty(B * T, D, dtype=torch.bfloat16, device=shared.device)
-        rc = lib.vqa_op_decoder_embed(_ptr(labels), _ptr(shared), _ptr(out), B, T, D, start_id, pad_id, _stream_ptr(shared.device))
-        _check(rc, None, "vqa_op_decoder_embed")
+        _call("vqa_op_decoder_embed", _ptr(labels), _ptr(shared), _ptr(out), B, T, D, start_id, pad_id, _stream_ptr(shared.device))
         return out
 
     @staticmethod
     def t5_bias_table(rel_emb: torch.Tensor, bucket_lut: torch.Tensor, max_distance: int, S: int, out=None):
         """The encoder's relative-position bias table fp32 [H, 2S - 1] from rel_emb bf16 [buckets, H] and a device bucket LUT."""
-        lib = _lib.load()
         H = rel_emb.shape[1]
         if out is None:
             out = torch.empty(H, 2 * S - 1, dtype=torch.float32, device=rel_emb.device)
-        rc = lib.vqa_op_t5_bias_table(_ptr(rel_emb), _ptr(bucket_lut), max_distance, _ptr(out), H, S, _stream_ptr(rel_emb.device))
-        _check(rc, None, "vqa_op_t5_bias_table")
+        _call("vqa_op_t5_bias_table", _ptr(rel_emb), _ptr(bucket_lut), max_distance, _ptr(out), H, S, _stream_ptr(rel_emb.device))
         return out
 
     @staticmethod
     def lmhead_score(h: torch.Tensor, w: torch.Tensor, labels: torch.Tensor, scores=None, logprobs=None):
         """The CLIP-FlanT5 score's lm_head and finalisation: h [B * T, K] against w [N, K], labels int32 [B, T]. Returns (scores fp32 [B],
         logprobs fp32 [B * T]); both are allocated NaN-filled when not given, and ignored positions of logprobs keep their value."""
-        lib = _lib.load()
         B, T = labels.shape
         N, K = w.shape[0], h.shape[1]
         if scores is None:
             scores = torch.full((B,), float("nan"), dtype=torch.float32, device=h.device)
         if logprobs is None:
             logprobs = torch.full((B * T,), float("nan"), dtype=torch.float32, device=h.device)
-        need = C.c_size_t(0)
+        st = _stream_ptr(h.device)
         args = (_ptr(h), h.stride(0), _ptr(w), w.stride(0), B, T, N, K, _ptr(labels), _ptr(scores), _ptr(logprobs))
-        rc = lib.vqa_op_lmhead_score(*args, None, 0, C.byref(need), _stream_ptr(h.device))
-        if rc != -4:        # a call without scratch stops at the scratch check and returns the size
-            _check(rc or -1, None, "vqa_op_lmhead_score")
-        scratch = torch.empty((need.value + 3) // 4, dtype=torch.float32, device=h.device)
-        rc = lib.vqa_op_lmhead_score(*args, _ptr(scratch), scratch.numel() * 4, None, _stream_ptr(h.device))
-        _check(rc, None, "vqa_op_lmhead_score")
+        need = _size_query("vqa_op_lmhead_score", C.c_size_t, args, (st,))
+        scratch = torch.empty((need + 3) // 4, dtype=torch.float32, device=h.device)
+        _call("vqa_op_lmhead_score", *args, _ptr(scratch), scratch.numel() * 4, None, st)
         return scores, logprobs
 
     @staticmethod
     def row_ssq(x: torch.Tensor, ssq: torch.Tensor):
         """Sum of squares of the rows of x bf16 [rows, D] into column 0 of ssq fp32 [rows, stride] (in place)."""
-        lib = _lib.load()
-        rc = lib.vqa_op_row_ssq(_ptr(x), _ptr(ssq), x.shape[0], x.shape[1], ssq.stride(0), _stream_ptr(x.device))
-        _check(rc, None, "vqa_op_row_ssq")
+        _call("vqa_op_row_ssq", _ptr(x), _ptr(ssq), x.shape[0], x.shape[1], ssq.stride(0), _stream_ptr(x.device))
         return ssq
 
     @staticmethod
     def gemm_f32acc(a: torch.Tensor, w: torch.Tensor, c: torch.Tensor, bias=None, variant=0):
         """The CLIP tower's residual GEMM: fp32 c[M, N] += bf16(a . w^T + bias), in place (row stride c.stride(0))."""
-        lib = _lib.load()
         M, K = a.shape
         N = w.shape[0]
-        rc = lib.vqa_op_gemm_bf16_f32acc(_ptr(a), a.stride(0), _ptr(w), w.stride(0), N, _ptr(c), c.stride(0), M, N, K, _ptr(bias), variant,
-                                         _stream_ptr(a.device))
-        _check(rc, None, "vqa_op_gemm_bf16_f32acc")
+        _call("vqa_op_gemm_bf16_f32acc", _ptr(a), a.stride(0), _ptr(w), w.stride(0), N, _ptr(c), c.stride(0), M, N, K, _ptr(bias), variant,
+              _stream_ptr(a.device))
         return c
 
     @staticmethod
@@ -680,12 +674,10 @@ class ops:
                      c_stride: int = 0, a_extent=None, w_extent=None, variant: int = 0):
         """`nb` store-GEMMs in one launch (see vqa_op_gemm_bf16_batched): batch b reads a at (row, k) + b * a_off, w at (row, k) + b * w_off
         and writes c.flatten()[b * c_stride + m * c.stride(0) + n]. a_extent / w_extent (rows, cols) default to the tensors' shapes."""
-        lib = _lib.load()
         a_rows, a_cols = a_extent or a.shape
         w_rows, w_cols = w_extent or w.shape
-        rc = lib.vqa_op_gemm_bf16_batched(_ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(c), c.stride(0), M, N, K, nb, a_off[0], a_off[1],
-                                          w_off[0], w_off[1], c_stride, a_rows, a_cols, w_rows, w_cols, variant, _stream_ptr(a.device))
-        _check(rc, None, "vqa_op_gemm_bf16_batched")
+        _call("vqa_op_gemm_bf16_batched", _ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(c), c.stride(0), M, N, K, nb, a_off[0], a_off[1],
+              w_off[0], w_off[1], c_stride, a_rows, a_cols, w_rows, w_cols, variant, _stream_ptr(a.device))
         return c
 
     @staticmethod
@@ -693,42 +685,33 @@ class ops:
                            mode: int = 0, round_scores: bool = False, out=None, workspace=None):
         """One CLIP-FlanT5 decoder cross-attention layer (see vqa_op_t5_cross_attention): mode 0 absorbed, mode 1 the reference association.
         Returns (out [B * T, H * 64], the uint8 workspace, whose mode-0 layout the header documents)."""
-        lib = _lib.load()
         Dm = x.shape[1]
         if out is None:
             out = torch.empty(B * T, H * 64, dtype=torch.bfloat16, device=q.device)
-        need = C.c_size_t(0)
+        st = _stream_ptr(q.device)
         args = (_ptr(q), _ptr(x), _ptr(seq_lens), _ptr(wkT), _ptr(wkv), _ptr(out), B, T, S, H, Dm, mode, 1 if round_scores else 0)
-        if workspace is None:   # a call without workspace stops at the workspace check and returns the size
-            rc = lib.vqa_op_t5_cross_attention(*args, None, 0, C.byref(need), _stream_ptr(q.device))
-            if rc != -4:
-                _check(rc or -1, None, "vqa_op_t5_cross_attention")
-            workspace = torch.empty(need.value, dtype=torch.uint8, device=q.device)
-        rc = lib.vqa_op_t5_cross_attention(*args, _ptr(workspace), workspace.numel(), C.byref(need), _stream_ptr(q.device))
-        _check(rc, None, "vqa_op_t5_cross_attention")
+        if workspace is None:
+            workspace = torch.empty(_size_query("vqa_op_t5_cross_attention", C.c_size_t, args, (st,)), dtype=torch.uint8, device=q.device)
+        _call("vqa_op_t5_cross_attention", *args, _ptr(workspace), workspace.numel(), None, st)
         return out, workspace
 
     @staticmethod
     def layernorm_f32(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5, out=None):
         """LayerNorm of an fp32 [rows, D] stream into bf16 (the CLIP tower's ln1 / ln2)."""
-        lib = _lib.load()
         if out is None:
             out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-        rc = lib.vqa_op_layernorm_f32(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), x.shape[0], x.shape[1], float(eps), _stream_ptr(x.device))
-        _check(rc, None, "vqa_op_layernorm_f32")
+        _call("vqa_op_layernorm_f32", _ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), x.shape[0], x.shape[1], float(eps), _stream_ptr(x.device))
         return out
 
     @staticmethod
     def clip_embed_ln(patch: torch.Tensor, cls: torch.Tensor, pos: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, n_images: int,
                       eps: float = 1e-5, out=None):
         """CLIP embeddings + pre_layrnorm: patch rows [n_images * P, D] -> fp32 [n_images * (P + 1), D]."""
-        lib = _lib.load()
         P, D = patch.shape[0] // n_images, patch.shape[1]
         if out is None:
             out = torch.empty(n_images * (P + 1), D, dtype=torch.float32, device=patch.device)
-        rc = lib.vqa_op_clip_embed_ln(_ptr(patch), _ptr(cls), _ptr(pos), _ptr(gamma), _ptr(beta), _ptr(out), n_images, P, D, float(eps),
-                                      _stream_ptr(patch.device))
-        _check(rc, None, "vqa_op_clip_embed_ln")
+        _call("vqa_op_clip_embed_ln", _ptr(patch), _ptr(cls), _ptr(pos), _ptr(gamma), _ptr(beta), _ptr(out), n_images, P, D, float(eps),
+              _stream_ptr(patch.device))
         return out
 
     @staticmethod
@@ -738,17 +721,15 @@ class ops:
         """Head-dim-128 attention on packed rows qkv [rows, ld] into out (row stride out.stride(0)), in place: fixed stride S with seq_lens
         [n_seq] (cu_seqlens None, vqa_op_attention_d128), or variable-length cu_seqlens [n_seq + 1] with the extras of
         vqa_op_attention_d128_ex. rows defaults to qkv.shape[0]."""
-        lib = _lib.load()
         rows = qkv.shape[0] if rows is None else rows
         st = _stream_ptr(qkv.device)
         if cu_seqlens is None:
-            rc = lib.vqa_op_attention_d128(_ptr(qkv), qkv.stride(0), rows, q_col0, k_col0, v_col0, _ptr(out), out.stride(0), n_seq, max_len, S,
-                                           q_heads, kv_group, None, _ptr(seq_lens), float(scale), 1 if causal else 0, st)
+            _call("vqa_op_attention_d128", _ptr(qkv), qkv.stride(0), rows, q_col0, k_col0, v_col0, _ptr(out), out.stride(0), n_seq, max_len, S,
+                  q_heads, kv_group, None, _ptr(seq_lens), float(scale), 1 if causal else 0, st)
         else:
-            rc = lib.vqa_op_attention_d128_ex(_ptr(qkv), qkv.stride(0), rows, q_col0, k_col0, v_col0, _ptr(out), out.stride(0), n_seq, max_len,
-                                              q_heads, kv_group, _ptr(cu_seqlens), _ptr(kv_prefix), float(scale), 1 if causal else 0,
-                                              1 if pair_sequences else 0, o_head_stride, d_out, st)
-        _check(rc, None, "vqa_op_attention_d128")
+            _call("vqa_op_attention_d128_ex", _ptr(qkv), qkv.stride(0), rows, q_col0, k_col0, v_col0, _ptr(out), out.stride(0), n_seq, max_len,
+                  q_heads, kv_group, _ptr(cu_seqlens), _ptr(kv_prefix), float(scale), 1 if causal else 0, 1 if pair_sequences else 0,
+                  o_head_stride, d_out, st)
         return out
 
     @staticmethod
@@ -757,36 +738,30 @@ class ops:
         """M-RoPE as the scoring path applies it: tables from positions int32 [n_axes, rows], axis_of_dim int32 / inv_freq fp32 [head_dim / 2]
         into cos_t / sin_t fp32 [rows, head_dim] (allocated when None), then n_heads heads of x bf16 [rows, ld] rotated in place.
         Returns (cos_t, sin_t)."""
-        lib = _lib.load()
         rows = positions.shape[1]
         if cos_t is None:
             cos_t = torch.empty(rows, head_dim, dtype=torch.float32, device=x.device)
             sin_t = torch.empty(rows, head_dim, dtype=torch.float32, device=x.device)
-        rc = lib.vqa_op_qwen_rope(_ptr(positions), rows, _ptr(axis_of_dim), _ptr(inv_freq), head_dim // 2, _ptr(cos_t), _ptr(sin_t), _ptr(x),
-                                  x.stride(0), col0, n_heads, head_stride, head_dim, 1 if text_mode else 0, _stream_ptr(x.device))
-        _check(rc, None, "vqa_op_qwen_rope")
+        _call("vqa_op_qwen_rope", _ptr(positions), rows, _ptr(axis_of_dim), _ptr(inv_freq), head_dim // 2, _ptr(cos_t), _ptr(sin_t), _ptr(x),
+              x.stride(0), col0, n_heads, head_stride, head_dim, 1 if text_mode else 0, _stream_ptr(x.device))
         return cos_t, sin_t
 
     @staticmethod
     def gather_rows(src: torch.Tensor, index: torch.Tensor, group: int, out=None):
         """out row r = src row index[r / group] * group + r % group, for every row of out (default: src's shape)."""
-        lib = _lib.load()
         if out is None:
             out = torch.empty_like(src)
-        rc = lib.vqa_op_gather_rows(_ptr(src), _ptr(out), _ptr(index), out.shape[0], group, out.shape[1], _stream_ptr(src.device))
-        _check(rc, None, "vqa_op_gather_rows")
+        _call("vqa_op_gather_rows", _ptr(src), _ptr(out), _ptr(index), out.shape[0], group, out.shape[1], _stream_ptr(src.device))
         return out
 
     @staticmethod
     def qwen_embed(ids: torch.Tensor, feat_index: torch.Tensor, seq_lens: torch.Tensor, embed: torch.Tensor, feats: torch.Tensor, S: int, out=None):
         """The embedding splice over rows = ids.numel() rows of S (packed rows: seq_lens = cu_seqlens[n_seq:], S = rows). Returns out [rows, D]."""
-        lib = _lib.load()
         rows, D = ids.numel(), embed.shape[1]
         if out is None:
             out = torch.empty(rows, D, dtype=torch.bfloat16, device=embed.device)
-        rc = lib.vqa_op_qwen_embed(_ptr(ids), _ptr(feat_index), _ptr(seq_lens), _ptr(embed), _ptr(feats), _ptr(out), rows, S, D,
-                                   _stream_ptr(embed.device))
-        _check(rc, None, "vqa_op_qwen_embed")
+        _call("vqa_op_qwen_embed", _ptr(ids), _ptr(feat_index), _ptr(seq_lens), _ptr(embed), _ptr(feats), _ptr(out), rows, S, D,
+              _stream_ptr(embed.device))
         return out
 
     @staticmethod
@@ -794,26 +769,22 @@ class ops:
                      max_prompt_len: int = 0, bitmap=None):
         """The repetition-penalty bitmap int32 [B, ceil(vocab / 32)] (zeroed here when not given) of padded prompts (seq_lens, S) or packed
         rows (cu_seqlens, kv_prefix, pair_seq, max_prompt_len)."""
-        lib = _lib.load()
         if bitmap is None:
             bitmap = torch.zeros(B, (vocab + 31) // 32, dtype=torch.int32, device=ids.device)
-        rc = lib.vqa_op_token_bitmap(_ptr(ids), _ptr(seq_lens), B, S, _ptr(cu_seqlens), _ptr(kv_prefix), _ptr(pair_seq), max_prompt_len, vocab,
-                                     _ptr(bitmap), _stream_ptr(ids.device))
-        _check(rc, None, "vqa_op_token_bitmap")
+        _call("vqa_op_token_bitmap", _ptr(ids), _ptr(seq_lens), B, S, _ptr(cu_seqlens), _ptr(kv_prefix), _ptr(pair_seq), max_prompt_len, vocab,
+              _ptr(bitmap), _stream_ptr(ids.device))
         return bitmap
 
     @staticmethod
     def topk_softmax(logits: torch.Tensor, K: int, V: Optional[int] = None, temperature: float = 1.0, pen_bitmap=None,
                      repetition_penalty: float = 1.0):
         """The trace top-K of bf16 logits [B, >= V] (row stride logits.stride(0)): (ids int32 [B, K], probabilities fp32 [B, K])."""
-        lib = _lib.load()
         B = logits.shape[0]
         V = logits.shape[1] if V is None else V
         ids = torch.full((B, K), -2, dtype=torch.int32, device=logits.device)
         probs = torch.full((B, K), float("nan"), dtype=torch.float32, device=logits.device)
-        rc = lib.vqa_op_topk_softmax(_ptr(logits), logits.stride(0), B, V, float(temperature), _ptr(pen_bitmap), float(repetition_penalty), K,
-                                     _ptr(ids), _ptr(probs), _stream_ptr(logits.device))
-        _check(rc, None, "vqa_op_topk_softmax")
+        _call("vqa_op_topk_softmax", _ptr(logits), logits.stride(0), B, V, float(temperature), _ptr(pen_bitmap), float(repetition_penalty), K,
+              _ptr(ids), _ptr(probs), _stream_ptr(logits.device))
         return ids, probs
 
 
@@ -855,6 +826,30 @@ CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
 
 
+def _upload_u8(items, dev: torch.device):
+    """The uint8 pixels of `items` (images [h, w, 3] or frame stacks [n, h, w, 3]) as one device byte buffer, item after item, and the
+    byte offset of every frame in it. A packed [n, h, w, 3] tensor of equal-size images is used in place on the device or sent with one
+    H2D copy; a list of device tensors is concatenated; a list with host tensors is staged once in pinned memory and copied once."""
+    offs, total = [], 0
+    for it in items:
+        step = int(it.shape[-3]) * int(it.shape[-2]) * 3
+        offs.extend(total + f * step for f in range(int(it.shape[0]) if it.dim() == 4 else 1))
+        total += int(it.numel())
+    if isinstance(items, torch.Tensor):
+        src = items.contiguous().view(-1)
+        src = src if src.is_cuda else src.to(dev, non_blocking=True)
+    elif all(it.is_cuda for it in items):
+        src = items[0].contiguous().view(-1) if len(items) == 1 else torch.cat([it.contiguous().view(-1) for it in items])
+    else:
+        stage = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+        o = 0
+        for it in items:
+            stage[o:o + it.numel()] = it.contiguous().view(-1)
+            o += it.numel()
+        src = stage.to(dev, non_blocking=True)
+    return src, offs
+
+
 def clip_preprocess_u8(images: Sequence[torch.Tensor], out_size: int, device, pad: bool = True, mean=CLIP_MEAN, std=CLIP_STD,
                        background=None, out_dtype: torch.dtype = torch.float32, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Decoded images (uint8 HWC RGB tensors, each [h, w, 3], on the host or on `device`) -> CLIP input [n, 3, S, S] on the device,
@@ -865,24 +860,11 @@ def clip_preprocess_u8(images: Sequence[torch.Tensor], out_size: int, device, pa
     dev = torch.device(device)
     n = len(images)
     assert n > 0
-    hs, ws, offs, total = [], [], [], 0
     for im in images:
         assert im.dtype == torch.uint8 and im.dim() == 3 and im.shape[2] == 3, "images must be uint8 [h, w, 3]"
-        hs.append(int(im.shape[0])); ws.append(int(im.shape[1])); offs.append(total)
-        total += int(im.numel())
-    if isinstance(images, torch.Tensor):      # one packed [n, h, w, 3] batch of equal-size images: no staging copy
-        src = images.contiguous().view(-1)
-        src = src if src.is_cuda else src.to(dev, non_blocking=True)
-    elif all(im.is_cuda for im in images):
-        src = images[0].contiguous().view(-1) if n == 1 else torch.cat([im.contiguous().view(-1) for im in images])
-    else:
-        stage = torch.empty(total, dtype=torch.uint8, pin_memory=True)
-        for im, o in zip(images, offs):
-            stage[o:o + im.numel()] = im.contiguous().view(-1)
-        src = stage.to(dev, non_blocking=True)
-    H = (C.c_int32 * n)(*hs)
-    W = (C.c_int32 * n)(*ws)
-    O = (C.c_int64 * n)(*offs)
+    src, offs = _upload_u8(images, dev)
+    H = (C.c_int32 * n)(*[int(im.shape[0]) for im in images])
+    W = (C.c_int32 * n)(*[int(im.shape[1]) for im in images])
     need = int(lib.vqa_clip_preprocess_workspace_bytes(H, W, n, out_size, 1 if pad else 0))
     if need == 0:
         raise RuntimeError(f"vqa_clip_preprocess_workspace_bytes: {_lib.last_error(None)}")
@@ -894,9 +876,9 @@ def clip_preprocess_u8(images: Sequence[torch.Tensor], out_size: int, device, pa
     ring = _staging(dev)
     hs = ring.acquire(need)
     with torch.cuda.device(dev):
-        rc = lib.vqa_clip_preprocess(_ptr(src), O, H, W, n, out_size, 1 if pad else 0, (C.c_uint8 * 3)(*bg), (C.c_float * 3)(*mean),
-                                     (C.c_float * 3)(*std), _ptr(out), _lib.VQA_DTYPE_F32 if out.dtype == torch.float32 else _lib.VQA_DTYPE_BF16,
-                                     _ptr(wsb), need, hs.data_ptr(), _stream_ptr(dev))
+        rc = lib.vqa_clip_preprocess(_ptr(src), (C.c_int64 * n)(*offs), H, W, n, out_size, 1 if pad else 0, (C.c_uint8 * 3)(*bg),
+                                     (C.c_float * 3)(*mean), (C.c_float * 3)(*std), _ptr(out), _dtype_code(out.dtype), _ptr(wsb), need,
+                                     hs.data_ptr(), _stream_ptr(dev))
     ring.release(dev)
     _check(rc, None, "vqa_clip_preprocess")
     # src / wsb stay referenced by the caching allocator's stream ordering: both were allocated on the current stream
@@ -927,58 +909,35 @@ def clip_preprocess_u8_sliced(images: Sequence[torch.Tensor], out_size: int, dev
     return out
 
 
+def _qwen_plan(n_frames, heights, widths, is_video, patch: int, temporal_patch: int, merge: int, min_pixels: int, max_pixels: int):
+    """vqa_qwen_preprocess_video_plan (host only) -> ([(t, gh, gw), ...], total patch rows, workspace bytes)."""
+    n = len(heights)
+    i32 = lambda v: (C.c_int32 * n)(*v)
+    grid = (C.c_int32 * (3 * n))()
+    rows, need = C.c_int64(0), C.c_size_t(0)
+    _call("vqa_qwen_preprocess_video_plan", i32(n_frames), i32(heights), i32(widths), i32(is_video), n, patch, temporal_patch, merge, min_pixels,
+          max_pixels, grid, C.byref(rows), C.byref(need))
+    return [tuple(int(grid[3 * i + k]) for k in range(3)) for i in range(n)], int(rows.value), int(need.value)
+
+
 def qwen_preprocess_plan(sizes_hw: Sequence[Sequence[int]], patch: int = 14, merge: int = 2, min_pixels: int = 56 * 56,
                          max_pixels: int = 14 * 14 * 4 * 1280):
     """Host-only geometry of the Qwen pre-processing (smart_resize): -> ([(1, gh, gw), ...], total patch rows, workspace bytes)."""
-    lib = _lib.load()
     n = len(sizes_hw)
-    H = (C.c_int32 * n)(*[int(s[0]) for s in sizes_hw])
-    W = (C.c_int32 * n)(*[int(s[1]) for s in sizes_hw])
-    grid = (C.c_int32 * (2 * n))()
-    total, wsb = C.c_int64(0), C.c_size_t(0)
-    _check(lib.vqa_qwen_preprocess_plan(H, W, n, patch, merge, min_pixels, max_pixels, grid, C.byref(total), C.byref(wsb)), None,
-           "vqa_qwen_preprocess_plan")
-    return [(1, int(grid[2 * i]), int(grid[2 * i + 1])) for i in range(n)], int(total.value), int(wsb.value)
+    # still images: the temporal patch size changes neither the rows nor the workspace
+    return _qwen_plan([1] * n, [int(s[0]) for s in sizes_hw], [int(s[1]) for s in sizes_hw], [0] * n, patch, 1, merge, min_pixels, max_pixels)
 
 
 def qwen_preprocess_u8(images: Sequence[torch.Tensor], device, patch: int = 14, temporal_patch: int = 2, merge: int = 2,
                        min_pixels: int = 56 * 56, max_pixels: int = 14 * 14 * 4 * 1280, mean=CLIP_MEAN, std=CLIP_STD,
                        out_dtype: torch.dtype = torch.float32):
-    """Decoded still images (uint8 HWC RGB, host or device) -> (pixel_patches [sum gh*gw, 3*temporal*patch^2] on the device,
-    [(1, gh, gw), ...]) by ONE kernel launch: smart_resize + PIL-exact bicubic + /255 + normalise + frame duplication + merge-order
-    patch rows -- bit-identical to models/vqascore_models/qwen_utils.qwen_image_to_patches (the CPU path)."""
-    lib = _lib.load()
-    dev = torch.device(device)
-    n = len(images)
-    assert n > 0
-    hs, ws, offs, total = [], [], [], 0
+    """Decoded still images (uint8 HWC RGB, host or device; a packed [n, h, w, 3] tensor is n stills) -> (pixel_patches
+    [sum gh*gw, 3*temporal*patch^2] on the device, [(1, gh, gw), ...]) by ONE kernel launch: smart_resize + PIL-exact bicubic + /255 +
+    normalise + frame duplication + merge-order patch rows -- bit-identical to models/vqascore_models/qwen_utils.qwen_image_to_patches
+    (the CPU path). The still-image case of qwen_preprocess_video_u8."""
     for im in images:
         assert im.dtype == torch.uint8 and im.dim() == 3 and im.shape[2] == 3, "images must be uint8 [h, w, 3]"
-        hs.append(int(im.shape[0])); ws.append(int(im.shape[1])); offs.append(total)
-        total += int(im.numel())
-    grids, rows, need = qwen_preprocess_plan(list(zip(hs, ws)), patch, merge, min_pixels, max_pixels)
-    if isinstance(images, torch.Tensor):
-        src = images.contiguous().view(-1)
-        src = src if src.is_cuda else src.to(dev, non_blocking=True)
-    elif all(im.is_cuda for im in images):
-        src = images[0].contiguous().view(-1) if n == 1 else torch.cat([im.contiguous().view(-1) for im in images])
-    else:
-        stage = torch.empty(total, dtype=torch.uint8, pin_memory=True)
-        for im, o in zip(images, offs):
-            stage[o:o + im.numel()] = im.contiguous().view(-1)
-        src = stage.to(dev, non_blocking=True)
-    out = torch.empty(rows, 3 * temporal_patch * patch * patch, dtype=out_dtype, device=dev)
-    wsb = torch.empty(max(need, 16), dtype=torch.uint8, device=dev)
-    ring = _staging(dev)
-    stage_buf = ring.acquire(wsb.numel())
-    with torch.cuda.device(dev):
-        rc = lib.vqa_qwen_preprocess(_ptr(src), (C.c_int64 * n)(*offs), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws), n, patch, temporal_patch,
-                                     merge, min_pixels, max_pixels, (C.c_float * 3)(*mean), (C.c_float * 3)(*std), _ptr(out),
-                                     _lib.VQA_DTYPE_F32 if out_dtype == torch.float32 else _lib.VQA_DTYPE_BF16, _ptr(wsb), wsb.numel(),
-                                     stage_buf.data_ptr(), _stream_ptr(dev))
-    ring.release(dev)
-    _check(rc, None, "vqa_qwen_preprocess")
-    return out, grids
+    return qwen_preprocess_video_u8(images, device, patch, temporal_patch, merge, min_pixels, max_pixels, mean, std, out_dtype)
 
 
 def qwen_preprocess_video_u8(items: Sequence[torch.Tensor], device, patch: int = 14, temporal_patch: int = 2, merge: int = 2,
@@ -988,46 +947,31 @@ def qwen_preprocess_video_u8(items: Sequence[torch.Tensor], device, patch: int =
     [sum t*gh*gw, 3*temporal*patch^2] on the device, [(t, gh, gw), ...]) by ONE kernel launch (vqa_qwen_preprocess_video): every frame
     gets the still-image pre-processing of qwen_preprocess_u8, and a stack's frames fill consecutive temporal slots of its patch rows, the
     last frame repeated into the slots a count that is not a multiple of temporal_patch leaves -- bit-identical to
-    models/vqascore_models/qwen_utils.qwen_video_to_patches. A still keeps grid t = 1 and the rows of qwen_preprocess_u8."""
+    models/vqascore_models/qwen_utils.qwen_video_to_patches. A still keeps grid t = 1 and the rows of qwen_preprocess_u8. A packed
+    [n, h, w, 3] tensor is n still images."""
     lib = _lib.load()
     dev = torch.device(device)
     n = len(items)
     assert n > 0
-    nf, hs, ws, vid, offs, total = [], [], [], [], [], 0
     for it in items:
         assert it.dtype == torch.uint8 and it.dim() in (3, 4) and it.shape[-1] == 3, "items must be uint8 [h, w, 3] or [n, h, w, 3]"
-        frames = int(it.shape[0]) if it.dim() == 4 else 1
-        nf.append(frames); hs.append(int(it.shape[-3])); ws.append(int(it.shape[-2])); vid.append(int(it.dim() == 4))
-        step = hs[-1] * ws[-1] * 3
-        offs.extend(total + f * step for f in range(frames))
-        total += int(it.numel())
+    nf = [int(it.shape[0]) if it.dim() == 4 else 1 for it in items]
+    hs, ws = [int(it.shape[-3]) for it in items], [int(it.shape[-2]) for it in items]
+    vid = [int(it.dim() == 4) for it in items]
+    grids, rows, need = _qwen_plan(nf, hs, ws, vid, patch, temporal_patch, merge, min_pixels, max_pixels)
+    src, offs = _upload_u8(items, dev)
+    out = torch.empty(rows, 3 * temporal_patch * patch * patch, dtype=out_dtype, device=dev)
+    wsb = torch.empty(max(need, 16), dtype=torch.uint8, device=dev)
     i32 = lambda v: (C.c_int32 * n)(*v)
-    NF, H, W, V = i32(nf), i32(hs), i32(ws), i32(vid)
-    grid = (C.c_int32 * (3 * n))()
-    rows, need = C.c_int64(0), C.c_size_t(0)
-    _check(lib.vqa_qwen_preprocess_video_plan(NF, H, W, V, n, patch, temporal_patch, merge, min_pixels, max_pixels, grid, C.byref(rows),
-                                              C.byref(need)), None, "vqa_qwen_preprocess_video_plan")
-    if all(it.is_cuda for it in items):
-        src = items[0].contiguous().view(-1) if n == 1 else torch.cat([it.contiguous().view(-1) for it in items])
-    else:
-        stage = torch.empty(total, dtype=torch.uint8, pin_memory=True)
-        o = 0
-        for it in items:
-            stage[o:o + it.numel()] = it.contiguous().view(-1)
-            o += it.numel()
-        src = stage.to(dev, non_blocking=True)
-    out = torch.empty(int(rows.value), 3 * temporal_patch * patch * patch, dtype=out_dtype, device=dev)
-    wsb = torch.empty(max(int(need.value), 16), dtype=torch.uint8, device=dev)
     ring = _staging(dev)
     stage_buf = ring.acquire(wsb.numel())
     with torch.cuda.device(dev):
-        rc = lib.vqa_qwen_preprocess_video(_ptr(src), (C.c_int64 * len(offs))(*offs), NF, H, W, V, n, patch, temporal_patch, merge, min_pixels,
-                                           max_pixels, (C.c_float * 3)(*mean), (C.c_float * 3)(*std), _ptr(out),
-                                           _lib.VQA_DTYPE_F32 if out_dtype == torch.float32 else _lib.VQA_DTYPE_BF16, _ptr(wsb), wsb.numel(),
-                                           stage_buf.data_ptr(), _stream_ptr(dev))
+        rc = lib.vqa_qwen_preprocess_video(_ptr(src), (C.c_int64 * len(offs))(*offs), i32(nf), i32(hs), i32(ws), i32(vid), n, patch,
+                                           temporal_patch, merge, min_pixels, max_pixels, (C.c_float * 3)(*mean), (C.c_float * 3)(*std),
+                                           _ptr(out), _dtype_code(out_dtype), _ptr(wsb), wsb.numel(), stage_buf.data_ptr(), _stream_ptr(dev))
     ring.release(dev)
     _check(rc, None, "vqa_qwen_preprocess_video")
-    return out, [tuple(int(grid[3 * i + k]) for k in range(3)) for i in range(n)]
+    return out, grids
 
 
 # Frames of a video file go to the device in slices of at most this many bytes (at least one frame), so that host and device staging
@@ -1102,8 +1046,7 @@ def qwen_preprocess_video_file_u8(frames, size, device, n_frames: Optional[int] 
         with torch.cuda.device(dev):
             rc = lib.vqa_qwen_preprocess_video_aa(_ptr(src), k, done, n_frames, hw[0], hw[1], rh, rw, ip(fh), fp(wh), th, ip(fv), fp(wv), tv,
                                                   patch, temporal_patch, merge, (C.c_float * 3)(*mean), (C.c_float * 3)(*std), _ptr(out),
-                                                  _lib.VQA_DTYPE_F32 if out_dtype == torch.float32 else _lib.VQA_DTYPE_BF16, _ptr(wsb),
-                                                  wsb.numel(), stage_buf.data_ptr(), _stream_ptr(dev))
+                                                  _dtype_code(out_dtype), _ptr(wsb), wsb.numel(), stage_buf.data_ptr(), _stream_ptr(dev))
         ring.release(dev)
         _check(rc, None, "vqa_qwen_preprocess_video_aa")
         done += k
@@ -1167,19 +1110,13 @@ def convert_qwen_state_dict(sd: Dict[str, torch.Tensor], cfg, device) -> Dict[st
     return out
 
 
-class QwenVLEngine:
+class QwenVLEngine(_Engine):
     """Qwen2.5-VL VQAScore engine: P(answer token | image, prompt) for a whole batch of prompts in one prefill."""
 
     def __init__(self, cfg, device="cuda:0", emulate_bf16_rounding: bool = True):
         from . import qwen_host
-        if not torch.cuda.is_available():
-            raise RuntimeError("QwenVLEngine needs a CUDA device (sm_90a); there is no CPU path")
         if cfg.head_dim != 128:
             raise ValueError("the language-model attention kernel is specialised for head_dim == 128")
-        self.lib = _lib.load()
-        self.cfg = cfg
-        self.device = torch.device(device)
-        idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
         mask = 0
         for l in cfg.fullatt_block_indexes:
             mask |= 1 << l
@@ -1188,28 +1125,12 @@ class QwenVLEngine:
                                    spatial_merge=cfg.spatial_merge_size, out_hidden=cfg.out_hidden, fullatt_mask=mask,
                                    hidden=cfg.hidden, layers=cfg.layers, heads=cfg.heads, kv_heads=cfg.kv_heads, mlp=cfg.mlp,
                                    vocab=cfg.vocab, rms_eps=cfg.rms_eps, emulate_bf16_rounding=1 if emulate_bf16_rounding else 0)
-        self._h = C.c_void_p()
-        with torch.cuda.device(idx):
-            _check(self.lib.vqa_create_qwen25vl(C.byref(c), idx, C.byref(self._h)), None, "vqa_create_qwen25vl")
+        super().__init__(cfg, device, "vqa_create_qwen25vl", c)
         t_inv, t_axis, v_inv, v_axis = qwen_host.rope_tables(cfg.head_dim, cfg.rope_theta, cfg.mrope_section, cfg.vit_head_dim)
         fp = lambda t: t.numpy().ctypes.data_as(C.POINTER(C.c_float))
         ip = lambda t: t.numpy().ctypes.data_as(C.POINTER(C.c_int32))
-        _check(self.lib.vqa_qwen25vl_set_rope(self._h, fp(t_inv), ip(t_axis), t_inv.numel(), fp(v_inv), ip(v_axis), v_inv.numel()),
-               self._h, "vqa_qwen25vl_set_rope")
-        self._weights: Dict[str, torch.Tensor] = {}
-        self._workspace: Optional[torch.Tensor] = None
+        self._run("vqa_qwen25vl_set_rope", fp(t_inv), ip(t_axis), t_inv.numel(), fp(v_inv), ip(v_axis), v_inv.numel())
         self._vision_cache: "collections.OrderedDict[tuple, dict]" = collections.OrderedDict()   # per-batch index sets, LRU-bounded
-
-    def __del__(self):
-        h = getattr(self, "_h", None)
-        if h is not None and h.value:
-            self.lib.vqa_destroy(h)
-            self._h = C.c_void_p()
-
-    bind_engine_tensors = ClipT5Engine.bind_engine_tensors
-    last_launch_count = ClipT5Engine.last_launch_count
-    set_profile = ClipT5Engine.set_profile
-    read_profile = ClipT5Engine.read_profile
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor]):
         self.bind_engine_tensors(convert_qwen_state_dict(sd, self.cfg, self.device))
@@ -1242,23 +1163,31 @@ class QwenVLEngine:
     def _prompts(self, pixel_patches, vi, input_ids, seq_lens, feat_index, position_ids, batch: int, seq_len: int = 0):
         """The vqa_qwen25vl_prompts of one prefill (packed rows: no seq_lens, seq_len 0). It holds raw device addresses: the caller keeps
         the tensors alive until the call that reads it has returned."""
-        pdt = _lib.VQA_DTYPE_F32 if pixel_patches.dtype == torch.float32 else _lib.VQA_DTYPE_BF16
         vision = {k: (_ptr(v) if torch.is_tensor(v) else v) for k, v in vi.items()}
-        return _lib.VqaQwen25VLPrompts(pixel_patches=_ptr(pixel_patches), pixel_dtype=pdt, input_ids=_ptr(input_ids), seq_lens=_ptr(seq_lens),
-                                       feat_index=_ptr(feat_index), position_ids=_ptr(position_ids), batch=batch, seq_len=seq_len, **vision)
+        return _lib.VqaQwen25VLPrompts(pixel_patches=_ptr(pixel_patches), pixel_dtype=_dtype_code(pixel_patches.dtype), input_ids=_ptr(input_ids),
+                                       seq_lens=_ptr(seq_lens), feat_index=_ptr(feat_index), position_ids=_ptr(position_ids), batch=batch,
+                                       seq_len=seq_len, **vision)
+
+    def _check_inputs(self, pixel_patches: torch.Tensor, vi: dict, *int32_tensors):
+        assert pixel_patches.is_cuda and pixel_patches.is_contiguous() and pixel_patches.shape == (vi["n_patches"], self.cfg.patch_dim)
+        assert pixel_patches.dtype in (torch.float32, torch.bfloat16)
+        for t in int32_tensors:
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+
+    def _indices(self, build, prompts, grid_thw, image_of_sample, second_per_grid_ts, **kw) -> dict:
+        """qwen_host.build_batch_indices or build_packed_indices (`build`) of id-list prompts over grid_thw; image_of_sample None: prompt b
+        shows item b."""
+        cfg = self.cfg
+        img = list(image_of_sample) if image_of_sample is not None else list(range(len(prompts)))
+        return build([list(map(int, p)) for p in prompts], [tuple(map(int, g)) for g in grid_thw], img, cfg.image_token_id,
+                     cfg.spatial_merge_size, cfg.tokens_per_second, video_token_id=cfg.video_token_id, second_per_grid_ts=second_per_grid_ts,
+                     **kw)
 
     def _score(self, prompts, packed, rows: int, answer_ids, temperature, repetition_penalty, out, logp):
         """One vqa_qwen25vl_score call over `rows` language-model rows: padded rows (packed None) or packed rows."""
-        dev = self.device
-        need = int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, prompts.batch, rows, prompts.n_patches))
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = None
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            rc = self.lib.vqa_qwen25vl_score(self._h, C.byref(prompts), None if packed is None else C.byref(packed), _ptr(answer_ids),
-                                             float(temperature), float(repetition_penalty), _ptr(out), _ptr(logp), _ptr(self._workspace),
-                                             self._workspace.numel(), _stream_ptr(dev))
-        _check(rc, self._h, "vqa_qwen25vl_score")
+        ws = self._grow("_workspace", int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, prompts.batch, rows, prompts.n_patches)), self._graphs)
+        self._run("vqa_qwen25vl_score", C.byref(prompts), None if packed is None else C.byref(packed), _ptr(answer_ids), float(temperature),
+                  float(repetition_penalty), _ptr(out), _ptr(logp), _ptr(ws), ws.numel(), _stream_ptr(self.device))
         self._last_call = (prompts.batch, rows, prompts.n_patches)     # what topk_last() needs to find the final hidden states again
 
     def score_tensors(self, pixel_patches: torch.Tensor, grid_thw, input_ids: torch.Tensor, seq_lens: torch.Tensor,
@@ -1270,10 +1199,7 @@ class QwenVLEngine:
         generation_config.json carries one, SURVEY F8). Returns probabilities [B] fp32 on the device."""
         dev = self.device
         vi = self.vision_indices(grid_thw)
-        assert pixel_patches.is_cuda and pixel_patches.is_contiguous() and pixel_patches.shape == (vi["n_patches"], self.cfg.patch_dim)
-        assert pixel_patches.dtype in (torch.float32, torch.bfloat16)
-        for t in (input_ids, seq_lens, feat_index, position_ids, answer_ids):
-            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+        self._check_inputs(pixel_patches, vi, input_ids, seq_lens, feat_index, position_ids, answer_ids)
         B, S = input_ids.shape
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=dev)
@@ -1292,16 +1218,14 @@ class QwenVLEngine:
         dev = self.device
         ids = torch.empty(B, k, dtype=torch.int32, device=dev)
         probs = torch.empty(B, k, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = self.lib.vqa_qwen25vl_topk(self._h, B, rows, n_patches, k, float(temperature), float(repetition_penalty), _ptr(ids), _ptr(probs),
-                                            _ptr(self._workspace), self._workspace.numel(), _stream_ptr(dev))
-        _check(rc, self._h, "vqa_qwen25vl_topk")
+        self._run("vqa_qwen25vl_topk", B, rows, n_patches, k, float(temperature), float(repetition_penalty), _ptr(ids), _ptr(probs),
+                  _ptr(self._workspace), self._workspace.numel(), _stream_ptr(dev))
         return ids, probs
 
     def debug_tensors(self, batch: int, seq_len: int, n_patches: int) -> Dict[str, torch.Tensor]:
         """Views into the workspace of the LAST call with these sizes (synchronise first). Parity investigations only."""
         off = (C.c_size_t * 4)()
-        _check(self.lib.vqa_qwen25vl_debug_layout(self._h, batch, batch * seq_len, n_patches, off, 4), self._h, "vqa_qwen25vl_debug_layout")
+        self._run("vqa_qwen25vl_debug_layout", batch, batch * seq_len, n_patches, off, 4)
         cfg, ws = self.cfg, self._workspace
         unit = cfg.spatial_merge_size ** 2
 
@@ -1315,7 +1239,7 @@ class QwenVLEngine:
         the K/V of their [chat prefix + vision tokens]."""
         dev = self.device
         vi = self.vision_indices(grid_thw)
-        assert pixel_patches.is_cuda and pixel_patches.is_contiguous() and pixel_patches.shape == (vi["n_patches"], self.cfg.patch_dim)
+        self._check_inputs(pixel_patches, vi)
         B, R = int(answer_ids.numel()), int(packed["total_rows"])
         if out is None:
             out = torch.empty(B, dtype=torch.float32, device=dev)
@@ -1335,29 +1259,19 @@ class QwenVLEngine:
         model once (KV-prefix sharing, exact under causal attention). The shared part is cut to whole key tiles of the attention kernel
         (ATTN_KEY_TILE rows), so a shared prefill is bit-identical to the unshared one; a prefix shorter than one tile is not shared."""
         from . import qwen_host
-        cfg, dev = self.cfg, self.device
-        B = len(prompts)
-        img = list(image_of_sample) if image_of_sample is not None else list(range(B))
+        dev = self.device
+        ans = torch.as_tensor(list(map(int, answer_ids)), dtype=torch.int32).to(dev)
         if share_prefix is None or share_prefix:
-            pk = qwen_host.build_packed_indices([list(map(int, p)) for p in prompts], [tuple(map(int, g)) for g in grid_thw], img,
-                                                cfg.image_token_id, cfg.spatial_merge_size, cfg.tokens_per_second,
-                                                video_token_id=cfg.video_token_id, second_per_grid_ts=second_per_grid_ts,
-                                                align=ATTN_KEY_TILE)
+            pk = self._indices(qwen_host.build_packed_indices, prompts, grid_thw, image_of_sample, second_per_grid_ts, align=ATTN_KEY_TILE)
             if pk["n_shared"] > 0 or share_prefix:
                 d = {k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in pk.items()}
-                ans = torch.as_tensor(list(map(int, answer_ids)), dtype=torch.int32).to(dev)
                 return self.score_packed(pixel_patches.to(dev), grid_thw, d, ans, temperature, repetition_penalty)
-        idx = qwen_host.build_batch_indices([list(map(int, p)) for p in prompts], [tuple(map(int, g)) for g in grid_thw], img,
-                                            cfg.image_token_id, cfg.spatial_merge_size, cfg.tokens_per_second,
-                                            video_token_id=cfg.video_token_id, second_per_grid_ts=second_per_grid_ts)
+        idx = self._indices(qwen_host.build_batch_indices, prompts, grid_thw, image_of_sample, second_per_grid_ts)
         d = {k: v.to(dev) for k, v in idx.items()}
-        ans = torch.as_tensor(list(map(int, answer_ids)), dtype=torch.int32).to(dev)
         return self.score_tensors(pixel_patches.to(dev), grid_thw, d["input_ids"], d["seq_lens"], d["feat_index"], d["position_ids"],
                                   ans, temperature, repetition_penalty=repetition_penalty)
 
     # ------------------------------------------------------------------------------------------ greedy generation
-    MAX_GEN_GRAPHS = 8
-
     def score_workspace_bytes(self, batch: int, seq_len: int, n_patches: int) -> int:
         """Device bytes of one padded scoring prefill (vqa_qwen25vl_workspace_bytes), the most score_prompts needs; 0 for invalid sizes."""
         return int(self.lib.vqa_qwen25vl_workspace_bytes(self._h, batch, batch * seq_len, n_patches))
@@ -1377,25 +1291,16 @@ class QwenVLEngine:
         from . import qwen_host
         cfg, dev = self.cfg, self.device
         B = len(prompts)
-        img = list(image_of_sample) if image_of_sample is not None else list(range(B))
-        idx = qwen_host.build_batch_indices([list(map(int, p)) for p in prompts], [tuple(map(int, g)) for g in grid_thw], img,
-                                            cfg.image_token_id, cfg.spatial_merge_size, cfg.tokens_per_second,
-                                            video_token_id=cfg.video_token_id, second_per_grid_ts=second_per_grid_ts)
+        idx = self._indices(qwen_host.build_batch_indices, prompts, grid_thw, image_of_sample, second_per_grid_ts)
         first = qwen_host.first_generated_positions(idx)
         vi = self.vision_indices(grid_thw)
         pixel_patches = pixel_patches.to(dev).contiguous()
-        assert pixel_patches.shape == (vi["n_patches"], cfg.patch_dim) and pixel_patches.dtype in (torch.float32, torch.bfloat16)
+        self._check_inputs(pixel_patches, vi)
         S, max_new = int(idx["input_ids"].shape[1]), int(max_new_tokens)
         eos = [int(e) for e in eos_ids]
         need = int(self.lib.vqa_qwen25vl_generate_workspace_bytes(self._h, B, S, vi["n_patches"], max_new))
         if need == 0:
             raise ValueError(f"bad generation size: batch {B}, prompt length {S}, max_new_tokens {max_new}")
-        gens = self.__dict__.setdefault("_gen_states", {})
-        ws = getattr(self, "_gen_workspace", None)
-        if ws is None or ws.numel() < need:
-            gens.clear()                         # captured step graphs point into the old workspace
-            self._gen_workspace = None
-            self._gen_workspace = torch.empty(need, dtype=torch.uint8, device=dev)
         key = (B, S, vi["n_patches"], max_new, float(repetition_penalty), len(eos))
         if score is not None:
             answers = [[int(t) for t in a] for a in score["answer_ids"]]
@@ -1403,11 +1308,11 @@ class QwenVLEngine:
                 raise ValueError("rollout scoring needs one non-empty answer id list per prompt")
             n_max, temp, top_k = max(len(a) for a in answers), float(score.get("temperature", 1.0)), int(score.get("top_k", 0))
             key += ("rollout", n_max, temp, top_k)
-        st = gens.get(key)
-        if st is None:
+
+        def make() -> dict:
             i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
-            st = gens[key] = dict(B=B, S=S, n_patches=vi["n_patches"], max_new=max_new, seq_lens=i32(B), first=i32(B), eos=i32(max(len(eos), 1)),
-                                  tokens=i32(B, max_new), lengths=i32(B), all_done=i32(1), graph=None, score=None)
+            st = dict(B=B, S=S, n_patches=vi["n_patches"], max_new=max_new, seq_lens=i32(B), first=i32(B), eos=i32(max(len(eos), 1)),
+                      tokens=i32(B, max_new), lengths=i32(B), all_done=i32(1), graph=None, score=None)
             # the vqa_qwen25vl_generation every call of this state passes, built once: its pointers are the state's own tensors
             st["gen"] = _lib.VqaQwen25VLGeneration(
                 seq_lens=_ptr(st["seq_lens"]), first_position=_ptr(st["first"]), eos_ids=_ptr(st["eos"]), n_eos=len(eos), max_new_tokens=max_new,
@@ -1422,8 +1327,8 @@ class QwenVLEngine:
                                                            temperature=temp, top_k=top_k, out_logp=_ptr(sc["logp"]),
                                                            out_topk_ids=_ptr(sc["topk_ids"]), out_topk_probs=_ptr(sc["topk_probs"]))
                 st["gen"].score = C.pointer(sc["struct"])
-            while len(gens) > self.MAX_GEN_GRAPHS:
-                gens.pop(next(iter(gens)))
+            return st
+        st = self._gen_state(key, need, make)
         st["seq_lens"].copy_(idx["seq_lens"], non_blocking=True)
         st["first"].copy_(first, non_blocking=True)
         if eos:
@@ -1443,20 +1348,17 @@ class QwenVLEngine:
 
         def prefill():
             prompts = self._prompts(pixel_patches, vi, d["input_ids"], st["seq_lens"], d["feat_index"], d["position_ids"], B, S)
-            with torch.cuda.device(dev):
-                rc = self.lib.vqa_qwen25vl_generate_prefill(self._h, C.byref(prompts), C.byref(st["gen"]), _ptr(self._gen_workspace),
-                                                            self._gen_workspace.numel(), _stream_ptr(dev))
-            _check(rc, self._h, "vqa_qwen25vl_generate_prefill")
+            ws = self._gen_workspace
+            self._run("vqa_qwen25vl_generate_prefill", C.byref(prompts), C.byref(st["gen"]), _ptr(ws), ws.numel(), _stream_ptr(dev))
         st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
         prefill()
         return st
 
     def generate_step(self, st: dict):
         """One decode step of the generation `st` (vqa_qwen25vl_generate_step), launched directly."""
-        with torch.cuda.device(self.device):
-            rc = self.lib.vqa_qwen25vl_generate_step(self._h, C.byref(st["gen"]), st["B"], st["S"], st["n_patches"], _ptr(self._gen_workspace),
-                                                     self._gen_workspace.numel(), _stream_ptr(self.device))
-        _check(rc, self._h, "vqa_qwen25vl_generate_step")
+        ws = self._gen_workspace
+        self._run("vqa_qwen25vl_generate_step", C.byref(st["gen"]), st["B"], st["S"], st["n_patches"], _ptr(ws), ws.numel(),
+                  _stream_ptr(self.device))
 
     def generate_prompts(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
                          repetition_penalty: float = 1.0, second_per_grid_ts=None, use_graph: bool = True, check_every: int = 16):
@@ -1466,9 +1368,7 @@ class QwenVLEngine:
         Returns each prompt's generated ids, the EOS id included when one ended it."""
         st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
                                  second_per_grid_ts)
-        _decode_loop(self, st, use_graph, check_every)
-        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
-        return [tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])]
+        return self._decode_loop(st, use_graph, check_every)[0]
 
     def rollout_scores(self, pixel_patches, grid_thw, prompts, answer_ids, max_new_tokens: int, eos_ids: Sequence[int],
                        temperature: float = 1.0, repetition_penalty: float = 1.0, top_k: int = 0, image_of_sample=None,
@@ -1481,9 +1381,7 @@ class QwenVLEngine:
         answer), topk_ids / topk_probs [B, max_new_tokens, top_k] or None)."""
         st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
                                  second_per_grid_ts, score=dict(answer_ids=answer_ids, temperature=temperature, top_k=top_k))
-        _decode_loop(self, st, use_graph, check_every)
+        tokens, lengths = self._decode_loop(st, use_graph, check_every)
         sc = st["score"]
-        tokens, lengths = st["tokens"].cpu(), st["lengths"].cpu()
         cpu = lambda t: None if t is None else t.cpu()
-        return dict(tokens=[tokens[b, :int(lengths[b])].tolist() for b in range(st["B"])], lengths=lengths, logp=cpu(sc["logp"]),
-                    topk_ids=cpu(sc["topk_ids"]), topk_probs=cpu(sc["topk_probs"]))
+        return dict(tokens=tokens, lengths=lengths, logp=cpu(sc["logp"]), topk_ids=cpu(sc["topk_ids"]), topk_probs=cpu(sc["topk_probs"]))

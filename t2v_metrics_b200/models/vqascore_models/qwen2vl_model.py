@@ -201,8 +201,8 @@ class Qwen2VLModel(VQAScoreModel):
         # the reference runs per image / per video
         import numpy as np
         from PIL import Image
-        from ...engine import qwen_preprocess_u8, qwen_preprocess_video_u8
-        raw, video = [], False
+        from ...engine import qwen_preprocess_video_u8
+        raw = []
         for p in image:
             if p.lower().endswith(".npy"):
                 # the reference's Qwen path takes the array as RGB, no channel flip (qwen2vl_model.py:146-153); a 4-D array is a frame
@@ -210,7 +210,6 @@ class Qwen2VLModel(VQAScoreModel):
                 arr = np.load(p)
                 if arr.ndim == 4:
                     arr = np.stack([np.asarray(Image.fromarray(f.astype("uint8"), "RGB"), dtype=np.uint8) for f in arr])
-                    video = True
                 elif arr.ndim == 3:
                     arr = np.asarray(Image.fromarray(arr.astype("uint8"), "RGB"), dtype=np.uint8)
                 else:
@@ -219,8 +218,7 @@ class Qwen2VLModel(VQAScoreModel):
                 with Image.open(p) as im:
                     arr = np.asarray(im.convert("RGB"), dtype=np.uint8)
             raw.append(torch.from_numpy(np.ascontiguousarray(arr)))
-        pre = qwen_preprocess_video_u8 if video else qwen_preprocess_u8
-        return pre(raw, self.engine.device, self.cfg.patch_size, self.cfg.temporal_patch_size, self.cfg.spatial_merge_size,
+        return qwen_preprocess_video_u8(raw, self.engine.device, self.cfg.patch_size, self.cfg.temporal_patch_size, self.cfg.spatial_merge_size,
                    min_pixels=self.min_pixels, max_pixels=self.max_pixels)
 
     def _load_video_file(self, path: str, fps):

@@ -8,10 +8,48 @@ from t2v_metrics_b200 import _lib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
+def header_text():
+    return re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "vqa_b200.h")).read(), flags=re.S)
+
+
 def declared_functions():
-    text = open(os.path.join(ROOT, "include", "vqa_b200.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(vqa_[a-z0-9_]+)\s*\(", text)))
+    return sorted(set(re.findall(r"\b(vqa_[a-z0-9_]+)\s*\(", header_text())))
+
+
+def declared_prototypes():
+    """{name: (return kind, [parameter kinds])} of every function declaration in the header."""
+    out = {}
+    for ret, name, params in re.findall(r"^\s*([A-Za-z_][\w\s]*?\**)\s*\b(vqa_\w+)\s*\(([^)]*)\)\s*;", header_text(), flags=re.M):
+        params = [p.strip() for p in params.split(",")]
+        args = [] if params == ["void"] else [c_kind(re.sub(r"\w+$", "", p)) for p in params]     # drop the parameter name
+        out[name] = (c_kind(ret), args)
+    return out
+
+
+C_KINDS = {"void": None, "int": "i32", "int32_t": "i32", "uint32_t": "i32", "int64_t": "i64", "size_t": "u64", "uint64_t": "u64",
+           "float": "f32", "double": "f64"}
+
+
+def c_kind(decl: str):
+    """The kind of a C type as written in the header (parameter name already removed)."""
+    if "*" in decl:
+        return "ptr"
+    return C_KINDS[decl.replace("const", "").strip()]
+
+
+def ctypes_kind(t):
+    """The kind of a ctypes type; on Linux c_size_t is c_uint64, so size_t and uint64_t are one kind."""
+    if t is None:
+        return None
+    if isinstance(t, type) and issubclass(t, (ctypes._Pointer, ctypes.c_void_p, ctypes.c_char_p)):
+        return "ptr"
+    code = t._type_
+    if code in "fd":
+        return {"f": "f32", "d": "f64"}[code]
+    assert code in "iIlLqQ", t
+    if ctypes.sizeof(t) == 4:
+        return "i32"
+    return "i64" if code.islower() else "u64"
 
 
 def test_header_symbols_exported():
@@ -20,7 +58,18 @@ def test_header_symbols_exported():
     assert len(names) >= 14
     for n in names:
         assert hasattr(lib, n), n
-    assert sorted(_lib.ABI_SYMBOLS) == names
+    assert sorted(_lib.PROTOTYPES) == names
+
+
+def test_prototypes_match_header():
+    # a wrong integer width or a missing argument is undefined behaviour at the foreign-call boundary: every entry of the ctypes table must
+    # have the header's return kind and parameter kinds, in order
+    declared = declared_prototypes()
+    assert sorted(declared) == declared_functions()
+    for name, (restype, argtypes) in _lib.PROTOTYPES.items():
+        ret, args = declared[name]
+        assert ctypes_kind(restype) == ret, f"{name}: return type"
+        assert [ctypes_kind(t) for t in argtypes] == args, f"{name}: parameters"
 
 
 def test_qwen_struct_layout_matches_header():

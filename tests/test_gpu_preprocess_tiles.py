@@ -68,8 +68,8 @@ def run_clip(images, size, pad, dtype, dev):
 
 
 def run_qwen(items, dtype, dev, pixels):
-    """Still images (uint8 [h, w, 3]) through vqa_qwen_preprocess, or a mix with frame stacks ([n, h, w, 3]) through
-    vqa_qwen_preprocess_video, packed back to back on the device -> (patch rows, [(t, gh, gw)])."""
+    """Still images (uint8 [h, w, 3]) and frame stacks ([n, h, w, 3]) through vqa_qwen_preprocess_video, packed back to back on the
+    device -> (patch rows, [(t, gh, gw)])."""
     lib, i32, i64 = _lib.load(), C.c_int32, C.c_int64
     n = len(items)
     arr = lambda t, v: (t * len(v))(*v)
@@ -91,13 +91,9 @@ def run_qwen(items, dtype, dev, pixels):
     mean, std = (C.c_float * 3)(*CLIP_MEAN), (C.c_float * 3)(*CLIP_STD)
     dt = _lib.VQA_DTYPE_F32 if dtype == torch.float32 else _lib.VQA_DTYPE_BF16
     stream = torch.cuda.current_stream(dev).cuda_stream
-    if any(vid):
-        rc = lib.vqa_qwen_preprocess_video(src.data_ptr(), arr(i64, offs), arr(i32, nf), arr(i32, hs), arr(i32, ws), arr(i32, vid), n, PATCH,
-                                           TEMPORAL, MERGE, pixels[0], pixels[1], mean, std, out.data_ptr(), dt, wsb.data_ptr(), wsb.numel(),
-                                           None, stream)
-    else:
-        rc = lib.vqa_qwen_preprocess(src.data_ptr(), arr(i64, offs), arr(i32, hs), arr(i32, ws), n, PATCH, TEMPORAL, MERGE, pixels[0],
-                                     pixels[1], mean, std, out.data_ptr(), dt, wsb.data_ptr(), wsb.numel(), None, stream)
+    rc = lib.vqa_qwen_preprocess_video(src.data_ptr(), arr(i64, offs), arr(i32, nf), arr(i32, hs), arr(i32, ws), arr(i32, vid), n, PATCH,
+                                       TEMPORAL, MERGE, pixels[0], pixels[1], mean, std, out.data_ptr(), dt, wsb.data_ptr(), wsb.numel(),
+                                       None, stream)
     if rc:
         raise RuntimeError(_lib.last_error(None))
     assert_guards(buf)

@@ -98,7 +98,7 @@ def test_workspace_sizing_and_errors():
 
 
 def test_qwen_plan_matches_python_smart_resize():
-    """vqa_qwen_preprocess_plan (C++ smart_resize incl. Python's round-half-even) == qwen_utils.smart_resize on a sweep of sizes,
+    """vqa_qwen_preprocess_video_plan (C++ smart_resize incl. Python's round-half-even) == qwen_utils.smart_resize on a sweep of sizes,
     including the min-pixel and max-pixel branches and exact .5 ties (h / 28 = k + 0.5)."""
     from t2v_metrics_b200.engine import qwen_preprocess_plan
     from t2v_metrics_b200.models.vqascore_models.qwen_utils import smart_resize
