@@ -256,8 +256,9 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnParams
 #pragma unroll
             for (int jb = 0; jb < D / 8; ++jb) {
                 const int col = jb * 8 + c0;
-                if (jb * 8 < p.d_out)
-                    *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16x2(o_acc[jb * 4 + 2 * hr] * inv, o_acc[jb * 4 + 2 * hr + 1] * inv);
+                if (jb * 8 < p.d_out)      // rows at or past len: +0 (O * 0 would be -0 where O < 0)
+                    *reinterpret_cast<uint32_t*>(orow + col) =
+                        qr < len ? pack_bf16x2(o_acc[jb * 4 + 2 * hr] * inv, o_acc[jb * 4 + 2 * hr + 1] * inv) : 0u;
             }
         }
     }

@@ -12,12 +12,11 @@ long-sequence cases run the 3-stage and 2-stage rings, which the bias row forces
 import pytest
 import torch
 
-from attention_ref import assert_attn, attn_bound, bf16_ulp, softmax_ref
+from attention_ref import assert_attn, attn_bound, bf16_ulp, exponent_reference, softmax_ref
 
 pytestmark = pytest.mark.gpu
 
 INVALID = -1
-LN2 = 0.6931471805599453
 
 # len mod 128 = 1, 16, 17, 32, 33, 64, 65, 96, 97, 127, 0 and lengths 0 / 1. 576: the second 64-row block of the last query tile is padding;
 # 640 / 256: whole 128-row query tiles are padding.
@@ -103,17 +102,6 @@ def d64_ref(q, k, v, n, S, table, scale, round_scores, r0=0, mistake=None, const
     n_keys = n + 1 if mistake == "one key past len" else n - 1 if mistake == "last valid key dropped" else n
     s[..., n_keys:] = float("-inf")
     return softmax_ref(s, v, exponent_reference(s))
-
-
-def exponent_reference(s):
-    """The kernel's exponent reference of each row: the maximum of its first 128-key tile, raised to a later tile's maximum only when that
-    exceeds it by more than 2^8 (8 ln 2 here, in the natural-log domain). A row dominated by one key then rounds that key's P as the kernel
-    does, not to an exact 1."""
-    tiles = [s[..., t:t + 128].amax(-1, keepdim=True) for t in range(0, s.shape[-1], 128)]
-    m = tiles[0]
-    for t in tiles[1:]:
-        m = torch.where(t > m + 8 * LN2, t, m)
-    return m
 
 
 def mistakes_for(n, S, table, scale, round_scores, const_from):
