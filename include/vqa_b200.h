@@ -293,6 +293,30 @@ int vqa_qwen25vl_generate_prefill(vqa_handle* h, const vqa_qwen25vl_prompts* pro
 int vqa_qwen25vl_generate_step(vqa_handle* h, const vqa_qwen25vl_generation* gen, int32_t batch, int32_t seq_len, int32_t n_patches,
                                void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Qwen2.5-VL sampled generation (reference Qwen2VLModel.generate with do_sample and temperature > 0, qwen2vl_model.py:495-563:
+ * generate(do_sample=True, temperature=T, top_p=p) with the checkpoint's top_k, default 50) ----
+ * The same prefill and steps as the greedy generation, with the selection replaced: HF's sampling distribution, built as its processors
+ * build it -- repetition penalty (as above), then scores / temperature (an fp32 division; none at 1.0), then top-k (every id whose score
+ * is >= the k-th largest stays, ties included), then top-p (in ascending order of (score, id), the ids whose cumulative probability is
+ * <= fp32(1 - top_p) go, the most probable always stays; lower ids of the group of equal scores at the cut go first) -- and one draw from
+ * the softmax of the kept scores: Gumbel-max with the uniforms of Philox4x32-10 keyed by seeds[b] at counter (id / 4, t, 0, 0), lane
+ * id % 4, where t is the index of the token. A prompt's tokens depend on its seed, prompt and sizes only, not on its batch position or
+ * on whether the step is replayed from a CUDA graph. A score that overflows fp32 (or a NaN logit) saturates to +-FLT_MAX (NaN to
+ * -FLT_MAX), where HF's softmax would be NaN; a top_p whose fp32(1 - top_p) rounds to 1 keeps only the most probable id, as HF does. Same workspace (vqa_qwen25vl_generate_workspace_bytes) and the same rules for it;
+ * gen->score must be NULL (a scored rollout is greedy). Refused with VQA_ERR_INVALID_ARG: a NULL seeds pointer, a temperature that is
+ * not positive and finite, top_k < 0, top_p outside (0, 1]. */
+typedef struct {
+    const uint64_t* seeds;  /* DEVICE [batch]: prompt b's key; its draws depend on (seeds[b], step, id) only */
+    float temperature;      /* > 0 and finite; 1.0 = no division */
+    int32_t top_k;          /* >= 0; 0 = off */
+    float top_p;            /* (0, 1]; 1.0 = off */
+} vqa_qwen25vl_sampling;
+
+int vqa_qwen25vl_generate_prefill_sampled(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
+                                          const vqa_qwen25vl_sampling* sampling, void* workspace, size_t workspace_bytes, void* stream);
+int vqa_qwen25vl_generate_step_sampled(vqa_handle* h, const vqa_qwen25vl_generation* gen, const vqa_qwen25vl_sampling* sampling, int32_t batch,
+                                       int32_t seq_len, int32_t n_patches, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Number of kernels, memsets and copies the last forward call on this handle (vqa_clipt5_score, vqa_qwen25vl_score, vqa_qwen25vl_topk,
  * a generate prefill or step) enqueued (for bench.py's gpu_launches). */
 int64_t vqa_last_launch_count(vqa_handle* h);
@@ -473,6 +497,15 @@ int vqa_op_decode_attention_d128(const void* q, int32_t ldq, const void* kc, con
 int vqa_op_greedy_select(const void* logits, int32_t B, int32_t V, uint32_t* pen_bitmap, float repetition_penalty, const int32_t* eos_ids,
                          int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
                          int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, void* stream);
+
+/* The token selection of the sampled generation (vqa_qwen25vl_generate_*_sampled) on caller-owned state: vqa_op_greedy_select with the
+ * arg-max replaced by a draw under `sampling` (HOST struct; its seeds DEVICE [B]); the draw of row b uses step t = lengths[b].
+ * kept: NULL, or DEVICE [B, ceil(V / 32)] that receives the bitmap of the ids each unfinished row kept after top-k and top-p (a debugging
+ * and test aid; the generation passes NULL). */
+int vqa_op_sample_select(const void* logits, int32_t B, int32_t V, uint32_t* pen_bitmap, float repetition_penalty, const int32_t* eos_ids,
+                         int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
+                         int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, const vqa_qwen25vl_sampling* sampling,
+                         uint32_t* kept, void* stream);
 
 /* Host-only (no GPU needed): T5's relative-position buckets (T5Attention._relative_position_bucket) of rel = -max_distance .. max_distance,
  * out[rel + max_distance], HOST int32 [2 * max_distance + 1] -- the table vqa_create_clipt5 builds for the encoder (bidirectional = 1) and

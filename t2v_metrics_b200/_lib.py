@@ -71,6 +71,10 @@ class VqaQwen25VLGeneration(C.Structure):
     ]
 
 
+class VqaQwen25VLSampling(C.Structure):
+    _fields_ = [("seeds", C.c_void_p), ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float)]
+
+
 class VqaTensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("shape", C.c_int64 * 4), ("ndim", C.c_int32),
                 ("dtype", C.c_int32)]
@@ -96,6 +100,9 @@ PROTOTYPES = {
     "vqa_qwen25vl_generate_workspace_bytes": (_sz, [_vp, _i32, _i32, _i32, _i32]),
     "vqa_qwen25vl_generate_prefill": (_i32, [_vp, _P(VqaQwen25VLPrompts), _P(VqaQwen25VLGeneration), _vp, _sz, _vp]),
     "vqa_qwen25vl_generate_step": (_i32, [_vp, _P(VqaQwen25VLGeneration), _i32, _i32, _i32, _vp, _sz, _vp]),
+    "vqa_qwen25vl_generate_prefill_sampled": (_i32, [_vp, _P(VqaQwen25VLPrompts), _P(VqaQwen25VLGeneration), _P(VqaQwen25VLSampling), _vp, _sz,
+                                                     _vp]),
+    "vqa_qwen25vl_generate_step_sampled": (_i32, [_vp, _P(VqaQwen25VLGeneration), _P(VqaQwen25VLSampling), _i32, _i32, _i32, _vp, _sz, _vp]),
     "vqa_last_launch_count": (_i64, [_vp]),
     "vqa_set_profile": (_i32, [_vp, _i32]),
     "vqa_profile_read": (_i32, [_vp, _P(_f32), _P(C.c_double), _P(C.c_double), _P(_i64)]),
@@ -130,6 +137,8 @@ PROTOTYPES = {
     "vqa_op_decode_attention_d128": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _f32, _i32, _vp, _sz, _P(_i32), _vp, _i32,
                                             _vp]),
     "vqa_op_greedy_select": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "vqa_op_sample_select": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                    _P(VqaQwen25VLSampling), _vp, _vp]),
     "vqa_t5_bucket_lut": (_i32, [_i32, _i32, _i32, _P(_i32)]),
     "vqa_op_t5_decoder_self_attn": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "vqa_op_t5_decode_self_attn": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),

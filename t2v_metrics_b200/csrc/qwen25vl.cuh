@@ -356,8 +356,9 @@ static QwenGenWorkspace qwen_gen_plan(const vqa_qwen25vl_config& c, int B, int S
 }
 
 // lm_head on w.lastn into [B, vocab] bf16 logits, then (rollout scoring) the answer log-probabilities of this step, then the greedy token
-// of every unfinished sequence and its bookkeeping
-static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g, int B, const vqa_qwen25vl_generation& a) {
+// (smp NULL) or the sampled one of every unfinished sequence and its bookkeeping
+static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g, int B, const vqa_qwen25vl_generation& a,
+                             const vqa_qwen25vl_sampling* smp) {
     const vqa_qwen25vl_config& c = q.cfg;
     const QwenWorkspace& w = g.w;
     bf16* logits = f.at(w.trace_logits);
@@ -366,13 +367,18 @@ static int qwen_select_token(Forward& f, QwenState& q, const QwenGenWorkspace& g
     uint32_t* bitmap = a.repetition_penalty != 1.0f ? f.at<uint32_t>(w.pen_bitmap) : nullptr;
     if (const vqa_qwen25vl_answer_score* s = a.score)
         TRY(answer_logprob(f, logits, B, c.vocab, bitmap, a.repetition_penalty, *s, a.max_new_tokens, a.out_lengths, f.at<int>(g.done)));
+    if (smp)
+        return sample_select(f, logits, B, c.vocab, bitmap, a.repetition_penalty, *smp, a.eos_ids, a.n_eos, a.max_new_tokens, a.first_position,
+                             a.out_tokens, a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done, f.at<int>(g.next_ids),
+                             f.at<int>(g.pos3));
     return greedy_select(f, logits, B, c.vocab, bitmap, a.repetition_penalty, a.eos_ids, a.n_eos, a.max_new_tokens, a.first_position, a.out_tokens,
                          a.out_lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done, f.at<int>(g.next_ids), f.at<int>(g.pos3));
 }
 
-// The prefill of vqa_qwen25vl_score over the padded rows, with every layer's K/V stored in the cache, then the first token.
-static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const vqa_qwen25vl_prompts& in, const vqa_qwen25vl_generation& a, void* workspace,
-                                 size_t workspace_bytes, cudaStream_t st) {
+// The prefill of vqa_qwen25vl_score over the padded rows, with every layer's K/V stored in the cache, then the first token (greedy when
+// smp is NULL, else sampled).
+static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const vqa_qwen25vl_prompts& in, const vqa_qwen25vl_generation& a,
+                                 const vqa_qwen25vl_sampling* smp, void* workspace, size_t workspace_bytes, cudaStream_t st) {
     const QwenGenWorkspace g = qwen_gen_plan(q.cfg, in.batch, in.seq_len, in.n_patches, a.max_new_tokens, h->num_sms);
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
@@ -380,7 +386,7 @@ static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const vqa_qwen25vl
     const QwenKVCache kv{f.at(g.kcache), f.at(g.vcache), g.layer_elems, g.cap};
     TRY(qwen_prefill(f, q, g.w, in, nullptr, &kv));
     TRY(qwen_last_position(f, q, g.w, in, nullptr, a.repetition_penalty));
-    return qwen_select_token(f, q, g, in.batch, a);
+    return qwen_select_token(f, q, g, in.batch, a, smp);
 }
 
 // One decode step: every sequence feeds its last token (finished ones recompute their frozen last step, which writes nothing new).
@@ -388,8 +394,8 @@ static int qwen_generate_prefill(vqa_handle* h, QwenState& q, const vqa_qwen25vl
 // of the 128-wide N tiles that splitk_slices() counts, far fewer than 132 SMs, so their K range is split (2, 4 and 4 slices:
 // tools/bench_generate.py measures the step with and without). gate_up (N = 2 x 18944) and the lm_head (N = 152064) already make
 // 296 and 1188 tiles and have no split.
-static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_patches, const vqa_qwen25vl_generation& a, void* workspace,
-                              size_t workspace_bytes, cudaStream_t st) {
+static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_patches, const vqa_qwen25vl_generation& a,
+                              const vqa_qwen25vl_sampling* smp, void* workspace, size_t workspace_bytes, cudaStream_t st) {
     const vqa_qwen25vl_config& c = q.cfg;
     const QwenGenWorkspace g = qwen_gen_plan(c, B, S, n_patches, a.max_new_tokens, h->num_sms);
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
@@ -424,5 +430,5 @@ static int qwen_generate_step(vqa_handle* h, QwenState& q, int B, int S, int n_p
         TRY(f.gemm(skinny(Gemm(P_(w.ff), Lw.down_w, P_(w.x), B, D, c.mlp).with_residual(P_(w.x))), "decode down gemm"));
     }
     TRY(f.rmsnorm(P_(w.x), q.final_norm, P_(w.lastn), B, D, c.rms_eps));
-    return qwen_select_token(f, q, g, B, a);
+    return qwen_select_token(f, q, g, B, a, smp);
 }

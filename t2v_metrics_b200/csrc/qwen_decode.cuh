@@ -1,7 +1,8 @@
-// Kernels of the Qwen2.5-VL greedy decode loop and their launches: the K/V cache write, flash-decoding attention over the cache, and greedy
-// token selection with the per-step bookkeeping. Every step-dependent value (generated lengths, finished flags, next input ids and
+// Kernels of the Qwen2.5-VL decode loop and their launches: the K/V cache write, flash-decoding attention over the cache, and greedy or
+// sampled token selection with the per-step bookkeeping. Every step-dependent value (generated lengths, finished flags, next input ids and
 // positions) lives in device memory, so the launches of one decode step take the same arguments at every step and replay from one CUDA graph.
 #pragma once
+#include <cfloat>
 #include "host.cuh"
 
 namespace vqa {
@@ -141,6 +142,53 @@ __global__ void generate_init_kernel(int B, int max_new, int* __restrict__ token
 // positions to keep). It finishes on an EOS id or at max_new tokens; the block that finishes the last sequence raises *all_done. A finished
 // sequence is left untouched.
 constexpr int SELECT_THREADS = 1024;
+
+// The per-token bookkeeping of both selection kernels, run by one thread of sequence b's block once its token `tok` is chosen.
+__device__ __forceinline__ void select_commit(int b, int tok, uint32_t* pen_bitmap, int pen_words, const int* eos_ids, int n_eos, int max_new,
+                                              const int* first_pos, int B, int* tokens, int* lengths, int* done, int* n_done, int* all_done,
+                                              int* next_ids, int* pos3) {
+    const int t = lengths[b];
+    tokens[(size_t)b * max_new + t] = tok;
+    lengths[b] = t + 1;
+    if (pen_bitmap) pen_bitmap[(size_t)b * pen_words + (tok >> 5)] |= 1u << (tok & 31);
+    next_ids[b] = tok;
+    if (pos3) {
+        const int p = first_pos[b] + t;
+        pos3[b] = p; pos3[B + b] = p; pos3[2 * B + b] = p;
+    }
+    bool fin = t + 1 >= max_new;
+    for (int e = 0; e < n_eos; ++e) fin |= tok == eos_ids[e];
+    if (fin) {
+        done[b] = 1;
+        if (atomicAdd(n_done, 1) + 1 == B) *all_done = 1;
+    }
+}
+
+// bf16 logit -> fp32 -> HF's RepetitionPenaltyLogitsProcessor when id n's bit is set in the row's bitmap pb (NULL = no penalty)
+__device__ __forceinline__ float penalised_logit(const __nv_bfloat16* lr, const uint32_t* pb, float penalty, int n) {
+    float x = __bfloat162float(lr[n]);
+    if (pb && ((pb[n >> 5] >> (n & 31)) & 1u)) x = x < 0.f ? x * penalty : __fdiv_rn(x, penalty);
+    return x;
+}
+
+// Block-wide arg-max of (best, bid) over SELECT_THREADS threads, ties to the lowest id; every thread gets the result. s_v / s_i hold
+// SELECT_THREADS / 32 entries.
+__device__ __forceinline__ int block_argmax(float best, int bid, float* s_v, int* s_i) {
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bid, o);
+        if (ov > best || (ov == best && oi < bid)) { best = ov; bid = oi; }
+    }
+    if ((tid & 31) == 0) { s_v[tid >> 5] = best; s_i[tid >> 5] = bid; }
+    __syncthreads();
+    best = s_v[0]; bid = s_i[0];
+    for (int w = 1; w < SELECT_THREADS / 32; ++w)
+        if (s_v[w] > best || (s_v[w] == best && s_i[w] < bid)) { best = s_v[w]; bid = s_i[w]; }
+    return bid;
+}
+
 __global__ void __launch_bounds__(SELECT_THREADS) greedy_select_kernel(
         const __nv_bfloat16* __restrict__ logits, int V, uint32_t* __restrict__ pen_bitmap, int pen_words, float penalty,
         const int* __restrict__ eos_ids, int n_eos, int max_new, const int* __restrict__ first_pos, int B, int* __restrict__ tokens,
@@ -156,36 +204,245 @@ __global__ void __launch_bounds__(SELECT_THREADS) greedy_select_kernel(
     float best = -INFINITY;
     int bid = 0x7fffffff;
     for (int n = tid; n < V; n += SELECT_THREADS) {
-        float x = __bfloat162float(lr[n]);
-        if (pb && ((pb[n >> 5] >> (n & 31)) & 1u)) x = x < 0.f ? x * penalty : __fdiv_rn(x, penalty);
+        const float x = penalised_logit(lr, pb, penalty, n);
         if (x > best || bid == 0x7fffffff) { best = x; bid = n; }      // ids rise along the scan: strict > keeps the lowest of equals
     }
+    const int tok = block_argmax(best, bid, s_v, s_i);
+    if (tid == 0)
+        select_commit(b, tok, pen_bitmap, pen_words, eos_ids, n_eos, max_new, first_pos, B, tokens, lengths, done, n_done, all_done, next_ids,
+                      pos3);
+}
+
+// ------------------------------------------------------------------------------------------------ sampled selection
+// Philox4x32-10 (Salmon, Moraes, Dror & Shaw, SC'11; the philox4x32 of Random123 with 10 rounds): counter c, key (k0, k1).
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bid, o);
-        if (ov > best || (ov == best && oi < bid)) { best = ov; bid = oi; }
+    for (int r = 0; r < 10; ++r) {
+        if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
     }
-    if ((tid & 31) == 0) { s_v[tid >> 5] = best; s_i[tid >> 5] = bid; }
+    return c;
+}
+
+// fp32 -> uint32 whose unsigned order is the float order (+0 and -0 must have been merged before)
+__device__ __forceinline__ uint32_t order_key(float x) {
+    const uint32_t u = __float_as_uint(x);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// Mass exp(x - max) of one token as an integer of 2^-40 units: sums of them are exact and independent of the summation order, so the
+// top-p cut is deterministic. A vocabulary of < 2^23 tokens, each <= 2^40, cannot overflow 64 bits; dropping terms below 2^-41 moves a
+// cumulative probability by < V * 2^-41 (7e-8 at V = 152,064).
+__device__ __forceinline__ unsigned long long mass_fx(float x, float mx) {
+    return (unsigned long long)(expf(x - mx) * 1099511627776.0f + 0.5f);
+}
+
+constexpr int SAMPLE_BINS = 2048;       // 11-bit radix digits: three passes (11, 11, 10 bits) select one 32-bit key
+constexpr int SAMPLE_UNROLL = 8;
+
+// Of the bins h[0, nb) taken from the highest when from_top (else from the lowest), the first whose inclusive running sum exceeds
+// *target; on return every thread sees that bin in *bin and *target reduced by the sum of the bins before it. With frac >= 0 the target is
+// first set to floor(frac * sum of all bins). A target at or past the sum of all bins (frac rounded to 1, e.g. fp32(1 - 1e-8)) is taken
+// as that sum - 1: the last unit then sits past it, so the last bin is found, as HF keeps its last id when every cumulative probability
+// is at or below the threshold. The callers' bins never sum to 0. Each thread owns two consecutive positions of the order; s_w holds 32
+// partial sums.
+__device__ void radix_find(const unsigned long long* h, int nb, bool from_top, float frac, unsigned long long* target, int* bin,
+                           unsigned long long* s_w) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    auto at = [&](int o) -> unsigned long long { return o < nb ? h[from_top ? nb - 1 - o : o] : 0ull; };
+    const unsigned long long a = at(2 * tid), c = at(2 * tid + 1);
+    unsigned long long incl = a + c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+    }
+    if (lane == 31) s_w[warp] = incl;
     __syncthreads();
-    if (tid != 0) return;
-    for (int w = 1; w < SELECT_THREADS / 32; ++w)
-        if (s_v[w] > best || (s_v[w] == best && s_i[w] < bid)) { best = s_v[w]; bid = s_i[w]; }
-    const int tok = bid, t = lengths[b];
-    tokens[(size_t)b * max_new + t] = tok;
-    lengths[b] = t + 1;
-    if (pen_bitmap) pen_bitmap[(size_t)b * pen_words + (tok >> 5)] |= 1u << (tok & 31);
-    next_ids[b] = tok;
-    if (pos3) {
-        const int p = first_pos[b] + t;
-        pos3[b] = p; pos3[B + b] = p; pos3[2 * B + b] = p;
+    unsigned long long before = 0, total = 0;
+    for (int w = 0; w < SELECT_THREADS / 32; ++w) {
+        if (w < warp) before += s_w[w];
+        total += s_w[w];
     }
-    bool fin = t + 1 >= max_new;
-    for (int e = 0; e < n_eos; ++e) fin |= tok == eos_ids[e];
-    if (fin) {
-        done[b] = 1;
-        if (atomicAdd(n_done, 1) + 1 == B) *all_done = 1;
+    const unsigned long long excl = before + incl - a - c;
+    unsigned long long tg = frac >= 0.f ? (unsigned long long)((double)frac * (double)total) : *target;
+    if (tg >= total) tg = total - 1;
+    __syncthreads();      // every thread has read *target and s_w
+    if (excl <= tg && tg < excl + a + c) {
+        const bool first = tg < excl + a;
+        const int o = 2 * tid + (first ? 0 : 1);
+        *bin = from_top ? nb - 1 - o : o;
+        *target = tg - (first ? excl : excl + a);
     }
+    __syncthreads();
+}
+
+// Sampled token selection, a drop-in for greedy_select_kernel (same bookkeeping through select_commit), one block per sequence. The
+// processed score of id n is HF's for generate(do_sample=True): the penalised fp32 logit, then TemperatureLogitsWarper (an IEEE fp32
+// division by `temperature`, skipped at 1), with -0 taken as +0 and saturated to [-FLT_MAX, FLT_MAX] (a score that overflows, or a NaN
+// logit, makes HF's softmax NaN and torch.multinomial raise; here +inf ties at FLT_MAX and -inf or NaN take -FLT_MAX, so the maximum is
+// finite, the mass of the maximum is 2^40 and a kept id always exists). Then, as HF's warpers in order:
+//   top-k (0 < top_k < V): the k-th largest score v_k, found by radix select; every id with score >= v_k stays, ties included;
+//   top-p (top_p < 1): in ascending (score, id) order, the ids whose cumulative probability among the kept ones is <= fp32(1 - top_p)
+//     go; the most probable id always stays. Within the group of equal scores at the cut, lower ids go first (what a stable ascending
+//     sort gives). The cut's score is found by radix select over the cumulative mass; the group's split by one pass in id order.
+// The token is the Gumbel-max over the kept ids: argmax((score_n - max) - log(-log u_n)) (ties to the lowest id), which draws id n with
+// probability softmax(kept scores)[n]. u_n is lane n & 3 of Philox4x32-10 with key seeds[b] (low word first) and counter
+// (n >> 2, t, 0, 0), t = lengths[b], as ((bits >> 8) + 0.5) * 2^-24 (-log u is taken without rounding u; both logs are the accurate
+// logf / log1pf): the draw depends on (seed, step, id) only, not on the batch position, the launch or the thread layout.
+// kept (debugging, NULL = none): the kept set as a bitmap [B, ceil(V / 32)], fully rewritten.
+__global__ void __launch_bounds__(SELECT_THREADS) sample_select_kernel(
+        const __nv_bfloat16* __restrict__ logits, int V, uint32_t* __restrict__ pen_bitmap, int pen_words, float penalty,
+        const unsigned long long* __restrict__ seeds, float temperature, int top_k, float top_p, const int* __restrict__ eos_ids, int n_eos,
+        int max_new, const int* __restrict__ first_pos, int B, int* __restrict__ tokens, int* __restrict__ lengths, int* __restrict__ done,
+        int* __restrict__ n_done, int* __restrict__ all_done, int* __restrict__ next_ids, int* __restrict__ pos3, uint32_t* __restrict__ kept) {
+    pdl_launch_dependents();
+    __shared__ unsigned long long s_h[SAMPLE_BINS];
+    __shared__ unsigned long long s_w[SELECT_THREADS / 32];
+    __shared__ float s_v[SELECT_THREADS / 32];
+    __shared__ int s_i[SELECT_THREADS / 32];
+    __shared__ unsigned long long s_target;
+    __shared__ int s_bin;
+    const int b = blockIdx.x, tid = threadIdx.x;
+    if (done[b]) return;
+    const __nv_bfloat16* lr = logits + (size_t)b * V;
+    const uint32_t* pb = pen_bitmap ? pen_bitmap + (size_t)b * pen_words : nullptr;
+    const int step = lengths[b];
+    auto score = [&](int n) {
+        float x = penalised_logit(lr, pb, penalty, n);
+        if (temperature != 1.0f) x = __fdiv_rn(x, temperature);
+        return x == 0.f ? 0.f : fminf(fmaxf(x, -FLT_MAX), FLT_MAX);      // fmaxf(NaN, -FLT_MAX) is -FLT_MAX
+    };
+    // fn(n, score(n)) for every id; a thread reads SAMPLE_UNROLL ids before it consumes them, so it has that many loads in flight
+    auto scan_row = [&](auto&& fn) {
+        for (int base = 0; base < V; base += SELECT_THREADS * SAMPLE_UNROLL) {
+            float x[SAMPLE_UNROLL];
+#pragma unroll
+            for (int u = 0; u < SAMPLE_UNROLL; ++u) {
+                const int n = base + u * SELECT_THREADS + tid;
+                x[u] = n < V ? score(n) : 0.f;
+            }
+#pragma unroll
+            for (int u = 0; u < SAMPLE_UNROLL; ++u) {
+                const int n = base + u * SELECT_THREADS + tid;
+                if (n < V) fn(n, x[u]);
+            }
+        }
+    };
+    // the maximum (the reference point of the masses)
+    float mx = -INFINITY;
+    scan_row([&](int, float x) { mx = fmaxf(mx, x); });
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((tid & 31) == 0) s_v[tid >> 5] = mx;
+    __syncthreads();
+    for (int w = 0; w < SELECT_THREADS / 32; ++w) mx = fmaxf(mx, s_v[w]);
+    __syncthreads();
+
+    // Three radix passes over the keys of the ids `in` admits: the key at which the running sum of add(n) -- taken from the highest key
+    // when from_top -- first exceeds the target; returns it, the target reduced by the sum of all keys before it.
+    auto radix_select = [&](auto&& in, auto&& add, bool from_top, float frac, unsigned long long target, uint32_t* key_out) {
+        uint32_t prefix = 0, mask = 0;
+        if (tid == 0) s_target = target;
+        for (int pass = 0; pass < 3; ++pass) {
+            const int shift = pass == 0 ? 21 : pass == 1 ? 10 : 0, nb = pass == 2 ? 1024 : 2048;
+            for (int i = tid; i < SAMPLE_BINS; i += SELECT_THREADS) s_h[i] = 0ull;
+            __syncthreads();
+            scan_row([&](int, float x) {
+                const uint32_t k = order_key(x);
+                if ((k & mask) == prefix && in(k)) atomicAdd(&s_h[(k >> shift) & (nb - 1)], add(x));
+            });
+            __syncthreads();
+            radix_find(s_h, nb, from_top, pass == 0 ? frac : -1.f, &s_target, &s_bin, s_w);
+            prefix |= (uint32_t)s_bin << shift;
+            mask |= (uint32_t)(nb - 1) << shift;
+        }
+        *key_out = prefix;
+        return s_target;
+    };
+    // top-k: the k-th largest key (k - 1 keys above it); ids below it are out
+    uint32_t key_k = 0;
+    if (top_k > 0 && top_k < V)
+        radix_select([](uint32_t) { return true; }, [](float) { return 1ull; }, true, -1.f, (unsigned long long)(top_k - 1), &key_k);
+    // top-p: the key whose group holds the cut, and how many of the group (lowest ids first) go
+    uint32_t key_p = 0;
+    int id_p = 0;
+    if (top_p < 1.0f) {
+        const float thr = (float)(1.0 - (double)top_p);
+        unsigned long long rest = radix_select([&](uint32_t k) { return k >= key_k; }, [&](float x) { return mass_fx(x, mx); }, false, thr,
+                                               0ull, &key_p);
+        // ids of the group at the cut with cumulative mass below + (j + 1) q <= limit go: the first floor(rest / q)
+        const float xv = __uint_as_float((key_p & 0x80000000u) ? (key_p & 0x7fffffffu) : ~key_p);
+        const unsigned long long q = mass_fx(xv, mx);
+        const int drop = (int)(rest / q);
+        if (drop > 0) {
+            // the id of group member `drop` in id order: each thread counts the members in its own contiguous id range
+            const int per = (V + SELECT_THREADS - 1) / SELECT_THREADS, n0 = min(V, tid * per), n1 = min(V, n0 + per);
+            int cnt = 0;
+            for (int n = n0; n < n1; ++n) cnt += order_key(score(n)) == key_p;
+            int incl = cnt;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, incl, o);
+                if ((tid & 31) >= o) incl += v;
+            }
+            if ((tid & 31) == 31) s_i[tid >> 5] = incl;
+            __syncthreads();
+            int before = incl - cnt;
+            for (int w = 0; w < (tid >> 5); ++w) before += s_i[w];
+            if (before <= drop && drop < before + cnt) {
+                int j = before;
+                for (int n = n0; n < n1; ++n)
+                    if (order_key(score(n)) == key_p && j++ == drop) { s_bin = n; break; }
+            }
+            __syncthreads();
+            id_p = s_bin;
+            __syncthreads();
+        }
+    }
+    // Gumbel-max over the kept ids; each thread takes four consecutive ids, the four lanes of one Philox block
+    const uint32_t seed_lo = (uint32_t)seeds[b], seed_hi = (uint32_t)(seeds[b] >> 32);
+    uint32_t* kb = kept ? kept + (size_t)b * pen_words : nullptr;
+    if (kb) {
+        for (int w = tid; w < pen_words; w += SELECT_THREADS) kb[w] = 0u;
+        __syncthreads();
+    }
+    float best = -INFINITY;
+    int bid = 0x7fffffff;
+    for (int g0 = 0; g0 * 4 < V; g0 += SELECT_THREADS * 2) {
+        float x[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int n = (g0 + (i >> 2) * SELECT_THREADS + tid) * 4 + (i & 3);
+            x[i] = n < V ? score(n) : 0.f;
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int g = g0 + h * SELECT_THREADS + tid;
+            uint4 r = make_uint4(0u, 0u, 0u, 0u);
+            bool drawn = false;
+#pragma unroll
+            for (int l = 0; l < 4; ++l) {
+                const int n = g * 4 + l;
+                const uint32_t k = order_key(x[h * 4 + l]);
+                if (n >= V || k < key_k || k < key_p || (k == key_p && n < id_p)) continue;
+                if (!drawn) { r = philox4x32_10(make_uint4((uint32_t)g, (uint32_t)step, 0u, 0u), seed_lo, seed_hi); drawn = true; }
+                // e = -log(u), u = (m + 0.5) 2^-24 without rounding u: for m >= 2^23, 1 - u = (2^24 - m - 0.5) 2^-24 is exact instead
+                const uint32_t m = (l == 0 ? r.x : l == 1 ? r.y : l == 2 ? r.z : r.w) >> 8;
+                const float e = m < (1u << 23) ? -logf(((float)m + 0.5f) * 5.9604644775390625e-8f)
+                                               : -log1pf(-((float)((1u << 24) - m) - 0.5f) * 5.9604644775390625e-8f);
+                const float v = (x[h * 4 + l] - mx) - logf(e);
+                if (v > best || bid == 0x7fffffff) { best = v; bid = n; }
+                if (kb) atomicOr(&kb[n >> 5], 1u << (n & 31));
+            }
+        }
+    }
+    const int tok = block_argmax(best, bid, s_v, s_i);
+    if (tid == 0)
+        select_commit(b, tok, pen_bitmap, pen_words, eos_ids, n_eos, max_new, first_pos, B, tokens, lengths, done, n_done, all_done, next_ids,
+                      pos3);
 }
 
 // Answer log-probabilities of one generation step (the scores a rollout is scored on), one block per sequence, launched between the
@@ -364,4 +621,13 @@ static int greedy_select(Forward& f, const bf16* logits, int B, int V, uint32_t*
                          int* pos3) {
     return f.launch(CAT_OTHER, 0, "greedy select", greedy_select_kernel, B, SELECT_THREADS, 0, logits, V, pen_bitmap, (V + 31) / 32, penalty,
                     eos_ids, n_eos, max_new, first_pos, B, tokens, lengths, done, n_done, all_done, next_ids, pos3);
+}
+
+// The sampled token of every unfinished sequence under `s` and the same bookkeeping as greedy_select (kept: see sample_select_kernel).
+static int sample_select(Forward& f, const bf16* logits, int B, int V, uint32_t* pen_bitmap, float penalty, const vqa_qwen25vl_sampling& s,
+                         const int* eos_ids, int n_eos, int max_new, const int* first_pos, int* tokens, int* lengths, int* done, int* n_done,
+                         int* all_done, int* next_ids, int* pos3, uint32_t* kept = nullptr) {
+    return f.launch(CAT_OTHER, 0, "sample select", sample_select_kernel, B, SELECT_THREADS, 0, logits, V, pen_bitmap, (V + 31) / 32, penalty,
+                    (const unsigned long long*)s.seeds, s.temperature, s.top_k, s.top_p, eos_ids, n_eos, max_new, first_pos, B, tokens,
+                    lengths, done, n_done, all_done, next_ids, pos3, kept);
 }

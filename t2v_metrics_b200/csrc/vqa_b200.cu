@@ -322,6 +322,8 @@ static_assert(sizeof(vqa_qwen25vl_packed) == 56 && offsetof(vqa_qwen25vl_packed,
 static_assert(sizeof(vqa_qwen25vl_answer_score) == 56 && offsetof(vqa_qwen25vl_answer_score, out_topk_probs) == 48,
               "vqa_qwen25vl_answer_score layout");
 static_assert(sizeof(vqa_qwen25vl_generation) == 72 && offsetof(vqa_qwen25vl_generation, score) == 64, "vqa_qwen25vl_generation layout");
+static_assert(sizeof(vqa_qwen25vl_sampling) == 24 && offsetof(vqa_qwen25vl_sampling, temperature) == 8 &&
+              offsetof(vqa_qwen25vl_sampling, top_k) == 12 && offsetof(vqa_qwen25vl_sampling, top_p) == 16, "vqa_qwen25vl_sampling layout");
 
 static int qwen_handle_check(vqa_handle* h) {
     if (!h || h->kind != 1) return fail(h, VQA_ERR_INVALID_ARG, "not a Qwen2.5-VL handle");
@@ -398,25 +400,60 @@ static int qwen_gen_check(vqa_handle* h, const vqa_qwen25vl_generation* a, int32
     return VQA_OK;
 }
 
+// A sampled generation's parameters; the reference's scored forward is always greedy, so no answer score goes with them.
+static int qwen_sampling_check(vqa_handle* h, const vqa_qwen25vl_sampling* s, const vqa_qwen25vl_answer_score* score) {
+    if (!s || !s->seeds) return fail(h, VQA_ERR_INVALID_ARG, "sampling: null sampling struct or seeds");
+    if (score) return fail(h, VQA_ERR_INVALID_ARG, "sampling: a scored rollout is greedy (gen->score must be NULL)");
+    if (!(s->temperature > 0.f) || !std::isfinite(s->temperature) || s->top_k < 0 || !(s->top_p > 0.f) || !(s->top_p <= 1.f))
+        return fail(h, VQA_ERR_INVALID_ARG, "sampling: bad parameters (temperature > 0 and finite, top_k >= 0, 0 < top_p <= 1)");
+    return VQA_OK;
+}
+
 extern "C" size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, int32_t max_new_tokens) {
     if (!h || h->kind != 1 || batch <= 0 || seq_len <= 0 || n_patches <= 0 || max_new_tokens <= 0) return 0;
     return qwen_gen_plan(h->qwen->cfg, batch, seq_len, n_patches, max_new_tokens, h->num_sms).total;
 }
 
-extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
-                                             void* workspace, size_t workspace_bytes, void* stream) {
+// The prefill and step of both generations: smp NULL = greedy, else sampled (checked by the _sampled entry points).
+static int qwen_gen_prefill_entry(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
+                                  const vqa_qwen25vl_sampling* smp, void* workspace, size_t workspace_bytes, void* stream) {
     if (!prompts) return fail(h, VQA_ERR_INVALID_ARG, "null prompts");
     if (int rc = qwen_gen_check(h, gen, prompts->batch, prompts->seq_len, prompts->n_patches, workspace)) return rc;
     if (int rc = qwen_prompts_check(h, prompts, false)) return rc;
     // the steps read the prompt lengths from gen->seq_lens: the prefill must have used the same ones
     if (gen->seq_lens != prompts->seq_lens) return fail(h, VQA_ERR_INVALID_ARG, "gen->seq_lens and prompts->seq_lens must be the same pointer");
-    return qwen_generate_prefill(h, *h->qwen, *prompts, *gen, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+    return qwen_generate_prefill(h, *h->qwen, *prompts, *gen, smp, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
+static int qwen_gen_step_entry(vqa_handle* h, const vqa_qwen25vl_generation* gen, const vqa_qwen25vl_sampling* smp, int32_t batch,
+                               int32_t seq_len, int32_t n_patches, void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = qwen_gen_check(h, gen, batch, seq_len, n_patches, workspace)) return rc;
+    return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, *gen, smp, workspace, workspace_bytes,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vqa_qwen25vl_generate_prefill(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
+                                             void* workspace, size_t workspace_bytes, void* stream) {
+    return qwen_gen_prefill_entry(h, prompts, gen, nullptr, workspace, workspace_bytes, stream);
 }
 
 extern "C" int vqa_qwen25vl_generate_step(vqa_handle* h, const vqa_qwen25vl_generation* gen, int32_t batch, int32_t seq_len, int32_t n_patches,
                                           void* workspace, size_t workspace_bytes, void* stream) {
-    if (int rc = qwen_gen_check(h, gen, batch, seq_len, n_patches, workspace)) return rc;
-    return qwen_generate_step(h, *h->qwen, batch, seq_len, n_patches, *gen, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+    return qwen_gen_step_entry(h, gen, nullptr, batch, seq_len, n_patches, workspace, workspace_bytes, stream);
+}
+
+extern "C" int vqa_qwen25vl_generate_prefill_sampled(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
+                                                     const vqa_qwen25vl_sampling* sampling, void* workspace, size_t workspace_bytes,
+                                                     void* stream) {
+    if (int rc = qwen_sampling_check(h, sampling, gen ? gen->score : nullptr)) return rc;
+    return qwen_gen_prefill_entry(h, prompts, gen, sampling, workspace, workspace_bytes, stream);
+}
+
+extern "C" int vqa_qwen25vl_generate_step_sampled(vqa_handle* h, const vqa_qwen25vl_generation* gen, const vqa_qwen25vl_sampling* sampling,
+                                                  int32_t batch, int32_t seq_len, int32_t n_patches, void* workspace, size_t workspace_bytes,
+                                                  void* stream) {
+    if (int rc = qwen_sampling_check(h, sampling, gen ? gen->score : nullptr)) return rc;
+    return qwen_gen_step_entry(h, gen, sampling, batch, seq_len, n_patches, workspace, workspace_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ kernel-level ABI
@@ -607,6 +644,21 @@ extern "C" int vqa_op_greedy_select(const void* logits, int32_t B, int32_t V, ui
     return glue_launch(stream, [&](Forward& f) {
         return greedy_select(f, (const bf16*)logits, B, V, pen_bitmap, repetition_penalty, eos_ids, n_eos, max_new, first_pos, tokens, lengths, done,
                              n_done, all_done, next_ids, pos3);
+    });
+}
+
+extern "C" int vqa_op_sample_select(const void* logits, int32_t B, int32_t V, uint32_t* pen_bitmap, float repetition_penalty, const int32_t* eos_ids,
+                                    int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
+                                    int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, const vqa_qwen25vl_sampling* sampling,
+                                    uint32_t* kept, void* stream) {
+    if (!logits || !tokens || !lengths || !done || !n_done || !all_done || !next_ids || (n_eos > 0 && !eos_ids) || (!first_pos != !pos3))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "sample select: null pointer (first_pos and pos3 are given together or not at all)");
+    if (B <= 0 || V <= 0 || max_new <= 0 || n_eos < 0 || !(repetition_penalty > 0.f))
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "sample select: bad size / repetition penalty");
+    if (int rc = qwen_sampling_check(nullptr, sampling, nullptr)) return rc;
+    return glue_launch(stream, [&](Forward& f) {
+        return sample_select(f, (const bf16*)logits, B, V, pen_bitmap, repetition_penalty, *sampling, eos_ids, n_eos, max_new, first_pos, tokens,
+                             lengths, done, n_done, all_done, next_ids, pos3, kept);
     });
 }
 

@@ -560,6 +560,19 @@ class ops:
               _stream_ptr(logits.device))
 
     @staticmethod
+    def sample_select(logits: torch.Tensor, seeds: torch.Tensor, temperature: float, top_k: int, top_p: float, tokens: torch.Tensor,
+                      lengths: torch.Tensor, done: torch.Tensor, n_done: torch.Tensor, all_done: torch.Tensor, next_ids: torch.Tensor, eos_ids=None,
+                      pen_bitmap=None, repetition_penalty: float = 1.0, first_pos=None, pos3=None, kept=None):
+        """One sampled selection step (vqa_op_sample_select): greedy_select's state and arguments, plus int64 seeds [B] on the device and
+        the warpers' (temperature, top_k, top_p). kept: None or int32 [B, ceil(V / 32)] that receives each unfinished row's kept-id bitmap."""
+        B, V = logits.shape
+        n_eos = eos_ids.numel() if eos_ids is not None else 0
+        smp = _lib.VqaQwen25VLSampling(seeds=_ptr(seeds), temperature=float(temperature), top_k=int(top_k), top_p=float(top_p))
+        _call("vqa_op_sample_select", _ptr(logits), B, V, _ptr(pen_bitmap), float(repetition_penalty), _ptr(eos_ids), n_eos, tokens.shape[1],
+              _ptr(first_pos), _ptr(tokens), _ptr(lengths), _ptr(done), _ptr(n_done), _ptr(all_done), _ptr(next_ids), _ptr(pos3), C.byref(smp),
+              _ptr(kept), _stream_ptr(logits.device))
+
+    @staticmethod
     def t5_bucket_lut(bidirectional: bool, num_buckets: int, max_distance: int) -> torch.Tensor:
         """The engine's relative-position bucket table (host): int32 [2 * max_distance + 1], entry rel + max_distance."""
         out = torch.empty(2 * max_distance + 1, dtype=torch.int32)
@@ -1281,13 +1294,17 @@ class QwenVLEngine(_Engine):
         return int(self.lib.vqa_qwen25vl_generate_workspace_bytes(self._h, batch, seq_len, n_patches, max_new_tokens))
 
     def generate_begin(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
-                       repetition_penalty: float = 1.0, second_per_grid_ts=None, score: Optional[dict] = None) -> dict:
+                       repetition_penalty: float = 1.0, second_per_grid_ts=None, score: Optional[dict] = None,
+                       sample: Optional[dict] = None) -> dict:
         """The prefill of a greedy generation (vqa_qwen25vl_generate_prefill): vision tower, padded prompt prefill into the K/V cache, first
         token. Returns the generation state that generate_step() advances: device tensors `tokens` [B, max_new_tokens] (-1 after a prompt's
         last token), `lengths` [B] and `all_done` [1], all owned by the state of this call shape.
         score = dict(answer_ids=[ids per prompt], temperature=T, top_k=k) makes it a scored rollout (an answer score in the generation): the
         state also holds `logp` [B, max_new_tokens, n_max] (NaN where nothing was written) and, with k > 0, `topk_ids` / `topk_probs`
-        [B, max_new_tokens, k]."""
+        [B, max_new_tokens, k].
+        sample = dict(seeds=[one int per prompt], temperature=T, top_k=k, top_p=p) makes it a sampled generation
+        (vqa_qwen25vl_generate_*_sampled). The seeds go to a device buffer of the state before each prefill, so one captured step graph
+        serves every seed."""
         from . import qwen_host
         cfg, dev = self.cfg, self.device
         B = len(prompts)
@@ -1308,11 +1325,17 @@ class QwenVLEngine(_Engine):
                 raise ValueError("rollout scoring needs one non-empty answer id list per prompt")
             n_max, temp, top_k = max(len(a) for a in answers), float(score.get("temperature", 1.0)), int(score.get("top_k", 0))
             key += ("rollout", n_max, temp, top_k)
+        if sample is not None:
+            seeds = [int(x) for x in sample["seeds"]]
+            if len(seeds) != B or not all(0 <= x < 1 << 64 for x in seeds):
+                raise ValueError("sampling needs one seed in [0, 2^64) per prompt")
+            smp_t, smp_k, smp_p = float(sample["temperature"]), int(sample["top_k"]), float(sample["top_p"])
+            key += ("sample", smp_t, smp_k, smp_p)
 
         def make() -> dict:
             i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
             st = dict(B=B, S=S, n_patches=vi["n_patches"], max_new=max_new, seq_lens=i32(B), first=i32(B), eos=i32(max(len(eos), 1)),
-                      tokens=i32(B, max_new), lengths=i32(B), all_done=i32(1), graph=None, score=None)
+                      tokens=i32(B, max_new), lengths=i32(B), all_done=i32(1), graph=None, score=None, sample=None)
             # the vqa_qwen25vl_generation every call of this state passes, built once: its pointers are the state's own tensors
             st["gen"] = _lib.VqaQwen25VLGeneration(
                 seq_lens=_ptr(st["seq_lens"]), first_position=_ptr(st["first"]), eos_ids=_ptr(st["eos"]), n_eos=len(eos), max_new_tokens=max_new,
@@ -1327,6 +1350,9 @@ class QwenVLEngine(_Engine):
                                                            temperature=temp, top_k=top_k, out_logp=_ptr(sc["logp"]),
                                                            out_topk_ids=_ptr(sc["topk_ids"]), out_topk_probs=_ptr(sc["topk_probs"]))
                 st["gen"].score = C.pointer(sc["struct"])
+            if sample is not None:
+                sm = st["sample"] = dict(seeds=torch.empty(B, dtype=torch.int64, device=dev))
+                sm["struct"] = _lib.VqaQwen25VLSampling(seeds=_ptr(sm["seeds"]), temperature=smp_t, top_k=smp_k, top_p=smp_p)
             return st
         st = self._gen_state(key, need, make)
         st["seq_lens"].copy_(idx["seq_lens"], non_blocking=True)
@@ -1344,21 +1370,32 @@ class QwenVLEngine(_Engine):
             if sc["top_k"] > 0:
                 sc["topk_ids"].fill_(-1)
                 sc["topk_probs"].fill_(float("nan"))
+        if st["sample"] is not None:
+            # uint64 seeds in an int64 buffer: the same 8 bytes
+            st["sample"]["seeds"].copy_(torch.tensor([x - (1 << 64) if x >= 1 << 63 else x for x in seeds], dtype=torch.int64), non_blocking=True)
         d = {k: v.to(dev) for k, v in idx.items()}
 
         def prefill():
             prompts = self._prompts(pixel_patches, vi, d["input_ids"], st["seq_lens"], d["feat_index"], d["position_ids"], B, S)
             ws = self._gen_workspace
-            self._run("vqa_qwen25vl_generate_prefill", C.byref(prompts), C.byref(st["gen"]), _ptr(ws), ws.numel(), _stream_ptr(dev))
+            if st["sample"] is None:
+                self._run("vqa_qwen25vl_generate_prefill", C.byref(prompts), C.byref(st["gen"]), _ptr(ws), ws.numel(), _stream_ptr(dev))
+            else:
+                self._run("vqa_qwen25vl_generate_prefill_sampled", C.byref(prompts), C.byref(st["gen"]), C.byref(st["sample"]["struct"]),
+                          _ptr(ws), ws.numel(), _stream_ptr(dev))
         st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
         prefill()
         return st
 
     def generate_step(self, st: dict):
-        """One decode step of the generation `st` (vqa_qwen25vl_generate_step), launched directly."""
+        """One decode step of the generation `st` (vqa_qwen25vl_generate_step, or _step_sampled), launched directly."""
         ws = self._gen_workspace
-        self._run("vqa_qwen25vl_generate_step", C.byref(st["gen"]), st["B"], st["S"], st["n_patches"], _ptr(ws), ws.numel(),
-                  _stream_ptr(self.device))
+        if st["sample"] is None:
+            self._run("vqa_qwen25vl_generate_step", C.byref(st["gen"]), st["B"], st["S"], st["n_patches"], _ptr(ws), ws.numel(),
+                      _stream_ptr(self.device))
+        else:
+            self._run("vqa_qwen25vl_generate_step_sampled", C.byref(st["gen"]), C.byref(st["sample"]["struct"]), st["B"], st["S"],
+                      st["n_patches"], _ptr(ws), ws.numel(), _stream_ptr(self.device))
 
     def generate_prompts(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], image_of_sample=None,
                          repetition_penalty: float = 1.0, second_per_grid_ts=None, use_graph: bool = True, check_every: int = 16):
@@ -1385,3 +1422,14 @@ class QwenVLEngine(_Engine):
         sc = st["score"]
         cpu = lambda t: None if t is None else t.cpu()
         return dict(tokens=tokens, lengths=lengths, logp=cpu(sc["logp"]), topk_ids=cpu(sc["topk_ids"]), topk_probs=cpu(sc["topk_probs"]))
+
+    def sample_prompts(self, pixel_patches, grid_thw, prompts, max_new_tokens: int, eos_ids: Sequence[int], seeds: Sequence[int],
+                       temperature: float, top_k: int, top_p: float, image_of_sample=None, repetition_penalty: float = 1.0,
+                       second_per_grid_ts=None, use_graph: bool = True, check_every: int = 16):
+        """Sampled generation (HF generate(do_sample=True) with the repetition penalty, temperature, top_k and top_p warpers) for a batch
+        of prompts, as generate_prompts runs greedy generation: one prefill, then decode steps replayed from a CUDA graph captured once per
+        (call shape, temperature, top_k, top_p). Prompt b's tokens depend on seeds[b] (an integer in [0, 2^64)), its prompt and the sizes,
+        not on its batch position. Returns each prompt's generated ids, the EOS id included when one ended it."""
+        st = self.generate_begin(pixel_patches, grid_thw, prompts, max_new_tokens, eos_ids, image_of_sample, repetition_penalty,
+                                 second_per_grid_ts, sample=dict(seeds=seeds, temperature=temperature, top_k=top_k, top_p=top_p))
+        return self._decode_loop(st, use_graph, check_every)[0]

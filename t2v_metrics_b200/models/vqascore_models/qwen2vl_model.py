@@ -93,6 +93,35 @@ def _require_rollout_engine(plugin) -> None:
                                   "plugin has none; without it only the single-prefill scoring of max_new_tokens=1 exists")
 
 
+# Warpers transformers adds for generate(do_sample=True) when generation_config.json enables them (generation/utils.py:1197-1230), with the
+# value that leaves each one off. The engine samples with repetition penalty, temperature, top-k and top-p only; a checkpoint that turns
+# one of these on is refused rather than sampled from another distribution.
+_UNSUPPORTED_WARPERS = {"min_p": None, "typical_p": 1.0, "epsilon_cutoff": 0.0, "eta_cutoff": 0.0, "top_h": None}
+HF_DEFAULT_TOP_K = 50      # GenerationConfig's top_k when neither the call nor generation_config.json sets one
+
+
+def sampling_params(checkpoint_path: str, do_sample: Optional[bool], temperature: float, top_p: float) -> Optional[tuple]:
+    """(temperature, top_k, top_p) of the reference's generate (qwen2vl_model.py:512-551), or None for greedy decoding. do_sample None means
+    temperature > 0, and only do_sample with temperature > 0 samples. The call passes temperature and top_p, so top_k is the one of the
+    generation_config.json beside the checkpoint, else transformers' default 50 (0 = off). A file that enables another warper raises."""
+    from ...checkpoint import generation_config_value
+    if do_sample is None:
+        do_sample = temperature > 0
+    if not (do_sample and temperature > 0):
+        return None
+    for key, off in _UNSUPPORTED_WARPERS.items():
+        v = generation_config_value(checkpoint_path, key, off)
+        if v != off:
+            raise NotImplementedError(f"generation_config.json sets {key} = {v!r}: sampling supports the repetition penalty, temperature, "
+                                      "top_k and top_p warpers only")
+    if not (0.0 < top_p <= 1.0) or not torch.isfinite(torch.tensor(float(temperature))):
+        raise ValueError(f"sampling needs a finite temperature > 0 and 0 < top_p <= 1 (got temperature {temperature}, top_p {top_p})")
+    top_k = int(generation_config_value(checkpoint_path, "top_k", HF_DEFAULT_TOP_K))
+    if top_k < 0:
+        raise ValueError(f"generation_config.json sets top_k = {top_k}")
+    return float(temperature), top_k, float(top_p)
+
+
 def _generation_config_penalty(checkpoint_path: str) -> float:
     """repetition_penalty of the generation_config.json stored beside the checkpoint (what `from_pretrained` would attach to
     `model.generation_config` in the reference, qwen2vl_model.py:116-130); 1.0 when there is none."""
@@ -376,18 +405,24 @@ class Qwen2VLModel(VQAScoreModel):
 
     @torch.no_grad()
     def generate(self, images: List[str], texts: List[str], fps=None, max_new_tokens: int = 2048, temperature: float = 0.0,
-                 do_sample: Optional[bool] = None, top_p: float = 0.9, eos_token_ids: Optional[List[int]] = None) -> List[str]:
-        """Greedy text generation, the reference's Qwen2VLModel.generate (qwen2vl_model.py:495-563) with its default temperature 0: per
-        sample, the chat prompt of the raw text and the image, generate(do_sample=False) under the checkpoint's repetition penalty, the
-        prompt cut off, decoded with skip_special_tokens and stripped. Here the whole batch is one prefill and one decode loop on the
-        device (a call with a video: as few as fit VIDEO_WORKSPACE_BUDGET); identical paths are encoded once. `fps` samples the frames
-        of a video file and does not change the output for a .npy frame stack (see HF_FRAME_LIST_FPS). Sampling (temperature > 0 or
-        do_sample=True, top-p) is not implemented."""
+                 do_sample: Optional[bool] = None, top_p: float = 0.9, eos_token_ids: Optional[List[int]] = None,
+                 generator: Optional[torch.Generator] = None) -> List[str]:
+        """Text generation, the reference's Qwen2VLModel.generate (qwen2vl_model.py:495-563): per sample, the chat prompt of the raw
+        text and the image, generate() under the checkpoint's repetition penalty, the prompt cut off, decoded with skip_special_tokens and
+        stripped. With the default temperature 0 it is greedy (do_sample=False). With do_sample (None: temperature > 0) and temperature > 0
+        it samples as generate(do_sample=True, temperature, top_p) does, with generation_config.json's top_k (default 50): see
+        sampling_params. Each prompt's draws come from a 63-bit seed taken from `generator` (None: torch's default generator, so
+        torch.manual_seed(s) before the call reproduces it). Here the whole batch is one prefill and one decode loop on the device (a call
+        with a video: as few as fit VIDEO_WORKSPACE_BUDGET); identical paths are encoded once. `fps` samples the frames of a video file and
+        does not change the output for a .npy frame stack (see HF_FRAME_LIST_FPS)."""
         assert len(images) == len(texts), "Number of images/videos and texts must match"
-        if do_sample is None:
-            do_sample = temperature > 0
+        sampling = None
         if do_sample or temperature > 0:
-            raise NotImplementedError("only greedy decoding is supported (temperature=0.0, do_sample=False); top-p sampling is not implemented")
+            # the engine's capability is looked up on its class, so nothing of the instance is touched before the refusal
+            if not callable(getattr(type(getattr(self, "engine", None)), "sample_prompts", None)):
+                raise NotImplementedError("this engine has only greedy decoding (temperature=0.0, do_sample=False): it has no "
+                                          "sample_prompts for top-k / top-p sampling")
+            sampling = sampling_params(self._checkpoint or QWEN2_VL_MODELS[self.model_name]["model"]["path"], do_sample, temperature, top_p)
         index, patches, grids, tokens, spg = self._vision(images, fps)
         unit = self.cfg.spatial_merge_size ** 2
         cache = self._memo()
@@ -397,12 +432,19 @@ class Qwen2VLModel(VQAScoreModel):
             prompts.append(build_prompt_ids(self.tokenizer, text, t * gh * gw // unit, tokens[img], cache))
         eos = self._eos_ids() if eos_token_ids is None else [int(e) for e in eos_token_ids]
         ws = lambda b, s, p: self.engine.generate_workspace_bytes(b, s, p, max_new_tokens)
+        if sampling is not None:
+            seeds = torch.randint(0, 2 ** 63 - 1, (len(prompts),), dtype=torch.int64, generator=generator).tolist()
         ids = []
         for sel in self._prefill_chunks(prompts, grids, spg, ws):
             pix, items, local = _subset(patches, grids, index, sel)
             video = {} if spg is None else dict(second_per_grid_ts=[spg[g] for g in items])
-            ids += self.engine.generate_prompts(pix, [grids[g] for g in items], [prompts[i] for i in sel], max_new_tokens, eos,
-                                                image_of_sample=local, repetition_penalty=self.repetition_penalty, **video)
+            args = (pix, [grids[g] for g in items], [prompts[i] for i in sel], max_new_tokens, eos)
+            if sampling is None:
+                ids += self.engine.generate_prompts(*args, image_of_sample=local, repetition_penalty=self.repetition_penalty, **video)
+            else:
+                t, k, p = sampling
+                ids += self.engine.sample_prompts(*args, [seeds[i] for i in sel], t, k, p, image_of_sample=local,
+                                                  repetition_penalty=self.repetition_penalty, **video)
         return [self.tokenizer.decode(x, skip_special_tokens=True, clean_up_tokenization_spaces=False).strip() for x in ids]
 
     def _prefill_chunks(self, prompts, grids, spg, workspace_bytes) -> List[List[int]]:
