@@ -317,6 +317,29 @@ int vqa_qwen25vl_generate_prefill_sampled(vqa_handle* h, const vqa_qwen25vl_prom
 int vqa_qwen25vl_generate_step_sampled(vqa_handle* h, const vqa_qwen25vl_generation* gen, const vqa_qwen25vl_sampling* sampling, int32_t batch,
                                        int32_t seq_len, int32_t n_patches, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- CLIP-FlanT5 sampled generation (HF T5ForConditionalGeneration.generate(inputs_embeds=<spliced prompt>, do_sample=True,
+ * temperature=T, top_k=k, top_p=p)) ----
+ * The greedy generation's prefill and steps (vqa_clipt5_generate_*) with the selection replaced by the draw the Qwen2.5-VL sampled
+ * generation makes: vqa_qwen25vl_sampling is shared by both models, with the same warpers (no repetition penalty here: FlanT5's generation
+ * config has none), the same tie rules, saturation and Philox4x32-10 uniforms. Sequence b's draws depend on (seeds[b], step, id) only:
+ * not on its slot, on the other sequences, or on whether the step is replayed from a CUDA graph.
+ * Encoder sharing: the prefill encodes n_prompts <= batch prompts (input_ids [n_prompts, text_len], text_lens / image_index [n_prompts])
+ * into sequence slots 0 .. n_prompts - 1, then copies prompt prompt_index[b] into every slot b >= n_prompts (the encoder output, its
+ * transposed copy and the prompt length; one launch, none when n_prompts == batch), so n draws of one (image, prompt) pair run the
+ * vision tower and the encoder once. prompt_index: DEVICE [batch], entries b < n_prompts unused, entries b >= n_prompts in
+ * [0, n_prompts) (others are clamped into that range); NULL when n_prompts == batch. The steps do not depend on n_prompts.
+ * Same workspace (vqa_clipt5_generate_workspace_bytes(batch, ...)) and the same rules for it. Refused with VQA_ERR_INVALID_ARG before any
+ * launch: a NULL seeds pointer, a temperature that is not positive and finite, top_k < 0, top_p outside (0, 1], n_prompts outside
+ * [1, batch], n_prompts < batch with a NULL prompt_index; cross_attention_mode 1 is refused as the greedy generation refuses it. */
+int vqa_clipt5_generate_prefill_sampled(vqa_handle* h, const void* pixels, int32_t pixel_dtype, int32_t n_images, const int32_t* image_index,
+                                        const int32_t* input_ids, const int32_t* text_lens, int32_t batch, int32_t text_len,
+                                        const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, int32_t* out_tokens,
+                                        int32_t* out_lengths, int32_t* all_done, int32_t n_prompts, const int32_t* prompt_index,
+                                        const vqa_qwen25vl_sampling* sampling, void* workspace, size_t workspace_bytes, void* stream);
+int vqa_clipt5_generate_step_sampled(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, const int32_t* eos_ids, int32_t n_eos,
+                                     int32_t max_new_tokens, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                     const vqa_qwen25vl_sampling* sampling, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Number of kernels, memsets and copies the last forward call on this handle (vqa_clipt5_score, vqa_qwen25vl_score, vqa_qwen25vl_topk,
  * a generate prefill or step) enqueued (for bench.py's gpu_launches). */
 int64_t vqa_last_launch_count(vqa_handle* h);
@@ -506,6 +529,13 @@ int vqa_op_sample_select(const void* logits, int32_t B, int32_t V, uint32_t* pen
                          int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
                          int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, const vqa_qwen25vl_sampling* sampling,
                          uint32_t* kept, void* stream);
+
+/* The encoder sharing of vqa_clipt5_generate_prefill_sampled on caller-owned buffers (tests): slots b >= n_prompts of xn bf16 [batch, S,
+ * d_model], xt bf16 [batch, d_model, Sp] (Sp = S rounded up to 8) and seq_lens int32 [batch] become copies of slot prompt_index[b]
+ * (clamped into [0, n_prompts)). All pointers DEVICE; xn and xt 16-byte aligned; d_model a multiple of 8; prompt_index may be NULL when
+ * n_prompts == batch (nothing is launched). */
+int vqa_op_clipt5_expand_prompts(void* xn, void* xt, int32_t* seq_lens, const int32_t* prompt_index, int32_t n_prompts, int32_t batch,
+                                 int32_t S, int32_t d_model, void* stream);
 
 /* Host-only (no GPU needed): T5's relative-position buckets (T5Attention._relative_position_bucket) of rel = -max_distance .. max_distance,
  * out[rel + max_distance], HOST int32 [2 * max_distance + 1] -- the table vqa_create_clipt5 builds for the encoder (bidirectional = 1) and

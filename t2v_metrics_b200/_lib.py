@@ -92,6 +92,9 @@ PROTOTYPES = {
     "vqa_clipt5_generate_workspace_bytes": (_sz, [_vp, _i32, _i32, _i32, _i32]),
     "vqa_clipt5_generate_prefill": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "vqa_clipt5_generate_step": (_i32, [_vp, _i32, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "vqa_clipt5_generate_prefill_sampled": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _vp,
+                                                   _P(VqaQwen25VLSampling), _vp, _sz, _vp]),
+    "vqa_clipt5_generate_step_sampled": (_i32, [_vp, _i32, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _P(VqaQwen25VLSampling), _vp, _sz, _vp]),
     "vqa_create_qwen25vl": (_i32, [_P(VqaQwen25VLConfig), _i32, _P(_vp)]),
     "vqa_qwen25vl_set_rope": (_i32, [_vp, _P(_f32), _P(_i32), _i32, _P(_f32), _P(_i32), _i32]),
     "vqa_qwen25vl_workspace_bytes": (_sz, [_vp, _i32, _i64, _i32]),
@@ -139,6 +142,7 @@ PROTOTYPES = {
     "vqa_op_greedy_select": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vqa_op_sample_select": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                     _P(VqaQwen25VLSampling), _vp, _vp]),
+    "vqa_op_clipt5_expand_prompts": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "vqa_t5_bucket_lut": (_i32, [_i32, _i32, _i32, _P(_i32)]),
     "vqa_op_t5_decoder_self_attn": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "vqa_op_t5_decode_self_attn": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),

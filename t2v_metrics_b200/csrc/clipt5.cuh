@@ -509,6 +509,43 @@ static ClipT5GenWorkspace clipt5_gen_plan(const vqa_handle* h, int B, int n_imag
     return g;
 }
 
+// Encoder sharing of a sampled prefill: slots [0, n_prompts) of xn [B, S, Dm], xt [B, Dm, Sp] and seq_lens [B] hold the encoded prompts;
+// every slot b >= n_prompts becomes a copy of slot prompt_index[b] (clamped to [0, n_prompts), so no index reaches outside the slots).
+// Reads only slots below n_prompts and writes only slots at or above it, so the copies are independent. blockIdx.y = b - n_prompts;
+// each slot is xn_vecs + xt_vecs 16-byte vectors, the padding columns of xt included.
+__global__ void __launch_bounds__(256) expand_prompts_kernel(const int* __restrict__ prompt_index, int n_prompts, uint4* xn, size_t xn_vecs,
+                                                             uint4* xt, size_t xt_vecs, int* seq_lens) {
+    pdl_launch_dependents();
+    const int b = n_prompts + blockIdx.y;
+    const int src = min(max(prompt_index[b], 0), n_prompts - 1);
+    if (blockIdx.x == 0 && threadIdx.x == 0) seq_lens[b] = seq_lens[src];
+    const size_t n = xn_vecs + xt_vecs, stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        if (i < xn_vecs) {
+            xn[b * xn_vecs + i] = xn[src * xn_vecs + i];
+        } else {
+            const size_t j = i - xn_vecs;
+            xt[b * xt_vecs + j] = xt[src * xt_vecs + j];
+        }
+    }
+}
+
+// Expands the n_prompts encoded prompts of xn / xt / seq_lens to B slots (expand_prompts_kernel); none when n_prompts == B. Profiled as
+// the bytes it moves: each further slot's xn and xt block read once and written once.
+static int clipt5_expand_prompts(Forward& f, const int* prompt_index, int n_prompts, int B, int S, int Dm, bf16* xn, bf16* xt, int* seq_lens) {
+    if (n_prompts >= B) return VQA_OK;
+    const int Sp = (S + 7) / 8 * 8;
+    const size_t xn_vecs = (size_t)S * Dm / 8, xt_vecs = (size_t)Dm * Sp / 8;
+    const int slots = B - n_prompts;
+    const double bytes = 2.0 * slots * (double)(xn_vecs + xt_vecs) * 16 + 8.0 * slots;
+    const unsigned gx = (unsigned)std::min<size_t>((xn_vecs + xt_vecs + 2047) / 2048, 4096);
+    return f.op(CAT_OTHER, 0.0, bytes, 1, "encoder expand", [&] {
+        expand_prompts_kernel<<<dim3(gx, slots), 256, 0, f.st>>>(prompt_index, n_prompts, reinterpret_cast<uint4*>(xn), xn_vecs,
+                                                                  reinterpret_cast<uint4*>(xt), xt_vecs, seq_lens);
+        return cudaGetLastError();
+    });
+}
+
 // Outputs and constants of a generation, the same for the prefill and every step
 struct ClipT5GenArgs {
     const int* eos_ids; int n_eos;
@@ -519,9 +556,10 @@ struct ClipT5GenArgs {
 };
 
 // One decoder position per sequence: the start token (first) or the last selected token (next_ids), through every decoder layer with
-// its self-attention K/V appended to the cache, then the final norm, the lm_head into [B, vocab] bf16 logits, and the greedy token of
-// every unfinished sequence. Finished sequences recompute their frozen last position, which changes nothing they output.
-static int clipt5_decode_step(Forward& f, const ClipT5GenWorkspace& g, int B, int S, const ClipT5GenArgs& a, bool first) {
+// its self-attention K/V appended to the cache, then the final norm, the lm_head into [B, vocab] bf16 logits, and the greedy (smp NULL)
+// or sampled token of every unfinished sequence. Finished sequences recompute their frozen last position, which changes nothing they output.
+static int clipt5_decode_step(Forward& f, const ClipT5GenWorkspace& g, int B, int S, const ClipT5GenArgs& a, const vqa_qwen25vl_sampling* smp,
+                              bool first) {
     vqa_handle* h = f.h;
     const vqa_clipt5_config& c = h->cfg;
     const ClipT5Workspace& w = g.w;
@@ -554,28 +592,34 @@ static int clipt5_decode_step(Forward& f, const ClipT5GenWorkspace& g, int B, in
     // The [B, vocab] bf16 logits are 64 KB per sequence against the 263 MB lm_head weight (xxl) that the GEMM streams either way.
     bf16* logits = f.at(g.logits);
     TRY(f.gemm(Gemm(P_(w.yn), h->lm_head, logits, B, c.vocab, Dm), "lm_head"));
+    if (smp)    // no repetition penalty and no positions: the arguments greedy selection gets
+        return sample_select(f, logits, B, c.vocab, nullptr, 1.0f, *smp, a.eos_ids, a.n_eos, a.max_new, nullptr, a.tokens, a.lengths,
+                             f.at<int>(g.done), f.at<int>(g.n_done), a.all_done, next_ids, nullptr);
     return greedy_select(f, logits, B, c.vocab, nullptr, 1.0f, a.eos_ids, a.n_eos, a.max_new, nullptr, a.tokens, a.lengths, f.at<int>(g.done),
                          f.at<int>(g.n_done), a.all_done, next_ids, nullptr);
 }
 
-// Encoder pass of vqa_clipt5_score, the generation state reset, then the first decoder position (the start token) and the first token.
-static int clipt5_generate_prefill(vqa_handle* h, const ClipT5Prompts& in, const ClipT5GenArgs& a, void* workspace, size_t workspace_bytes,
-                                   cudaStream_t st) {
-    const ClipT5GenWorkspace g = clipt5_gen_plan(h, in.B, in.n_images, in.L, a.max_new);
+// Encoder pass of vqa_clipt5_score over the in.B prompts, copied to the `batch` sequence slots by prompt_index when in.B < batch
+// (clipt5_expand_prompts), the generation state reset, then the first decoder position (the start token) and the first token.
+static int clipt5_generate_prefill(vqa_handle* h, const ClipT5Prompts& in, int batch, const int* prompt_index, const ClipT5GenArgs& a,
+                                   const vqa_qwen25vl_sampling* smp, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    const ClipT5GenWorkspace g = clipt5_gen_plan(h, batch, in.n_images, in.L, a.max_new);
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
-    TRY(clipt5_encode(f, g.w, in));
-    TRY(generate_init(f, in.B, a.max_new, a.tokens, a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
     const int P = (h->cfg.image_size / h->cfg.patch_size) * (h->cfg.image_size / h->cfg.patch_size);
-    return clipt5_decode_step(f, g, in.B, in.L - 1 + P, a, true);
+    const int S = in.L - 1 + P;
+    TRY(clipt5_encode(f, g.w, in));
+    TRY(clipt5_expand_prompts(f, prompt_index, in.B, batch, S, h->cfg.d_model, f.at(g.w.xn), f.at(g.w.xt), f.at<int>(g.w.seq_lens)));
+    TRY(generate_init(f, batch, a.max_new, a.tokens, a.lengths, f.at<int>(g.done), f.at<int>(g.n_done), a.all_done));
+    return clipt5_decode_step(f, g, batch, S, a, smp, true);
 }
 
 // One decode step: every sequence feeds its last selected token.
-static int clipt5_generate_step(vqa_handle* h, int B, int n_images, int L, const ClipT5GenArgs& a, void* workspace, size_t workspace_bytes,
-                                cudaStream_t st) {
+static int clipt5_generate_step(vqa_handle* h, int B, int n_images, int L, const ClipT5GenArgs& a, const vqa_qwen25vl_sampling* smp,
+                                void* workspace, size_t workspace_bytes, cudaStream_t st) {
     const ClipT5GenWorkspace g = clipt5_gen_plan(h, B, n_images, L, a.max_new);
     if (workspace_bytes < g.total) return fail(h, VQA_ERR_WORKSPACE, "workspace too small");
     Forward f(h, workspace, st);
     const int P = (h->cfg.image_size / h->cfg.patch_size) * (h->cfg.image_size / h->cfg.patch_size);
-    return clipt5_decode_step(f, g, B, L - 1 + P, a, false);
+    return clipt5_decode_step(f, g, B, L - 1 + P, a, smp, false);
 }

@@ -150,25 +150,70 @@ extern "C" size_t vqa_clipt5_generate_workspace_bytes(vqa_handle* h, int32_t bat
     return clipt5_gen_plan(h, batch, n_images, text_len, max_new_tokens).total;
 }
 
+// A sampled generation's parameters (both models); the reference's scored forward is always greedy, so no answer score goes with them.
+static int sampling_check(vqa_handle* h, const vqa_qwen25vl_sampling* s, const vqa_qwen25vl_answer_score* score) {
+    if (!s || !s->seeds) return fail(h, VQA_ERR_INVALID_ARG, "sampling: null sampling struct or seeds");
+    if (score) return fail(h, VQA_ERR_INVALID_ARG, "sampling: a scored rollout is greedy (gen->score must be NULL)");
+    if (!(s->temperature > 0.f) || !std::isfinite(s->temperature) || s->top_k < 0 || !(s->top_p > 0.f) || !(s->top_p <= 1.f))
+        return fail(h, VQA_ERR_INVALID_ARG, "sampling: bad parameters (temperature > 0 and finite, top_k >= 0, 0 < top_p <= 1)");
+    return VQA_OK;
+}
+
+// The prefill and step of both CLIP-FlanT5 generations: smp NULL = greedy (n_prompts == batch, no prompt_index), else sampled.
+static int clipt5_gen_prefill_entry(vqa_handle* h, const void* pixels, int32_t pixel_dtype, int32_t n_images, const int32_t* image_index,
+                                    const int32_t* input_ids, const int32_t* text_lens, int32_t batch, int32_t text_len, const ClipT5GenArgs& a,
+                                    int32_t n_prompts, const int32_t* prompt_index, const vqa_qwen25vl_sampling* smp, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+    if (int rc = clipt5_gen_check(h, batch, n_images, text_len, a, workspace)) return rc;
+    if (!pixels || !input_ids || !text_lens) return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
+    if (n_prompts < 1 || n_prompts > batch) return fail(h, VQA_ERR_INVALID_ARG, "1 <= n_prompts <= batch");
+    if (n_prompts < batch && !prompt_index) return fail(h, VQA_ERR_INVALID_ARG, "prompt_index == NULL requires n_prompts == batch");
+    if (!image_index && n_images != n_prompts) return fail(h, VQA_ERR_INVALID_ARG, "image_index == NULL requires n_images == n_prompts");
+    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
+    const ClipT5Prompts in{pixels, pixel_dtype, n_images, image_index, input_ids, text_lens, n_prompts, text_len};
+    return clipt5_generate_prefill(h, in, batch, prompt_index, a, smp, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
+static int clipt5_gen_step_entry(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, const ClipT5GenArgs& a,
+                                 const vqa_qwen25vl_sampling* smp, void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = clipt5_gen_check(h, batch, n_images, text_len, a, workspace)) return rc;
+    return clipt5_generate_step(h, batch, n_images, text_len, a, smp, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+
 extern "C" int vqa_clipt5_generate_prefill(vqa_handle* h, const void* pixels, int32_t pixel_dtype, int32_t n_images, const int32_t* image_index,
                                            const int32_t* input_ids, const int32_t* text_lens, int32_t batch, int32_t text_len,
                                            const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens, int32_t* out_tokens,
                                            int32_t* out_lengths, int32_t* all_done, void* workspace, size_t workspace_bytes, void* stream) {
     const ClipT5GenArgs a{eos_ids, n_eos, max_new_tokens, out_tokens, out_lengths, all_done};
-    if (int rc = clipt5_gen_check(h, batch, n_images, text_len, a, workspace)) return rc;
-    if (!pixels || !input_ids || !text_lens) return fail(h, VQA_ERR_INVALID_ARG, "null device pointer");
-    if (!image_index && n_images != batch) return fail(h, VQA_ERR_INVALID_ARG, "image_index == NULL requires n_images == batch");
-    if (pixel_dtype != VQA_DTYPE_F32 && pixel_dtype != VQA_DTYPE_BF16) return fail(h, VQA_ERR_INVALID_ARG, "pixel_dtype must be F32 or BF16");
-    const ClipT5Prompts in{pixels, pixel_dtype, n_images, image_index, input_ids, text_lens, batch, text_len};
-    return clipt5_generate_prefill(h, in, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+    return clipt5_gen_prefill_entry(h, pixels, pixel_dtype, n_images, image_index, input_ids, text_lens, batch, text_len, a, batch, nullptr,
+                                    nullptr, workspace, workspace_bytes, stream);
 }
 
 extern "C" int vqa_clipt5_generate_step(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, const int32_t* eos_ids, int32_t n_eos,
                                         int32_t max_new_tokens, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, void* workspace,
                                         size_t workspace_bytes, void* stream) {
     const ClipT5GenArgs a{eos_ids, n_eos, max_new_tokens, out_tokens, out_lengths, all_done};
-    if (int rc = clipt5_gen_check(h, batch, n_images, text_len, a, workspace)) return rc;
-    return clipt5_generate_step(h, batch, n_images, text_len, a, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+    return clipt5_gen_step_entry(h, batch, n_images, text_len, a, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int vqa_clipt5_generate_prefill_sampled(vqa_handle* h, const void* pixels, int32_t pixel_dtype, int32_t n_images,
+                                                   const int32_t* image_index, const int32_t* input_ids, const int32_t* text_lens, int32_t batch,
+                                                   int32_t text_len, const int32_t* eos_ids, int32_t n_eos, int32_t max_new_tokens,
+                                                   int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done, int32_t n_prompts,
+                                                   const int32_t* prompt_index, const vqa_qwen25vl_sampling* sampling, void* workspace,
+                                                   size_t workspace_bytes, void* stream) {
+    if (int rc = sampling_check(h, sampling, nullptr)) return rc;
+    const ClipT5GenArgs a{eos_ids, n_eos, max_new_tokens, out_tokens, out_lengths, all_done};
+    return clipt5_gen_prefill_entry(h, pixels, pixel_dtype, n_images, image_index, input_ids, text_lens, batch, text_len, a, n_prompts,
+                                    prompt_index, sampling, workspace, workspace_bytes, stream);
+}
+
+extern "C" int vqa_clipt5_generate_step_sampled(vqa_handle* h, int32_t batch, int32_t n_images, int32_t text_len, const int32_t* eos_ids,
+                                                int32_t n_eos, int32_t max_new_tokens, int32_t* out_tokens, int32_t* out_lengths, int32_t* all_done,
+                                                const vqa_qwen25vl_sampling* sampling, void* workspace, size_t workspace_bytes, void* stream) {
+    if (int rc = sampling_check(h, sampling, nullptr)) return rc;
+    const ClipT5GenArgs a{eos_ids, n_eos, max_new_tokens, out_tokens, out_lengths, all_done};
+    return clipt5_gen_step_entry(h, batch, n_images, text_len, a, sampling, workspace, workspace_bytes, stream);
 }
 
 // Byte offsets inside the caller's workspace of the tensors a parity investigation wants to look at after a call has completed.
@@ -400,15 +445,6 @@ static int qwen_gen_check(vqa_handle* h, const vqa_qwen25vl_generation* a, int32
     return VQA_OK;
 }
 
-// A sampled generation's parameters; the reference's scored forward is always greedy, so no answer score goes with them.
-static int qwen_sampling_check(vqa_handle* h, const vqa_qwen25vl_sampling* s, const vqa_qwen25vl_answer_score* score) {
-    if (!s || !s->seeds) return fail(h, VQA_ERR_INVALID_ARG, "sampling: null sampling struct or seeds");
-    if (score) return fail(h, VQA_ERR_INVALID_ARG, "sampling: a scored rollout is greedy (gen->score must be NULL)");
-    if (!(s->temperature > 0.f) || !std::isfinite(s->temperature) || s->top_k < 0 || !(s->top_p > 0.f) || !(s->top_p <= 1.f))
-        return fail(h, VQA_ERR_INVALID_ARG, "sampling: bad parameters (temperature > 0 and finite, top_k >= 0, 0 < top_p <= 1)");
-    return VQA_OK;
-}
-
 extern "C" size_t vqa_qwen25vl_generate_workspace_bytes(vqa_handle* h, int32_t batch, int32_t seq_len, int32_t n_patches, int32_t max_new_tokens) {
     if (!h || h->kind != 1 || batch <= 0 || seq_len <= 0 || n_patches <= 0 || max_new_tokens <= 0) return 0;
     return qwen_gen_plan(h->qwen->cfg, batch, seq_len, n_patches, max_new_tokens, h->num_sms).total;
@@ -445,14 +481,14 @@ extern "C" int vqa_qwen25vl_generate_step(vqa_handle* h, const vqa_qwen25vl_gene
 extern "C" int vqa_qwen25vl_generate_prefill_sampled(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
                                                      const vqa_qwen25vl_sampling* sampling, void* workspace, size_t workspace_bytes,
                                                      void* stream) {
-    if (int rc = qwen_sampling_check(h, sampling, gen ? gen->score : nullptr)) return rc;
+    if (int rc = sampling_check(h, sampling, gen ? gen->score : nullptr)) return rc;
     return qwen_gen_prefill_entry(h, prompts, gen, sampling, workspace, workspace_bytes, stream);
 }
 
 extern "C" int vqa_qwen25vl_generate_step_sampled(vqa_handle* h, const vqa_qwen25vl_generation* gen, const vqa_qwen25vl_sampling* sampling,
                                                   int32_t batch, int32_t seq_len, int32_t n_patches, void* workspace, size_t workspace_bytes,
                                                   void* stream) {
-    if (int rc = qwen_sampling_check(h, sampling, gen ? gen->score : nullptr)) return rc;
+    if (int rc = sampling_check(h, sampling, gen ? gen->score : nullptr)) return rc;
     return qwen_gen_step_entry(h, gen, sampling, batch, seq_len, n_patches, workspace, workspace_bytes, stream);
 }
 
@@ -655,10 +691,21 @@ extern "C" int vqa_op_sample_select(const void* logits, int32_t B, int32_t V, ui
         return fail(nullptr, VQA_ERR_INVALID_ARG, "sample select: null pointer (first_pos and pos3 are given together or not at all)");
     if (B <= 0 || V <= 0 || max_new <= 0 || n_eos < 0 || !(repetition_penalty > 0.f))
         return fail(nullptr, VQA_ERR_INVALID_ARG, "sample select: bad size / repetition penalty");
-    if (int rc = qwen_sampling_check(nullptr, sampling, nullptr)) return rc;
+    if (int rc = sampling_check(nullptr, sampling, nullptr)) return rc;
     return glue_launch(stream, [&](Forward& f) {
         return sample_select(f, (const bf16*)logits, B, V, pen_bitmap, repetition_penalty, *sampling, eos_ids, n_eos, max_new, first_pos, tokens,
                              lengths, done, n_done, all_done, next_ids, pos3, kept);
+    });
+}
+
+extern "C" int vqa_op_clipt5_expand_prompts(void* xn, void* xt, int32_t* seq_lens, const int32_t* prompt_index, int32_t n_prompts, int32_t batch,
+                                            int32_t S, int32_t d_model, void* stream) {
+    if (!xn || !xt || !seq_lens || (n_prompts < batch && !prompt_index)) return fail(nullptr, VQA_ERR_INVALID_ARG, "expand prompts: null pointer");
+    if (n_prompts < 1 || n_prompts > batch || S <= 0 || d_model <= 0 || d_model % 8)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "expand prompts: bad size (1 <= n_prompts <= batch, d_model a multiple of 8)");
+    if (!aligned(xn, 16) || !aligned(xt, 16)) return fail(nullptr, VQA_ERR_INVALID_ARG, "expand prompts: xn and xt must be 16-byte aligned");
+    return glue_launch(stream, [&](Forward& f) {
+        return clipt5_expand_prompts(f, prompt_index, n_prompts, batch, S, d_model, (bf16*)xn, (bf16*)xt, seq_lens);
     });
 }
 

@@ -386,42 +386,76 @@ class ClipT5Engine(_Engine):
 
     # ------------------------------------------------------------------------------------------ greedy generation
     def generate_begin(self, pixel_values: torch.Tensor, input_ids: torch.Tensor, text_lens: torch.Tensor, max_new_tokens: int,
-                       eos_ids: Sequence[int], image_index: Optional[torch.Tensor] = None) -> dict:
+                       eos_ids: Sequence[int], image_index: Optional[torch.Tensor] = None, sample: Optional[dict] = None,
+                       prompt_index: Optional[torch.Tensor] = None) -> dict:
         """The prefill of a greedy generation (vqa_clipt5_generate_prefill): the encoder pass of score_tensors over the same inputs (no
         labels), then the decoder start token and the first token. Returns the generation state that generate_step() advances: device
         tensors `tokens` [B, max_new_tokens] (-1 after a prompt's last token), `lengths` [B] and `all_done` [1], all owned by the state of
-        this call shape. The generation workspace is separate from the scoring one, so scoring graphs are never invalidated by it."""
+        this call shape. The generation workspace is separate from the scoring one, so scoring graphs are never invalidated by it.
+        sample = dict(seeds=[one int per sequence], temperature=T, top_k=k, top_p=p) makes it a sampled generation
+        (vqa_clipt5_generate_*_sampled) of B = len(seeds) sequences over the input_ids.shape[0] prompts: with fewer prompts than
+        sequences, prompt_index (int32 [B] on the device) names each slot's prompt, and slot b < input_ids.shape[0] must be prompt b. The
+        seeds go to a device buffer of the state before each prefill, so one captured step graph serves every seed."""
         dev = self.device
         self._check_inputs(pixel_values, image_index, input_ids, text_lens)
-        B, L = input_ids.shape
+        n_prompts, L = input_ids.shape
+        B = n_prompts
         NI = pixel_values.shape[0]
         max_new = int(max_new_tokens)
         eos = [int(e) for e in eos_ids]
+        key = (B, NI, L, max_new, len(eos))
+        if sample is not None:
+            seeds = [int(x) for x in sample["seeds"]]
+            B = len(seeds)
+            if not all(0 <= x < 1 << 64 for x in seeds):
+                raise ValueError("sampling needs one seed in [0, 2^64) per sequence")
+            if B < n_prompts or (B > n_prompts and prompt_index is None):
+                raise ValueError(f"{B} sequences over {n_prompts} prompts: need at least one sequence per prompt and, with more, prompt_index")
+            if prompt_index is not None:
+                assert prompt_index.is_cuda and prompt_index.dtype == torch.int32 and prompt_index.shape == (B,)
+            smp_t, smp_k, smp_p = float(sample["temperature"]), int(sample["top_k"]), float(sample["top_p"])
+            key = (B, NI, L, max_new, len(eos), "sample", smp_t, smp_k, smp_p)
         need = int(self.lib.vqa_clipt5_generate_workspace_bytes(self._h, B, NI, L, max_new))
         if need == 0:
             raise ValueError(f"bad generation size: batch {B}, images {NI}, prompt length {L}, max_new_tokens {max_new}")
         i32 = lambda *shape: torch.empty(*shape, dtype=torch.int32, device=dev)
-        st = self._gen_state((B, NI, L, max_new, len(eos)), need, lambda: dict(
-            B=B, NI=NI, L=L, max_new=max_new, n_eos=len(eos), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new), lengths=i32(B),
-            all_done=i32(1), graph=None))
+
+        def make() -> dict:
+            st = dict(B=B, NI=NI, L=L, max_new=max_new, n_eos=len(eos), eos=i32(max(len(eos), 1)), tokens=i32(B, max_new), lengths=i32(B),
+                      all_done=i32(1), graph=None, sample=None)
+            if sample is not None:
+                sm = st["sample"] = dict(seeds=torch.empty(B, dtype=torch.int64, device=dev))
+                sm["struct"] = _lib.VqaQwen25VLSampling(seeds=_ptr(sm["seeds"]), temperature=smp_t, top_k=smp_k, top_p=smp_p)
+            return st
+        st = self._gen_state(key, need, make)
         if eos:
             st["eos"].copy_(torch.as_tensor(eos, dtype=torch.int32), non_blocking=True)
+        if st["sample"] is not None:
+            # uint64 seeds in an int64 buffer: the same 8 bytes
+            st["sample"]["seeds"].copy_(torch.tensor([x - (1 << 64) if x >= 1 << 63 else x for x in seeds], dtype=torch.int64), non_blocking=True)
         pdt = _dtype_code(pixel_values.dtype)
 
         def prefill():
             ws = self._gen_workspace
-            self._run("vqa_clipt5_generate_prefill", _ptr(pixel_values), pdt, NI, _ptr(image_index), _ptr(input_ids), _ptr(text_lens), B, L,
-                      _ptr(st["eos"]), len(eos), max_new, _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(ws),
-                      ws.numel(), _stream_ptr(dev))
+            head = (_ptr(pixel_values), pdt, NI, _ptr(image_index), _ptr(input_ids), _ptr(text_lens), B, L, _ptr(st["eos"]), len(eos), max_new,
+                    _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]))
+            if st["sample"] is None:
+                self._run("vqa_clipt5_generate_prefill", *head, _ptr(ws), ws.numel(), _stream_ptr(dev))
+            else:
+                self._run("vqa_clipt5_generate_prefill_sampled", *head, n_prompts, _ptr(prompt_index), C.byref(st["sample"]["struct"]), _ptr(ws),
+                          ws.numel(), _stream_ptr(dev))
         st["prefill"] = prefill          # relaunches this prefill on the same device inputs (no host work)
         prefill()
         return st
 
     def generate_step(self, st: dict):
-        """One decode step of the generation `st` (vqa_clipt5_generate_step), launched directly."""
+        """One decode step of the generation `st` (vqa_clipt5_generate_step, or _step_sampled), launched directly."""
         ws = self._gen_workspace
-        self._run("vqa_clipt5_generate_step", st["B"], st["NI"], st["L"], _ptr(st["eos"]), st["n_eos"], st["max_new"], _ptr(st["tokens"]),
-                  _ptr(st["lengths"]), _ptr(st["all_done"]), _ptr(ws), ws.numel(), _stream_ptr(self.device))
+        head = (st["B"], st["NI"], st["L"], _ptr(st["eos"]), st["n_eos"], st["max_new"], _ptr(st["tokens"]), _ptr(st["lengths"]), _ptr(st["all_done"]))
+        if st["sample"] is None:
+            self._run("vqa_clipt5_generate_step", *head, _ptr(ws), ws.numel(), _stream_ptr(self.device))
+        else:
+            self._run("vqa_clipt5_generate_step_sampled", *head, C.byref(st["sample"]["struct"]), _ptr(ws), ws.numel(), _stream_ptr(self.device))
 
     def generate_tensors(self, pixel_values: torch.Tensor, input_ids: torch.Tensor, text_lens: torch.Tensor, max_new_tokens: int,
                          eos_ids: Sequence[int], image_index: Optional[torch.Tensor] = None, use_graph: bool = True, check_every: int = 16):
@@ -431,6 +465,38 @@ class ClipT5Engine(_Engine):
         never synchronises in between. Returns each prompt's generated ids, the EOS id included when one ended it."""
         st = self.generate_begin(pixel_values, input_ids, text_lens, max_new_tokens, eos_ids, image_index)
         return self._decode_loop(st, use_graph, check_every)[0]
+
+    def sample_tensors(self, pixel_values: torch.Tensor, input_ids: torch.Tensor, text_lens: torch.Tensor, max_new_tokens: int,
+                       eos_ids: Sequence[int], seeds: Sequence[int], temperature: float, top_k: int, top_p: float,
+                       image_index: Optional[torch.Tensor] = None, prompt_of_sample: Optional[Sequence[int]] = None, use_graph: bool = True,
+                       check_every: int = 16):
+        """Sampled generation (HF generate(do_sample=True) with the temperature, top_k and top_p warpers) of len(seeds) samples over the
+        input_ids.shape[0] prompts laid out as for generate_tensors: sample s continues prompt prompt_of_sample[s] (None: sample s is
+        prompt s) under seeds[s] (an integer in [0, 2^64)). Each prompt is encoded once however many samples it has, and sample s's tokens
+        depend on its seed, prompt and the sizes only. Every prompt needs at least one sample. One prefill, then decode steps replayed from
+        a CUDA graph captured once per (call shape, temperature, top_k, top_p). Returns each sample's generated ids in the caller's order,
+        the EOS id included when one ended it."""
+        n_prompts, B = input_ids.shape[0], len(seeds)
+        owner = list(range(B)) if prompt_of_sample is None else [int(p) for p in prompt_of_sample]
+        if len(owner) != B or not all(0 <= p < n_prompts for p in owner):
+            raise ValueError(f"prompt_of_sample needs one prompt in [0, {n_prompts}) per sample ({B} samples)")
+        firsts = {}
+        for s, p in enumerate(owner):
+            firsts.setdefault(p, s)
+        if len(firsts) != n_prompts:
+            raise ValueError(f"prompts {sorted(set(range(n_prompts)) - set(firsts))} have no sample")
+        # slot p < n_prompts is prompt p's first sample (the encoded prompt itself); the other samples follow in the caller's order
+        order = [firsts[p] for p in range(n_prompts)] + [s for s in range(B) if firsts[owner[s]] != s]
+        prompt_index = None
+        if B > n_prompts:
+            prompt_index = torch.tensor([owner[s] for s in order], dtype=torch.int32).to(self.device)
+        st = self.generate_begin(pixel_values, input_ids, text_lens, max_new_tokens, eos_ids, image_index, prompt_index=prompt_index,
+                                 sample=dict(seeds=[int(seeds[s]) for s in order], temperature=temperature, top_k=top_k, top_p=top_p))
+        ids = self._decode_loop(st, use_graph, check_every)[0]
+        out: list = [None] * B
+        for slot, s in enumerate(order):
+            out[s] = ids[slot]
+        return out
 
 
 # ------------------------------------------------------------------------------------------------ single-kernel ops
@@ -571,6 +637,15 @@ class ops:
         _call("vqa_op_sample_select", _ptr(logits), B, V, _ptr(pen_bitmap), float(repetition_penalty), _ptr(eos_ids), n_eos, tokens.shape[1],
               _ptr(first_pos), _ptr(tokens), _ptr(lengths), _ptr(done), _ptr(n_done), _ptr(all_done), _ptr(next_ids), _ptr(pos3), C.byref(smp),
               _ptr(kept), _stream_ptr(logits.device))
+
+    @staticmethod
+    def clipt5_expand_prompts(xn: torch.Tensor, xt: torch.Tensor, seq_lens: torch.Tensor, n_prompts: int, prompt_index=None):
+        """The encoder sharing of the sampled CLIP-FlanT5 prefill (vqa_op_clipt5_expand_prompts), in place: slots b >= n_prompts of xn
+        bf16 [B, S, d_model], xt bf16 [B, d_model, Sp] and seq_lens int32 [B] become copies of slot prompt_index[b] (int32 [B])."""
+        B, S, D = xn.shape
+        assert xt.shape == (B, D, (S + 7) // 8 * 8) and seq_lens.shape == (B,)
+        _call("vqa_op_clipt5_expand_prompts", _ptr(xn), _ptr(xt), _ptr(seq_lens), _ptr(prompt_index), int(n_prompts), B, S, D,
+              _stream_ptr(xn.device))
 
     @staticmethod
     def t5_bucket_lut(bidirectional: bool, num_buckets: int, max_distance: int) -> torch.Tensor:

@@ -14,6 +14,7 @@ import torch
 from ...config import CLIPT5_MODELS as _MODEL_TABLE, ClipT5Config
 from ...constants import HF_CACHE_DIR, CONTEXT_LEN, SYSTEM_MSG, IGNORE_INDEX, DEFAULT_IMAGE_TOKEN, IMAGE_TOKEN_INDEX
 from .mm_utils import t5_tokenizer_image_token, clip_preprocess, video_canvas
+from .sampling import sampling_params
 from .vqa_model import VQAScoreModel
 
 default_question_template = 'Does this figure show "{}"? Please answer yes or no.'  # V_3.0_README.md:211-215
@@ -167,45 +168,103 @@ class CLIPT5Model(VQAScoreModel):
 
     @torch.no_grad()
     def generate(self, images: List[str], texts: List[str], max_new_tokens: int = 256, temperature: float = 0.0,
-                 do_sample: Optional[bool] = None, eos_token_ids: Optional[List[int]] = None) -> List[str]:
-        """Greedy text generation with CLIP-FlanT5 (V_3.0_README.md:316-325: `model.generate(images=..., texts=...) -> List[str]`).
+                 do_sample: Optional[bool] = None, top_p: float = 0.9, eos_token_ids: Optional[List[int]] = None,
+                 generator: Optional[torch.Generator] = None) -> List[str]:
+        """Text generation with CLIP-FlanT5 (V_3.0_README.md:316-325: `model.generate(images=..., texts=...) -> List[str]`).
 
         Per sample the prompt is format_question(text) -- the raw text, no question template -- through t5_tokenizer_image_token,
         truncated to context_len, i.e. the scoring path's prompt; identical image paths are encoded once. Decoding is HF
-        T5ForConditionalGeneration.generate(inputs_embeds=<spliced prompt>, attention_mask=<its mask>, do_sample=False, num_beams=1): the
-        decoder starts from decoder_start_id, each token is the arg-max of the fp32-cast bf16 logits over the whole vocabulary (ties to
-        the lowest id) with no logits processors (FlanT5's generation config has no repetition penalty), and a sample stops on an EOS id
-        (kept, then dropped by the decode) or after max_new_tokens tokens. EOS ids come from generation_config.json beside the checkpoint,
-        else the tokenizer; `eos_token_ids=` overrides both. Output: tokenizer.decode(ids, skip_special_tokens=True).strip().
+        T5ForConditionalGeneration.generate(inputs_embeds=<spliced prompt>, attention_mask=<its mask>, num_beams=1) from decoder_start_id;
+        a sample stops on an EOS id (kept, then dropped by the decode) or after max_new_tokens tokens. EOS ids come from
+        generation_config.json beside the checkpoint, else the tokenizer; `eos_token_ids=` overrides both. Output:
+        tokenizer.decode(ids, skip_special_tokens=True).strip().
 
-        The v3.0 wrapper's default length is not recoverable from the reference; 256 is this implementation's choice and sizes the K/V
-        cache (393 KB per sample per token at xxl width). The batch runs as one encoder pass and one decode loop on the device, in calls of
-        at most GENERATE_MAX_PAIRS pairs. Sampling (temperature > 0 or do_sample=True) is not implemented."""
+        With the default temperature 0 decoding is greedy (do_sample=False): each token is the arg-max of the fp32-cast bf16 logits over
+        the whole vocabulary (ties to the lowest id), with no logits processors (FlanT5's generation config has no repetition penalty).
+        With do_sample (None: temperature > 0) and temperature > 0 it samples as generate(do_sample=True, temperature, top_p) does, with
+        generation_config.json's top_k (default 50): see sampling_params; a generation_config.json with a repetition penalty is refused,
+        since the sampled T5 step applies none. Each pair's draws come from a 63-bit seed taken, in the caller's order, from `generator`
+        (None: torch's default generator, so torch.manual_seed(s) before the call reproduces it). Identical (image, text) pairs of a sampled
+        call run the vision tower and the encoder once and draw their samples from that one encoding.
+
+        The v3.0 wrapper's own generate signature is not recoverable from the reference (SURVEY App. A): the sampling keywords and their
+        defaults (top_p=0.9) are those of the reference's Qwen2VLModel.generate. Its default length is not recoverable either; 256 is this
+        implementation's choice and sizes the K/V cache (393 KB per sample per token at xxl width). The batch runs as one encoder pass and
+        one decode loop on the device, in calls of at most GENERATE_MAX_PAIRS pairs."""
         assert len(images) == len(texts), "Number of images and texts must match"
         if any(p[-4:].lower() in VIDEO_EXTENSIONS for p in images):
             raise NotImplementedError("generate takes image files; video files are scored by forward only")
-        if do_sample is None:
-            do_sample = temperature > 0
+        sampling = None
         if do_sample or temperature > 0:
-            raise NotImplementedError("only greedy decoding is supported (temperature=0.0, do_sample=False)")
+            # the engine's capability is looked up on its class, so nothing of the instance is touched before the refusal
+            if not callable(getattr(type(getattr(self, "engine", None)), "sample_tensors", None)):
+                raise NotImplementedError("this engine has only greedy decoding (temperature=0.0, do_sample=False): it has no "
+                                          "sample_tensors for top-k / top-p sampling")
+            from ...checkpoint import generation_config_value
+            ckpt = self._checkpoint or CLIP_T5_MODELS[self.model_name]["model"]["path"]
+            sampling = sampling_params(ckpt, do_sample, temperature, top_p)
+            penalty = generation_config_value(ckpt, "repetition_penalty", 1.0)
+            if sampling is not None and penalty != 1.0:
+                raise NotImplementedError(f"generation_config.json sets repetition_penalty = {penalty!r}: the sampled CLIP-FlanT5 step applies "
+                                          "no repetition penalty")
         prompts = self._prompt_ids([format_question(t, self.conversational_style) for t in texts])
         eos = self._eos_ids() if eos_token_ids is None else [int(e) for e in eos_token_ids]
+        if sampling is not None:
+            seeds = torch.randint(0, 2 ** 63 - 1, (len(prompts),), dtype=torch.int64, generator=generator).tolist()
+            return self._sample(images, texts, prompts, seeds, sampling, max_new_tokens, eos)
         out: List[str] = []
         for lo in range(0, len(images), self.GENERATE_MAX_PAIRS):
             chunk_images, chunk_prompts = images[lo:lo + self.GENERATE_MAX_PAIRS], prompts[lo:lo + self.GENERATE_MAX_PAIRS]
-            uniq: Dict[str, int] = {}
-            index = [uniq.setdefault(p, len(uniq)) for p in chunk_images]
-            pixels = self.load_images(list(uniq.keys()))
-            dev = self.engine.device
-            L = max(map(len, chunk_prompts))
-            pad = getattr(self.tokenizer, "pad_token_id", 0) or 0
-            input_ids = torch.full((len(chunk_prompts), L), pad, dtype=torch.int32)
-            for i, row in enumerate(chunk_prompts):
-                input_ids[i, :len(row)] = torch.tensor(row, dtype=torch.int32)
-            lens = torch.tensor([len(r) for r in chunk_prompts], dtype=torch.int32)
-            image_index = torch.tensor(index, dtype=torch.int32).to(dev) if len(uniq) != len(chunk_images) else None
-            ids = self.engine.generate_tensors(pixels, input_ids.to(dev), lens.to(dev), max_new_tokens, eos, image_index=image_index)
+            pixels, input_ids, lens, image_index = self._generate_inputs(chunk_images, chunk_prompts)
+            ids = self.engine.generate_tensors(pixels, input_ids, lens, max_new_tokens, eos, image_index=image_index)
             out.extend(self.tokenizer.decode(x, skip_special_tokens=True).strip() for x in ids)
+        return out
+
+    def _generate_inputs(self, images: List[str], prompts: List[List[int]]):
+        """Device inputs of one engine generation call: pixels of the distinct image paths, padded input_ids, text_lens and image_index
+        (None when every path differs)."""
+        uniq: Dict[str, int] = {}
+        index = [uniq.setdefault(p, len(uniq)) for p in images]
+        pixels = self.load_images(list(uniq.keys()))
+        dev = self.engine.device
+        L = max(map(len, prompts))
+        pad = getattr(self.tokenizer, "pad_token_id", 0) or 0
+        input_ids = torch.full((len(prompts), L), pad, dtype=torch.int32)
+        for i, row in enumerate(prompts):
+            input_ids[i, :len(row)] = torch.tensor(row, dtype=torch.int32)
+        lens = torch.tensor([len(r) for r in prompts], dtype=torch.int32)
+        image_index = torch.tensor(index, dtype=torch.int32).to(dev) if len(uniq) != len(images) else None
+        return pixels, input_ids.to(dev), lens.to(dev), image_index
+
+    def _sample(self, images, texts, prompts, seeds, sampling, max_new_tokens: int, eos) -> List[str]:
+        """The sampled generate: identical (image, text) pairs form a group whose samples share one encoding; groups are packed into engine
+        calls of at most GENERATE_MAX_PAIRS samples, a group kept whole where it fits; strings come back in the caller's order."""
+        groups: Dict[tuple, List[int]] = {}
+        for i, pair in enumerate(zip(images, texts)):
+            groups.setdefault(pair, []).append(i)
+        cap = self.GENERATE_MAX_PAIRS
+        chunks: List[List[int]] = [[]]
+        for members in groups.values():
+            while members:
+                if len(chunks[-1]) + len(members) > cap and chunks[-1] and len(members) <= cap:
+                    chunks.append([])          # a group that fits in a call of its own is not split
+                room = cap - len(chunks[-1])
+                chunks[-1] += members[:room]
+                members = members[room:]
+                if len(chunks[-1]) == cap:
+                    chunks.append([])
+        out: List[Optional[str]] = [None] * len(images)
+        T, k, p = sampling
+        for chunk in (c for c in chunks if c):
+            firsts: Dict[tuple, int] = {}
+            prompt_of_sample = [firsts.setdefault((images[i], texts[i]), len(firsts)) for i in chunk]
+            distinct = list(firsts)
+            rep = {pair: next(i for i in chunk if (images[i], texts[i]) == pair) for pair in distinct}
+            pixels, input_ids, lens, image_index = self._generate_inputs([pair[0] for pair in distinct], [prompts[rep[pair]] for pair in distinct])
+            ids = self.engine.sample_tensors(pixels, input_ids, lens, max_new_tokens, eos, [seeds[i] for i in chunk], T, k, p,
+                                             image_index=image_index, prompt_of_sample=prompt_of_sample)
+            for i, x in zip(chunk, ids):
+                out[i] = self.tokenizer.decode(x, skip_special_tokens=True).strip()
         return out
 
     # ---- scoring -------------------------------------------------------------------------------------------------
