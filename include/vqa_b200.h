@@ -387,6 +387,17 @@ int vqa_debug_preprocess_geometry(int32_t layout, const int32_t* n_frames, const
                                   const int32_t* is_video, int32_t n_items, int32_t out_size, int32_t pad_to_square, int32_t patch,
                                   int32_t temporal_patch, int32_t merge, int64_t min_pixels, int64_t max_pixels, int32_t* geometry);
 
+/* Process-wide override of the output rows per CTA of the antialiased video-file resize (vqa_qwen_preprocess_video_aa; tests): any
+ * tile_rows in 1..32. A plan call whose forced band of input rows does not fit the kernel's shared memory fails with an error naming
+ * this override. 0 = the automatic plan (the default). */
+int vqa_debug_set_preprocess_aa_rows(int32_t tile_rows);
+
+/* Host-only: the launch geometry of vqa_qwen_preprocess_video_aa for these windows (arguments as vqa_qwen_preprocess_video_aa_plan),
+ * with any override above. geometry HOST [3] = (tile_rows, band_rows, tiles_x): output rows per CTA, input rows of the tallest band,
+ * 64-column tiles per row tile. */
+int vqa_debug_preprocess_aa_geometry(int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w, const int32_t* first_h, int32_t htaps,
+                                     const int32_t* first_v, int32_t vtaps, int32_t patch, int32_t merge, int32_t* geometry);
+
 const char* vqa_last_error(vqa_handle* h);
 void vqa_destroy(vqa_handle* h);
 

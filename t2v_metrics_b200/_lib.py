@@ -117,6 +117,8 @@ PROTOTYPES = {
     "vqa_debug_set_preprocess_tiles": (_i32, [_i32, _i32, _i32]),
     "vqa_debug_preprocess_geometry": (_i32, [_i32, _P(_i32), _P(_i32), _P(_i32), _P(_i32), _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64,
                                              _P(_i32)]),
+    "vqa_debug_set_preprocess_aa_rows": (_i32, [_i32]),
+    "vqa_debug_preprocess_aa_geometry": (_i32, [_i32, _i32, _i32, _i32, _P(_i32), _i32, _P(_i32), _i32, _i32, _i32, _P(_i32)]),
     "vqa_last_error": (C.c_char_p, [_vp]),
     "vqa_destroy": (None, [_vp]),
     "vqa_clip_preprocess_workspace_bytes": (_sz, [_P(_i32), _P(_i32), _i32, _i32, _i32]),

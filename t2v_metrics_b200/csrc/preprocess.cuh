@@ -638,8 +638,12 @@ video_resize_aa_kernel(const uint8_t* __restrict__ src, const int* __restrict__ 
     }
 }
 
+// Process-wide forced output rows per CTA of video_resize_aa_kernel (vqa_debug_set_preprocess_aa_rows; tests): 1 ... 32, 0 = the
+// planner's choice.
+inline int g_pre_aa_rows_override = 0;
+
 // Host checks and launch geometry of video_resize_aa_kernel: every window inside its axis and the vertical windows monotonic; the
-// output rows per CTA (<= 32, a power of two) are the most whose band of input rows fits PRE_AA_MAX_SMEM.
+// output rows per CTA (<= 32, a power of two) are the most whose band of input rows fits PRE_AA_MAX_SMEM, or the forced count.
 inline bool pre_plan_aa(int in_h, int in_w, int out_h, int out_w, const int32_t* first_h, int htaps, const int32_t* first_v, int vtaps,
                         int patch, int merge, PreAAGeom& g, std::string& error) {
     if (in_h <= 0 || in_w <= 0 || out_h <= 0 || out_w <= 0 || htaps <= 0 || vtaps <= 0 || htaps > in_w || vtaps > in_h) {
@@ -655,12 +659,26 @@ inline bool pre_plan_aa(int in_h, int in_w, int out_h, int out_w, const int32_t*
             return false;
         }
     g = PreAAGeom{in_h, in_w, out_h, out_w, htaps, vtaps, 0, 0, (out_w + PRE_AA_TX - 1) / PRE_AA_TX, 0, 0};
-    for (int tile = 32; tile >= 1; tile >>= 1) {
+    auto band_of = [&](int tile) {       // input rows of the tallest band of `tile` output rows
         int band = 0;
         for (int y0 = 0; y0 < out_h; y0 += tile) {
             const int y1 = (y0 + tile < out_h ? y0 + tile : out_h) - 1;
             if (first_v[y1] + vtaps - first_v[y0] > band) band = first_v[y1] + vtaps - first_v[y0];
         }
+        return band;
+    };
+    if (const int tile = g_pre_aa_rows_override) {
+        const int band = band_of(tile);
+        if (pre_aa_smem_bytes(band) > (size_t)PRE_AA_MAX_SMEM) {
+            error = "the forced row tile of vqa_debug_set_preprocess_aa_rows needs " + std::to_string(pre_aa_smem_bytes(band)) +
+                    " bytes of shared memory for this resize, over the " + std::to_string(PRE_AA_MAX_SMEM) + "-byte budget";
+            return false;
+        }
+        g.tile_rows = tile; g.band_rows = band;
+        return true;
+    }
+    for (int tile = 32; tile >= 1; tile >>= 1) {
+        const int band = band_of(tile);
         if (pre_aa_smem_bytes(band) <= (size_t)PRE_AA_MAX_SMEM) { g.tile_rows = tile; g.band_rows = band; return true; }
     }
     error = "downscale too steep for the device resize (vertical window exceeds shared memory)";

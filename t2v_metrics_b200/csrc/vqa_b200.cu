@@ -1252,6 +1252,24 @@ extern "C" int vqa_qwen_preprocess_video_aa_plan(int32_t in_h, int32_t in_w, int
     return VQA_OK;
 }
 
+// Process-wide forced output rows per CTA of video_resize_aa_kernel (tests): 1 ... 32, 0 = the planner's choice (pre_plan_aa).
+extern "C" int vqa_debug_set_preprocess_aa_rows(int32_t tile_rows) {
+    if (tile_rows < 0 || tile_rows > 32) return fail(nullptr, VQA_ERR_INVALID_ARG, "preprocess aa rows: tile_rows in [1, 32], or 0");
+    g_pre_aa_rows_override = tile_rows;
+    return VQA_OK;
+}
+
+// Host-only: the launch geometry vqa_qwen_preprocess_video_aa would use for these windows, geometry[3] = (tile_rows, band_rows, tiles_x).
+extern "C" int vqa_debug_preprocess_aa_geometry(int32_t in_h, int32_t in_w, int32_t out_h, int32_t out_w, const int32_t* first_h,
+                                                int32_t htaps, const int32_t* first_v, int32_t vtaps, int32_t patch, int32_t merge,
+                                                int32_t* geometry) {
+    if (!geometry) return fail(nullptr, VQA_ERR_INVALID_ARG, "bad argument");
+    PreAAGeom g;
+    if (int rc = qwen_video_aa_args(in_h, in_w, out_h, out_w, first_h, htaps, first_v, vtaps, patch, 1, merge, 1, g)) return rc;
+    geometry[0] = g.tile_rows; geometry[1] = g.band_rows; geometry[2] = g.tiles_x;
+    return VQA_OK;
+}
+
 extern "C" int vqa_qwen_preprocess_video_aa(const void* src, int32_t n_frames, int32_t frame0, int32_t total_frames, int32_t in_h, int32_t in_w,
                                             int32_t out_h, int32_t out_w, const int32_t* first_h, const float* weights_h, int32_t htaps,
                                             const int32_t* first_v, const float* weights_v, int32_t vtaps, int32_t patch, int32_t temporal_patch,

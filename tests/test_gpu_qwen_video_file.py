@@ -1,6 +1,8 @@
 """Qwen2.5-VL video FILES on a real H100: the device's antialiased bicubic resize against torchvision on the host CPU (equal except at
 rounding ties), its patch rows bit for bit against the restatement built from the device's own uint8 frames, one kernel per slice, and
-the plugin's forward / forward_with_trace / generate / k = 4 rollout on the committed clip against the HF golden."""
+the plugin's forward / forward_with_trace / generate / k = 4 rollout on the committed clip against the HF golden. The bit-exact tests of
+the device resize, against a host restatement of its fp32 arithmetic under every row-tile plan, are in test_gpu_qwen_video_aa_exact.py;
+the torchvision comparison here stays the check against the reference's own implementation."""
 import ctypes as C
 import dataclasses
 import math
