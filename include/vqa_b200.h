@@ -302,14 +302,16 @@ int vqa_qwen25vl_generate_step(vqa_handle* h, const vqa_qwen25vl_generation* gen
  * the softmax of the kept scores: Gumbel-max with the uniforms of Philox4x32-10 keyed by seeds[b] at counter (id / 4, t, 0, 0), lane
  * id % 4, where t is the index of the token. A prompt's tokens depend on its seed, prompt and sizes only, not on its batch position or
  * on whether the step is replayed from a CUDA graph. A score that overflows fp32 (or a NaN logit) saturates to +-FLT_MAX (NaN to
- * -FLT_MAX), where HF's softmax would be NaN; a top_p whose fp32(1 - top_p) rounds to 1 keeps only the most probable id, as HF does. Same workspace (vqa_qwen25vl_generate_workspace_bytes) and the same rules for it;
- * gen->score must be NULL (a scored rollout is greedy). Refused with VQA_ERR_INVALID_ARG: a NULL seeds pointer, a temperature that is
+ * -FLT_MAX), where HF's softmax would be NaN; a top_p whose fp32(1 - top_p) rounds to 1 keeps only the most probable id, as HF does.
+ * 1 - top_p is taken in double and rounded to fp32 once, as HF's TopPLogitsWarper compares its fp32 cumulative probabilities with
+ * 1 - top_p of the caller's Python float (a float top_p, rounded before the subtraction, would move the threshold by up to 10 fp32 ulps).
+ * Same workspace (vqa_qwen25vl_generate_workspace_bytes) and the same rules for it; gen->score must be NULL (a scored rollout is greedy). Refused with VQA_ERR_INVALID_ARG: a NULL seeds pointer, a temperature that is
  * not positive and finite, top_k < 0, top_p outside (0, 1]. */
 typedef struct {
     const uint64_t* seeds;  /* DEVICE [batch]: prompt b's key; its draws depend on (seeds[b], step, id) only */
     float temperature;      /* > 0 and finite; 1.0 = no division */
     int32_t top_k;          /* >= 0; 0 = off */
-    float top_p;            /* (0, 1]; 1.0 = off */
+    double top_p;           /* (0, 1]; 1.0 = off. A double, as the caller's Python float: the threshold is fp32(1 - top_p) of it, as HF's */
 } vqa_qwen25vl_sampling;
 
 int vqa_qwen25vl_generate_prefill_sampled(vqa_handle* h, const vqa_qwen25vl_prompts* prompts, const vqa_qwen25vl_generation* gen,
@@ -540,6 +542,17 @@ int vqa_op_sample_select(const void* logits, int32_t B, int32_t V, uint32_t* pen
                          int32_t n_eos, int32_t max_new, const int32_t* first_pos, int32_t* tokens, int32_t* lengths, int32_t* done,
                          int32_t* n_done, int32_t* all_done, int32_t* next_ids, int32_t* pos3, const vqa_qwen25vl_sampling* sampling,
                          uint32_t* kept, void* stream);
+
+/* The per-id terms vqa_op_sample_select decides on (a test aid), computed by the same device functions as its kernel, for every row b < B
+ * (finished or not) at step t = lengths[b], with the same logits, penalty bitmap, penalty and sampling struct (top_k and top_p unused but
+ * checked). All pointers DEVICE; every output [B, V] except row_max [B]:
+ *   score     fp32 processed score (penalty, / temperature, -0 as +0, saturated)      row_max  the row's maximum score
+ *   expv      fp32 expf(score - row_max)          mass     uint64 its mass in 2^-40 units, as the top-p cut sums it
+ *   bits      uint32 Philox4x32-10 lane id % 4 of key seeds[b], counter (id / 4, t, 0, 0)
+ *   gumbel_e  fp32 -log(u) of those bits          perturbed  fp32 (score - row_max) - log(gumbel_e), the draw's arg-max value */
+int vqa_debug_sample_terms(const void* logits, int32_t B, int32_t V, const uint32_t* pen_bitmap, float repetition_penalty, const int32_t* lengths,
+                           const vqa_qwen25vl_sampling* sampling, float* score, float* row_max, float* expv, uint64_t* mass, uint32_t* bits,
+                           float* gumbel_e, float* perturbed, void* stream);
 
 /* The encoder sharing of vqa_clipt5_generate_prefill_sampled on caller-owned buffers (tests): slots b >= n_prompts of xn bf16 [batch, S,
  * d_model], xt bf16 [batch, d_model, Sp] (Sp = S rounded up to 8) and seq_lens int32 [batch] become copies of slot prompt_index[b]

@@ -72,7 +72,8 @@ class VqaQwen25VLGeneration(C.Structure):
 
 
 class VqaQwen25VLSampling(C.Structure):
-    _fields_ = [("seeds", C.c_void_p), ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float)]
+    # top_p is a double: the kernels compare against fp32(1 - top_p) of the caller's value, as HF does
+    _fields_ = [("seeds", C.c_void_p), ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_double)]
 
 
 class VqaTensor(C.Structure):
@@ -144,6 +145,7 @@ PROTOTYPES = {
     "vqa_op_greedy_select": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vqa_op_sample_select": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                     _P(VqaQwen25VLSampling), _vp, _vp]),
+    "vqa_debug_sample_terms": (_i32, [_vp, _i32, _i32, _vp, _f32, _vp, _P(VqaQwen25VLSampling), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "vqa_op_clipt5_expand_prompts": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "vqa_t5_bucket_lut": (_i32, [_i32, _i32, _i32, _P(_i32)]),
     "vqa_op_t5_decoder_self_attn": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),

@@ -232,12 +232,35 @@ __device__ __forceinline__ uint32_t order_key(float x) {
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
+// The processed score of id n for sampling (see sample_select_kernel): the penalised logit, / temperature (none at 1), -0 as +0,
+// saturated to [-FLT_MAX, FLT_MAX] (fmaxf(NaN, -FLT_MAX) is -FLT_MAX)
+__device__ __forceinline__ float sample_score(const __nv_bfloat16* lr, const uint32_t* pb, float penalty, float temperature, int n) {
+    float x = penalised_logit(lr, pb, penalty, n);
+    if (temperature != 1.0f) x = __fdiv_rn(x, temperature);
+    return x == 0.f ? 0.f : fminf(fmaxf(x, -FLT_MAX), FLT_MAX);
+}
+
 // Mass exp(x - max) of one token as an integer of 2^-40 units: sums of them are exact and independent of the summation order, so the
 // top-p cut is deterministic. A vocabulary of < 2^23 tokens, each <= 2^40, cannot overflow 64 bits; dropping terms below 2^-41 moves a
-// cumulative probability by < V * 2^-41 (7e-8 at V = 152,064).
-__device__ __forceinline__ unsigned long long mass_fx(float x, float mx) {
-    return (unsigned long long)(expf(x - mx) * 1099511627776.0f + 0.5f);
+// cumulative probability by < V * 2^-41 (7e-8 at V = 152,064). mass_of_exp is the quantisation of the fp32 ex = expf(x - max).
+__device__ __forceinline__ unsigned long long mass_of_exp(float ex) {
+    return (unsigned long long)(ex * 1099511627776.0f + 0.5f);
 }
+__device__ __forceinline__ unsigned long long mass_fx(float x, float mx) { return mass_of_exp(expf(x - mx)); }
+
+// The Philox block of ids 4g .. 4g + 3 at step t under seed (lo, hi), and lane l of it (id 4g + l)
+__device__ __forceinline__ uint4 sample_philox(int g, int step, uint32_t seed_lo, uint32_t seed_hi) {
+    return philox4x32_10(make_uint4((uint32_t)g, (uint32_t)step, 0u, 0u), seed_lo, seed_hi);
+}
+__device__ __forceinline__ uint32_t philox_lane(uint4 r, int l) { return l == 0 ? r.x : l == 1 ? r.y : l == 2 ? r.z : r.w; }
+
+// The Gumbel term of one id from its Philox lane bits: e = -log(u), u = (m + 0.5) 2^-24 with m = bits >> 8, taken without rounding u:
+// for m >= 2^23, 1 - u = (2^24 - m - 0.5) 2^-24 is exact instead. The perturbed score is (x - max) - log(e).
+__device__ __forceinline__ float gumbel_e(uint32_t bits) {
+    const uint32_t m = bits >> 8;
+    return m < (1u << 23) ? -logf(((float)m + 0.5f) * 5.9604644775390625e-8f) : -log1pf(-((float)((1u << 24) - m) - 0.5f) * 5.9604644775390625e-8f);
+}
+__device__ __forceinline__ float gumbel_perturbed(float x, float mx, float e) { return (x - mx) - logf(e); }
 
 constexpr int SAMPLE_BINS = 2048;       // 11-bit radix digits: three passes (11, 11, 10 bits) select one 32-bit key
 constexpr int SAMPLE_UNROLL = 8;
@@ -295,7 +318,7 @@ __device__ void radix_find(const unsigned long long* h, int nb, bool from_top, f
 // kept (debugging, NULL = none): the kept set as a bitmap [B, ceil(V / 32)], fully rewritten.
 __global__ void __launch_bounds__(SELECT_THREADS) sample_select_kernel(
         const __nv_bfloat16* __restrict__ logits, int V, uint32_t* __restrict__ pen_bitmap, int pen_words, float penalty,
-        const unsigned long long* __restrict__ seeds, float temperature, int top_k, float top_p, const int* __restrict__ eos_ids, int n_eos,
+        const unsigned long long* __restrict__ seeds, float temperature, int top_k, double top_p, const int* __restrict__ eos_ids, int n_eos,
         int max_new, const int* __restrict__ first_pos, int B, int* __restrict__ tokens, int* __restrict__ lengths, int* __restrict__ done,
         int* __restrict__ n_done, int* __restrict__ all_done, int* __restrict__ next_ids, int* __restrict__ pos3, uint32_t* __restrict__ kept) {
     pdl_launch_dependents();
@@ -310,11 +333,7 @@ __global__ void __launch_bounds__(SELECT_THREADS) sample_select_kernel(
     const __nv_bfloat16* lr = logits + (size_t)b * V;
     const uint32_t* pb = pen_bitmap ? pen_bitmap + (size_t)b * pen_words : nullptr;
     const int step = lengths[b];
-    auto score = [&](int n) {
-        float x = penalised_logit(lr, pb, penalty, n);
-        if (temperature != 1.0f) x = __fdiv_rn(x, temperature);
-        return x == 0.f ? 0.f : fminf(fmaxf(x, -FLT_MAX), FLT_MAX);      // fmaxf(NaN, -FLT_MAX) is -FLT_MAX
-    };
+    auto score = [&](int n) { return sample_score(lr, pb, penalty, temperature, n); };
     // fn(n, score(n)) for every id; a thread reads SAMPLE_UNROLL ids before it consumes them, so it has that many loads in flight
     auto scan_row = [&](auto&& fn) {
         for (int base = 0; base < V; base += SELECT_THREADS * SAMPLE_UNROLL) {
@@ -369,8 +388,8 @@ __global__ void __launch_bounds__(SELECT_THREADS) sample_select_kernel(
     // top-p: the key whose group holds the cut, and how many of the group (lowest ids first) go
     uint32_t key_p = 0;
     int id_p = 0;
-    if (top_p < 1.0f) {
-        const float thr = (float)(1.0 - (double)top_p);
+    if (top_p < 1.0) {
+        const float thr = (float)(1.0 - top_p);      // HF's threshold: the caller's 1 - top_p in double, compared in fp32
         unsigned long long rest = radix_select([&](uint32_t k) { return k >= key_k; }, [&](float x) { return mass_fx(x, mx); }, false, thr,
                                                0ull, &key_p);
         // ids of the group at the cut with cumulative mass below + (j + 1) q <= limit go: the first floor(rest / q)
@@ -428,12 +447,8 @@ __global__ void __launch_bounds__(SELECT_THREADS) sample_select_kernel(
                 const int n = g * 4 + l;
                 const uint32_t k = order_key(x[h * 4 + l]);
                 if (n >= V || k < key_k || k < key_p || (k == key_p && n < id_p)) continue;
-                if (!drawn) { r = philox4x32_10(make_uint4((uint32_t)g, (uint32_t)step, 0u, 0u), seed_lo, seed_hi); drawn = true; }
-                // e = -log(u), u = (m + 0.5) 2^-24 without rounding u: for m >= 2^23, 1 - u = (2^24 - m - 0.5) 2^-24 is exact instead
-                const uint32_t m = (l == 0 ? r.x : l == 1 ? r.y : l == 2 ? r.z : r.w) >> 8;
-                const float e = m < (1u << 23) ? -logf(((float)m + 0.5f) * 5.9604644775390625e-8f)
-                                               : -log1pf(-((float)((1u << 24) - m) - 0.5f) * 5.9604644775390625e-8f);
-                const float v = (x[h * 4 + l] - mx) - logf(e);
+                if (!drawn) { r = sample_philox(g, step, seed_lo, seed_hi); drawn = true; }
+                const float v = gumbel_perturbed(x[h * 4 + l], mx, gumbel_e(philox_lane(r, l)));
                 if (v > best || bid == 0x7fffffff) { best = v; bid = n; }
                 if (kb) atomicOr(&kb[n >> 5], 1u << (n & 31));
             }
@@ -443,6 +458,40 @@ __global__ void __launch_bounds__(SELECT_THREADS) sample_select_kernel(
     if (tid == 0)
         select_commit(b, tok, pen_bitmap, pen_words, eos_ids, n_eos, max_new, first_pos, B, tokens, lengths, done, n_done, all_done, next_ids,
                       pos3);
+}
+
+// The per-id terms sample_select_kernel decides on, through the same helpers, for tests: for row b and id n (t = lengths[b])
+//   score[b, n] = sample_score, row_max[b] = the row's maximum score, ex[b, n] = expf(score - max), mass[b, n] = mass_of_exp(ex),
+//   bits[b, n] = lane n & 3 of the Philox block (seeds[b], n >> 2, t), e[b, n] = gumbel_e(bits), v[b, n] = gumbel_perturbed(score, max, e).
+// Every row is written, finished or not (the maximum is exact in any order). One block per row.
+constexpr int SAMPLE_TERMS_THREADS = 256;
+__global__ void __launch_bounds__(SAMPLE_TERMS_THREADS) sample_terms_kernel(
+        const __nv_bfloat16* __restrict__ logits, int V, const uint32_t* __restrict__ pen_bitmap, int pen_words, float penalty,
+        const unsigned long long* __restrict__ seeds, float temperature, const int* __restrict__ lengths, float* __restrict__ score,
+        float* __restrict__ row_max, float* __restrict__ ex, unsigned long long* __restrict__ mass, uint32_t* __restrict__ bits,
+        float* __restrict__ e_out, float* __restrict__ v_out) {
+    pdl_launch_dependents();
+    __shared__ float s_m[SAMPLE_TERMS_THREADS / 32];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    const __nv_bfloat16* lr = logits + (size_t)b * V;
+    const uint32_t* pb = pen_bitmap ? pen_bitmap + (size_t)b * pen_words : nullptr;
+    float mx = -INFINITY;
+    for (int n = tid; n < V; n += SAMPLE_TERMS_THREADS) mx = fmaxf(mx, sample_score(lr, pb, penalty, temperature, n));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((tid & 31) == 0) s_m[tid >> 5] = mx;
+    __syncthreads();
+    for (int w = 0; w < SAMPLE_TERMS_THREADS / 32; ++w) mx = fmaxf(mx, s_m[w]);
+    if (tid == 0) row_max[b] = mx;
+    const uint32_t seed_lo = (uint32_t)seeds[b], seed_hi = (uint32_t)(seeds[b] >> 32);
+    const int step = lengths[b];
+    for (int n = tid; n < V; n += SAMPLE_TERMS_THREADS) {
+        const size_t i = (size_t)b * V + n;
+        const float x = sample_score(lr, pb, penalty, temperature, n), xe = expf(x - mx);
+        const uint32_t u = philox_lane(sample_philox(n >> 2, step, seed_lo, seed_hi), n & 3);
+        const float e = gumbel_e(u);
+        score[i] = x; ex[i] = xe; mass[i] = mass_of_exp(xe); bits[i] = u; e_out[i] = e; v_out[i] = gumbel_perturbed(x, mx, e);
+    }
 }
 
 // Answer log-probabilities of one generation step (the scores a rollout is scored on), one block per sequence, launched between the
@@ -630,4 +679,13 @@ static int sample_select(Forward& f, const bf16* logits, int B, int V, uint32_t*
     return f.launch(CAT_OTHER, 0, "sample select", sample_select_kernel, B, SELECT_THREADS, 0, logits, V, pen_bitmap, (V + 31) / 32, penalty,
                     (const unsigned long long*)s.seeds, s.temperature, s.top_k, s.top_p, eos_ids, n_eos, max_new, first_pos, B, tokens,
                     lengths, done, n_done, all_done, next_ids, pos3, kept);
+}
+
+// The per-id terms of sample_select's draw for rows [0, B) at steps lengths[b] (tests; see sample_terms_kernel), each output [B, V]
+// except row_max [B].
+static int sample_terms(Forward& f, const bf16* logits, int B, int V, const uint32_t* pen_bitmap, float penalty, const vqa_qwen25vl_sampling& s,
+                        const int* lengths, float* score, float* row_max, float* ex, unsigned long long* mass, uint32_t* bits, float* e,
+                        float* v) {
+    return f.launch(CAT_OTHER, 0, "sample terms", sample_terms_kernel, B, SAMPLE_TERMS_THREADS, 0, logits, V, pen_bitmap, (V + 31) / 32,
+                    penalty, (const unsigned long long*)s.seeds, s.temperature, lengths, score, row_max, ex, mass, bits, e, v);
 }

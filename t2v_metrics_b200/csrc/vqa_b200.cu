@@ -154,7 +154,7 @@ extern "C" size_t vqa_clipt5_generate_workspace_bytes(vqa_handle* h, int32_t bat
 static int sampling_check(vqa_handle* h, const vqa_qwen25vl_sampling* s, const vqa_qwen25vl_answer_score* score) {
     if (!s || !s->seeds) return fail(h, VQA_ERR_INVALID_ARG, "sampling: null sampling struct or seeds");
     if (score) return fail(h, VQA_ERR_INVALID_ARG, "sampling: a scored rollout is greedy (gen->score must be NULL)");
-    if (!(s->temperature > 0.f) || !std::isfinite(s->temperature) || s->top_k < 0 || !(s->top_p > 0.f) || !(s->top_p <= 1.f))
+    if (!(s->temperature > 0.f) || !std::isfinite(s->temperature) || s->top_k < 0 || !(s->top_p > 0.0) || !(s->top_p <= 1.0))
         return fail(h, VQA_ERR_INVALID_ARG, "sampling: bad parameters (temperature > 0 and finite, top_k >= 0, 0 < top_p <= 1)");
     return VQA_OK;
 }
@@ -695,6 +695,19 @@ extern "C" int vqa_op_sample_select(const void* logits, int32_t B, int32_t V, ui
     return glue_launch(stream, [&](Forward& f) {
         return sample_select(f, (const bf16*)logits, B, V, pen_bitmap, repetition_penalty, *sampling, eos_ids, n_eos, max_new, first_pos, tokens,
                              lengths, done, n_done, all_done, next_ids, pos3, kept);
+    });
+}
+
+extern "C" int vqa_debug_sample_terms(const void* logits, int32_t B, int32_t V, const uint32_t* pen_bitmap, float repetition_penalty,
+                                      const int32_t* lengths, const vqa_qwen25vl_sampling* sampling, float* score, float* row_max, float* expv,
+                                      uint64_t* mass, uint32_t* bits, float* gumbel_e, float* perturbed, void* stream) {
+    if (!logits || !lengths || !score || !row_max || !expv || !mass || !bits || !gumbel_e || !perturbed)
+        return fail(nullptr, VQA_ERR_INVALID_ARG, "sample terms: null pointer");
+    if (B <= 0 || V <= 0 || !(repetition_penalty > 0.f)) return fail(nullptr, VQA_ERR_INVALID_ARG, "sample terms: bad size / repetition penalty");
+    if (int rc = sampling_check(nullptr, sampling, nullptr)) return rc;
+    return glue_launch(stream, [&](Forward& f) {
+        return sample_terms(f, (const bf16*)logits, B, V, pen_bitmap, repetition_penalty, *sampling, lengths, score, row_max, expv,
+                            (unsigned long long*)mass, bits, gumbel_e, perturbed);
     });
 }
 

@@ -630,7 +630,8 @@ class ops:
                       lengths: torch.Tensor, done: torch.Tensor, n_done: torch.Tensor, all_done: torch.Tensor, next_ids: torch.Tensor, eos_ids=None,
                       pen_bitmap=None, repetition_penalty: float = 1.0, first_pos=None, pos3=None, kept=None):
         """One sampled selection step (vqa_op_sample_select): greedy_select's state and arguments, plus int64 seeds [B] on the device and
-        the warpers' (temperature, top_k, top_p). kept: None or int32 [B, ceil(V / 32)] that receives each unfinished row's kept-id bitmap."""
+        the warpers' (temperature, top_k, top_p; top_p goes to the kernel as the double it is, so its threshold is HF's fp32(1 - top_p)).
+        kept: None or int32 [B, ceil(V / 32)] that receives each unfinished row's kept-id bitmap."""
         B, V = logits.shape
         n_eos = eos_ids.numel() if eos_ids is not None else 0
         smp = _lib.VqaQwen25VLSampling(seeds=_ptr(seeds), temperature=float(temperature), top_k=int(top_k), top_p=float(top_p))

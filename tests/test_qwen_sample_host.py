@@ -208,3 +208,7 @@ def test_sampling_struct_layout_matches_header():
     cls = _lib.VqaQwen25VLSampling
     assert [f[0] for f in cls._fields_] == re.findall(r"(\w+);", body)
     assert ctypes.sizeof(cls) == 24 and cls.temperature.offset == 8 and cls.top_k.offset == 12 and cls.top_p.offset == 16
+    # top_p is a double in the header and the binding: a float field would round the caller's top_p before 1 - top_p is formed
+    assert re.search(r"\bdouble\s+top_p;", body) and dict(cls._fields_)["top_p"] is ctypes.c_double
+    s = cls(top_p=0.9)
+    assert s.top_p == 0.9
